@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py - scan-pairs/sec of DGR's pairwise-registration hot path on B200.
+"""bench.py - scan-pairs/sec of DGR's pairwise-registration hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \\
         --master-port P bench.py --gpus N --steps K --warmup W
 
@@ -16,6 +16,8 @@ Prints ONE JSON line (rank 0).  `value` = pairs/s with the raw scans resident in
 `e2e` = pairs/s through DeepGlobalRegistration.register(host ndarrays) including the H2D
 copy of both scans and the D2H read of the pose.  `--impl reference` times the CPU oracle
 port of the same path (MinkowskiEngine cannot be installed offline) on a bounded sample.
+`--dump-outputs DIR` writes the pose the timed loop computed in its last step as DIR/pose.npy (float64
+[4, 4]); the inputs are generated from fixed seeds, so two builds can be compared output for output.
 """
 import argparse
 import gc
@@ -59,7 +61,7 @@ def base_config(n_gpus):
   (voxel counts seen, sample notes) goes into other keys of the line."""
   return {'workload': WORKLOAD, 'n_raw_points_per_scan': N_RAW, 'voxel_size': VOXEL, 'feat_dim': 32,
           'fcgf_model': 'ResUNetBN2C(D=3,conv1_k=7)', 'inlier_model': 'ResUNetBN2C(D=6,conv1_k=3)',
-          'conv_arithmetic': 'tcgen05 split products, fp32 accumulate: 3xFP16 hi/lo on the wide layers, 3xTF32 elsewhere (both fp32-accurate: features within 5e-5 of the fp32 oracle at full size); fp32 adds for conv1',
+          'conv_arithmetic': 'wgmma split products, fp32 accumulate: 3xFP16 hi/lo on the wide layers, 3xTF32 elsewhere (both fp32-accurate: features within 5e-5 of the fp32 oracle at full size); fp32 adds for conv1',
           'parallelism': f'pair-sharded dp{n_gpus}', 'pairs_per_step_per_gpu': 1,
           'excluded_on_both_arms': 'ICP fine-tune and RANSAC safeguard (both built; the benchmarked unit is SURVEY 8(d)\'s: through the SE(3) refinement, and the benchmark pairs take the Procrustes branch)',
           'l2_policy': 'inputs larger than L2: every step streams the 944 MB inlier-net weights '
@@ -287,7 +289,7 @@ def stage_isolated_parity(dgr, pair_dev):
 
 def run_reference(args):
   """The reference's CPU implementation of the path (the oracle port: MinkowskiEngine is not installable
-  offline, nothing of the reference compiles into oracle/_ref) on the SAME configuration as the B200 arm:
+  offline, nothing of the reference compiles into oracle/_ref) on the SAME configuration as the H100 arm:
   full-size pairs of the same generator and seeds.  One such pair is minutes of CPU, so the run executes as
   many of the K steps as fit REF_TIME_BUDGET_S after the first (at least one) and says how many
   (cpu_baseline.steps_executed); pairs/s is per executed full-size pair, nothing is extrapolated."""
@@ -322,7 +324,7 @@ def run_reference(args):
           'ms_per_step': 1e3 * dt / n_exec, 'higher_is_better': True, 'scaling': 'weak',
           'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic', 'config': base_config(args.gpus),
           'cpu_baseline': {'value': val, 'unit': 'pairs/s', 'cores': cores, 'kind': 'port',
-                           'sample': f'{n_exec} FULL-SIZE pair(s) of the workload (same generator and seeds as the B200 arm: '
+                           'sample': f'{n_exec} FULL-SIZE pair(s) of the workload (same generator and seeds as the H100 arm: '
                                      f'{N_RAW} raw points per scan -> N0={info["n0"]}, N1={info["n1"]} voxels), not a reduced sample; '
                                      'CPU path = oracle port (torch-CPU index_select/mm/index_add per kernel offset, the algorithm '
                                      "of MinkowskiEngine's CPU backend) + restated kNN / Procrustes / Adam refinement",
@@ -334,7 +336,7 @@ def run_reference(args):
 
 
 # ------------------------------------------------------------------------------------------
-# the B200 arm
+# the H100 arm
 # ------------------------------------------------------------------------------------------
 def run_ours(args):
   import torch.distributed as dist
@@ -452,6 +454,8 @@ def run_ours(args):
   t_start = time.time()
   thr0 = cgroup_throttled_ms()
   res = timed(K, host_inputs=False)               # `value`: scans resident in HBM
+  if args.dump_outputs and rank == 0:
+    dump_outputs(args.dump_outputs, res['last'])
   res_e2e = timed(K, host_inputs=True)            # `e2e`: host buffers in, pose out
   t_end = time.time()
   thr1 = cgroup_throttled_ms()
@@ -489,14 +493,14 @@ def run_ours(args):
   e2e = n_total / (res_e2e['ms'] / 1e3)
 
   # ---- roofline of the dominant kernel (live CUDA events around every launch, serial pass) ------------
-  peaks, peak_src = None, 'fallback (B200_PROFILING.md: 6650 GB/s, 1590 TFLOP/s bf16)'
+  peaks, peak_src = None, 'fallback (H100 SXM data sheet: 3350 GB/s, 989 TFLOP/s dense bf16)'
   try:
     peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
     peak_src = 'measured (MEASURED_PEAKS.json)'
   except Exception:   # noqa: BLE001
     pass
-  hbm_peak = float(peaks['hbm_gbs']) if peaks else 6650.0
-  bf16_peak = float(peaks.get('bf16_tflops_sustained', peaks['bf16_tflops'])) if peaks else 1400.0
+  hbm_peak = float(peaks['hbm_gbs']) if peaks else 3350.0
+  bf16_peak = float(peaks.get('bf16_tflops_sustained', peaks['bf16_tflops'])) if peaks else 989.0
   roofline, roofline_tensor, kernel_share = None, None, None
   if prof_rows is not None and len(prof_rows):
     names = {0: 'spconv_tc_kernel', 1: 'spconv_fwd_kernel', 2: 'spconv_table_kernel'}
@@ -511,15 +515,8 @@ def run_ours(args):
     n, ms, flops, nbytes = by[dom]
     gbs = nbytes / (ms * 1e-3) / 1e9
     tfs = flops / (ms * 1e-3) / 1e12
-    traffic = None
-    for name in ('r02_spconv_tc_traffic.json', 'r01_spconv_tc_traffic.json'):
-      try:   # per-launch DRAM bytes from the committed ncu --set full capture, if present
-        traffic = json.load(open(os.path.join(ROOT, 'profiles', name)))['dram_bytes_per_launch']
-        break
-      except Exception:   # noqa: BLE001
-        pass
     roofline = {'kernel': dom, 'bound': 'hbm', 'achieved': gbs, 'peak': hbm_peak, 'unit': 'GB/s',
-                'frac': gbs / hbm_peak, 'traffic': traffic, 'peak_source': peak_src,
+                'frac': gbs / hbm_peak, 'peak_source': peak_src,
                 'launches_per_step': n / n_prof, 'avg_launch_ms': ms / n,
                 'algorithmic_bytes_per_launch': nbytes / n,
                 'bytes_model': 'SURVEY 8(d) gather-scatter model: P*(Cin+Cout)*4 + 8*P + K_nonempty*Cin*Cout*4',
@@ -597,6 +594,14 @@ def run_ours(args):
     dist.destroy_process_group()
 
 
+def dump_outputs(dirname, last):
+  """The last timed step's result as a caller of register() receives it: the 4x4 pose, float64."""
+  T = last[0]
+  T = T.detach().cpu().numpy() if torch.is_tensor(T) else np.asarray(T)
+  os.makedirs(dirname, exist_ok=True)
+  np.save(os.path.join(dirname, 'pose.npy'), T.astype(np.float64))
+
+
 def main():
   # keep stdout clean for the ONE JSON line: libraries (NCCL's version banner, ...) write to fd 1
   real_stdout = os.dup(1)
@@ -606,10 +611,12 @@ def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--gpus', type=int, default=1)
   ap.add_argument('--steps', type=int, default=None,
-                  help='timed steps (default 100 for the B200 arm: ~1.5 s per region, so that one ~0.3 s host stall '
+                  help='timed steps (default 100 for the H100 arm, so that one ~0.3 s host stall '
                        'of a shared box costs 10-20 %% instead of halving the number; 10 for --impl reference)')
   ap.add_argument('--warmup', type=int, default=3)
   ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
+  ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                  help='write what the timed loop computed in its last step (the pose) to DIR/pose.npy')
   ap.add_argument('--pairs', type=int, default=0,
                   help='BASELINE config 4: register this many pairs (seeds 0..pairs-1) round-robin over the ranks - '
                        'the same total at every N (strong scaling); 0 = the contract mode (K steps per rank, weak)')

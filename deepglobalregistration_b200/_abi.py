@@ -2,7 +2,7 @@
 
 torch is used here for device memory and the current CUDA stream only; every
 computation happens inside the library.  There is no CPU fallback: importing this
-module without a built library, or calling into it without an sm_100 device,
+module without a built library, or calling into it without an sm_90 device,
 raises.
 """
 import ctypes as C
@@ -51,7 +51,7 @@ SIGNATURES = {
     'dgr_spconv_fwd': [_p, _i32, _p, _i32, _p, _p, _p, _p, _p, _i32, _i32, _i32, _p, _p],
     'dgr_spconv_tc_supported': [_i32, _i32],
     'dgr_pack_weight_tf32': [_p, _i32, _i32, _i32, _p, _p],
-    'dgr_spconv_tc_fwd': [_p, _i32, _p, _i32, _p, _p, _p, _p, _p, _i32, _i32, _i32, _i32, _p, _p],
+    'dgr_spconv_tc_fwd': [_p, _i32, _p, _i32, _p, _p, _p, _p, _p, _i32, _i32, _i32, _p, _p],
     'dgr_spconv_table_fwd': [_p, _i32, _p, _i32, _p, _i32, _i64, _p, _p, _p, _p],
     'dgr_linear_fwd': [_p, _i32, _p, _i32, _i64, _p, _i32, _p, _i32, _i32, _p, _p],
     'dgr_affine_act': [_p, _i64, _i32, _p, _p, _p, _i32, _p, _p],
@@ -164,7 +164,7 @@ _checked_devices = set()
 def require_device(device):
   device = torch.device(device)
   if device.type != 'cuda':
-    raise DgrError(f'libdgr_b200 computes on CUDA (sm_100a) only, got device {device}; there is no '
+    raise DgrError(f'libdgr_b200 computes on CUDA (sm_90a) only, got device {device}; there is no '
                    'CPU fallback')
   idx = device.index if device.index is not None else torch.cuda.current_device()
   if idx not in _checked_devices:
@@ -329,7 +329,7 @@ class KernelMap:
                'tile_k', 'tile_start', 'n_tiles', '_paired')
 
   def paired_tiles(self):
-    """(tile_k, tile_start, n_tiles) with an even tile count per offset (2-CTA cluster kernel)."""
+    """(tile_k, tile_start, n_tiles) with an even tile count per offset (the extra tiles are empty)."""
     if getattr(self, '_paired', None) is None:
       counts = self.kofs_host[1:] - self.kofs_host[:-1]
       per_k = (counts + TILE_ROWS - 1) // TILE_ROWS
@@ -456,15 +456,6 @@ def pack_weight_tf32(weight, K, cin, cout):
   return packed
 
 
-# kernel variant of the tensor-core convolution: 1 = one CTA per tile, both operands in shared
-# memory (default), 0 = A operand in tensor memory, 2 = CTA pairs with multicast weight tiles,
-# 3 = cta_group::2 (one M = 256 MMA per tile pair, half of every weight tile per CTA; used for
-# cout >= TC_PAIR_MIN_COUT, else 1).  All four are parity-tested.  With the line-coalesced epilogue
-# variant 3 is ~6 % faster on the wide layers (profiles/r01_spconv_tc_experiments.txt); default since
-# round 2 (the whole GPU suite runs with it).
-TC_VARIANT = int(os.environ.get('DGR_TC_VARIANT', '3'))
-TC_PAIR_MIN_COUT = int(os.environ.get('DGR_TC_PAIR_MIN_COUT', '128'))
-
 # When set to a list, every sparse-convolution launch appends
 # (kernel name, start event, end event, algorithmic flops, gather-scatter-model bytes):
 # bench.py's live per-kernel roofline measurement (CUDA events on the launching stream).
@@ -486,28 +477,20 @@ def _conv_profiled(name, km, cin, cout, fn):
   CONV_PROFILE.append((name, e0, e1, flops, nbytes))
 
 
-def spconv_tc_fwd(feat, weight_t, km, out, passes=3, cluster=None):
+def spconv_tc_fwd(feat, weight_t, km, out, passes=3):
   """Tensor-core gather-GEMM-scatter: out[km.out_idx] += feat[km.in_idx] @ W[kappa]."""
   _chk(feat, torch.float32, 'feat'); _chk(weight_t, torch.float32, 'weight_t'); _chk(out, torch.float32, 'out')
   cin, cout = feat.shape[1], out.shape[1]
   assert weight_t.numel() == 2 * km.K * cin * cout
   assert feat.shape[0] == km.n_in and out.shape[0] == km.n_out
-  if cluster is None:
-    cluster = TC_VARIANT
-    if cluster == 3 and cout < TC_PAIR_MIN_COUT:
-      cluster = 1               # narrow layers are bound by the gather, not by weight ingress: no pairing
-  if cluster in (2, 3):
-    tk, ts, nt = km.paired_tiles()
-  else:
-    tk, ts, nt = km.tile_k, km.tile_start, km.n_tiles
   _conv_profiled('spconv_tc_kernel', km, cin, cout, lambda: call(
       'dgr_spconv_tc_fwd', ptr(feat), cin, ptr(weight_t), cout, ptr(km.in_idx), ptr(km.out_idx),
-      ptr(km.kofs), ptr(tk), ptr(ts), nt, TILE_ROWS, int(passes), cluster, ptr(out), stream()))
+      ptr(km.kofs), ptr(km.tile_k), ptr(km.tile_start), km.n_tiles, TILE_ROWS, int(passes), ptr(out), stream()))
   return out
 
 
 def spconv_tc_f16_fwd(feat, weight, km, out, amax=None):
-  """3xFP16 cta_group::2 convolution (weight: the fp32 [K, cin, cout] kernel; packed per call - test helper)."""
+  """3xFP16 tensor-core convolution (weight: the fp32 [K, cin, cout] kernel; packed per call - test helper)."""
   _chk(feat, torch.float32, 'feat'); _chk(weight, torch.float32, 'weight'); _chk(out, torch.float32, 'out')
   cin, cout = feat.shape[1], out.shape[1]
   packed = torch.empty(4 * km.K * cin * cout, dtype=torch.uint8, device=feat.device)
@@ -516,9 +499,8 @@ def spconv_tc_f16_fwd(feat, weight, km, out, amax=None):
   if amax is None:
     amax = torch.empty(1, dtype=torch.float32, device=feat.device)
     call('dgr_absmax_f32', ptr(feat), feat.numel(), ptr(amax), stream())
-  tk, ts, nt = km.paired_tiles()
   call('dgr_spconv_tc_f16_fwd', ptr(feat), cin, ptr(packed), cout, ptr(km.in_idx), ptr(km.out_idx), ptr(km.kofs),
-       ptr(tk), ptr(ts), nt, TILE_ROWS, ptr(amax), ptr(wscale), ptr(out), stream())
+       ptr(km.tile_k), ptr(km.tile_start), km.n_tiles, TILE_ROWS, ptr(amax), ptr(wscale), ptr(out), stream())
   return out
 
 

@@ -1,4 +1,4 @@
-"""Build libdgr_b200.so in-tree with nvcc for sm_100a (no torch headers in the ABI, so a
+"""Build libdgr_b200.so in-tree with nvcc for sm_90a (no torch headers in the ABI, so a
 full rebuild takes well under a minute and needs no GPU).
 
     python -m deepglobalregistration_b200.build [--force]
@@ -16,9 +16,9 @@ INCLUDE = os.path.join(ROOT, 'include')
 LIB = os.path.join(HERE, 'libdgr_b200.so')
 OBJ_DIR = os.path.join(HERE, 'build')
 
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr', '-I', INCLUDE, '-I', CSRC]
-NVCC_FLAGS += os.environ.get('DGR_EXTRA_NVCC_FLAGS', '').split()      # A/B build switches (e.g. -DDGR_GATHER_CG)
+NVCC_FLAGS += os.environ.get('DGR_EXTRA_NVCC_FLAGS', '').split()      # extra build flags (A/B experiments)
 
 
 def _nvcc():
@@ -44,7 +44,7 @@ def _fingerprint():
 
 
 def build(force=False, verbose=False):
-  """Compile every csrc/*.cu for sm_100a and link libdgr_b200.so.  Returns its path."""
+  """Compile every csrc/*.cu for sm_90a and link libdgr_b200.so.  Returns its path."""
   os.makedirs(OBJ_DIR, exist_ok=True)
   stamp = os.path.join(OBJ_DIR, 'fingerprint')
   fp = _fingerprint()

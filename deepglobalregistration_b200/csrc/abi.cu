@@ -35,8 +35,8 @@ int32_t dgr_device_check(int32_t device) {
     dgr_set_error("cudaGetDeviceProperties(%d): %s", device, cudaGetErrorString(e));
     return DGR_ERR_DEVICE;
   }
-  if (prop.major != 10) {
-    dgr_set_error("device %d is sm_%d%d; libdgr_b200 is built for sm_100a (B200) only", device,
+  if (prop.major != 9 || prop.minor != 0) {
+    dgr_set_error("device %d is sm_%d%d; libdgr_b200 is built for sm_90a (H100) only", device,
                   prop.major, prop.minor);
     return DGR_ERR_DEVICE;
   }

@@ -596,9 +596,9 @@ static size_t probe_smem_bytes(int k_per_block, int64_t n_bloom_words) {
          (size_t)n_bloom_words * 4;
 }
 static int probe_k_per_block(int K, unsigned row_blocks) {
-  // kappa chunks: enough blocks for ~2 waves of the 148 SMs at 2 blocks per SM, at most 96 offsets per block
+  // kappa chunks: enough blocks for ~2 waves of the 132 SMs at 2 blocks per SM, at most 96 offsets per block
   int k_per_block = K;
-  while (k_per_block > 16 && (int64_t)row_blocks * ((K + k_per_block - 1) / k_per_block) < 592) k_per_block = (k_per_block + 1) / 2;
+  while (k_per_block > 16 && (int64_t)row_blocks * ((K + k_per_block - 1) / k_per_block) < 528) k_per_block = (k_per_block + 1) / 2;
   if (k_per_block > 96) k_per_block = 96;
   return (k_per_block + 3) & ~3;
 }

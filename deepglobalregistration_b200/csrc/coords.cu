@@ -445,7 +445,7 @@ int32_t dgr_coords_minmax(const int32_t* coords, int64_t n, int32_t ncols, int32
   minmax_init_kernel<<<1, 32, 0, st>>>(minmax, ncols);
   if (n > 0) {
     unsigned blocks = dgr_blocks(n, kThreads * 4);
-    if (blocks > 1184) blocks = 1184;   // 148 SMs x 8
+    if (blocks > 1056) blocks = 1056;   // 132 SMs x 8
     minmax_kernel<<<blocks, kThreads, 0, st>>>(coords, n, ncols, minmax);
   }
   dgr_note_launches(n > 0 ? 2 : 1);

@@ -43,10 +43,9 @@ constexpr int kMetaNetBase = 8;       // meta[0..8): pair counts (N, N0, N1, key
 constexpr int kMetaPerMap = 5;
 constexpr int kKeyMargin = 32;        // spare cells around the bounding box (7^3 kernels, stride-8 flooring)
 
-int tc_variant();
 bool tc_f16_enabled();
 bool tc_os_enabled();
-int tc_pair_min_cout();
+int tc_f16_min_cout();
 
 #define DGR_TRY(expr)                 \
   do {                                \
@@ -314,9 +313,8 @@ struct KMap {
   int32_t* cnt = nullptr;
   int32_t* kofs = nullptr;
   int32_t* meta = nullptr;
-  int P = 0, n_tiles = 0, n_ptiles = 0, nonempty = 0;
-  int32_t *in_idx = nullptr, *out_idx = nullptr, *tile_k = nullptr, *tile_start = nullptr, *ptile_k = nullptr,
-          *ptile_start = nullptr;
+  int P = 0, n_tiles = 0, nonempty = 0;
+  int32_t *in_idx = nullptr, *out_idx = nullptr, *tile_k = nullptr, *tile_start = nullptr;
   int32_t* nbr = nullptr;
   int64_t nbr_stride = 0;
 };
@@ -450,7 +448,7 @@ int32_t plan_finish(dgr_ctx* c, Plan& p) {
       m.nonempty = m.dense ? m.K : mm[3];
       continue;
     }
-    m.P = mm[0]; m.n_tiles = mm[1]; m.n_ptiles = mm[2]; m.nonempty = mm[3];
+    m.P = mm[0]; m.n_tiles = mm[1]; m.nonempty = mm[3];
     if (mm[4] != 0) {
       dgr_set_error("coordinate extent does not fit a 63-bit packed key");
       return DGR_ERR_ARG;
@@ -461,13 +459,10 @@ int32_t plan_finish(dgr_ctx* c, Plan& p) {
     DGR_TRY(aalloc(c, m.P, &m.out_idx));
     DGR_TRY(aalloc(c, m.n_tiles, &m.tile_k));
     DGR_TRY(aalloc(c, m.n_tiles, &m.tile_start));
-    DGR_TRY(aalloc(c, m.n_ptiles, &m.ptile_k));
-    DGR_TRY(aalloc(c, m.n_ptiles, &m.ptile_start));
     if (m.P > 0) {
       DGR_TRY(dgr_kmap_fill(m.bits, m.cnt, m.K, Lout.n_max > 0 ? Lout.n_max : 1, Lout.coords, p.ncols, p.spec, Lin.keys,
                             Lin.vals, Lin.cap, m.offsets, m.in_idx, m.out_idx, st));
-      DGR_TRY(dgr_kernel_map_tiles2(m.kofs, m.K, kTileRows, m.n_tiles, m.n_ptiles, m.tile_k, m.tile_start, m.ptile_k,
-                                    m.ptile_start, st));
+      DGR_TRY(dgr_kernel_map_tiles(m.kofs, m.K, kTileRows, m.n_tiles, 0, m.tile_k, m.tile_start, st));
     }
   }
   return DGR_OK;
@@ -486,14 +481,6 @@ struct LayerExec {
   bool bits;      // conv1 on an all-ones input from the occupancy masks
 };
 
-int tc_variant() {
-  static const int v = [] {
-    const char* e = getenv("DGR_TC_VARIANT");
-    const int x = e ? atoi(e) : 3;
-    return (x < 0 || x > 3) ? 1 : x;
-  }();
-  return v;
-}
 bool tc_f16_enabled() {
   static const bool v = [] {
     const char* e = getenv("DGR_TC_F16");
@@ -504,13 +491,13 @@ bool tc_f16_enabled() {
 bool tc_os_enabled() {
   static const bool v = [] {
     const char* e = getenv("DGR_TC_OS");      // output-stationary kernel for the 3-D stride-1 layers: opt-in (measured
-    return e ? atoi(e) != 0 : false;          // slower than the pair-list kernel on B200, see DESIGN.md)
+    return e ? atoi(e) != 0 : false;          // slower than the pair-list kernel, see DESIGN.md)
   }();
   return v;
 }
-int tc_pair_min_cout() {
+int tc_f16_min_cout() {
   static const int v = [] {
-    const char* e = getenv("DGR_TC_PAIR_MIN_COUT");
+    const char* e = getenv("DGR_TC_F16_MIN_COUT");
     return e ? atoi(e) : 128;
   }();
   return v;
@@ -557,16 +544,12 @@ int32_t run_conv(dgr_ctx* c, const LayerExec& L, const float* feat, const float*
           DGR_TRY(dgr_absmax_f32(feat, (int64_t)L.n_in * cv.cin, amax, st));
           if (prof) cudaEventRecord(rec.e0, c->stream);      // the timed launch is the convolution itself
         }
-        DGR_TRY(dgr_spconv_tc_f16_fwd(feat, cv.cin, cv.packed16, cv.cout, in_idx, out_idx, m.kofs, m.ptile_k,
-                                      m.ptile_start, m.n_ptiles, kTileRows, amax, cv.wscale, out, st));
+        DGR_TRY(dgr_spconv_tc_f16_fwd(feat, cv.cin, cv.packed16, cv.cout, in_idx, out_idx, m.kofs, m.tile_k,
+                                      m.tile_start, m.n_tiles, kTileRows, amax, cv.wscale, out, st));
         rec.kind = 0;
       } else if (cv.tc) {
-        int variant = tc_variant();
-        if (variant == 3 && cv.cout < tc_pair_min_cout()) variant = 1;
-        const bool paired = variant == 2 || variant == 3;
-        DGR_TRY(dgr_spconv_tc_fwd(feat, cv.cin, cv.packed, cv.cout, in_idx, out_idx, m.kofs,
-                                  paired ? m.ptile_k : m.tile_k, paired ? m.ptile_start : m.tile_start,
-                                  paired ? m.n_ptiles : m.n_tiles, kTileRows, 3, variant, out, st));
+        DGR_TRY(dgr_spconv_tc_fwd(feat, cv.cin, cv.packed, cv.cout, in_idx, out_idx, m.kofs, m.tile_k, m.tile_start,
+                                  m.n_tiles, kTileRows, 3, out, st));
         rec.kind = 0;
       } else {
         DGR_TRY(dgr_spconv_fwd(feat, cv.cin, cv.w, cv.cout, in_idx, out_idx, m.kofs, m.tile_k, m.tile_start, m.n_tiles,
@@ -835,7 +818,7 @@ int32_t dgr_net_create(int32_t device, int32_t D, int32_t in_ch, int32_t out_ch,
     cv.w = params[pi++]; cv.scale = params[pi++]; cv.shift = params[pi++];
     cv.cin = cin; cv.cout = cout; cv.ksize = ksize; cv.K = K;
     cv.tc = dgr_spconv_tc_supported(cin, cout) != 0;
-    cv.f16 = cv.tc && !os && tc_f16_enabled() && tc_variant() == 3 && cout >= tc_pair_min_cout() &&
+    cv.f16 = cv.tc && !os && tc_f16_enabled() && cout >= tc_f16_min_cout() &&
              dgr_spconv_tc_f16_supported(cin, cout) != 0;
     if (cv.f16) {
       DGR_CUDA_CHECK(cudaMalloc(&cv.packed16, (size_t)4 * K * cin * cout));

@@ -13,8 +13,6 @@
 // sqrt is monotone, so a candidate can only win if d2 < best_d2; only then is the exact
 // root evaluated.  The row result is the lexicographic minimum of (root, index), merged
 // across column splits with one 64-bit atomicMin on (root_bits << 32 | index).
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace {
@@ -113,115 +111,6 @@ knn_top1_kernel(const float* __restrict__ f0, int n0, const float* __restrict__ 
   }
 }
 
-// Packed-math variant: Blackwell issues two fp32 operations per lane with FADD2 / FFMA2
-// (PTX sub.f32x2 / fma.rn.f32x2).  Rows are paired (a_2p, a_2p+1) straight out of the
-// transposed A tile; every B value is stored duplicated (b, b) so one 64-bit shared load
-// feeds both halves.  Per channel a thread issues 32 FADD2 + 32 FFMA2 for its 8x8 block -
-// half the instructions of the scalar kernel, bit-identical results (same fma chain).
-__device__ __forceinline__ unsigned long long f2_sub(unsigned long long a, unsigned long long b) {
-  unsigned long long d;
-  asm("sub.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ unsigned long long f2_fma(unsigned long long a, unsigned long long b,
-                                                     unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-
-template <int C>
-__global__ void __launch_bounds__(kThreads, 2)
-knn_top1_f2_kernel(const float* __restrict__ f0, int n0, const float* __restrict__ f1, int n1,
-                   int cols_per_split, unsigned long long* __restrict__ packed) {
-  // A: [C][kBM] transposed floats; B: [kBN][C + 1] duplicated pairs (b, b)
-  extern __shared__ __align__(16) float knn_smem[];
-  float* As = knn_smem;
-  float2* Bs = reinterpret_cast<float2*>(knn_smem + C * kBM);
-  const int t = threadIdx.x;
-  const int tx = t & 15, ty = t >> 4;
-  const int row0 = blockIdx.x * kBM;
-  const int col_begin = blockIdx.y * cols_per_split;
-  const int col_end = min(n1, col_begin + cols_per_split);
-
-  for (int e = t; e < kBM * C; e += kThreads) {
-    int r = e / C, c = e - r * C;
-    As[c * kBM + r] = (row0 + r < n0) ? f0[(int64_t)(row0 + r) * C + c] : 0.f;
-  }
-
-  float best_s[8], best_d2[8];
-  int best_j[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    best_s[i] = __int_as_float(0x7f800000);
-    best_d2[i] = __int_as_float(0x7f800000);
-    best_j[i] = 0x7fffffff;
-  }
-
-  for (int j0 = col_begin; j0 < col_end; j0 += kBN) {
-    __syncthreads();
-    for (int e = t; e < kBN * C; e += kThreads) {
-      int r = e / C, c = e - r * C;
-      float v = (j0 + r < col_end) ? f1[(int64_t)(j0 + r) * C + c] : 0.f;
-      Bs[r * (C + 1) + c] = make_float2(v, v);
-    }
-    __syncthreads();
-    unsigned long long acc[4][8];
-#pragma unroll
-    for (int p = 0; p < 4; ++p)
-#pragma unroll
-      for (int j = 0; j < 8; ++j) acc[p][j] = 0ull;
-#pragma unroll 4
-    for (int c = 0; c < C; ++c) {
-      const ulonglong2 a01 = *reinterpret_cast<const ulonglong2*>(As + c * kBM + ty * 8);
-      const ulonglong2 a23 = *reinterpret_cast<const ulonglong2*>(As + c * kBM + ty * 8 + 4);
-      const unsigned long long a[4] = {a01.x, a01.y, a23.x, a23.y};
-      unsigned long long b[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        b[j] = *reinterpret_cast<const unsigned long long*>(Bs + (tx + 16 * j) * (C + 1) + c);
-#pragma unroll
-      for (int p = 0; p < 4; ++p)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const unsigned long long d = f2_sub(a[p], b[j]);
-          acc[p][j] = f2_fma(d, d, acc[p][j]);
-        }
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int col = j0 + tx + 16 * j;
-      if (col < col_end) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const unsigned long long pk = acc[i >> 1][j];
-          const float d2 = __uint_as_float((i & 1) ? (unsigned)(pk >> 32) : (unsigned)(pk & 0xffffffffu));
-          if (d2 < best_d2[i]) {
-            float s = sqrtf(d2 + 1e-7f);
-            if (s < best_s[i]) {
-              best_s[i] = s;
-              best_d2[i] = d2;
-              best_j[i] = col;
-            }
-          }
-        }
-      }
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    unsigned long long p =
-        ((unsigned long long)__float_as_uint(best_s[i]) << 32) | (unsigned)best_j[i];
-#pragma unroll
-    for (int d = 8; d > 0; d >>= 1) {
-      unsigned long long o = __shfl_xor_sync(0xffffffffu, p, d);
-      p = o < p ? o : p;
-    }
-    const int row = row0 + ty * 8 + i;
-    if (tx == 0 && row < n0) atomicMin(packed + row, p);
-  }
-}
-
 // any channel count: one thread per (row, column-split) - correctness path for odd C
 __global__ void knn_top1_generic_kernel(const float* __restrict__ f0, int n0,
                                         const float* __restrict__ f1, int n1, int c,
@@ -269,30 +158,19 @@ extern "C" int32_t dgr_knn_top1(const float* f0, int64_t n0, const float* f1, in
   unsigned long long* packed = reinterpret_cast<unsigned long long*>(packed_ws);
   knn_init_kernel<<<dgr_blocks(n0, kThreads), kThreads, 0, st>>>(packed, n0);
   const int row_tiles = (int)((n0 + kBM - 1) / kBM);
-  // split the columns so that the grid fills 148 SMs x 2 resident CTAs a few times over
-  int splits = (148 * 2 * 2 + row_tiles - 1) / row_tiles;
+  // split the columns so that the grid fills 132 SMs x 2 resident CTAs a few times over
+  int splits = (132 * 2 * 2 + row_tiles - 1) / row_tiles;
   const int col_tiles = (int)((n1 + kBN - 1) / kBN);
   if (splits > col_tiles) splits = col_tiles;
   if (splits < 1) splits = 1;
   const int cols_per_split = ((col_tiles + splits - 1) / splits) * kBN;
   splits = (int)((n1 + cols_per_split - 1) / cols_per_split);
   dim3 grid(row_tiles, splits);
-  static const bool scalar_variant = getenv("DGR_KNN_SCALAR") != nullptr;   // A/B switch
 #define DGR_LAUNCH_KNN(CC)                                                                         \
   do {                                                                                             \
-    if (scalar_variant) {                                                                          \
-      const int smem = (CC * kBM + kBN * (CC + 1)) * (int)sizeof(float);                           \
-      DGR_CUDA_CHECK(cudaFuncSetAttribute(knn_top1_kernel<CC>,                                     \
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem));     \
-      knn_top1_kernel<CC><<<grid, kThreads, smem, st>>>(f0, (int)n0, f1, (int)n1, cols_per_split, \
-                                                        packed);                                   \
-    } else {                                                                                       \
-      const int smem = (CC * kBM + 2 * kBN * (CC + 1)) * (int)sizeof(float);                       \
-      DGR_CUDA_CHECK(cudaFuncSetAttribute(knn_top1_f2_kernel<CC>,                                  \
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem));     \
-      knn_top1_f2_kernel<CC><<<grid, kThreads, smem, st>>>(f0, (int)n0, f1, (int)n1,               \
-                                                           cols_per_split, packed);                \
-    }                                                                                              \
+    const int smem = (CC * kBM + kBN * (CC + 1)) * (int)sizeof(float);                             \
+    DGR_CUDA_CHECK(cudaFuncSetAttribute(knn_top1_kernel<CC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
+    knn_top1_kernel<CC><<<grid, kThreads, smem, st>>>(f0, (int)n0, f1, (int)n1, cols_per_split, packed); \
   } while (0)
   switch (c) {
     case 16: DGR_LAUNCH_KNN(16); break;

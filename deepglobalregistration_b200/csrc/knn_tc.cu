@@ -1,17 +1,11 @@
 // Exact feature nearest neighbour with a tensor-core pre-filter (C % 32 == 0).
 //
 // The fp32 brute-force kernel (knn.cu) spends 2 instructions per (i, j, c) term on the fp32
-// pipe.  Here the same answer - bit-identical indices - is produced in two tcgen05 sweeps:
+// pipe.  Here the same answer - bit-identical indices - is produced in two wgmma sweeps:
 //
-//   pass 1  D = F0_tile . F1_tile^T on the tensor cores (TF32, accumulator in TMEM);
-//           the epilogue (thread = F0 row = TMEM lane) forms d~2 = |a|^2 + |b|^2 - 2 D and
-//           keeps the row minimum m~_i.  (Round 2 measured a pass 1 over every 8th column tile - any
-//           upper bound of the minimum keeps the candidate set a superset: pass 1 fell from 0.55 to
-//           0.09 ms but pass 2 grew from 0.91 to 1.68 ms on the looser bound; and 3xTF32 products
-//           (kFine, a ~150x narrower band) cost more in operand staging than they save: 2.0 ms.
-//           The full single-product sweep stays.  A SINGLE sweep with a running bound and a candidate buffer
-//           (PASS 3 below, DGR_KNN_SWEEPS=1) is bit-identical too but measured 6.6 ms against 1.5 ms on the
-//           benchmark's tightly clustered random-init features: profiles/r02_experiments.txt.)
+//   pass 1  D = F0_tile . F1_tile^T on the tensor cores (TF32, fp32 accumulator in registers);
+//           the epilogue (each thread holds two F0 rows, two columns of every 8-column group) forms
+//           d~2 = |a|^2 + |b|^2 - 2 D and keeps the row minimum m~_i;
 //   pass 2  the same products again; every column with d~2 <= m~_i + 2 E_i is a CANDIDATE and
 //           only candidates are evaluated with the reference arithmetic
 //           (fp32 sum_c (a - b)^2 in ascending c, sqrt(d2 + 1e-7), lowest index on ties) - the
@@ -21,8 +15,6 @@
 // product is off by at most 2^-10 |a||b| (+ accumulation slack), and d~2 by twice that.  The
 // true nearest neighbour j* satisfies d~2(j*) <= d2(j*) + E <= d2(j) + E <= d~2(j) + 2E for
 // every j, hence it is always among the candidates and the result equals the fp32 kernel's.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -30,19 +22,11 @@ namespace {
 
 using namespace tc;
 
-constexpr int kLoadWarps = 4;
-constexpr int kLoadThreads = kLoadWarps * 32;
-constexpr int kMmaWarpK = kLoadWarps;
-constexpr int kEpiWarps = 8;                          // two per TMEM lane group: column halves
-constexpr int kThreadsK = (kLoadWarps + 1 + kEpiWarps) * 32;   // 416
+constexpr int kThreadsK = 256;        // two warpgroups: F0 rows 0..63 and 64..127 of the tile
 constexpr int kRowsA = 128;
-constexpr int kColsB = 256;
+constexpr int kColsB = 128;
 constexpr int kATile = kRowsA * 128;    // bytes per 32-float chunk
 constexpr int kBTile = kColsB * 128;
-constexpr int kCandCap = 16;           // single-sweep mode: buffered candidates per (row, column half)
-constexpr int kEpiThreads = kEpiWarps * 32;
-constexpr size_t kCandBytes = (size_t)2 * kCandCap * kEpiThreads * 4;   // column index + estimate
-constexpr int kPass1Stride = 1;        // pass 1 column-tile stride (a sampled pass 1 was measured: see header)
 
 __global__ void row_norms_kernel(const float* __restrict__ f, int64_t n, int c, float* __restrict__ n2,
                                  unsigned* __restrict__ max_bits) {
@@ -73,47 +57,26 @@ __global__ void knn_tc_init_kernel(unsigned* __restrict__ rowmin_bits, unsigned 
   if (i == 0) *max_bits = 0u;
 }
 
-// thr_i = m~_i + 2 E_i with E_i = 2 * (dot-product error bound).
-// coarse (one TF32 product): operands rounded to TF32, |a.b error| <= 2^-10 * 1.25 |a||b| (+ accumulation slack);
-// fine (3xTF32, hi*hi + lo*hi + hi*lo): the dropped lo*lo term and the truncation of the lo parts are each
-// <= 2^-22 |a||b|, fp32 accumulation of 32 products <= 32 * 2^-24 |a||b|: 4e-6 |a||b| covers them with margin.
-// Both add the slack of the fp32 norms.
-__device__ __forceinline__ float knn_error_bound(float na, float nb, bool fine) {
-  const float rel = fine ? 4e-6f : (0.0009765625f * 1.25f + 4e-5f);
-  return rel * na * nb + 1e-6f * (na + nb) * (na + nb) + 1e-7f;
+// thr_i = m~_i + 2 E_i with E_i = 2 * (dot-product error bound): operands rounded to TF32,
+// |a.b error| <= 2^-10 * 1.25 |a||b| (+ accumulation slack), plus the slack of the fp32 norms.
+__device__ __forceinline__ float knn_error_bound(float na, float nb) {
+  return (0.0009765625f * 1.25f + 4e-5f) * na * nb + 1e-6f * (na + nb) * (na + nb) + 1e-7f;
 }
 __global__ void knn_tc_threshold_kernel(const unsigned* __restrict__ rowmin_bits, const float* __restrict__ na2,
-                                        const unsigned* __restrict__ nb2_max_bits, int64_t n0, int fine,
+                                        const unsigned* __restrict__ nb2_max_bits, int64_t n0,
                                         float* __restrict__ thr) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n0) return;
   const float na = sqrtf(na2[i]), nb = sqrtf(__uint_as_float(*nb2_max_bits));
-  const float e = knn_error_bound(na, nb, fine != 0);
+  const float e = knn_error_bound(na, nb);
   // stored in the epilogue's units: candidates satisfy (0.5 |b|^2 - a.b) <= thr'
   thr[i] = 0.5f * (__uint_as_float(rowmin_bits[i]) + 4.f * e - na2[i]);
 }
-
-struct KnnShared {
-  unsigned long long full[2];
-  unsigned long long acc_full[2];
-  unsigned long long acc_empty[2];
-  uint32_t tmem_base;
-  float nb[2][kColsB];
-};
 
 __device__ __forceinline__ void round_store(float4 v, unsigned char* tile, int row, int piece) {
   float4 h;
   h.x = tf32_round(v.x); h.y = tf32_round(v.y); h.z = tf32_round(v.z); h.w = tf32_round(v.w);
   *reinterpret_cast<float4*>(tile + row * 128 + ((piece ^ (row & 7)) << 4)) = h;
-}
-
-__device__ __forceinline__ void split_store2(float4 v, unsigned char* hi_tile, unsigned char* lo_tile, int row, int piece) {
-  float4 h, l;
-  h.x = tf32_round(v.x); h.y = tf32_round(v.y); h.z = tf32_round(v.z); h.w = tf32_round(v.w);
-  l.x = v.x - h.x; l.y = v.y - h.y; l.z = v.z - h.z; l.w = v.w - h.w;
-  const int off = row * 128 + ((piece ^ (row & 7)) << 4);
-  *reinterpret_cast<float4*>(hi_tile + off) = h;
-  *reinterpret_cast<float4*>(lo_tile + off) = l;
 }
 
 // exact reference arithmetic for one candidate column, as in knn.cu
@@ -141,332 +104,129 @@ __device__ __noinline__ void knn_exact_candidate(const float* __restrict__ f0, c
   }
 }
 
-// the same arithmetic for candidates met in ANY order (single-sweep mode evaluates its buffered candidates after
-// the sweep, overflowed ones during it): smallest sqrt distance, lowest index among equal ones - what the ascending
-// walk above yields.  best_d2 is the smallest exact d2 seen; it only tightens the candidate bound.
-template <int C>
-__device__ __noinline__ void knn_exact_candidate_unordered(const float* __restrict__ f0, const float* __restrict__ f1,
-                                                           int gi, int j, float& best_s, float& best_d2, int& best_j) {
-  const float4* a = reinterpret_cast<const float4*>(f0 + (size_t)gi * C);
-  const float4* b = reinterpret_cast<const float4*>(f1 + (size_t)j * C);
-  float d2 = 0.f;
-#pragma unroll
-  for (int k = 0; k < C / 4; ++k) {
-    const float4 x = __ldg(a + k), y = __ldg(b + k);
-    float df = x.x - y.x; d2 = fmaf(df, df, d2);
-    df = x.y - y.y; d2 = fmaf(df, df, d2);
-    df = x.z - y.z; d2 = fmaf(df, df, d2);
-    df = x.w - y.w; d2 = fmaf(df, df, d2);
-  }
-  const float sq = sqrtf(d2 + 1e-7f);
-  if (sq < best_s || (sq == best_s && j < best_j)) {
-    best_s = sq;
-    best_j = j;
-  }
-  best_d2 = fminf(best_d2, d2);
-}
-
-__device__ __forceinline__ void tc_ld32_issue(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]),
-        "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]),
-        "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]),
-        "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-template <int C, int PASS, bool kFine>
-__global__ void __launch_bounds__(kThreadsK, 1)
+template <int C, int PASS>
+__global__ void __launch_bounds__(kThreadsK)
 knn_tc_kernel(const float* __restrict__ f0, int n0, const float* __restrict__ f1, int n1,
               const float* __restrict__ na2, const float* __restrict__ nb2, int cols_per_split,
               unsigned* __restrict__ rowmin_bits, const float* __restrict__ thr,
               unsigned long long* __restrict__ packed, const unsigned* __restrict__ nb2_max_bits) {
   constexpr int kChunks = C / 32;
-  constexpr int kParts = kFine ? 2 : 1;            // operand tiles per chunk: TF32 hi (+ residual lo)
   extern __shared__ __align__(16) unsigned char smem_dyn[];
-  KnnShared& sh = *reinterpret_cast<KnnShared*>(smem_dyn);
+  float* nb_sh = reinterpret_cast<float*>(smem_dyn);          // 0.5 |b|^2 of the tile's columns
   unsigned char* a_tile = reinterpret_cast<unsigned char*>(
-      (reinterpret_cast<uintptr_t>(smem_dyn) + sizeof(KnnShared) + 1023) & ~(uintptr_t)1023);
-  unsigned char* b_stage0 = a_tile + kParts * kChunks * kATile;
-  constexpr int kStageBytes = kParts * kChunks * kBTile;
-  const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
+      (reinterpret_cast<uintptr_t>(smem_dyn) + kColsB * sizeof(float) + 1023) & ~(uintptr_t)1023);
+  unsigned char* b_tile = a_tile + kChunks * kATile;
+  const int t = threadIdx.x, wg = t >> 7, lane = t & 31;
   const int row0 = blockIdx.x * kRowsA;
   const int col_begin = blockIdx.y * cols_per_split;
   const int col_end = min(n1, col_begin + cols_per_split);
-  constexpr int kTS = PASS == 1 ? kPass1Stride : 1;               // tile stride of this pass
-  const int n_tiles_all = (col_end - col_begin + kColsB - 1) / kColsB;
-  const int n_tiles = (n_tiles_all + kTS - 1) / kTS;
+  const int n_tiles = (col_end - col_begin + kColsB - 1) / kColsB;
+  const int piece = t & 7, rgrp = t >> 3;   // 8 lanes per 128-byte row, 32 row groups
 
-  if (t == 0) {
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&sh.full[s]), kLoadThreads);
-      mbar_init(smem_u32(&sh.acc_full[s]), 1);
-      mbar_init(smem_u32(&sh.acc_empty[s]), kEpiWarps * 32);
+  // the F0 tile, once
+#pragma unroll
+  for (int ch = 0; ch < kChunks; ++ch)
+#pragma unroll
+    for (int i = 0; i < kRowsA / 32; ++i) {
+      const int r = i * 32 + rgrp;
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (row0 + r < n0) v = __ldg(reinterpret_cast<const float4*>(f0 + (size_t)(row0 + r) * C + ch * 32 + piece * 4));
+      round_store(v, a_tile + ch * kATile, r, piece);
     }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == kMmaWarpK) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(&sh.tmem_base)),
-                 "r"(512u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = sh.tmem_base;
-
-  if (warp < kLoadWarps) {
-    // ================================ loaders ============================================
-    const int piece = t & 7, rgrp = t >> 3;   // 16 row groups
-    // the F0 tile, once
+  float4 bv[kChunks][kColsB / 32];
+  float nbv = 0.f;
+  auto load_b = [&](int it) {
+    const int j0 = col_begin + it * kColsB;
 #pragma unroll
     for (int ch = 0; ch < kChunks; ++ch)
 #pragma unroll
-      for (int i = 0; i < kRowsA / 16; ++i) {
-        const int r = i * 16 + rgrp;
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (row0 + r < n0) v = __ldg(reinterpret_cast<const float4*>(f0 + (size_t)(row0 + r) * C + ch * 32 + piece * 4));
-        if (kFine) split_store2(v, a_tile + (2 * ch) * kATile, a_tile + (2 * ch + 1) * kATile, r, piece);
-        else round_store(v, a_tile + ch * kATile, r, piece);
+      for (int i = 0; i < kColsB / 32; ++i) {
+        const int r = i * 32 + rgrp;
+        bv[ch][i] = (j0 + r < col_end)
+                        ? __ldg(reinterpret_cast<const float4*>(f1 + (size_t)(j0 + r) * C + ch * 32 + piece * 4))
+                        : make_float4(0.f, 0.f, 0.f, 0.f);
       }
-    for (int it = 0; it < n_tiles; ++it) {
-      const int s = it & 1;
-      const uint32_t ph = (it >> 1) & 1;
-      const int j0 = col_begin + it * kTS * kColsB;
-      float4 bv[kChunks][kColsB / 16];
+    if (t < kColsB) nbv = (j0 + t < col_end) ? nb2[j0 + t] : 0.f;
+  };
+
+  // epilogue state: this thread's rows r and r + 8 (h = 0, 1) of its warpgroup
+  const int r = wg * 64 + ((t >> 5) & 3) * 16 + (lane >> 2);
+  int gi[2];
+  bool valid[2];
+  float th[2], na2_i[2], e4[2], rmin[2], best_s[2], best_d2[2];
+  int best_j[2];
 #pragma unroll
-      for (int ch = 0; ch < kChunks; ++ch)
-#pragma unroll
-        for (int i = 0; i < kColsB / 16; ++i) {
-          const int r = i * 16 + rgrp;
-          bv[ch][i] = (j0 + r < col_end)
-                          ? __ldg(reinterpret_cast<const float4*>(f1 + (size_t)(j0 + r) * C + ch * 32 + piece * 4))
-                          : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      const float nb_a = (j0 + t < col_end) ? nb2[j0 + t] : 0.f;
-      const float nb_b = (j0 + 128 + t < col_end) ? nb2[j0 + 128 + t] : 0.f;
-      // stage s (B tile + norms) and accumulator s travel together: both are free once the
-      // epilogue has drained accumulator s of tile it - 2
-      mbar_wait(smem_u32(&sh.acc_empty[s]), ph ^ 1);
-      unsigned char* b_tile = b_stage0 + (size_t)s * kStageBytes;
-#pragma unroll
-      for (int ch = 0; ch < kChunks; ++ch)
-#pragma unroll
-        for (int i = 0; i < kColsB / 16; ++i) {
-          if (kFine) split_store2(bv[ch][i], b_tile + (2 * ch) * kBTile, b_tile + (2 * ch + 1) * kBTile, i * 16 + rgrp, piece);
-          else round_store(bv[ch][i], b_tile + ch * kBTile, i * 16 + rgrp, piece);
-        }
-      sh.nb[s][t] = 0.5f * nb_a;          // the epilogue works with 0.5 |b|^2 - a.b
-      sh.nb[s][128 + t] = 0.5f * nb_b;
-      fence_proxy_async();
-      mbar_arrive(smem_u32(&sh.full[s]));
-    }
-  } else if (warp == kMmaWarpK) {
-    // ================================ MMA issuer =========================================
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(kColsB >> 3) << 17) |
-                           ((uint32_t)(kRowsA >> 4) << 24);
-    for (int it = 0; it < n_tiles; ++it) {
-      const int s = it & 1;
-      const uint32_t ph = (it >> 1) & 1;
-      mbar_wait(smem_u32(&sh.acc_empty[s]), ph ^ 1);
-      mbar_wait(smem_u32(&sh.full[s]), ph);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t a0 = smem_u32(a_tile);
-        const uint32_t b0 = smem_u32(b_stage0 + (size_t)s * kStageBytes);
-#pragma unroll
-        for (int ch = 0; ch < kChunks; ++ch)
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint32_t td = tmem_base + (uint32_t)s * kColsB;
-            if (kFine) {
-              const uint64_t ah = umma_desc(a0 + (2 * ch) * kATile + ks * 32), al = umma_desc(a0 + (2 * ch + 1) * kATile + ks * 32);
-              const uint64_t bh = umma_desc(b0 + (2 * ch) * kBTile + ks * 32), bl = umma_desc(b0 + (2 * ch + 1) * kBTile + ks * 32);
-              tc_mma_tf32(td, ah, bh, idesc, (ch | ks) != 0);
-              tc_mma_tf32(td, al, bh, idesc, 1);
-              tc_mma_tf32(td, ah, bl, idesc, 1);
-            } else {
-              tc_mma_tf32(td, umma_desc(a0 + ch * kATile + ks * 32), umma_desc(b0 + ch * kBTile + ks * 32), idesc,
-                          (ch | ks) != 0);
-            }
-          }
-        tc_commit(smem_u32(&sh.acc_full[s]));
-      }
-      __syncwarp();
-    }
-  } else if (PASS == 3) {
-    // ================================ single sweep: thread = (F0 row, column half) ========
-    // One pass over the products.  The candidate bound follows the RUNNING row minimum of this thread's columns
-    // (any upper bound of the final minimum keeps the candidate set a superset, see the header): columns within the
-    // bound are buffered in shared memory (column, estimate) and evaluated exactly after the sweep against the
-    // final - tightest - bound; a full buffer evaluates the newcomer on the spot.
-    const int lane_grp = warp & 3;
-    const int half = (warp - kLoadWarps - 1) >> 2;
-    const int gi = row0 + lane_grp * 32 + lane;
-    const bool valid = gi < n0;
-    const int etid = (warp - kLoadWarps - 1) * 32 + lane;                  // 0 .. kEpiThreads-1
-    int* cand_j = reinterpret_cast<int*>(b_stage0 + 2 * (size_t)kStageBytes) + etid;       // [slot][thread]
-    float* cand_g = reinterpret_cast<float*>(cand_j - etid + kCandCap * kEpiThreads) + etid;
-    const float ninf = -__int_as_float(0x7f800000), pinf = __int_as_float(0x7f800000);
-    const float na2_i = valid ? na2[gi] : 0.f;
-    const float e4 = valid ? 4.f * knn_error_bound(sqrtf(na2_i), sqrtf(__uint_as_float(*nb2_max_bits)), kFine) : 0.f;
-    float rmin = pinf, th_exact = pinf;
-    float best_s = pinf, best_d2 = pinf;
-    int best_j = 0x7fffffff, cnt = 0;
-    // bound in the epilogue's units (0.5 |b|^2 - a.b), from the running minimum: thr kernel's formula
-    auto bound = [&](float m) { return 0.5f * (fmaxf(fmaf(2.f, m, na2_i), 0.f) + e4 - na2_i); };
-    auto take = [&](int j, float g) {
-      if (cnt < kCandCap) {
-        cand_j[cnt * kEpiThreads] = j;
-        cand_g[cnt * kEpiThreads] = g;
-        ++cnt;
-      } else {
-        knn_exact_candidate_unordered<C>(f0, f1, gi, j, best_s, best_d2, best_j);
-        th_exact = fminf(th_exact, 0.5f * (best_d2 + e4 - na2_i));
-      }
-    };
-    for (int it = 0; it < n_tiles; ++it) {
-      const int s = it & 1;
-      const uint32_t ph = (it >> 1) & 1;
-      const int j0 = col_begin + it * kColsB + half * 128;
-      mbar_wait(smem_u32(&sh.acc_full[s]), ph);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t)s * kColsB + half * 128 + ((uint32_t)(lane_grp * 32) << 16);
-      const float* hb = sh.nb[s] + half * 128;
-      uint32_t va[32], vb[32];
-      tc_ld32_issue(taddr, va);
-#pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {
-        tc_ld_wait();
-        uint32_t(&cur)[32] = (cc & 1) ? vb : va;
-        uint32_t(&nxt)[32] = (cc & 1) ? va : vb;
-        if (cc < 3) tc_ld32_issue(taddr + (cc + 1) * 32, nxt);
-        const int jc = j0 + cc * 32;
-        if (jc < col_end) {
-          const int nq = min(32, col_end - jc);
-          float cmin = pinf;
-#pragma unroll
-          for (int q = 0; q < 32; ++q)
-            cmin = fminf(cmin, q < nq ? hb[cc * 32 + q] - __uint_as_float(cur[q]) : pinf);
-          rmin = fminf(rmin, cmin);
-          float th = valid ? fminf(th_exact, bound(rmin)) : ninf;
-          if (cmin <= th) {
-#pragma unroll
-            for (int q = 0; q < 32; ++q) {
-              const float g = hb[cc * 32 + q] - __uint_as_float(cur[q]);
-              if (q < nq && g <= th) {
-                take(jc + q, g);
-                th = fminf(th, th_exact);
-              }
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(smem_u32(&sh.acc_empty[s]));
-    }
-    if (valid) {
-      float th = fminf(th_exact, bound(rmin));
-      for (int k = 0; k < cnt; ++k) {
-        if (cand_g[k * kEpiThreads] <= th) {
-          knn_exact_candidate_unordered<C>(f0, f1, gi, cand_j[k * kEpiThreads], best_s, best_d2, best_j);
-          th = fminf(th, 0.5f * (best_d2 + e4 - na2_i));
-        }
-      }
-      if (best_j != 0x7fffffff)
-        atomicMin(packed + gi, ((unsigned long long)__float_as_uint(best_s) << 32) | (unsigned)best_j);
-    }
-  } else {
-    // ================================ epilogue: thread = (F0 row, column half) ============
-    const int lane_grp = warp & 3;
-    const int half = (warp - kLoadWarps - 1) >> 2;      // 0: columns 0..127, 1: columns 128..255
-    const int r = lane_grp * 32 + lane;
-    const int gi = row0 + r;
-    const bool valid = gi < n0;
-    float th = (PASS == 2 && valid) ? thr[gi] : -__int_as_float(0x7f800000);
+  for (int h = 0; h < 2; ++h) {
+    gi[h] = row0 + r + 8 * h;
+    valid[h] = gi[h] < n0;
     // pass 2 tightens its bound with every exact distance it learns: a later column can only win if its true
     // d2 is below the best exact d2 so far, i.e. if its estimate is below best_d2 + (estimate error)
-    const float na2_i = (PASS == 2 && valid) ? na2[gi] : 0.f;
-    const float e4 = (PASS == 2 && valid)
-                         ? 4.f * knn_error_bound(sqrtf(na2_i), sqrtf(__uint_as_float(*nb2_max_bits)), kFine)
-                         : 0.f;
-    float rmin = __int_as_float(0x7f800000);     // min over columns of 0.5 |b|^2 - a.b
-    float best_s = __int_as_float(0x7f800000), best_d2 = best_s;
-    int best_j = 0x7fffffff;
-    for (int it = 0; it < n_tiles; ++it) {
-      const int s = it & 1;
-      const uint32_t ph = (it >> 1) & 1;
-      const int j0 = col_begin + it * kTS * kColsB + half * 128;
-      mbar_wait(smem_u32(&sh.acc_full[s]), ph);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t)s * kColsB + half * 128 + ((uint32_t)(lane_grp * 32) << 16);
-      const float* hb = sh.nb[s] + half * 128;
-      uint32_t va[32], vb[32];
-      tc_ld32_issue(taddr, va);
+    th[h] = (PASS == 2 && valid[h]) ? thr[gi[h]] : -__int_as_float(0x7f800000);
+    na2_i[h] = (PASS == 2 && valid[h]) ? na2[gi[h]] : 0.f;
+    e4[h] = (PASS == 2 && valid[h])
+                ? 4.f * knn_error_bound(sqrtf(na2_i[h]), sqrtf(__uint_as_float(*nb2_max_bits)))
+                : 0.f;
+    rmin[h] = __int_as_float(0x7f800000);     // min over columns of 0.5 |b|^2 - a.b
+    best_s[h] = best_d2[h] = __int_as_float(0x7f800000);
+    best_j[h] = 0x7fffffff;
+  }
+
+  load_b(0);
+  for (int it = 0; it < n_tiles; ++it) {
+    __syncthreads();     // every thread is done with the previous tile's operands and norms
 #pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {
-        tc_ld_wait();
-        uint32_t(&cur)[32] = (cc & 1) ? vb : va;
-        uint32_t(&nxt)[32] = (cc & 1) ? va : vb;
-        if (cc < 3) tc_ld32_issue(taddr + (cc + 1) * 32, nxt);
-        const int jc = j0 + cc * 32;
+    for (int ch = 0; ch < kChunks; ++ch)
+#pragma unroll
+      for (int i = 0; i < kColsB / 32; ++i) round_store(bv[ch][i], b_tile + ch * kBTile, i * 32 + rgrp, piece);
+    if (t < kColsB) nb_sh[t] = 0.5f * nbv;          // the epilogue works with 0.5 |b|^2 - a.b
+    if (it + 1 < n_tiles) load_b(it + 1);           // in flight during the MMAs and the epilogue
+    fence_proxy_async();
+    __syncthreads();
+    float acc[kColsB / 2];
+#pragma unroll
+    for (int i = 0; i < kColsB / 2; ++i) acc[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int ch = 0; ch < kChunks; ++ch) {
+      const uint32_t a = smem_u32(a_tile + ch * kATile) + wg * (kATile / 2), b = smem_u32(b_tile + ch * kBTile);
+      mma_chunk<kColsB, false, 1>(acc, a, a, b, b);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(acc);
+    // columns in ascending order per row: the exact evaluation keeps the lowest index on ties
+    const int j0 = col_begin + it * kColsB;
+#pragma unroll
+    for (int i = 0; i < kColsB / 8; ++i)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = 8 * i + 2 * (lane & 3) + e;
+        const int jc = j0 + col;
         if (jc < col_end) {
-          if (jc + 32 <= col_end) {
-            // both passes reduce the chunk to its minimum first (branch-free); pass 2 walks the
-            // chunk element by element only when that minimum is within the candidate bound
-            float cmin = __int_as_float(0x7f800000);
 #pragma unroll
-            for (int q = 0; q < 32; ++q) cmin = fminf(cmin, hb[cc * 32 + q] - __uint_as_float(cur[q]));
+          for (int h = 0; h < 2; ++h) {
+            const float g = nb_sh[col] - acc[4 * i + 2 * h + e];
             if (PASS == 1) {
-              rmin = fminf(rmin, cmin);
-            } else if (cmin <= th) {
-#pragma unroll
-              for (int q = 0; q < 32; ++q) {
-                const float g = hb[cc * 32 + q] - __uint_as_float(cur[q]);
-                if (g <= th) {
-                  knn_exact_candidate<C>(f0, f1, gi, jc + q, best_s, best_d2, best_j);
-                  th = fminf(th, 0.5f * (best_d2 + e4 - na2_i));
-                }
-              }
-            }
-          } else {
-#pragma unroll
-            for (int q = 0; q < 32; ++q) {
-              const float g = hb[cc * 32 + q] - __uint_as_float(cur[q]);
-              if (jc + q < col_end) {
-                if (PASS == 1) rmin = fminf(rmin, g);
-                else if (g <= th) {
-                  knn_exact_candidate<C>(f0, f1, gi, jc + q, best_s, best_d2, best_j);
-                  th = fminf(th, 0.5f * (best_d2 + e4 - na2_i));
-                }
-              }
+              rmin[h] = fminf(rmin[h], g);
+            } else if (g <= th[h]) {
+              knn_exact_candidate<C>(f0, f1, gi[h], jc, best_s[h], best_d2[h], best_j[h]);
+              th[h] = fminf(th[h], 0.5f * (best_d2[h] + e4[h] - na2_i[h]));
             }
           }
         }
       }
-      tc_fence_before();
-      mbar_arrive(smem_u32(&sh.acc_empty[s]));
-    }
-    if (valid) {
-      if (PASS == 1) {
-        atomicMin(rowmin_bits + gi, __float_as_uint(fmaxf(fmaf(2.f, rmin, na2[gi]), 0.f)));
-      } else if (best_j != 0x7fffffff) {
-        atomicMin(packed + gi, ((unsigned long long)__float_as_uint(best_s) << 32) | (unsigned)best_j);
-      }
-    }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarpK) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (PASS == 1) {
+      // the four lanes of a quad share the row
+      rmin[h] = fminf(rmin[h], __shfl_xor_sync(0xffffffffu, rmin[h], 1));
+      rmin[h] = fminf(rmin[h], __shfl_xor_sync(0xffffffffu, rmin[h], 2));
+      if (valid[h] && (lane & 3) == 0)
+        atomicMin(rowmin_bits + gi[h], __float_as_uint(fmaxf(fmaf(2.f, rmin[h], na2[gi[h]]), 0.f)));
+    } else if (valid[h] && best_j[h] != 0x7fffffff) {
+      atomicMin(packed + gi[h], ((unsigned long long)__float_as_uint(best_s[h]) << 32) | (unsigned)best_j[h]);
+    }
   }
 }
 
@@ -479,48 +239,31 @@ __global__ void knn_tc_unpack_kernel(const unsigned long long* __restrict__ pack
   if (dist != nullptr) dist[i] = __uint_as_float((unsigned)(p >> 32));
 }
 
-// single sweep (DGR_KNN_SWEEPS=1): no row-minimum pass, no threshold kernel
 template <int C>
-int32_t launch_knn_tc_single(const float* f0, int64_t n0, const float* f1, int64_t n1, float* na2, float* nb2,
-                             unsigned* max_bits, unsigned long long* packed, cudaStream_t st) {
-  constexpr int kChunks = C / 32;
-  const size_t smem = sizeof(KnnShared) + 1024 + (size_t)kChunks * kATile + 2 * (size_t)kChunks * kBTile + kCandBytes;
-  DGR_ENSURE_SMEM((knn_tc_kernel<C, 3, false>), smem);
-  const int row_tiles = (int)((n0 + kRowsA - 1) / kRowsA);
-  const int col_tiles = (int)((n1 + kColsB - 1) / kColsB);
-  int splits = (148 * 4 + row_tiles - 1) / row_tiles;
-  if (splits > col_tiles) splits = col_tiles;
-  if (splits < 1) splits = 1;
-  const int cols_per_split = ((col_tiles + splits - 1) / splits) * kColsB;
-  splits = (int)((n1 + cols_per_split - 1) / cols_per_split);
-  dim3 grid(row_tiles, splits);
-  knn_tc_kernel<C, 3, false><<<grid, kThreadsK, smem, st>>>(f0, (int)n0, f1, (int)n1, na2, nb2, cols_per_split,
-                                                            nullptr, nullptr, packed, max_bits);
-  return DGR_OK;
-}
-
-template <int C, bool kFine>
 int32_t launch_knn_tc(const float* f0, int64_t n0, const float* f1, int64_t n1, float* na2, float* nb2,
                       unsigned* rowmin, float* thr, unsigned* max_bits, unsigned long long* packed,
                       cudaStream_t st) {
   constexpr int kChunks = C / 32;
-  constexpr int kParts = kFine ? 2 : 1;
-  const size_t smem = sizeof(KnnShared) + 1024 + (size_t)kParts * kChunks * kATile + 2 * (size_t)kParts * kChunks * kBTile;
-  DGR_ENSURE_SMEM((knn_tc_kernel<C, 1, kFine>), smem);
-  DGR_ENSURE_SMEM((knn_tc_kernel<C, 2, kFine>), smem);
+  const size_t smem = kColsB * sizeof(float) + 1024 + (size_t)kChunks * (kATile + kBTile);
+  DGR_ENSURE_SMEM((knn_tc_kernel<C, 1>), smem);
+  DGR_ENSURE_SMEM((knn_tc_kernel<C, 2>), smem);
+  int dev = 0, sms = 0;
+  DGR_CUDA_CHECK(cudaGetDevice(&dev));
+  DGR_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  // split the columns so that the grid fills every SM a few times over
   const int row_tiles = (int)((n0 + kRowsA - 1) / kRowsA);
   const int col_tiles = (int)((n1 + kColsB - 1) / kColsB);
-  int splits = (148 * 4 + row_tiles - 1) / row_tiles;
+  int splits = (sms * 4 + row_tiles - 1) / row_tiles;
   if (splits > col_tiles) splits = col_tiles;
   if (splits < 1) splits = 1;
   const int cols_per_split = ((col_tiles + splits - 1) / splits) * kColsB;
   splits = (int)((n1 + cols_per_split - 1) / cols_per_split);
   dim3 grid(row_tiles, splits);
-  knn_tc_kernel<C, 1, kFine><<<grid, kThreadsK, smem, st>>>(f0, (int)n0, f1, (int)n1, na2, nb2, cols_per_split,
-                                                            rowmin, thr, packed, max_bits);
-  knn_tc_threshold_kernel<<<dgr_blocks(n0, 256), 256, 0, st>>>(rowmin, na2, max_bits, n0, kFine ? 1 : 0, thr);
-  knn_tc_kernel<C, 2, kFine><<<grid, kThreadsK, smem, st>>>(f0, (int)n0, f1, (int)n1, na2, nb2, cols_per_split,
-                                                            rowmin, thr, packed, max_bits);
+  knn_tc_kernel<C, 1><<<grid, kThreadsK, smem, st>>>(f0, (int)n0, f1, (int)n1, na2, nb2, cols_per_split, rowmin, thr,
+                                                     packed, max_bits);
+  knn_tc_threshold_kernel<<<dgr_blocks(n0, 256), 256, 0, st>>>(rowmin, na2, max_bits, n0, thr);
+  knn_tc_kernel<C, 2><<<grid, kThreadsK, smem, st>>>(f0, (int)n0, f1, (int)n1, na2, nb2, cols_per_split, rowmin, thr,
+                                                     packed, max_bits);
   return DGR_OK;
 }
 
@@ -534,7 +277,7 @@ int64_t dgr_knn_tc_ws_elems(int64_t n0, int64_t n1) { return 3 * n0 + n1 + 8; }
 // 1 if the tensor-core pre-filter supports the channel count
 int32_t dgr_knn_tc_supported(int32_t c) { return (c == 32 || c == 64) ? 1 : 0; }
 
-// Same result as dgr_knn_top1 (bit-identical indices and distances), two tcgen05 sweeps
+// Same result as dgr_knn_top1 (bit-identical indices and distances), two wgmma sweeps
 // plus exact fp32 evaluation of the few candidates per row.  ws: dgr_knn_tc_ws_elems floats.
 int32_t dgr_knn_top1_tc(const float* f0, int64_t n0, const float* f1, int64_t n1, int32_t c,
                         uint64_t* packed_ws, float* ws, int32_t* idx, float* dist, void* stream) {
@@ -552,23 +295,8 @@ int32_t dgr_knn_top1_tc(const float* f0, int64_t n0, const float* f1, int64_t n1
   knn_tc_init_kernel<<<dgr_blocks(n0, 256), 256, 0, st>>>(rowmin, packed, n0, max_bits);
   row_norms_kernel<<<dgr_blocks(n0 * 8, 256), 256, 0, st>>>(f0, n0, c, na2, nullptr);
   row_norms_kernel<<<dgr_blocks(n1 * 8, 256), 256, 0, st>>>(f1, n1, c, nb2, max_bits);
-  // default: single TF32 product per term.  DGR_KNN_FINE=1 (c = 32 only): 3xTF32 products, a ~150x narrower
-  // candidate band, measured slower (the hi + lo tiles double the operand staging)
-  static const bool coarse = getenv("DGR_KNN_FINE") == nullptr;        // A/B switch: 3xTF32 pre-filter (slower)
-  // DGR_KNN_SWEEPS=1: the single-sweep variant (running bound + candidate buffer)
-  static const bool single = getenv("DGR_KNN_SWEEPS") != nullptr && atoi(getenv("DGR_KNN_SWEEPS")) == 1;
-  if (single) {
-    int32_t rc1 = (c == 32) ? launch_knn_tc_single<32>(f0, n0, f1, n1, na2, nb2, max_bits, packed, st)
-                            : launch_knn_tc_single<64>(f0, n0, f1, n1, na2, nb2, max_bits, packed, st);
-    if (rc1 != DGR_OK) return rc1;
-    knn_tc_unpack_kernel<<<dgr_blocks(n0, 256), 256, 0, st>>>(packed, n0, idx, dist);
-    dgr_note_launches(5);
-    DGR_LAUNCH_CHECK();
-    return DGR_OK;
-  }
-  int32_t rc = (c == 32) ? (coarse ? launch_knn_tc<32, false>(f0, n0, f1, n1, na2, nb2, rowmin, thr, max_bits, packed, st)
-                                   : launch_knn_tc<32, true>(f0, n0, f1, n1, na2, nb2, rowmin, thr, max_bits, packed, st))
-                         : launch_knn_tc<64, false>(f0, n0, f1, n1, na2, nb2, rowmin, thr, max_bits, packed, st);
+  int32_t rc = (c == 32) ? launch_knn_tc<32>(f0, n0, f1, n1, na2, nb2, rowmin, thr, max_bits, packed, st)
+                         : launch_knn_tc<64>(f0, n0, f1, n1, na2, nb2, rowmin, thr, max_bits, packed, st);
   if (rc != DGR_OK) return rc;
   knn_tc_unpack_kernel<<<dgr_blocks(n0, 256), 256, 0, st>>>(packed, n0, idx, dist);
   dgr_note_launches(7);

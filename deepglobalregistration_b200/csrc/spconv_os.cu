@@ -8,14 +8,13 @@
 // pass.  With only 27 offsets and ~64 % of the (row, offset) slots occupied, the output-stationary
 // order is the better one:
 //
-//   tile          = 128 consecutive OUTPUT rows; the accumulator (TMEM, fp32) lives through all
+//   tile          = 128 consecutive OUTPUT rows; the accumulator (registers of two warpgroups, fp32) lives through all
 //                   27 offsets x Cin/32 chunks: D[128, Cout] += A_kappa[128, 32] . W[kappa][32, Cout]
-//   A_kappa       = input rows nbr[kappa][j] gathered by the loader warps (missing neighbours are
+//   A_kappa       = input rows nbr[kappa][j] gathered by all threads (missing neighbours are
 //                   zero rows), split hi / lo as in the 3xTF32 kernel, K-major SWIZZLE_128B tiles
 //   weights       = the same packed hi | lo slabs, one cp.async.bulk per stage
-//   epilogue      = tcgen05.ld, y = acc * scale + shift (+ residual), ReLU, transposed through shared
-//                   memory so that 8 lanes write one row's 128-byte line: every output row is
-//                   written exactly once with plain stores - no atomics, no memset, deterministic
+//   epilogue      = y = acc * scale + shift (+ residual), ReLU on the accumulator fragments: every output
+//                   row is written exactly once with plain stores - no atomics, no memset, deterministic
 //
 // 1.56x the MMA work of the pair lists (zero rows are multiplied too) on layers whose tensor pipe is
 // ~6-13 % busy; gather bytes unchanged (P x Cin x 4), output bytes N x Cout x 4 instead of the
@@ -29,248 +28,149 @@ namespace {
 
 using namespace tc;
 
-constexpr int kLoaderWarps = 8;
-constexpr int kLoaderThreads = kLoaderWarps * 32;
-constexpr int kMmaWarp = kLoaderWarps;
-constexpr int kThreadsOS = (kLoaderWarps + 5) * 32;   // 8 loader warps, 1 MMA warp, 4 epilogue warps
+constexpr int kThreadsOS = 256;          // two warpgroups: tile rows 0..63 and 64..127
 constexpr int kTileM = 128;
 constexpr int kChunk = 32;
 constexpr int kATileBytes = kTileM * 128;
-constexpr int kEpiStageBytes = 4 * 4096;
-
-__device__ __forceinline__ void split_store(float4 v, unsigned char* hi_tile, unsigned char* lo_tile, uint32_t off) {
-  float4 h, l;
-  h.x = tf32_round(v.x); h.y = tf32_round(v.y); h.z = tf32_round(v.z); h.w = tf32_round(v.w);
-  l.x = v.x - h.x; l.y = v.y - h.y; l.z = v.z - h.z; l.w = v.w - h.w;
-  *reinterpret_cast<float4*>(hi_tile + off) = h;
-  *reinterpret_cast<float4*>(lo_tile + off) = l;
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   dst_smem),
-               "l"(src), "r"(bytes), "r"(bar)
-               : "memory");
-}
+constexpr int kStages = 2;
 
 struct OsShared {
-  unsigned long long full[4];      // gathered A tiles (256 arrivals) + B hi tile bytes
-  unsigned long long full_lo[4];   // B lo tile bytes
-  unsigned long long empty[4];
-  unsigned long long acc_full[2];
-  unsigned long long acc_empty[2];
-  uint32_t tmem_base;
+  unsigned long long full[kStages];     // weight slab of the stage has landed (bulk-copy bytes)
 };
 
+constexpr size_t os_smem_bytes(int nt) {
+  return sizeof(OsShared) + 1024 + (size_t)kStages * (2 * kATileBytes + 2 * nt * 128);
+}
+
+template <int NT>
 __global__ void __launch_bounds__(kThreadsOS, 1)
 spconv_os_kernel(const float* __restrict__ in_feat, int cin, const float* __restrict__ wt, int cout,
-                 const int32_t* __restrict__ nbr, int64_t nbr_stride, int K, int n_out, int n_stages, int tmem_cols,
+                 const int32_t* __restrict__ nbr, int64_t nbr_stride, int K, int n_out,
                  const float* __restrict__ scale, const float* __restrict__ shift, const float* __restrict__ residual,
                  int relu, float* __restrict__ out) {
+  constexpr int kBTileBytes = NT * 128;          // B tile in shared memory: rows >= cout stay zero
+  constexpr int kStageBytes = 2 * kATileBytes + 2 * kBTileBytes;
   extern __shared__ __align__(16) unsigned char smem_dyn[];
   OsShared& sh = *reinterpret_cast<OsShared*>(smem_dyn);
   unsigned char* stage0 = reinterpret_cast<unsigned char*>(
       (reinterpret_cast<uintptr_t>(smem_dyn) + sizeof(OsShared) + 1023) & ~(uintptr_t)1023);
-  const int b_tile_bytes = cout * 128;
-  const int stage_bytes = 2 * kATileBytes + 2 * b_tile_bytes;
-  const int t = threadIdx.x;
-  const int warp = t >> 5, lane = t & 31;
+  const int t = threadIdx.x, wg = t >> 7;
   const int n_chunks = cin / kChunk;
-  const int n_tiles = (n_out + kTileM - 1) / kTileM;
-  const int steps_per_tile = K * n_chunks;                // pipeline stages consumed per output tile
-  const uint32_t acc_stride = (uint32_t)tmem_cols >> 1;
+  const int steps = K * n_chunks;                 // (kappa, chunk) steps of the tile
+  const uint32_t b_tile_bytes = (uint32_t)cout * 128;
+  const uint32_t slab_bytes = 2 * b_tile_bytes;
+  const int j0 = blockIdx.x * kTileM;
 
   if (t == 0) {
-    for (int s = 0; s < n_stages; ++s) {
-      mbar_init(smem_u32(&sh.full[s]), kLoaderThreads);
-      mbar_init(smem_u32(&sh.full_lo[s]), 1);
-      mbar_init(smem_u32(&sh.empty[s]), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(smem_u32(&sh.acc_full[b]), 1);
-      mbar_init(smem_u32(&sh.acc_empty[b]), 128);
-    }
+    for (int s = 0; s < kStages; ++s) mbar_init(smem_u32(&sh.full[s]), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sh.tmem_base)),
-                 "r"((uint32_t)tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  if (NT > cout) {     // zero the padding rows of every B tile once: the bulk copies never write them
+    const int pad_pieces = (NT - cout) * 8;
+    for (int i = t; i < kStages * 2 * pad_pieces; i += kThreadsOS) {
+      const int tile = i / pad_pieces, e = i % pad_pieces;
+      *reinterpret_cast<uint4*>(stage0 + (tile >> 1) * kStageBytes + 2 * kATileBytes + (tile & 1) * kBTileBytes +
+                                (cout + (e >> 3)) * 128 + (e & 7) * 16) = make_uint4(0u, 0u, 0u, 0u);
+    }
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = sh.tmem_base;
 
-  if (warp < kLoaderWarps) {
-    // ================================ loaders ============================================
-    const int piece = t & 7, rgrp = t >> 3;           // 8 lanes cover one 128-byte row; 32 row groups
-    const uint32_t a_off = (uint32_t)(rgrp * 128 + ((piece ^ (rgrp & 7)) << 4));
-    const uint32_t slab_bytes = 2u * (uint32_t)b_tile_bytes;
-    // flattened work sequence of this CTA: (tile, kappa, chunk); the gather runs ONE step ahead of the store
-    auto rows_of = [&](int tile, int kappa, int (&src)[4]) {
-      const int j0 = tile * kTileM;
+  // gather: 8 lanes cover one 128-byte row; 32 row groups, rows rgrp + 32 i
+  const int piece = t & 7, rgrp = t >> 3;
+  const uint32_t a_off = (uint32_t)(rgrp * 128 + ((piece ^ (rgrp & 7)) << 4));
+  int src[4];
+  auto rows_of = [&](int kappa) {
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = j0 + i * 32 + rgrp;
-        src[i] = (r < n_out) ? __ldg(nbr + (int64_t)kappa * nbr_stride + r) : -1;
-      }
-    };
-    auto load_a = [&](const int (&src)[4], int c, float4 (&v)[4]) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        v[i] = src[i] >= 0 ? __ldg(reinterpret_cast<const float4*>(in_feat + (size_t)src[i] * cin + c * kChunk + piece * 4))
-                           : make_float4(0.f, 0.f, 0.f, 0.f);
-    };
-    // prefetch cursor
-    int pf_tile = blockIdx.x, pf_k = 0, pf_c = 0;
-    int pf_src[4];
-    float4 cur[4], nxt[4];
-    if (pf_tile < n_tiles) {
-      rows_of(pf_tile, 0, pf_src);
-      load_a(pf_src, 0, cur);
+    for (int i = 0; i < 4; ++i) {
+      const int r = j0 + i * 32 + rgrp;
+      src[i] = (r < n_out) ? __ldg(nbr + (int64_t)kappa * nbr_stride + r) : -1;
     }
-    auto advance = [&]() {            // move the cursor one step; reload the row indices at a new (tile, kappa)
-      if (++pf_c == n_chunks) {
-        pf_c = 0;
-        if (++pf_k == K) {
-          pf_k = 0;
-          pf_tile += gridDim.x;
-        }
-        if (pf_tile < n_tiles) rows_of(pf_tile, pf_k, pf_src);
-      }
-    };
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      for (int kappa = 0; kappa < K; ++kappa) {
-        const float* slab = wt + (size_t)kappa * n_chunks * (slab_bytes / 4);
-        for (int c = 0; c < n_chunks; ++c, ++it) {
-          const int s = it % n_stages;
-          const uint32_t ph = (it / n_stages) & 1;
-          advance();
-          if (pf_tile < n_tiles) load_a(pf_src, pf_c, nxt);      // next step's rows are in flight during the wait
-          mbar_wait(smem_u32(&sh.empty[s]), ph ^ 1);
-          unsigned char* a_hi = stage0 + (size_t)s * stage_bytes;
-          unsigned char* a_lo = a_hi + kATileBytes;
-          if (t == 0) {
-            const float* src = slab + (size_t)c * (slab_bytes / 4);
-            mbar_expect_tx(smem_u32(&sh.full[s]), (uint32_t)b_tile_bytes);
-            mbar_arrive_expect_tx(smem_u32(&sh.full_lo[s]), (uint32_t)b_tile_bytes);
-            bulk_g2s(smem_u32(a_lo + kATileBytes), src, (uint32_t)b_tile_bytes, smem_u32(&sh.full[s]));
-            bulk_g2s(smem_u32(a_lo + kATileBytes + b_tile_bytes), src + b_tile_bytes / 4, (uint32_t)b_tile_bytes,
-                     smem_u32(&sh.full_lo[s]));
-          }
+  };
+  float4 v[4];
+  auto load_a = [&](int c) {
 #pragma unroll
-          for (int i = 0; i < 4; ++i) split_store(cur[i], a_hi, a_lo, a_off + i * 4096);
-          fence_proxy_async();
-          mbar_arrive(smem_u32(&sh.full[s]));
+    for (int i = 0; i < 4; ++i)
+      v[i] = src[i] >= 0 ? __ldg(reinterpret_cast<const float4*>(in_feat + (size_t)src[i] * cin + c * kChunk + piece * 4))
+                         : make_float4(0.f, 0.f, 0.f, 0.f);
+  };
+
+  float acc[NT / 2];
 #pragma unroll
-          for (int i = 0; i < 4; ++i) cur[i] = nxt[i];
-        }
-      }
+  for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+  rows_of(0);
+  load_a(0);
+  for (int step = 0; step < steps; ++step) {
+    const int s = step % kStages;
+    const uint32_t ph = (step / kStages) & 1;
+    unsigned char* a_hi = stage0 + (size_t)s * kStageBytes;
+    unsigned char* a_lo = a_hi + kATileBytes;
+    unsigned char* b_hi = a_lo + kATileBytes;
+    __syncthreads();       // every warpgroup has retired the MMAs of step - kStages: stage s is free
+    if (t == 0) {
+      const unsigned char* bsrc = reinterpret_cast<const unsigned char*>(wt) + (size_t)step * slab_bytes;
+      mbar_arrive_expect_tx(smem_u32(&sh.full[s]), slab_bytes);
+      bulk_g2s(smem_u32(b_hi), bsrc, b_tile_bytes, smem_u32(&sh.full[s]));
+      bulk_g2s(smem_u32(b_hi + kBTileBytes), bsrc + b_tile_bytes, b_tile_bytes, smem_u32(&sh.full[s]));
     }
-  } else if (warp == kMmaWarp) {
-    // ================================ MMA issuer =========================================
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(cout >> 3) << 17) |
-                           ((uint32_t)(kTileM >> 4) << 24);
-    uint32_t it = 0, tile_iter = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tile_iter) {
-      const uint32_t buf = tile_iter & 1;
-      const uint32_t tmem_d = tmem_base + buf * acc_stride;
-      mbar_wait(smem_u32(&sh.acc_empty[buf]), ((tile_iter >> 1) & 1) ^ 1);
-      tc_fence_after();
-      for (int step = 0; step < steps_per_tile; ++step, ++it) {
-        const int s = it % n_stages;
-        const uint32_t ph = (it / n_stages) & 1;
-        mbar_wait(smem_u32(&sh.full[s]), ph);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t a_hi = smem_u32(stage0 + (size_t)s * stage_bytes);
-          const uint32_t a_lo = a_hi + kATileBytes;
-          const uint32_t b_hi = a_lo + kATileBytes;
 #pragma unroll
-          for (int ks = 0; ks < kChunk / 8; ++ks) {
-            const uint32_t ko = ks * 32;
-            const uint64_t dbh = umma_desc(b_hi + ko);
-            tc_mma_tf32(tmem_d, umma_desc(a_hi + ko), dbh, idesc, (step | ks) != 0);
-            tc_mma_tf32(tmem_d, umma_desc(a_lo + ko), dbh, idesc, 1);
-          }
-        }
-        mbar_wait(smem_u32(&sh.full_lo[s]), ph);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t a_hi = smem_u32(stage0 + (size_t)s * stage_bytes);
-          const uint32_t b_lo = a_hi + 2 * kATileBytes + b_tile_bytes;
-#pragma unroll
-          for (int ks = 0; ks < kChunk / 8; ++ks)
-            tc_mma_tf32(tmem_d, umma_desc(a_hi + ks * 32), umma_desc(b_lo + ks * 32), idesc, 1);
-          tc_commit(smem_u32(&sh.empty[s]));
-          if (step == steps_per_tile - 1) tc_commit(smem_u32(&sh.acc_full[buf]));
-        }
-        __syncwarp();
-      }
+    for (int i = 0; i < 4; ++i) split_store(v[i], a_hi, a_lo, a_off + i * 4096);
+    if (step + 1 < steps) {                 // the next step's rows are in flight while this one multiplies
+      const int c = (step + 1) % n_chunks;
+      if (c == 0) rows_of((step + 1) / n_chunks);
+      load_a(c);
     }
-  } else {
-    // ================================ epilogue ===========================================
-    const int lane_grp = warp & 3;            // TMEM lanes 32 * (warp % 4) .. + 31
-    unsigned char* stg = stage0 + (size_t)n_stages * stage_bytes + (warp - kLoaderWarps - 1) * 4096;
-    uint32_t tile_iter = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tile_iter) {
-      const uint32_t buf = tile_iter & 1;
-      const int row_base = tile * kTileM + lane_grp * 32;       // this warp's 32 output rows
-      mbar_wait(smem_u32(&sh.acc_full[buf]), (tile_iter >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + buf * acc_stride + ((uint32_t)(lane_grp * 32) << 16);
-      for (int col = 0; col < cout; col += 32) {
-        uint32_t v[32];
-        tc_ld32(taddr + col, v);
-        // thread = row  ->  transposed through a 4 KB XOR-swizzled tile  ->  8 lanes per row's 128-byte line
+    fence_proxy_async();
+    __syncthreads();
+    mbar_wait(smem_u32(&sh.full[s]), ph);
+    wgmma_fence();
+    const uint32_t a0 = smem_u32(a_hi) + wg * (kATileBytes / 2);
+    mma_chunk<NT, false, 3>(acc, a0, a0 + kATileBytes, smem_u32(b_hi), smem_u32(b_hi) + kBTileBytes);
+    wgmma_commit();
+    wgmma_wait<1>();
+  }
+  wgmma_wait<0>();
+  fence_acc(acc);
+
+  // epilogue: thread holds rows r and r + 8 of its warpgroup, two adjacent columns per 8-column group
+  const int lane = t & 31;
+  const int r = j0 + wg * 64 + ((t >> 5) & 3) * 16 + (lane >> 2);
 #pragma unroll
-        for (int q = 0; q < 8; ++q)
-          *reinterpret_cast<uint4*>(stg + lane * 128 + ((q ^ (lane & 7)) << 4)) =
-              make_uint4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-        __syncwarp();
-        const int p = lane & 7, rsub = lane >> 3;
-        const float4 sc = scale != nullptr ? __ldg(reinterpret_cast<const float4*>(scale + col + p * 4))
-                                           : make_float4(1.f, 1.f, 1.f, 1.f);
-        const float4 sf = shift != nullptr ? __ldg(reinterpret_cast<const float4*>(shift + col + p * 4))
-                                           : make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int i = 0; i < NT / 8; ++i) {
+    const int col = 8 * i + 2 * (lane & 3);
+    if (col < cout) {
+      const float2 sc = scale != nullptr ? __ldg(reinterpret_cast<const float2*>(scale + col)) : make_float2(1.f, 1.f);
+      const float2 sf = shift != nullptr ? __ldg(reinterpret_cast<const float2*>(shift + col)) : make_float2(0.f, 0.f);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const int R = rsub + 4 * k;
-          const int j = row_base + R;
-          float4 x = *reinterpret_cast<const float4*>(stg + R * 128 + ((p ^ (R & 7)) << 4));
-          if (j < n_out) {
-            x.x = fmaf(x.x, sc.x, sf.x); x.y = fmaf(x.y, sc.y, sf.y); x.z = fmaf(x.z, sc.z, sf.z); x.w = fmaf(x.w, sc.w, sf.w);
-            const size_t o = (size_t)j * cout + col + p * 4;
-            if (residual != nullptr) {
-              const float4 r4 = __ldg(reinterpret_cast<const float4*>(residual + o));
-              x.x += r4.x; x.y += r4.y; x.z += r4.z; x.w += r4.w;
-            }
-            if (relu) {
-              x.x = fmaxf(x.x, 0.f); x.y = fmaxf(x.y, 0.f); x.z = fmaxf(x.z, 0.f); x.w = fmaxf(x.w, 0.f);
-            }
-            *reinterpret_cast<float4*>(out + o) = x;
+      for (int h = 0; h < 2; ++h) {
+        const int j = r + 8 * h;
+        if (j < n_out) {
+          float2 x = make_float2(fmaf(acc[4 * i + 2 * h], sc.x, sf.x), fmaf(acc[4 * i + 2 * h + 1], sc.y, sf.y));
+          const size_t o = (size_t)j * cout + col;
+          if (residual != nullptr) {
+            const float2 r2 = __ldg(reinterpret_cast<const float2*>(residual + o));
+            x.x += r2.x; x.y += r2.y;
           }
+          if (relu) {
+            x.x = fmaxf(x.x, 0.f); x.y = fmaxf(x.y, 0.f);
+          }
+          *reinterpret_cast<float2*>(out + o) = x;
         }
-        __syncwarp();
       }
-      tc_fence_before();
-      mbar_arrive(smem_u32(&sh.acc_empty[buf]));
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)tmem_cols)
-                 : "memory");
-  }
+}
+
+// one instantiation per kernel: DGR_ENSURE_SMEM keeps its attribute state per call site
+template <int NT>
+int32_t launch_spconv_os(const float* in_feat, int cin, const float* wt, int cout, const int32_t* nbr,
+                         int64_t nbr_stride, int K, int n_out, const float* scale, const float* shift,
+                         const float* residual, int relu, float* out, cudaStream_t st) {
+  const size_t smem = os_smem_bytes(NT);
+  DGR_ENSURE_SMEM(spconv_os_kernel<NT>, smem);
+  spconv_os_kernel<NT><<<(n_out + kTileM - 1) / kTileM, kThreadsOS, smem, st>>>(
+      in_feat, cin, wt, cout, nbr, nbr_stride, K, n_out, scale, shift, residual, relu, out);
+  dgr_note_launches(1);
+  DGR_LAUNCH_CHECK();
+  return DGR_OK;
 }
 
 }  // namespace
@@ -294,26 +194,10 @@ int32_t dgr_spconv_os_fwd(const float* in_feat, int32_t cin, const float* weight
   DGR_ARG_CHECK((scale == nullptr) == (shift == nullptr), "scale and shift go together");
   DGR_ARG_CHECK(K >= 1 && nbr_stride >= n_out && n_out < (1ll << 31), "bad neighbour table extents");
   if (n_out == 0) return DGR_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int stage_bytes = 2 * kATileBytes + 2 * cout * 128;
-  int n_stages = (200 * 1024) / stage_bytes;
-  if (n_stages > 4) n_stages = 4;
-  if (n_stages < 2) n_stages = 2;
-  const size_t smem = sizeof(OsShared) + 1024 + (size_t)n_stages * stage_bytes + kEpiStageBytes;
-  int acc_cols = 32;
-  while (acc_cols < cout) acc_cols <<= 1;
-  const int tmem_cols = 2 * acc_cols;
-  int dev = 0, sms = 148;
-  DGR_CUDA_CHECK(cudaGetDevice(&dev));
-  DGR_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const int n_tiles = (int)((n_out + kTileM - 1) / kTileM);
-  const int grid = n_tiles < sms ? n_tiles : sms;
-  DGR_ENSURE_SMEM(spconv_os_kernel, smem);
-  spconv_os_kernel<<<grid, kThreadsOS, smem, st>>>(in_feat, cin, weight_t, cout, nbr, nbr_stride, K, (int)n_out, n_stages,
-                                                   tmem_cols, scale, shift, residual, relu, out);
-  dgr_note_launches(1);
-  DGR_LAUNCH_CHECK();
-  return DGR_OK;
+  auto launch = cout <= 32 ? launch_spconv_os<32> : cout <= 64 ? launch_spconv_os<64>
+                : cout <= 128 ? launch_spconv_os<128> : launch_spconv_os<256>;
+  return launch(in_feat, cin, weight_t, cout, nbr, nbr_stride, K, (int)n_out, scale, shift, residual, relu, out,
+                (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -1,7 +1,10 @@
-// tcgen05 / TMEM / mbarrier primitives shared by the tensor-core kernels (sm_100a inline PTX).
+// wgmma / mbarrier / bulk-copy primitives shared by the tensor-core kernels (sm_90a inline PTX).
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace tc {
 
@@ -10,9 +13,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
@@ -29,80 +29,46 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
 }
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads, bulk copies)
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
+// 1-D bulk copy global -> shared (TMA engine), completion signalled on an mbarrier
+__device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                   dst_smem),
+               "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-__device__ __forceinline__ void tc_mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A operand taken from tensor memory (lane = row, consecutive columns = K), B from shared memory
-__device__ __forceinline__ void tc_mma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// registers -> tensor memory: thread's lane, 32 consecutive 32-bit columns
-__device__ __forceinline__ void tc_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-        "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]),
-        "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]),
-        "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tc_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]),
-        "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]),
-        "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]),
-        "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// K-major SWIZZLE_128B operand descriptor: 8-row groups of 128-byte rows, 1024 bytes apart.
+// A k-step inside the 128-byte row advances the start address by its byte offset.
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);   // start address
+  d |= (uint64_t)1 << 16;                         // leading byte offset (unused for SW128 K-major)
+  d |= (uint64_t)(1024 >> 4) << 32;               // stride byte offset: next 8-row group
+  d |= (uint64_t)1 << 62;                         // SWIZZLE_128B
+  return d;
 }
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]),
-        "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory");
 }
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d)
-               : "memory");
+// pins the accumulator registers in place across wgmma_wait: no read may be hoisted above it
+template <int R>
+__device__ __forceinline__ void fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 __device__ __forceinline__ float tf32_round(float x) {
   uint32_t r;
@@ -110,16 +76,61 @@ __device__ __forceinline__ float tf32_round(float x) {
   return __uint_as_float(r);
 }
 
-// K-major SWIZZLE_128B operand descriptor: 8-row groups of 128-byte rows, 1024 bytes apart.
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);   // start address
-  d |= (uint64_t)1 << 16;                         // leading byte offset (unused for SW128 K-major)
-  d |= (uint64_t)(1024 >> 4) << 32;               // stride byte offset: next 8-row group
-  d |= (uint64_t)1 << 46;                         // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                         // SWIZZLE_128B
-  return d;
+// split one float4 into a TF32 "hi" part (round to nearest) and the exact fp32 residual "lo"
+// (the tensor core truncates lo to TF32: 2^-21 relative overall) and store both 16-byte pieces
+__device__ __forceinline__ void split_store(float4 v, unsigned char* hi_tile, unsigned char* lo_tile, uint32_t off) {
+  float4 h, l;
+  h.x = tf32_round(v.x); h.y = tf32_round(v.y); h.z = tf32_round(v.z); h.w = tf32_round(v.w);
+  l.x = v.x - h.x; l.y = v.y - h.y; l.z = v.z - h.z; l.w = v.w - h.w;
+  *reinterpret_cast<float4*>(hi_tile + off) = h;
+  *reinterpret_cast<float4*>(lo_tile + off) = l;
 }
 
+// 3xFP16 split: fp16 carries the same 11 significant bits as TF32 at half the bytes and twice the tensor
+// rate.  x is first scaled by a power of two `sx` (exact) that maps the tensor's absolute maximum into
+// [2^14, 2^15) - below fp16's 65504, far above its 2^-14 normal floor - then split into hi = fp16(x'),
+// lo = fp16(x' - hi): the same hi*hi + lo*hi + hi*lo products as 3xTF32, 2^-21 relative (an element more
+// than 2^17 below the tensor's maximum loses bits of its lo part: <= 2^-39 of the maximum).
+__device__ __forceinline__ void split_store_f16(float4 a, float4 b, float sx, unsigned char* hi_tile,
+                                                unsigned char* lo_tile, uint32_t off) {
+  const float x[8] = {a.x * sx, a.y * sx, a.z * sx, a.w * sx, b.x * sx, b.y * sx, b.z * sx, b.w * sx};
+  uint32_t h[4], l[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const __half2 hh = __floats2half2_rn(x[2 * i], x[2 * i + 1]);
+    const float2 hf = __half22float2(hh);
+    const __half2 ll = __floats2half2_rn(x[2 * i] - hf.x, x[2 * i + 1] - hf.y);
+    h[i] = *reinterpret_cast<const uint32_t*>(&hh);
+    l[i] = *reinterpret_cast<const uint32_t*>(&ll);
+  }
+  *reinterpret_cast<uint4*>(hi_tile + off) = make_uint4(h[0], h[1], h[2], h[3]);
+  *reinterpret_cast<uint4*>(lo_tile + off) = make_uint4(l[0], l[1], l[2], l[3]);
+}
+// power of two that maps `amax` into [2^14, 2^15); 1 for amax == 0 / non-finite
+__device__ __forceinline__ float f16_scale_for(float amax) {
+  const uint32_t b = __float_as_uint(amax);
+  const int e = (int)((b >> 23) & 255u);
+  if (e == 0 || e == 255) return 1.f;
+  int se = 14 - (e - 127) + 127;
+  se = se < 1 ? 1 : (se > 254 ? 254 : se);
+  return __uint_as_float((uint32_t)se << 23);
+}
+
+// One 128-byte K chunk (4 k-steps of 32 bytes) of a warpgroup's D[64, N] += A . B^T.
+// kPasses = 3: hi*hi + lo*hi + hi*lo (split operands, fp32-accurate); kPasses = 1: hi*hi only.
+template <int N, bool kF16, int kPasses>
+__device__ __forceinline__ void mma_chunk(float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
+                                          uint32_t b_lo) {
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    const uint32_t ko = ks * 32;
+    const uint64_t dbh = wgmma_desc(b_hi + ko);
+    Wgmma<N, kF16>::mma(d, wgmma_desc(a_hi + ko), dbh);
+    if (kPasses == 3) {
+      Wgmma<N, kF16>::mma(d, wgmma_desc(a_lo + ko), dbh);
+      Wgmma<N, kF16>::mma(d, wgmma_desc(a_hi + ko), wgmma_desc(b_lo + ko));
+    }
+  }
+}
 
 }  // namespace tc

@@ -24,8 +24,8 @@ from . import utils  # noqa: F401  (ME.utils.sparse_quantize / batched_coordinat
 __version__ = '0.5.4+dgr_b200'
 
 # Arithmetic of the sparse convolution sub-GEMMs:
-#   'tc3'  tcgen05 3xTF32 (hi*hi + lo*hi + hi*lo), fp32-accurate - the default
-#   'tc1'  tcgen05 single TF32 product (~1e-3 relative), opt-in fast mode
+#   'tc3'  wgmma 3xTF32 (hi*hi + lo*hi + hi*lo), fp32-accurate - the default
+#   'tc1'  wgmma single TF32 product (~1e-3 relative), opt-in fast mode
 #   'simt' fp32 FFMA kernel (also the fallback for shapes the tensor-core path rejects)
 _CONV_MODE = 'tc3'
 

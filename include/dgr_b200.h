@@ -1,5 +1,5 @@
 /*
- * dgr_b200.h - C ABI of libdgr_b200.so: the B200-native (sm_100a) replacement for the
+ * dgr_b200.h - C ABI of libdgr_b200.so: the H100-native (sm_90a) replacement for the
  * native layer underneath Deep Global Registration's pairwise-registration hot path.
  *
  * The reference (chrischoy/DeepGlobalRegistration) has no native code of its own; the
@@ -19,7 +19,7 @@
  *   - all row indices are int32; feature matrices are row-major float32 [rows, channels];
  *     coordinate matrices are row-major int32 [rows, ncols] with column 0 = batch index
  *     (ME.utils.batched_coordinates layout, core/deep_global_registration.py:158);
- *   - there is no CPU fallback: on a machine without an sm_100 device every compute
+ *   - there is no CPU fallback: on a machine without an sm_90 device every compute
  *     entry point fails with DGR_ERR_DEVICE.
  */
 #ifndef DGR_B200_H_
@@ -57,7 +57,7 @@ int32_t dgr_version(void);
 const char* dgr_last_error(void);
 /* Number of CUDA kernels this library has launched in this process (all threads). */
 int64_t dgr_launch_count(void);
-/* 0 if device `device` is sm_100 (B200); DGR_ERR_DEVICE otherwise.  Host-only query. */
+/* 0 if device `device` is sm_90 (H100); DGR_ERR_DEVICE otherwise.  Host-only query. */
 int32_t dgr_device_check(int32_t device);
 
 /* ---- voxelisation: ME.utils.sparse_quantize + re-floor of preprocess()
@@ -134,8 +134,8 @@ int32_t dgr_kernel_map_fill(const int32_t* nbr, int32_t K, int64_t n_out, const 
 /* Work list of the gather-GEMM-scatter kernel: tile t covers pairs
  * [tile_start[t], min(tile_start[t] + tile_rows, kofs[tile_k[t] + 1])) of bucket tile_k[t].
  * n_tiles = sum_k ceil(count_k / tile_rows) is computed by the caller from kofs.  pair != 0
- * rounds every offset's tile count up to even (the extra tile is empty) - the list the 2-CTA
- * cluster variant of the tensor-core convolution consumes. */
+ * rounds every offset's tile count up to even (the extra tile is empty); the convolutions skip
+ * empty tiles, so either list serves them. */
 int32_t dgr_kernel_map_tiles(const int32_t* kofs, int32_t K, int32_t tile_rows, int32_t n_tiles, int32_t pair,
                              int32_t* tile_k, int32_t* tile_start, void* stream);
 /* Both lists (pair = 0 and pair = 1) in one launch. */
@@ -153,29 +153,21 @@ int32_t dgr_spconv_fwd(const float* in_feat, int32_t cin, const float* weight, i
                        const int32_t* in_idx, const int32_t* out_idx, const int32_t* kofs,
                        const int32_t* tile_k, const int32_t* tile_start, int32_t n_tiles,
                        int32_t tile_rows, int32_t relu_in, float* out, void* stream);
-/* Tensor-core (tcgen05.mma kind::tf32, TMEM accumulator) variant of dgr_spconv_fwd for
+/* Tensor-core (wgmma, TF32 operands, fp32 register accumulator) variant of dgr_spconv_fwd for
  * cin % 32 == 0 and cout in {16, 32, ..., 256} (dgr_spconv_tc_supported returns 1).
  * weight_t is the layer's weight in the packed layout of dgr_pack_weight_tf32
  * ([K][cin/32][2][cout][32]: per offset and 32-channel chunk the TF32 hi tile and the lo
  * residual tile in shared-memory image order; the host caches it per layer; 2 * K * cin * cout
  * floats).  passes = 3 evaluates every
  * product as hi*hi + lo*hi + hi*lo on TF32 splits (fp32-accurate); passes = 1 is plain
- * TF32 (~1e-3 relative), offered as an opt-in fast mode.  `cluster` selects the kernel variant:
- * 1 = both operands in shared memory (default); 0 = A operand split straight into tensor memory
- * (tcgen05.st), shared memory holds only the weight slabs; 2 = as 1 with thread-block clusters of
- * two CTAs that work on two tiles of the same offset and receive each weight tile by ONE multicast
- * bulk copy; 3 = tcgen05 cta_group::2: the CTA pair issues ONE M = 256 MMA per two tiles of the same
- * offset and every CTA holds only half of each weight tile (2 and 3 need the paired tile list of
- * dgr_kernel_map_tiles(pair = 1)).  All variants scatter through a shared-memory transpose so that a
- * warp instruction writes whole 128-byte lines of the output rows.  Process-level tuning knobs read
- * once from the environment: DGR_TC_PREFETCH (gather lookahead in chunks, 1..3, default 1),
- * DGR_TC_EPILOGUE (0 = scatter one row per lane, the pre-transposition epilogue; default 1). */
+ * TF32 (~1e-3 relative), offered as an opt-in fast mode.  One CTA per 128-pair tile; the weight
+ * slab of each 32-channel chunk arrives by one bulk copy. */
 int32_t dgr_spconv_tc_supported(int32_t cin, int32_t cout);
 int32_t dgr_pack_weight_tf32(const float* w, int32_t K, int32_t cin, int32_t cout, float* packed, void* stream);
 int32_t dgr_spconv_tc_fwd(const float* in_feat, int32_t cin, const float* weight_t, int32_t cout,
                           const int32_t* in_idx, const int32_t* out_idx, const int32_t* kofs,
                           const int32_t* tile_k, const int32_t* tile_start, int32_t n_tiles,
-                          int32_t tile_rows, int32_t passes, int32_t cluster, float* out, void* stream);
+                          int32_t tile_rows, int32_t passes, float* out, void* stream);
 /* Output-stationary variant for few input channels (conv1: cin == 1): reads the dense
  * neighbour table, no atomics, optional fused per-channel affine (eval BatchNorm):
  *   out[j, :] = (sum_kappa in[nbr[kappa, j], :] @ W[kappa]) * scale + shift. */
@@ -210,7 +202,7 @@ int32_t dgr_l2_normalize(const float* x, int64_t n, int32_t c, float* out, void*
 int32_t dgr_knn_top1(const float* f0, int64_t n0, const float* f1, int64_t n1, int32_t c,
                      uint64_t* packed_ws, int32_t* idx, float* dist, void* stream);
 
-/* Tensor-core variant for c in {32, 64} (dgr_knn_tc_supported): two tcgen05 (TF32) sweeps
+/* Tensor-core variant for c in {32, 64} (dgr_knn_tc_supported): two wgmma (TF32) sweeps
  * find, per row, the candidate columns whose approximate distance is within a proven error
  * bound of the row minimum; only those are evaluated with the exact fp32 arithmetic above.
  * Results are bit-identical to dgr_knn_top1.  ws: dgr_knn_tc_ws_elems(n0, n1) floats. */
@@ -288,7 +280,7 @@ int32_t dgr_spconv_wgrad(const float* in_feat, int32_t cin, const float* grad_ou
                          const int32_t* in_idx, const int32_t* out_idx, const int32_t* kofs, int32_t K, float* dw,
                          void* stream);
 
-/* ---- 3xFP16 mode of the cta_group::2 tensor-core convolution ---------------------------------
+/* ---- 3xFP16 mode of the tensor-core convolution ----------------------------------------------
  * fp16 has TF32's 11 significant bits at half the bytes and twice the tensor rate; operands are scaled by
  * powers of two (exact) so that the tensor's absolute maximum lands in [2^14, 2^15), then split hi / lo as
  * in the 3xTF32 path: same 2^-21 relative accuracy, 1.5 TF32-MMA equivalents per product instead of 3. */
@@ -303,7 +295,7 @@ int32_t dgr_spconv_tc_f16_supported(int32_t cin, int32_t cout);     /* cin % 64 
  * scale_ws: device float[2] = (1 / weight scale, max |W|). */
 int32_t dgr_pack_weight_f16(const float* w, int32_t K, int32_t cin, int32_t cout, void* packed, float* scale_ws,
                             void* stream);
-/* Same contract as dgr_spconv_tc_fwd(cluster = 3) (paired tile list).  amax_in: device float >= max |in_feat|
+/* Same contract as dgr_spconv_tc_fwd (plain or paired tile list).  amax_in: device float >= max |in_feat|
  * (dgr_absmax_f32); w_scale: scale_ws of dgr_pack_weight_f16. */
 int32_t dgr_spconv_tc_f16_fwd(const float* in_feat, int32_t cin, const void* weight_h, int32_t cout,
                               const int32_t* in_idx, const int32_t* out_idx, const int32_t* kofs,
@@ -369,7 +361,7 @@ int32_t dgr_kmap_dense(const int32_t* out_coords, int64_t n_out_max, const int32
 /* ---- output-stationary tensor-core convolution with the fused layer epilogue (csrc/spconv_os.cu) ----------
  * For stride-1 layers whose neighbour table is dense enough (3^3 kernels of the 3-D network, ~64 % occupied):
  *   out[j, :] = act((sum_kappa in_feat[nbr[kappa * nbr_stride + j], :] @ W[kappa]) * scale + shift + residual[j, :])
- * tile = 128 output rows, accumulator in TMEM across all offsets, 3xTF32 from the packed slabs of
+ * tile = 128 output rows, accumulator in registers across all offsets, 3xTF32 from the packed slabs of
  * dgr_pack_weight_tf32; every output row is written once with plain stores (no atomics, no pre-zeroed buffer,
  * deterministic); eval BatchNorm (model/common.py:13), the residual add and ReLU of BasicBlockBase.forward
  * (model/residual_block.py:118-134) ride in the epilogue.  scale / shift / residual may be NULL. */

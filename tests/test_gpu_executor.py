@@ -291,7 +291,7 @@ def test_safeguard_branch_native_equals_stagewise(dgr):
                                                     (6, 256, 256, 3000, 3, 300.0), (3, 64, 32, 600, 5, 1.0),
                                                     (3, 192, 160, 2500, 8, 7.0)])
 def test_conv_3xfp16_matches_fp32_and_3xtf32(abi, D, cin, cout, n, ext, scale):
-  """The 3xFP16 mode of the cta_group::2 kernel against the fp32 FFMA kernel (and the 3xTF32 mode) on data of very
+  """The 3xFP16 mode of the tensor-core kernel against the fp32 FFMA kernel (and the 3xTF32 mode) on data of very
   different magnitudes, with heavy-tailed activations: the power-of-two scaling keeps fp16 in range."""
   from deepglobalregistration_b200.me.coords import CoordinateMapKey
   coords = _cloud(D, n, ext, seed=cin + cout)
@@ -314,7 +314,7 @@ def test_conv_3xfp16_matches_fp32_and_3xtf32(abi, D, cin, cout, n, ext, scale):
       ref64.index_add_(0, jj[a:b], feat[ii[a:b]].double() @ W[kap].double())
   out16 = abi.spconv_tc_f16_fwd(feat, W, km, torch.zeros(nrow, cout, device='cuda'))
   out32 = abi.spconv_tc_fwd(feat, abi.pack_weight_tf32(W, 3 ** D, cin, cout), km, torch.zeros(nrow, cout, device='cuda'),
-                            passes=3, cluster=3)
+                            passes=3)
   torch.cuda.synchronize()
   mag = float(ref64.abs().max())
   e16 = float((out16.double() - ref64).abs().max()) / mag

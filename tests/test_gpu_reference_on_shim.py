@@ -1,15 +1,7 @@
-"""Boundary b2 (SURVEY 8b): the reference's own code on this stack.
-
-* The open3d stand-in's registration pipeline (o3d_registration.py: registration_icp /
-  registration_ransac_based_on_correspondence behind `open3d.pipelines.registration`) called the way
-  core/deep_global_registration.py:50-64,317-322 and util/pointcloud.py:15-23 call open3d, against the library
-  entry points and the oracle.  Runs on any GPU box.
-* The reference's UNMODIFIED `core/deep_global_registration.py::DeepGlobalRegistration` and `model/resunet.py`
-  imported from /root/reference over shims.install() (MinkowskiEngine -> me, open3d -> the stand-in), on cuda,
-  against this package's class and the oracle.  Needs BOTH a GPU and the reference tree; the reference tree is
-  not allowed to travel to the GPU box (no reference sources in the repo), so there these tests skip - they are
-  the recipe a maintainer with both at hand runs (INTEGRATION.md section 1)."""
-import os
+"""Boundary b2 (SURVEY 8b): the open3d stand-in's registration pipeline (o3d_registration.py: registration_icp /
+registration_ransac_based_on_correspondence behind `open3d.pipelines.registration`) called the way
+core/deep_global_registration.py:50-64,317-322 and util/pointcloud.py:15-23 of the reference call open3d, against
+the library entry points and the oracle."""
 import sys
 import types
 
@@ -20,7 +12,6 @@ import torch
 from deepglobalregistration_b200 import synthetic as syn
 
 pytestmark = pytest.mark.gpu
-REF = '/root/reference'
 EXTENT = (1.8, 1.5, 1.25)
 
 
@@ -85,100 +76,3 @@ def test_standin_ransac_equals_library(setup):
   assert np.allclose(res.transformation, lib[:16].reshape(4, 4), atol=1e-12)
   te, re = syn.rte_rre(res.transformation, T_gt)
   assert te <= 0.02 and re <= 0.02 and res.fitness > 0.25
-
-
-# ------------------------------------------------------------------------------------------------------------
-# the reference's own files (need /root/reference AND a GPU)
-# ------------------------------------------------------------------------------------------------------------
-needs_reference = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, 'core')),
-                                     reason='reference tree not present on this box (it may not travel)')
-_REF_PACKAGES = ('model', 'core', 'util')
-
-
-@pytest.fixture
-def reference_modules(monkeypatch):
-  from deepglobalregistration_b200 import shims
-  saved = {k: sys.modules.get(k) for k in list(sys.modules)
-           if k.split('.')[0] in _REF_PACKAGES + ('open3d', 'MinkowskiEngine', 'easydict')}
-  for k in saved:
-    del sys.modules[k]
-  shims.install(force=True)
-  sys.path.insert(0, REF)
-  real_load = torch.load
-  preloaded = {}
-  monkeypatch.setattr(torch, 'load', lambda f, *a, **k: preloaded[str(f)] if str(f) in preloaded
-                      else real_load(f, *a, **dict(k, weights_only=False)))
-  cwd = os.getcwd()
-  try:
-    yield preloaded
-  finally:
-    os.chdir(cwd)
-    sys.path.remove(REF)
-    for k in [k for k in sys.modules if k.split('.')[0] in _REF_PACKAGES + ('open3d', 'MinkowskiEngine', 'easydict')]:
-      del sys.modules[k]
-    sys.modules.update({k: v for k, v in saved.items() if v is not None})
-
-
-@needs_reference
-def test_reference_class_on_cuda_equals_ours_and_oracle(reference_modules, tmp_path, setup):
-  from oracle import pipeline as op
-  d, state, _, _ = setup
-  from core.deep_global_registration import DeepGlobalRegistration as RefDGR      # the reference's file, unmodified
-  path = tmp_path / 'ckpt.pth'
-  path.write_bytes(b'')
-  reference_modules[str(path)] = state
-  ref = RefDGR(types.SimpleNamespace(weights=str(path), clip_weight_thresh=0.05), device=torch.device('cuda'))
-  xyz0, xyz1, _ = syn.room_pair(2, n_raw=20000, extent=EXTENT)
-  T_ref = ref.register(xyz0, xyz1)                          # ME -> me, open3d ICP -> dgr_icp_point_to_point
-  d.use_icp = True
-  T_ours = d.register(xyz0, xyz1)
-  te, re = syn.rte_rre(T_ref, T_ours)
-  assert te <= 1e-5 and re <= 1e-5, (te, re)
-  T_o, _ = op.register(state, xyz0, xyz1, use_icp=True)
-  te, re = syn.rte_rre(T_ref, T_o)
-  assert te <= 1e-3 and re <= 1e-3, (te, re)
-
-
-@needs_reference
-def test_reference_resunet_forward_on_cuda_equals_oracle(reference_modules):
-  import MinkowskiEngine as ME
-  from model.resunet import ResUNetBN2C                      # the reference's file, unmodified
-  from oracle.resunet import resunet_forward
-  sd = syn.resunet_state_dict(5, 1, 32, 7, 3)
-  net = ResUNetBN2C(1, 32, bn_momentum=0.05, conv1_kernel_size=7, normalize_feature=True, D=3)
-  net.load_state_dict(sd)
-  net = net.cuda().eval()
-  g = np.random.default_rng(0)
-  coords = np.unique(g.integers(-12, 12, size=(6000, 3)), axis=0)
-  coords = np.concatenate([np.zeros((len(coords), 1), np.int64), coords], 1).astype(np.int32)
-  with torch.no_grad():
-    out = net(ME.SparseTensor(torch.ones(len(coords), 1), coordinates=torch.from_numpy(coords), device='cuda')).F
-  want = resunet_forward(sd, coords, torch.ones(len(coords), 1), 7, True)
-  assert float((out.cpu() - want).abs().max()) <= 5e-5
-
-
-@needs_reference
-def test_reference_demo_flow_on_two_ply_files(reference_modules, tmp_path, setup):
-  """demo.py:28-48 without its download: read two PLY files with (stand-in) open3d, register with the reference's
-  class, transform, 'draw'."""
-  import open3d as o3d
-  from core.deep_global_registration import DeepGlobalRegistration as RefDGR
-  from deepglobalregistration_b200 import io as dio
-  d, state, _, _ = setup
-  path = tmp_path / 'ckpt.pth'
-  path.write_bytes(b'')
-  reference_modules[str(path)] = state
-  xyz0, xyz1, _ = syn.room_pair(6, n_raw=15000, extent=EXTENT)
-  dio.write_ply(str(tmp_path / 'a.ply'), xyz0, dtype='double')
-  dio.write_ply(str(tmp_path / 'b.ply'), xyz1, dtype='double')
-  dgr = RefDGR(types.SimpleNamespace(weights=str(path), clip_weight_thresh=0.05, pcd0=str(tmp_path / 'a.ply'),
-                                     pcd1=str(tmp_path / 'b.ply')))
-  pcd0 = o3d.io.read_point_cloud(str(tmp_path / 'a.ply'))
-  pcd0.estimate_normals() if hasattr(pcd0, 'estimate_normals') else None
-  pcd1 = o3d.io.read_point_cloud(str(tmp_path / 'b.ply'))
-  T01 = dgr.register(pcd0, pcd1)
-  o3d.visualization.draw_geometries([pcd0, pcd1])
-  pcd0.transform(T01)
-  d.use_icp = True
-  te, re = syn.rte_rre(T01, d.register(xyz0, xyz1))
-  assert te <= 1e-5 and re <= 1e-5

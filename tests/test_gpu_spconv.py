@@ -68,7 +68,7 @@ def test_spconv_stride1(abi, D, cin, cout, ks):
                                         (3, 256, 256), (3, 256, 128), (3, 128, 64), (3, 96, 48), (6, 32, 32),
                                         (6, 256, 256), (3, 32, 16), (3, 64, 240)])
 def test_spconv_tensor_core(abi, D, cin, cout):
-  """tcgen05 path: 3xTF32 must match the fp32 oracle like the FFMA kernel does; single-pass
+  """wgmma path: 3xTF32 must match the fp32 oracle like the FFMA kernel does; single-pass
   TF32 within 5e-3 of the result's scale."""
   from deepglobalregistration_b200.me.coords import CoordinateManager, CoordinateMapKey
   assert abi.tc_supported(cin, cout)
@@ -95,24 +95,23 @@ def test_spconv_tensor_core(abi, D, cin, cout):
   assert torch.equal(unsw, want_w)
   out = torch.zeros(n, cout, device='cuda')
   abi.spconv_tc_fwd(feat.cuda(), Wt, km, out, passes=3)
-  _close(out, want, what='tcgen05 3xTF32')
+  _close(out, want, what='wgmma 3xTF32')
   out1 = torch.zeros(n, cout, device='cuda')
   abi.spconv_tc_fwd(feat.cuda(), Wt, km, out1, passes=1)
   scale = float(want.abs().max())
-  assert float((out1.cpu() - want).abs().max()) <= 5e-3 * scale, 'tcgen05 1xTF32'
+  assert float((out1.cpu() - want).abs().max()) <= 5e-3 * scale, 'wgmma 1xTF32'
   # accumulate onto a non-zero initial value, twice in a row (persistent CTAs, phase tracking)
   init = torch.randn(n, cout, generator=g)
   out2 = init.clone().cuda()
   abi.spconv_tc_fwd(feat.cuda(), Wt, km, out2, passes=3)
   abi.spconv_tc_fwd(feat.cuda(), Wt, km, out2, passes=3)
-  _close(out2, init + 2 * want, what='tcgen05 accumulate')
+  _close(out2, init + 2 * want, what='wgmma accumulate')
 
 
 @pytest.mark.parametrize('D,cin,cout', [(3, 256, 256), (3, 128, 128), (6, 64, 240), (3, 32, 32)])
 def test_spconv_tensor_core_cta_pairs(abi, D, cin, cout):
-  """Every kernel variant - cta_group::2 (one M = 256 MMA per tile pair, half of each weight tile
-  per CTA), 2-CTA cluster with multicast weight tiles, A in shared memory, A in tensor memory -
-  on the paired tile list (empty padding tiles) or the plain one must match the oracle."""
+  """The tensor-core convolution on the paired tile list (an even tile count per offset, as CTA pairs consume it,
+  with empty padding tiles) and on the plain one must match the oracle, run after run."""
   from deepglobalregistration_b200.me.coords import CoordinateManager, CoordinateMapKey
   coords = _coords(cin + 7 * cout + D, 4000, D, 10 if D == 3 else 3)
   n = len(coords)
@@ -127,11 +126,12 @@ def test_spconv_tensor_core_cta_pairs(abi, D, cin, cout):
   assert nt % 2 == 0 and nt >= km.n_tiles
   tkh = tk.cpu().numpy()[:nt]
   assert (tkh[0::2] == tkh[1::2]).all()              # both tiles of a pair share the kernel offset
-  for variant, name in ((3, 'cta_group::2'), (2, '2-CTA cluster'), (1, 'A in smem'), (0, 'A in TMEM')):
+  for (tl_k, tl_s, tl_n), name in (((tk, ts, nt), 'paired tile list'), ((km.tile_k, km.tile_start, km.n_tiles), 'plain tile list')):
     for rep in range(2):
       out = torch.zeros(n, cout, device='cuda')
-      abi.spconv_tc_fwd(feat.cuda(), Wt, km, out, passes=3, cluster=variant)
-      _close(out, want, what=f'tcgen05 {name}')
+      abi.call('dgr_spconv_tc_fwd', abi.ptr(feat.cuda()), cin, abi.ptr(Wt), cout, abi.ptr(km.in_idx), abi.ptr(km.out_idx),
+               abi.ptr(km.kofs), abi.ptr(tl_k), abi.ptr(tl_s), tl_n, abi.TILE_ROWS, 3, abi.ptr(out), abi.stream())
+      _close(out, want, what=f'wgmma {name}')
 
 
 def test_tc_unsupported_shapes_fall_back(abi):

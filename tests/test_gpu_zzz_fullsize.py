@@ -100,7 +100,7 @@ def test_conv_adjoint_and_linear_full_size(abi, cloud):
 
 
 def test_knn_tensor_core_equals_fp32_kernel_full_size(abi):
-  """51k x 40k x 32 unit-norm features with planted exact duplicates: the tcgen05 pre-filter path returns
+  """51k x 40k x 32 unit-norm features with planted exact duplicates: the wgmma pre-filter path returns
   exactly the fp32 kernel's indices and distances."""
   g = torch.Generator().manual_seed(3)
   n0, n1, c = 51_381, 39_881, 32
