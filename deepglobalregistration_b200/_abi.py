@@ -66,6 +66,9 @@ SIGNATURES = {
     'dgr_icp_point_to_point': [_p, _i64, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _p, _i32, _f64, _f64, _p, _p, _p],
     'dgr_ransac_ws_elems': [_i64, _i64, _p],
     'dgr_ransac_correspondence': [_p, _p, _p, _p, _i64, _f64, _i64, C.c_uint64, _p, _p, _p],
+    'dgr_ransac_fm_ws_elems': [_i64, _i64, _i64, _p],
+    'dgr_ransac_feature_matching': [_p, _i64, _p, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _f64, _f64, _i64, _i64,
+                                    C.c_uint64, _p, _p, _p],
     'dgr_se3_register': [_p, _p, _p, _p, _i64, _f32, _i32, _i32, _f32, _f32, _f32, _p, _p, _p, _p],
     # ---- round 2: coordinate planning with device-side counts (csrc/coordplan.cu) ----
     'dgr_spconv_table_fwd_strided': [_p, _i32, _p, _i32, _p, _i32, _i64, _i64, _p, _p, _p, _p],
@@ -641,4 +644,26 @@ def ransac_correspondence(x, y, idx0, idx1, max_dist, num_hyp=4000000, seed=0):
   call('dgr_ransac_correspondence', ptr(x), ptr(y), ptr(idx0) if idx0 is not None else None,
        ptr(idx1) if idx1 is not None else None, n, float(max_dist), int(num_hyp), int(seed) & (2**64 - 1),
        ptr(ws), ptr(res), stream())
+  return res
+
+
+def ransac_feature_matching(src, tgt, nn, spec, table, cell, max_dist, edge_ratio=0.0, check_dist=0.0,
+                            max_iteration=80000, max_validation=1000, seed=0, batch=0):
+  """Feature-matching RANSAC (open3d 0.10 registration_ransac_based_on_feature_matching): hypotheses of 4
+  source points src[i] paired with tgt[nn[i]], scored on all of src through tgt's voxel hash (spec / table of
+  a dgr_unique_first table at `cell`, one point per cell, rows = rows of tgt, batch column `batch`).
+  edge_ratio 0 / check_dist <= 0 turn the edge-length / distance checkers off.  src / tgt: CUDA float32
+  [n, 3]; nn: int32 [len(src)].  -> device double [24] (pose 16, fitness, inlier RMSE, winning hypothesis,
+  matched points, validated hypotheses scored, hypotheses drawn until the max_validation-th validation)."""
+  _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt'); _chk(nn, torch.int32, 'nn')
+  if nn.numel() != src.shape[0]:
+    raise DgrError('nn must hold one target row per source point')
+  dev = src.device
+  words = C.c_int64(0)
+  call('dgr_ransac_fm_ws_elems', src.shape[0], int(max_iteration), int(max_validation), C.byref(words))
+  ws = scratch('ransac_fm', words.value, torch.int64, dev)
+  res = torch.empty(24, dtype=torch.float64, device=dev)
+  call('dgr_ransac_feature_matching', ptr(src), src.shape[0], ptr(tgt), ptr(nn), ptr(spec), ptr(table.keys),
+       ptr(table.vals), table.cap, int(batch), float(cell), float(max_dist), float(edge_ratio), float(check_dist),
+       int(max_iteration), int(max_validation), int(seed) & (2**64 - 1), ptr(ws), ptr(res), stream())
   return res

@@ -101,6 +101,89 @@ __device__ __forceinline__ int32_t dgr_hash_lookup(const uint64_t* __restrict__ 
   }
 }
 
+// Nearest target row strictly within sqrt(best) of the point p, through a voxel hash holding at most one
+// target point per cell of size `cell` (the cells within `reach` = ceil(radius / cell) of p's cell on every
+// side are the candidates).  8 lanes share one query point: an aligned group of 8 lanes of the warp, lane
+// `sub` probing cells sub, sub + 8, ... (a thread per point walking all (2 reach + 1)^3 cells serially waits
+// on that many dependent L2 round trips).  The group's best (smaller d2, then lower row) is reduced with
+// shuffles, so the answer does not depend on the probe order and every lane of the group leaves with it.
+// Whole warps must call it; lanes with have == false probe nothing.  best: in = radius^2, out = its d2;
+// best_j: -1 when nothing is within the radius.
+__device__ __forceinline__ void dgr_voxel_nearest8(const double p[3], bool have, int sub, const float* __restrict__ tgt,
+                                                   const dgr_keyspec_t& s, const uint64_t* __restrict__ keys,
+                                                   const int32_t* __restrict__ vals, uint64_t mask, int32_t batch,
+                                                   double cell, int reach, double& best, int& best_j) {
+  const int side = 2 * reach + 1, n_cells = side * side * side;
+  int c3[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) c3[a] = (int)floor(p[a] / cell);
+  best_j = -1;
+  for (int c = sub; c < n_cells && have; c += 8) {
+    const int dx = c % side - reach, dy = (c / side) % side - reach, dz = c / (side * side) - reach;
+    const int32_t row[4] = {batch, c3[0] + dx, c3[1] + dy, c3[2] + dz};
+    bool inside = true;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const long long d = (long long)row[q] - s.lo[q];
+      inside = inside && d >= 0 && d < (1ll << s.bits[q]);
+    }
+    if (!inside) continue;
+    const int32_t j = dgr_hash_lookup(keys, vals, mask, dgr_pack_key(row, s));
+    if (j < 0) continue;
+    const double ex = p[0] - tgt[3 * (int64_t)j], ey = p[1] - tgt[3 * (int64_t)j + 1],
+                 ez = p[2] - tgt[3 * (int64_t)j + 2];
+    const double d2 = ex * ex + ey * ey + ez * ez;
+    if (d2 < best || (d2 == best && (best_j < 0 || j < best_j))) {
+      best = d2;
+      best_j = j;
+    }
+  }
+#pragma unroll
+  for (int d = 1; d < 8; d <<= 1) {
+    const double ob = __shfl_xor_sync(0xffffffffu, best, d);
+    const int oj = __shfl_xor_sync(0xffffffffu, best_j, d);
+    if (oj >= 0 && (best_j < 0 || ob < best || (ob == best && oj < best_j))) {
+      best = ob;
+      best_j = oj;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------
+// exclusive scan of `nb` ints in place with one block; returns the total (valid in every thread)
+// ---------------------------------------------------------------------------------------
+__device__ __forceinline__ int dgr_block_scan_inplace(int32_t* cnt, int64_t nb) {
+  __shared__ int carry_s;
+  __shared__ int wsum[32];
+  if (threadIdx.x == 0) carry_s = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int64_t base = 0; base < nb; base += blockDim.x) {
+    const int64_t i = base + threadIdx.x;
+    const int v = (i < nb) ? cnt[i] : 0;
+    int inc = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, inc, d);
+      if (lane >= d) inc += t;
+    }
+    if (lane == 31) wsum[warp] = inc;
+    __syncthreads();
+    int wbase = 0, tot = 0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) {
+      const int sm = wsum[w];
+      if (w < warp) wbase += sm;
+      tot += sm;
+    }
+    const int carry = carry_s;
+    if (i < nb) cnt[i] = carry + wbase + inc - v;
+    __syncthreads();
+    if (threadIdx.x == 0) carry_s = carry + tot;
+    __syncthreads();
+  }
+  return carry_s;
+}
+
 // ---------------------------------------------------------------------------------------
 // block-wide exclusive scan of one int per thread (blockDim.x == 256)
 // ---------------------------------------------------------------------------------------

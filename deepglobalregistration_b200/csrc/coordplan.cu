@@ -170,44 +170,11 @@ __global__ void coarse_flag_kernel(const int32_t* __restrict__ n_dev, int64_t n_
   }
 }
 
-// exclusive scan of `nb` ints in place with one block; returns the total (valid in every thread)
-__device__ int block_scan_inplace(int32_t* cnt, int64_t nb) {
-  __shared__ int carry_s;
-  __shared__ int wsum[32];
-  if (threadIdx.x == 0) carry_s = 0;
-  __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int64_t base = 0; base < nb; base += blockDim.x) {
-    const int64_t i = base + threadIdx.x;
-    const int v = (i < nb) ? cnt[i] : 0;
-    int inc = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, inc, d);
-      if (lane >= d) inc += t;
-    }
-    if (lane == 31) wsum[warp] = inc;
-    __syncthreads();
-    int wbase = 0, tot = 0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) {
-      const int sm = wsum[w];
-      if (w < warp) wbase += sm;
-      tot += sm;
-    }
-    const int carry = carry_s;
-    if (i < nb) cnt[i] = carry + wbase + inc - v;
-    __syncthreads();
-    if (threadIdx.x == 0) carry_s = carry + tot;
-    __syncthreads();
-  }
-  return carry_s;
-}
-
 __global__ void coarse_scan_kernel(const int32_t* __restrict__ n_dev, int64_t n_max, CoarseArgs a) {
   const int n = dev_count(n_dev, n_max);
   const int l = blockIdx.x;
   const int64_t nb = (n + kScanElems - 1) / kScanElems;
-  const int total = block_scan_inplace(a.scan[l], nb);
+  const int total = dgr_block_scan_inplace(a.scan[l], nb);
   if (threadIdx.x == 0) a.n_out[l][0] = total;
 }
 
@@ -412,7 +379,7 @@ kmap_probe_kernel(const int32_t* __restrict__ out_coords, const int32_t* __restr
 __global__ void kmap_scan_kernel(int32_t* cnt, int K, int bpk, int tile_rows, int32_t* kofs,
                                  int32_t* meta, const dgr_keyspec_t* spec) {
   const int64_t nb = (int64_t)K * bpk;
-  const int total = block_scan_inplace(cnt, nb);
+  const int total = dgr_block_scan_inplace(cnt, nb);
   if (threadIdx.x == 0) cnt[nb] = total;
   __syncthreads();
   __shared__ int red[3][32];

@@ -43,17 +43,11 @@ __device__ __forceinline__ uint32_t ransac_pick(uint64_t seed, uint64_t h, int s
   return (uint32_t)(((z >> 32) * (uint64_t)n) >> 32);
 }
 
-// Umeyama without scaling on the 4 sampled correspondences, fp64
-__device__ void ransac_hypothesis(const float4* __restrict__ src, const float4* __restrict__ tgt, uint32_t n,
-                                  uint64_t seed, uint64_t h, double R[3][3], double t[3]) {
-  double p[4][3], q[4][3], mp[3] = {0, 0, 0}, mq[3] = {0, 0, 0};
-  for (int j = 0; j < 4; ++j) {
-    uint32_t i = ransac_pick(seed, h, j, n);
-    float4 a = __ldg(src + i), b = __ldg(tgt + i);
-    p[j][0] = a.x; p[j][1] = a.y; p[j][2] = a.z;
-    q[j][0] = b.x; q[j][1] = b.y; q[j][2] = b.z;
+// Umeyama without scaling: the pose (R, t) minimising sum |R p_j + t - q_j|^2 over 4 pairs, fp64
+__device__ void ransac_fit4(const double p[4][3], const double q[4][3], double R[3][3], double t[3]) {
+  double mp[3] = {0, 0, 0}, mq[3] = {0, 0, 0};
+  for (int j = 0; j < 4; ++j)
     for (int c = 0; c < 3; ++c) { mp[c] += p[j][c]; mq[c] += q[j][c]; }
-  }
   for (int c = 0; c < 3; ++c) { mp[c] *= 0.25; mq[c] *= 0.25; }
   double S[3][3];
   for (int r = 0; r < 3; ++r)
@@ -64,6 +58,19 @@ __device__ void ransac_hypothesis(const float4* __restrict__ src, const float4* 
     }
   kabsch_rotation(S, R);
   for (int r = 0; r < 3; ++r) t[r] = mq[r] - (R[r][0] * mp[0] + R[r][1] * mp[1] + R[r][2] * mp[2]);
+}
+
+// the pose of hypothesis h over the packed correspondence list
+__device__ void ransac_hypothesis(const float4* __restrict__ src, const float4* __restrict__ tgt, uint32_t n,
+                                  uint64_t seed, uint64_t h, double R[3][3], double t[3]) {
+  double p[4][3], q[4][3];
+  for (int j = 0; j < 4; ++j) {
+    uint32_t i = ransac_pick(seed, h, j, n);
+    float4 a = __ldg(src + i), b = __ldg(tgt + i);
+    p[j][0] = a.x; p[j][1] = a.y; p[j][2] = a.z;
+    q[j][0] = b.x; q[j][1] = b.y; q[j][2] = b.z;
+  }
+  ransac_fit4(p, q, R, t);
 }
 
 // (inliers, sum d^2) -> a key whose unsigned order is open3d's IsBetterRANSACThan: more
@@ -217,6 +224,223 @@ inline uint32_t ransac_blocks(int64_t num_hyp) {
   return (uint32_t)((num_hyp + per_block - 1) / per_block);
 }
 
+// ---------------------------------------------------------------------------------------
+// Feature-matching RANSAC: open3d 0.10's registration_ransac_based_on_feature_matching as the reference
+// calls it (core/deep_global_registration.py:29-47), restated in oracle/ransac_fm.py.  Hypothesis h draws
+// 4 SOURCE points with ransac_pick and pairs each with its nearest target feature (nn, computed once by the
+// caller); the checkers run before / after the fp64 Umeyama fit; the first max_validation hypotheses that
+// pass every checker are scored on ALL source points (nearest target point strictly within max_dist of
+// R s + t, through the target's voxel hash).  Five launches, no host read:
+//   fm_hypothesis_kernel  one thread per hypothesis: draw, edge checker, fit, distance checker -> flag, pose
+//   fm_scan_kernel        exclusive scan of the per-block validated counts (the coordplan.cu pattern)
+//   fm_select_kernel      the first V validated hypothesis numbers, in hypothesis order
+//   fm_score_kernel       (selected hypothesis x 1024-point chunk) per block, 8 lanes per point
+//                         (dgr_voxel_nearest8, shared with the ICP); fixed-order block partials
+//   fm_final_kernel       partials summed in chunk order, best by (count, smaller sum d^2, lower h)
+// The scoring is fp64 end to end and its partials are reduced in a fixed order, so the (count, sum d^2)
+// a hypothesis is ranked by are the numbers the result reports, and a call is bit-reproducible.
+// ---------------------------------------------------------------------------------------
+constexpr int kFmThreads = 256;
+constexpr int kFmChunk = 1024;          // source points per scoring block: 32 groups of 8 lanes x 32 rounds
+constexpr int64_t kFmMaxChunks = 65535; // gridDim.y of the scoring launch
+
+struct FmWs {
+  double* pose;       // [M][12] row-major [R | t] of every hypothesis that reached the fit
+  int32_t* flag;      // [M] passed every checker
+  int32_t* blk;       // [n_hblk + 1] validated per hypothesis block -> exclusive offsets; [n_hblk] = total
+  int32_t* sel;       // [Vc] selected hypothesis numbers
+  double* part;       // [Vc][n_chunk][2] (matched, sum d^2) per scoring block
+};
+
+inline int64_t fm_words(int64_t n_int32) { return (n_int32 + 1) / 2; }
+
+// workspace size in 8-byte words; carves `base` into the regions when it is not null
+int64_t fm_layout(int64_t n_src, int64_t M, int64_t V, uint64_t* base, FmWs* w) {
+  const int64_t Vc = V < M ? V : M;
+  const int64_t n_hblk = (M + kFmThreads - 1) / kFmThreads;
+  const int64_t n_chunk = (n_src + kFmChunk - 1) / kFmChunk;
+  const int64_t sizes[5] = {12 * M, fm_words(M), fm_words(n_hblk + 1), fm_words(Vc), 2 * Vc * n_chunk};
+  int64_t ofs[5], total = 0;
+  for (int k = 0; k < 5; ++k) { ofs[k] = total; total += sizes[k]; }
+  if (base != nullptr) {
+    w->pose = reinterpret_cast<double*>(base + ofs[0]);
+    w->flag = reinterpret_cast<int32_t*>(base + ofs[1]);
+    w->blk = reinterpret_cast<int32_t*>(base + ofs[2]);
+    w->sel = reinterpret_cast<int32_t*>(base + ofs[3]);
+    w->part = reinterpret_cast<double*>(base + ofs[4]);
+  }
+  return total;
+}
+
+__global__ void __launch_bounds__(kFmThreads)
+fm_hypothesis_kernel(const float* __restrict__ src, uint32_t n_src, const float* __restrict__ tgt,
+                     const int32_t* __restrict__ nn, uint64_t seed, int64_t M, double edge_ratio, double check_dist,
+                     double* __restrict__ pose, int32_t* __restrict__ flag, int32_t* __restrict__ blk_cnt) {
+  const int64_t h = (int64_t)blockIdx.x * kFmThreads + threadIdx.x;
+  int ok = 0;
+  if (h < M) {
+    double p[4][3], q[4][3];
+    for (int j = 0; j < 4; ++j) {
+      const int64_t i = ransac_pick(seed, (uint64_t)h, j, n_src);
+      const int64_t k = __ldg(nn + i);
+      for (int c = 0; c < 3; ++c) { p[j][c] = __ldg(src + 3 * i + c); q[j][c] = __ldg(tgt + 3 * k + c); }
+    }
+    ok = 1;
+    // CorrespondenceCheckerBasedOnEdgeLength: every edge of the sample similar in length on both sides
+    if (edge_ratio > 0) {
+      for (int a = 1; a < 4; ++a)
+        for (int b = 0; b < a; ++b) {
+          double ds = 0, dt = 0;
+          for (int c = 0; c < 3; ++c) {
+            ds += (p[a][c] - p[b][c]) * (p[a][c] - p[b][c]);
+            dt += (q[a][c] - q[b][c]) * (q[a][c] - q[b][c]);
+          }
+          ds = sqrt(ds);
+          dt = sqrt(dt);
+          if (ds < edge_ratio * dt || dt < edge_ratio * ds) ok = 0;
+        }
+    }
+    if (ok) {
+      double R[3][3], t[3];
+      ransac_fit4(p, q, R, t);
+      // CorrespondenceCheckerBasedOnDistance: every sampled pair within check_dist after alignment
+      if (check_dist > 0) {
+        for (int j = 0; j < 4; ++j) {
+          double e2 = 0;
+          for (int r = 0; r < 3; ++r) {
+            const double e = R[r][0] * p[j][0] + R[r][1] * p[j][1] + R[r][2] * p[j][2] + t[r] - q[j][r];
+            e2 += e * e;
+          }
+          if (sqrt(e2) > check_dist) ok = 0;
+        }
+      }
+      double* T = pose + 12 * h;
+      for (int r = 0; r < 3; ++r) {
+        for (int c = 0; c < 3; ++c) T[4 * r + c] = R[r][c];
+        T[4 * r + 3] = t[r];
+      }
+    }
+    flag[h] = ok;
+  }
+  const int cnt = __syncthreads_count(ok);
+  if (threadIdx.x == 0) blk_cnt[blockIdx.x] = cnt;
+}
+
+__global__ void __launch_bounds__(1024) fm_scan_kernel(int32_t* blk, int64_t n_hblk) {
+  const int total = dgr_block_scan_inplace(blk, n_hblk);
+  if (threadIdx.x == 0) blk[n_hblk] = total;
+}
+
+__global__ void __launch_bounds__(kFmThreads)
+fm_select_kernel(const int32_t* __restrict__ flag, const int32_t* __restrict__ blk, int64_t M, int64_t Vc,
+                 int32_t* __restrict__ sel) {
+  const int base = blk[blockIdx.x];
+  if (base >= Vc) return;                              // uniform per block
+  const int64_t h = (int64_t)blockIdx.x * kFmThreads + threadIdx.x;
+  const int f = h < M ? flag[h] : 0;
+  const int pos = base + dgr_block_exclusive_scan_256(f, nullptr);
+  if (f && pos < Vc) sel[pos] = (int32_t)h;
+}
+
+__global__ void __launch_bounds__(kFmThreads, 4)   // <= 64 registers: 32 warps per SM hide the probe latency
+fm_score_kernel(const float* __restrict__ src, int64_t n_src, const float* __restrict__ tgt,
+                const dgr_keyspec_t* __restrict__ spec_p, const uint64_t* __restrict__ keys,
+                const int32_t* __restrict__ vals, uint64_t mask, int32_t batch, double cell, double max_dist,
+                const double* __restrict__ pose, const int32_t* __restrict__ sel, const int32_t* __restrict__ n_valid,
+                int64_t Vc, double* __restrict__ part) {
+  const int64_t slot = blockIdx.x;
+  if (slot >= min((int64_t)*n_valid, Vc)) return;      // uniform per block
+  const dgr_keyspec_t s = *spec_p;
+  double T[12];
+  const double* Tp = pose + 12 * (int64_t)sel[slot];
+#pragma unroll
+  for (int k = 0; k < 12; ++k) T[k] = __ldg(Tp + k);
+  const int reach = (int)ceil(max_dist / cell);
+  const int sub = threadIdx.x & 7;
+  const int64_t lo = (int64_t)blockIdx.y * kFmChunk, hi = min(n_src, lo + kFmChunk);
+  const int64_t end = lo + ((hi - lo + kFmThreads / 8 - 1) / (kFmThreads / 8)) * (kFmThreads / 8);
+  uint32_t cnt = 0;
+  double err = 0.0;
+  for (int64_t i0 = lo + (threadIdx.x >> 3); i0 < end; i0 += kFmThreads / 8) {
+    const bool have = i0 < hi;                         // whole warps stay in the loop for the shuffles
+    const int64_t i = have ? i0 : lo;
+    const double x = src[3 * i], y = src[3 * i + 1], z = src[3 * i + 2];
+    const double p[3] = {T[0] * x + T[1] * y + T[2] * z + T[3], T[4] * x + T[5] * y + T[6] * z + T[7],
+                         T[8] * x + T[9] * y + T[10] * z + T[11]};
+    double best = max_dist * max_dist;
+    int best_j;
+    dgr_voxel_nearest8(p, have, sub, tgt, s, keys, vals, mask, batch, cell, reach, best, best_j);
+    if (have && sub == 0 && best_j >= 0) {
+      ++cnt;
+      err += best;
+    }
+  }
+  // fixed reduction order (butterfly, then warps in order): the partial does not depend on scheduling
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, d);
+    err += __shfl_xor_sync(0xffffffffu, err, d);
+  }
+  __shared__ uint32_t s_cnt[kFmThreads / 32];
+  __shared__ double s_err[kFmThreads / 32];
+  if ((threadIdx.x & 31) == 0) { s_cnt[threadIdx.x >> 5] = cnt; s_err[threadIdx.x >> 5] = err; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    cnt = 0;
+    err = 0.0;
+    for (int w = 0; w < kFmThreads / 32; ++w) { cnt += s_cnt[w]; err += s_err[w]; }
+    double* o = part + 2 * (slot * gridDim.y + blockIdx.y);
+    o[0] = (double)cnt;
+    o[1] = err;
+  }
+}
+
+// (c2, e2, s2) ranks before (c1, e1, s1): open3d's IsBetterRANSACThan with the earlier hypothesis keeping a
+// tie; slot -1 = nothing (open3d's initial result, fitness 0, which no hypothesis without a match beats)
+__device__ __forceinline__ bool fm_better(double c2, double e2, int s2, double c1, double e1, int s1) {
+  return s2 >= 0 && (s1 < 0 || c2 > c1 || (c2 == c1 && (e2 < e1 || (e2 == e1 && s2 < s1))));
+}
+
+__global__ void __launch_bounds__(1024)
+fm_final_kernel(const double* __restrict__ pose, const int32_t* __restrict__ sel, const int32_t* __restrict__ n_valid,
+                int64_t Vc, int64_t V, int64_t M, int64_t n_chunk, const double* __restrict__ part, int64_t n_src,
+                double* __restrict__ result) {
+  __shared__ double s_c[32], s_e[32];
+  __shared__ int s_s[32];
+  const int total = *n_valid;
+  const int64_t nv = min((int64_t)total, Vc);
+  double bc = 0, be = 0;
+  int bs = -1;
+  for (int64_t v = threadIdx.x; v < nv; v += blockDim.x) {
+    double c = 0, e = 0;
+    for (int64_t k = 0; k < n_chunk; ++k) {
+      c += part[2 * (v * n_chunk + k)];
+      e += part[2 * (v * n_chunk + k) + 1];
+    }
+    if (c > 0 && fm_better(c, e, (int)v, bc, be, bs)) { bc = c; be = e; bs = (int)v; }
+  }
+  for (int d = 16; d > 0; d >>= 1) {
+    const double oc = __shfl_xor_sync(0xffffffffu, bc, d), oe = __shfl_xor_sync(0xffffffffu, be, d);
+    const int os = __shfl_xor_sync(0xffffffffu, bs, d);
+    if (fm_better(oc, oe, os, bc, be, bs)) { bc = oc; be = oe; bs = os; }
+  }
+  if ((threadIdx.x & 31) == 0) { s_c[threadIdx.x >> 5] = bc; s_e[threadIdx.x >> 5] = be; s_s[threadIdx.x >> 5] = bs; }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
+    if (fm_better(s_c[w], s_e[w], s_s[w], bc, be, bs)) { bc = s_c[w]; be = s_e[w]; bs = s_s[w]; }
+  const int64_t h = bs >= 0 ? (int64_t)sel[bs] : -1;
+  for (int k = 0; k < 12; ++k) result[k] = h >= 0 ? pose[12 * h + k] : (k % 5 == 0 ? 1.0 : 0.0);
+  result[12] = 0; result[13] = 0; result[14] = 0; result[15] = 1;
+  result[16] = bs >= 0 ? bc / (double)n_src : 0.0;         // fitness
+  result[17] = bs >= 0 ? sqrt(be / bc) : 0.0;              // inlier RMSE
+  result[18] = (double)h;                                  // winning hypothesis
+  result[19] = bc;                                         // matched source points
+  result[20] = (double)nv;                                 // validated hypotheses scored
+  result[21] = total >= V ? (double)(sel[V - 1] + 1) : (double)M;   // drawn until the V-th validation
+  for (int k = 22; k < 24; ++k) result[k] = 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -246,6 +470,46 @@ int32_t dgr_ransac_correspondence(const float* x, const float* y, const int32_t*
   ransac_final_kernel<<<1, 1024, 0, st>>>(src, tgt, (uint32_t)n_corr, seed, blk_key, blk_hyp, n_blk, max_dist,
                                           result);
   dgr_note_launches(3);
+  DGR_LAUNCH_CHECK();
+  return DGR_OK;
+}
+
+int32_t dgr_ransac_fm_ws_elems(int64_t n_src, int64_t max_iteration, int64_t max_validation, int64_t* n_elems) {
+  DGR_ARG_CHECK(n_elems != nullptr && n_src >= 0 && max_iteration >= 0 && max_validation >= 0, "bad arguments");
+  *n_elems = fm_layout(n_src, max_iteration, max_validation, nullptr, nullptr);
+  return DGR_OK;
+}
+
+int32_t dgr_ransac_feature_matching(const float* src, int64_t n_src, const float* tgt, const int32_t* nn,
+                                    const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap,
+                                    int32_t batch, double cell, double max_dist, double edge_ratio, double check_dist,
+                                    int64_t max_iteration, int64_t max_validation, uint64_t seed, uint64_t* ws,
+                                    double* result, void* stream) {
+  DGR_ARG_CHECK(src != nullptr && tgt != nullptr && nn != nullptr && spec != nullptr && keys != nullptr &&
+                vals != nullptr && ws != nullptr && result != nullptr, "null pointer");
+  DGR_ARG_CHECK(n_src >= 1 && n_src <= kFmChunk * kFmMaxChunks, "source point count out of range");
+  DGR_ARG_CHECK(max_iteration >= 1 && max_iteration <= (1ll << 30), "hypothesis count out of range");
+  DGR_ARG_CHECK(max_validation >= 1, "max_validation must be positive");
+  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
+  DGR_ARG_CHECK(cell > 0 && max_dist > 0, "cell and max_dist must be positive");
+  DGR_ARG_CHECK(max_dist / cell <= 4.0, "search radius above 4 cells is not supported");
+  DGR_ARG_CHECK(edge_ratio >= 0, "edge_ratio must be >= 0 (0 = no edge-length checker)");
+  cudaStream_t st = (cudaStream_t)stream;
+  FmWs w;
+  fm_layout(n_src, max_iteration, max_validation, ws, &w);
+  const int64_t Vc = max_validation < max_iteration ? max_validation : max_iteration;
+  const uint32_t n_hblk = (uint32_t)((max_iteration + kFmThreads - 1) / kFmThreads);
+  const int64_t n_chunk = (n_src + kFmChunk - 1) / kFmChunk;
+  fm_hypothesis_kernel<<<n_hblk, kFmThreads, 0, st>>>(src, (uint32_t)n_src, tgt, nn, seed, max_iteration, edge_ratio,
+                                                      check_dist, w.pose, w.flag, w.blk);
+  fm_scan_kernel<<<1, 1024, 0, st>>>(w.blk, n_hblk);
+  fm_select_kernel<<<n_hblk, kFmThreads, 0, st>>>(w.flag, w.blk, max_iteration, Vc, w.sel);
+  fm_score_kernel<<<dim3((unsigned)Vc, (unsigned)n_chunk), kFmThreads, 0, st>>>(
+      src, n_src, tgt, spec, keys, vals, (uint64_t)cap - 1, batch, cell, max_dist, w.pose, w.sel, w.blk + n_hblk, Vc,
+      w.part);
+  fm_final_kernel<<<1, 1024, 0, st>>>(w.pose, w.sel, w.blk + n_hblk, Vc, max_validation, max_iteration, n_chunk, w.part,
+                                      n_src, result);
+  dgr_note_launches(5);
   DGR_LAUNCH_CHECK();
   return DGR_OK;
 }

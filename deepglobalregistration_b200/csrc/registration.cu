@@ -468,10 +468,7 @@ icp_match_kernel(const float* __restrict__ src, int64_t n_src, const float* __re
 #pragma unroll
   for (int k = 0; k < 17; ++k) acc[k] = 0.0;
   const int reach = (int)ceil(max_dist / voxel);     // cells to search on every side (2 for DGR)
-  const int side = 2 * reach + 1, n_cells = side * side * side;
-  // 8 lanes share one source point: the (2 reach + 1)^3 = 125 candidate cells are probed 8 at a time (a thread
-  // per point walked them serially - 125 dependent L2 round trips - and left the SMs 92 % idle), then the lanes'
-  // best (d2, then lower row) is reduced with shuffles; lane 0 of the group accumulates the moments
+  // 8 lanes share one source point (dgr_voxel_nearest8); lane 0 of the group accumulates the moments
   const int sub = threadIdx.x & 7;
   const int64_t groups = ((int64_t)gridDim.x * blockDim.x) >> 3;
   for (int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 3; i0 < ((n_src + groups - 1) / groups) * groups;
@@ -481,40 +478,9 @@ icp_match_kernel(const float* __restrict__ src, int64_t n_src, const float* __re
     const double x = src[3 * i], y = src[3 * i + 1], z = src[3 * i + 2];
     const double p[3] = {T[0] * x + T[1] * y + T[2] * z + T[3], T[4] * x + T[5] * y + T[6] * z + T[7],
                          T[8] * x + T[9] * y + T[10] * z + T[11]};
-    int cell[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) cell[a] = (int)floor(p[a] / voxel);
     double best = max_dist * max_dist;
-    int best_j = -1;
-    for (int c = sub; c < n_cells && have; c += 8) {
-      const int dx = c % side - reach, dy = (c / side) % side - reach, dz = c / (side * side) - reach;
-      const int32_t row[4] = {batch, cell[0] + dx, cell[1] + dy, cell[2] + dz};
-      bool inside = true;
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const long long d = (long long)row[q] - s.lo[q];
-        inside = inside && d >= 0 && d < (1ll << s.bits[q]);
-      }
-      if (!inside) continue;
-      const int32_t j = dgr_hash_lookup(keys, vals, mask, dgr_pack_key(row, s));
-      if (j < 0) continue;
-      const double ex = p[0] - tgt[3 * (int64_t)j], ey = p[1] - tgt[3 * (int64_t)j + 1],
-                   ez = p[2] - tgt[3 * (int64_t)j + 2];
-      const double d2 = ex * ex + ey * ey + ez * ez;
-      if (d2 < best || (d2 == best && (best_j < 0 || j < best_j))) {
-        best = d2;
-        best_j = j;
-      }
-    }
-#pragma unroll
-    for (int d = 1; d < 8; d <<= 1) {                  // nearest, lower row index on ties: order-independent
-      const double ob = __shfl_xor_sync(0xffffffffu, best, d);
-      const int oj = __shfl_xor_sync(0xffffffffu, best_j, d);
-      if (oj >= 0 && (best_j < 0 || ob < best || (ob == best && oj < best_j))) {
-        best = ob;
-        best_j = oj;
-      }
-    }
+    int best_j;
+    dgr_voxel_nearest8(p, have, sub, tgt, s, keys, vals, mask, batch, voxel, reach, best, best_j);
     if (have && sub == 0 && best_j >= 0) {
       const double q[3] = {tgt[3 * (int64_t)best_j], tgt[3 * (int64_t)best_j + 1], tgt[3 * (int64_t)best_j + 2]};
       acc[0] += 1.0;

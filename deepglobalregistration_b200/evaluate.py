@@ -197,6 +197,14 @@ def main(argv=None):
   ap.add_argument('--success_rte_thresh', type=float, default=0.3, help='m (config.py:127; KITTI: 0.6)')
   ap.add_argument('--success_rre_thresh', type=float, default=15.0, help='deg (config.py:128; KITTI: 5)')
   ap.add_argument('--no_icp', action='store_true')
+  ap.add_argument('--method', choices=('dgr', 'fcgf_ransac'), default='dgr',
+                  help='dgr: DeepGlobalRegistration.register; fcgf_ransac: the FCGF + RANSAC baseline on the same '
+                  'checkpoint (core/fcgf_ransac.py)')
+  ap.add_argument('--ransac_max_iteration', type=int, default=80000, help='fcgf_ransac: hypotheses drawn at most')
+  ap.add_argument('--ransac_max_validation', type=int, default=1000,
+                  help='fcgf_ransac: hypotheses scored (the ones that pass the checkers first)')
+  ap.add_argument('--ransac_edge_ratio', type=float, default=0.0,
+                  help='fcgf_ransac: edge-length checker similarity threshold (open3d uses 0.9); 0 = off')
   ap.add_argument('--out_dir', default='.')
   args = ap.parse_args(argv)
 
@@ -210,6 +218,12 @@ def main(argv=None):
   cfg = argparse.Namespace(weights=args.weights, clip_weight_thresh=args.clip_weight_thresh, verbose=False)
   dgr = DeepGlobalRegistration(cfg, device=torch.device('cuda', local))
   dgr.use_icp = not args.no_icp
+  method = dgr
+  if args.method == 'fcgf_ransac':
+    from .core.fcgf_ransac import FCGFRansac
+    method = FCGFRansac(dgr)
+    method.max_iteration, method.max_validation = args.ransac_max_iteration, args.ransac_max_validation
+    method.edge_ratio = args.ransac_edge_ratio
   if args.threed_match_dir:
     pairs = threedmatch_pairs(args.threed_match_dir)
   elif args.kitti_dir:
@@ -225,13 +239,14 @@ def main(argv=None):
     except OSError as e:
       print(f'cannot create {out_dir!r} ({e}); saving to the current directory')
       out_dir = '.'
-  result = evaluate(dgr, pairs, args.success_rte_thresh, args.success_rre_thresh,
+  result = evaluate(method, pairs, args.success_rte_thresh, args.success_rre_thresh,
                     log=print if rank == 0 else None, device=torch.device('cuda', local))
   if rank == 0:
     summary = summarize(result)
     print(json.dumps(dict(summary, world_size=world)))          # the summary first: a failing save loses nothing
-    out = os.path.join(out_dir, 'dgr-b200-stats.npz')
-    np.savez(out, stats=result['stats'][None], names=['DGR'], poses=result['poses'], groups=result['groups'])
+    stem, name = ('dgr-b200', 'DGR') if args.method == 'dgr' else ('fcgf-ransac-b200', 'RANSAC')
+    out = os.path.join(out_dir, f'{stem}-stats.npz')
+    np.savez(out, stats=result['stats'][None], names=[name], poses=result['poses'], groups=result['groups'])
     print(json.dumps(dict(summary, world_size=world, saved=out)))
   if world > 1:
     dist.destroy_process_group()

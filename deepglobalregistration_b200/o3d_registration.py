@@ -1,4 +1,4 @@
-"""``open3d.pipelines.registration`` stand-in backed by libdgr_b200 - the two calls the reference's
+"""``open3d.pipelines.registration`` stand-in backed by libdgr_b200 - the three calls the reference's
 ``core/deep_global_registration.py`` makes into open3d, with open3d's signatures and result objects:
 
   registration_icp(source, target, max_correspondence_distance, init, ...)             (:317-322)
@@ -9,6 +9,10 @@
          correspondences (the reference passes its 80000 into the confidence slot, so open3d >= 0.12 never
          exits early; under 0.10 / 0.11 the same argument bounded the VALIDATED hypotheses instead - this
          stand-in follows the >= 0.12 reading, INTEGRATION.md).
+  registration_ransac_based_on_feature_matching(source, target, source_feature, target_feature, ...)  (:29-47)
+      -> dgr_knn_top1 + dgr_ransac_feature_matching: open3d 0.10's form (RANSACConvergenceCriteria(max_iteration,
+         max_validation)), the edge-length and distance checkers, every validated hypothesis scored on all source
+         points through a voxel hash of the target.
 
 With ``shims.install()`` these are reachable as ``open3d.pipelines.registration`` (and the pre-0.12 alias
 ``open3d.registration``) whenever the real open3d is absent, so the reference's own class runs on this stack
@@ -36,11 +40,36 @@ class RANSACConvergenceCriteria:
   def __init__(self, max_iteration=100000, confidence=0.999):
     self.max_iteration = int(max_iteration)
     self.confidence = min(float(confidence), 1.0)       # open3d clamps; DGR passes 80000 here
+    # open3d 0.10 / 0.11 read the second argument as max_validation (what the feature-matching RANSAC uses;
+    # DGR passes 1000 there at core/deep_global_registration.py:44); 1000 was that version's default
+    is_count = isinstance(confidence, (int, np.integer)) and not isinstance(confidence, bool) and confidence >= 1
+    self.max_validation = int(confidence) if is_count else 1000
 
 
 class CorrespondenceCheckerBasedOnDistance:
   def __init__(self, distance_threshold):
     self.distance_threshold = distance_threshold
+
+
+class CorrespondenceCheckerBasedOnEdgeLength:
+  def __init__(self, similarity_threshold=0.9):
+    self.similarity_threshold = similarity_threshold
+
+
+class Feature:
+  """Per-point feature vectors, stored as open3d does: data [dimension, num] float64."""
+
+  def __init__(self):
+    self.data = np.zeros((0, 0), dtype=np.float64)
+
+  def resize(self, dim, n):
+    self.data = np.zeros((int(dim), int(n)), dtype=np.float64)
+
+  def dimension(self):
+    return int(np.asarray(self.data).shape[0])
+
+  def num(self):
+    return int(np.asarray(self.data).shape[1])
 
 
 class RegistrationResult:
@@ -116,4 +145,56 @@ def registration_ransac_based_on_correspondence(source, target, corres, max_corr
   idx1 = torch.from_numpy(np.ascontiguousarray(corres[:, 1], dtype=np.int32)).to(dev)
   r = _abi.ransac_correspondence(src, tgt, idx0, idx1, float(max_correspondence_distance),
                                  num_hyp=criteria.max_iteration, seed=seed).cpu().numpy()
+  return RegistrationResult(r[:16], r[16], r[17], r[19])
+
+
+def _feature_checkers(checkers):
+  """(edge_ratio, check_dist) of the checker list (0 = that checker is off); several of one kind combine to the
+  strictest."""
+  edge, dist = 0.0, 0.0
+  for c in checkers or ():
+    if isinstance(c, CorrespondenceCheckerBasedOnEdgeLength):
+      edge = max(edge, float(c.similarity_threshold))
+    elif isinstance(c, CorrespondenceCheckerBasedOnDistance):
+      d = float(c.distance_threshold)
+      dist = d if dist == 0.0 else min(dist, d)
+    else:
+      raise NotImplementedError(f'{type(c).__name__}: only the edge-length and distance checkers are built')
+  return edge, dist
+
+
+def registration_ransac_based_on_feature_matching(source, target, source_feature, target_feature,
+                                                  max_correspondence_distance, estimation_method=None, ransac_n=3,
+                                                  checkers=None, criteria=None, seed=0, **kwargs):
+  """open3d 0.10's argument order (the reference's :29-47).  Every source point's nearest target feature
+  (dgr_knn_top1, fp32) proposes its match; dgr_ransac_feature_matching draws criteria.max_iteration
+  hypotheses of 4 source points, and the first criteria.max_validation that pass the checkers are scored on
+  every source point."""
+  if 'mutual_filter' in kwargs or isinstance(max_correspondence_distance, (bool, np.bool_)):
+    raise NotImplementedError('the open3d >= 0.12 form (mutual_filter) is not built; DGR calls the 0.10 form')
+  if kwargs:
+    raise TypeError(f'unexpected arguments {sorted(kwargs)}')
+  if int(ransac_n) != 4:
+    raise NotImplementedError('ransac_n = 4 (what DGR passes) is the built sample size')
+  if not (estimation_method is None or isinstance(estimation_method, TransformationEstimationPointToPoint)):
+    raise NotImplementedError('only point-to-point estimation is built (what DGR calls)')
+  edge_ratio, check_dist = _feature_checkers(checkers)
+  criteria = criteria or RANSACConvergenceCriteria()
+  fs = np.asarray(source_feature.data, dtype=np.float32).T
+  ft = np.asarray(target_feature.data, dtype=np.float32).T
+  if fs.shape[1] != ft.shape[1]:
+    raise ValueError(f'feature dimensions differ: {fs.shape[1]} vs {ft.shape[1]}')
+  dev = _abi.require_device('cuda')
+  _abi.refresh_stream()
+  src64, tgt64 = _points(source, dev), _points(target, dev)
+  if len(fs) != len(src64) or len(ft) != len(tgt64):
+    raise ValueError('one feature per point is required')
+  if len(src64) == 0 or len(tgt64) == 0:
+    return RegistrationResult(np.eye(4))
+  d = float(max_correspondence_distance)
+  cell, spec, table = _target_hash(tgt64, d)
+  nn = _abi.knn_top1(torch.from_numpy(np.ascontiguousarray(fs)).to(dev), torch.from_numpy(np.ascontiguousarray(ft)).to(dev))
+  r = _abi.ransac_feature_matching(src64.float().contiguous(), tgt64.float().contiguous(), nn, spec, table, cell, d,
+                                   edge_ratio, check_dist, criteria.max_iteration, criteria.max_validation,
+                                   seed=seed).cpu().numpy()
   return RegistrationResult(r[:16], r[16], r[17], r[19])

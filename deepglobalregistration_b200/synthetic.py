@@ -277,3 +277,29 @@ def correspondence_set(seed, n=1500, inlier_frac=0.3, noise=0.004):
   tgt = np.empty_like(Q)
   tgt[perm] = Q
   return P, tgt.astype(np.float32), np.arange(n), perm, T, ~out
+
+
+def feature_matching_pair(seed, n=2000, match_frac=0.3, spacing=0.1, noise=0.003, dim=16):
+  """Clouds and features for the feature-matching RANSAC tests.  Source = n jittered points of a lattice
+  of pitch `spacing` (so no two share a cell of a voxel hash finer than spacing / 2); target = a random pose
+  (<= 40 deg, <= 0.5 m) of the source plus N(0, noise), rows shuffled.  Features: random unit vectors on the
+  target; a source point's feature is its true partner's feature for `match_frac` of the points and a
+  random other target row's otherwise (plus 1e-3 noise, far from any near-tie).
+  -> (src f32 [n,3], tgt f32 [n,3], feat_src f32 [n,dim], feat_tgt f32 [n,dim], T_gt, partner [n],
+  identified mask [n])."""
+  g = np.random.default_rng(seed)
+  side = int(np.ceil(n ** (1 / 3))) + 2
+  lattice = np.stack(np.meshgrid(*[np.arange(side)] * 3, indexing='ij'), -1).reshape(-1, 3)
+  P = (lattice[g.choice(len(lattice), n, replace=False)] - side / 2) * spacing
+  P = (P + g.uniform(-0.1, 0.1, size=P.shape) * spacing).astype(np.float32)
+  T = random_se3(g, 40.0, 0.5)
+  Q = apply_se3(T, P.astype(np.float64)) + g.normal(0, noise, size=(n, 3))
+  perm = g.permutation(n)                          # source i <-> target row perm[i]
+  tgt = np.empty_like(Q)
+  tgt[perm] = Q
+  ft = g.normal(size=(n, dim))
+  ft /= np.linalg.norm(ft, axis=1, keepdims=True)
+  ident = g.random(n) < match_frac
+  wrong = (perm + g.integers(1, n, size=n)) % n
+  fs = ft[np.where(ident, perm, wrong)] + g.normal(0, 1e-3, size=(n, dim))
+  return P, tgt.astype(np.float32), fs.astype(np.float32), ft.astype(np.float32), T, perm, ident

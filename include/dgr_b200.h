@@ -261,6 +261,29 @@ int32_t dgr_ransac_correspondence(const float* x, const float* y, const int32_t*
                                   int64_t n_corr, double max_dist, int64_t num_hyp, uint64_t seed,
                                   uint64_t* ws, double* result, void* stream);
 
+/* ---- Feature-matching RANSAC: open3d 0.10 registration_ransac_based_on_feature_matching as called at
+ *      core/deep_global_registration.py:29-47 (the FCGF + RANSAC baseline) ------------------------ */
+/* nn[i] = row of the target feature nearest to source feature i (dgr_knn_top1 / dgr_knn_top1_tc).
+ * Hypotheses h = 0 .. max_iteration-1 each draw 4 SOURCE points (the counter hash of
+ * dgr_ransac_correspondence) paired with their nn; edge_ratio > 0 enables the edge-length checker
+ * (every sampled edge |S_a - S_b| >= r |T_a - T_b| and vice versa), then the fp64 Umeyama fit
+ * without scaling, then check_dist > 0 the distance checker (every sampled residual <= check_dist).
+ * The first max_validation hypotheses that pass are scored on ALL source points: a point matches its
+ * nearest target point strictly within max_dist of R s + t, searched through the TARGET's voxel hash
+ * (keys / vals / spec of a dgr_unique_first table at `cell`, at most one point per cell, rows = rows of
+ * tgt, `batch` = its batch column; max_dist / cell <= 4).  Best = more matches, then a smaller sum of
+ * squared distances, then the lower hypothesis.  All fp64, reproducible bit for bit; no host read.
+ * ws: dgr_ransac_fm_ws_elems() 8-byte words; result: device double[24] = 4x4 pose (identity when no
+ * hypothesis matched a point), fitness, inlier RMSE, winning hypothesis (-1 if none), matched source
+ * points, validated hypotheses scored, hypotheses drawn until the max_validation-th validation
+ * (max_iteration if it is never reached), 2 zeros. */
+int32_t dgr_ransac_fm_ws_elems(int64_t n_src, int64_t max_iteration, int64_t max_validation, int64_t* n_elems);
+int32_t dgr_ransac_feature_matching(const float* src, int64_t n_src, const float* tgt, const int32_t* nn,
+                                    const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap,
+                                    int32_t batch, double cell, double max_dist, double edge_ratio, double check_dist,
+                                    int64_t max_iteration, int64_t max_validation, uint64_t seed, uint64_t* ws,
+                                    double* result, void* stream);
+
 /* ======================================================================================
  * Round 2: coordinate planning with device-side counts, and the native executor.
  * ====================================================================================== */
