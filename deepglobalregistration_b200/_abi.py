@@ -69,6 +69,9 @@ SIGNATURES = {
     'dgr_ransac_fm_ws_elems': [_i64, _i64, _i64, _p],
     'dgr_ransac_feature_matching': [_p, _i64, _p, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _f64, _f64, _i64, _i64,
                                     C.c_uint64, _p, _p, _p],
+    'dgr_fgr_ws_elems': [_i64, _i64, _i64, _i32, _p],
+    'dgr_fgr_feature_matching': [_p, _i64, _p, _i64, _p, _p, _f64, _i32, _i32, _f64, _i32, _f64, _i64, _i32, C.c_uint64,
+                                 _p, _p, _p, _p],
     'dgr_se3_register': [_p, _p, _p, _p, _i64, _f32, _i32, _i32, _f32, _f32, _f32, _p, _p, _p, _p],
     # ---- round 2: coordinate planning with device-side counts (csrc/coordplan.cu) ----
     'dgr_spconv_table_fwd_strided': [_p, _i32, _p, _i32, _p, _i32, _i64, _i64, _p, _p, _p, _p],
@@ -667,3 +670,34 @@ def ransac_feature_matching(src, tgt, nn, spec, table, cell, max_dist, edge_rati
        ptr(table.vals), table.cap, int(batch), float(cell), float(max_dist), float(edge_ratio), float(check_dist),
        int(max_iteration), int(max_validation), int(seed) & (2**64 - 1), ptr(ws), ptr(res), stream())
   return res
+
+
+def fgr_feature_matching(src, tgt, nn_st, nn_ts, division_factor=1.4, use_absolute_scale=False, decrease_mu=True,
+                         maximum_correspondence_distance=0.025, iteration_number=64, tuple_scale=0.95,
+                         maximum_tuple_count=1000, tuple_test=True, seed=0, return_correspondences=False):
+  """Fast Global Registration over feature matches (open3d registration_fast_based_on_feature_matching):
+  nn_st[i] = nearest target feature of source point i, nn_ts[j] = nearest source feature of target point j
+  (knn_top1 both ways).  src / tgt: CUDA float32 [n, 3]; nn: int32.  -> device double [24] (pose 16 mapping src
+  into tgt, mutual pairs, correspondences used, tuple trials drawn, final mu, optimiser ran, clouds swapped);
+  with return_correspondences also the int32 [n_max, 2] (source, target) buffer whose first res[17] rows are
+  the correspondences the optimiser used."""
+  _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
+  _chk(nn_st, torch.int32, 'nn_st'); _chk(nn_ts, torch.int32, 'nn_ts')
+  n_s, n_t = src.shape[0], tgt.shape[0]
+  if nn_st.numel() != n_s or nn_ts.numel() != n_t:
+    raise DgrError('nn_st / nn_ts must hold one row per source / target point')
+  dev = src.device
+  words = C.c_int64(0)
+  call('dgr_fgr_ws_elems', n_s, n_t, int(maximum_tuple_count), int(bool(tuple_test)), C.byref(words))
+  ws = scratch('fgr', words.value, torch.int64, dev)
+  res = torch.empty(24, dtype=torch.float64, device=dev)
+  corres = None
+  if return_correspondences:
+    n_min = min(n_s, n_t)
+    n_max = 3 * min(int(maximum_tuple_count), 100 * n_min) if tuple_test else n_min
+    corres = torch.full((max(n_max, 1), 2), -1, dtype=torch.int32, device=dev)
+  call('dgr_fgr_feature_matching', ptr(src), n_s, ptr(tgt), n_t, ptr(nn_st), ptr(nn_ts), float(division_factor),
+       int(bool(use_absolute_scale)), int(bool(decrease_mu)), float(maximum_correspondence_distance),
+       int(iteration_number), float(tuple_scale), int(maximum_tuple_count), int(bool(tuple_test)),
+       int(seed) & (2**64 - 1), ptr(ws), ptr(corres), ptr(res), stream())
+  return (res, corres) if return_correspondences else res

@@ -10,6 +10,8 @@ Voxelise both clouds -> FCGF features of both in one pass -> nearest target feat
 core/deep_global_registration.py:29-47 asks of open3d 0.10) -> optionally point-to-point ICP, as the
 stagewise path does.  The wrapped object's preprocessing, FCGF network, voxel size and ``use_icp`` are
 used as they are: no second checkpoint is loaded.
+
+``FCGFBaseline`` is that skeleton with the search step left to the subclass (core/fcgf_fgr.py uses it too).
 """
 import numpy as np
 import torch
@@ -18,15 +20,14 @@ from .. import _abi
 from ..util.timer import Timer
 
 
-class FCGFRansac:
+class FCGFBaseline:
+  """Voxelise -> FCGF on both clouds in one pass -> ``_search`` (device result whose first 12 entries are the
+  [R | t] rows of the pose) -> optional ICP from that pose -> one readback."""
+  branch = None      # last_branch after a call
+  label = None       # name in the timing log line
+
   def __init__(self, dgr):
     self.dgr = dgr
-    # what the reference's function receives from its safeguard call (:306-313, :43-44):
-    # RANSACConvergenceCriteria(num_iterations = 80000, 1000) and only the distance checker
-    self.max_iteration = 80000
-    self.max_validation = 1000
-    self.edge_ratio = 0.0         # CorrespondenceCheckerBasedOnEdgeLength threshold; 0 = not used
-    self.seed = 0                 # open3d draws from std::random_device; here a call is reproducible
     self.reg_timer = Timer()
     self.last_branch = None
     self.last_info = {}
@@ -39,6 +40,14 @@ class FCGFRansac:
   def use_icp(self):
     return self.dgr.use_icp
 
+  def _search(self, p0, p1, f0, f1, manager1):
+    """-> device double result of the global search; manager1: cloud 1's coordinate manager (voxel hash)."""
+    raise NotImplementedError
+
+  def _info(self, res):
+    """last_info entries of the search's host result."""
+    raise NotImplementedError
+
   def register(self, xyz0, xyz1):
     """-> 4x4 float64 ndarray mapping cloud 0 into cloud 1's frame."""
     d = self.dgr
@@ -49,22 +58,44 @@ class FCGFRansac:
       p0, c0, _ = d.preprocess(xyz0, 0, _batch=0)
       p1, c1, _ = d.preprocess(xyz1, 1, _batch=1)
       f0, f1 = d.fcgf_feature_extraction_pair(c0, c1)
-      nn = _abi.knn_top1(f0.contiguous(), f1.contiguous())
       m = c1._dgr_manager
-      res = _abi.ransac_feature_matching(p0, p1, nn, m.spec, m._maps[1].table, vs, 2 * vs, self.edge_ratio, 2 * vs,
-                                         self.max_iteration, self.max_validation, seed=self.seed, batch=1)
+      res = self._search(p0, p1, f0.contiguous(), f1.contiguous(), m)
       parts = [res]
       if self.use_icp:
         parts.append(_abi.icp_point_to_point(p0, p1, m, vs, 2 * vs, res[:12].contiguous(), batch=1))
       host = torch.cat(parts).cpu().numpy()
+    n_res = res.numel()
     T = host[:16].reshape(4, 4).copy()
-    self.last_branch = 'ransac'
-    self.last_info = dict(n0=len(p0), n1=len(p1), ransac_fitness=float(host[16]), ransac_inlier_rmse=float(host[17]),
-                          ransac_hypothesis=int(host[18]), ransac_inliers=int(host[19]),
-                          ransac_validated=int(host[20]), ransac_drawn=int(host[21]))
+    self.last_branch = self.branch
+    self.last_info = dict(n0=len(p0), n1=len(p1), **self._info(host[:n_res]))
     if self.use_icp:
-      icp = host[24:44]
+      icp = host[n_res:n_res + 20]
       T = icp[:16].reshape(4, 4).copy()
       self.last_info.update(icp_fitness=float(icp[16]), icp_inlier_rmse=float(icp[17]), icp_iterations=int(icp[18]))
-    d._log(f'=> FCGF + RANSAC takes {self.reg_timer.toc():.2} s')
+    d._log(f'=> {self.label} takes {self.reg_timer.toc():.2} s')
     return np.asarray(T, dtype=np.float64)
+
+
+class FCGFRansac(FCGFBaseline):
+  branch = 'ransac'
+  label = 'FCGF + RANSAC'
+
+  def __init__(self, dgr):
+    super().__init__(dgr)
+    # what the reference's function receives from its safeguard call (:306-313, :43-44):
+    # RANSACConvergenceCriteria(num_iterations = 80000, 1000) and only the distance checker
+    self.max_iteration = 80000
+    self.max_validation = 1000
+    self.edge_ratio = 0.0         # CorrespondenceCheckerBasedOnEdgeLength threshold; 0 = not used
+    self.seed = 0                 # open3d draws from std::random_device; here a call is reproducible
+
+  def _search(self, p0, p1, f0, f1, manager1):
+    vs = self.voxel_size
+    nn = _abi.knn_top1(f0, f1)
+    return _abi.ransac_feature_matching(p0, p1, nn, manager1.spec, manager1._maps[1].table, vs, 2 * vs,
+                                        self.edge_ratio, 2 * vs, self.max_iteration, self.max_validation,
+                                        seed=self.seed, batch=1)
+
+  def _info(self, res):
+    return dict(ransac_fitness=float(res[16]), ransac_inlier_rmse=float(res[17]), ransac_hypothesis=int(res[18]),
+                ransac_inliers=int(res[19]), ransac_validated=int(res[20]), ransac_drawn=int(res[21]))

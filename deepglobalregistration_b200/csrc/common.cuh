@@ -76,6 +76,13 @@ __device__ __forceinline__ uint64_t dgr_mix64(uint64_t x) {
   return x;
 }
 
+// Draw number `draw` of the counter-hash stream of `seed`: uniform in [0, n).  RANSAC hypothesis h takes draws
+// 4h .. 4h + 3, an FGR tuple trial k draws 3k .. 3k + 2; oracle/ransac.py restates it (sample_indices).
+__device__ __forceinline__ uint32_t dgr_counter_pick(uint64_t seed, uint64_t draw, uint32_t n) {
+  const uint64_t z = dgr_mix64(seed + (draw + 1) * 0x9E3779B97F4A7C15ull);
+  return (uint32_t)(((z >> 32) * (uint64_t)n) >> 32);
+}
+
 // Claim (or find) the slot of `key`; linear probing.
 __device__ __forceinline__ uint32_t dgr_hash_insert(uint64_t* keys, uint64_t mask, uint64_t key) {
   uint64_t s = dgr_mix64(key) & mask;
@@ -208,4 +215,18 @@ __device__ __forceinline__ int dgr_block_exclusive_scan_256(int v, int* total) {
   __syncthreads();
   if (total) *total = tot;
   return base + inc - v;
+}
+
+// ---------------------------------------------------------------------------------------
+// "the first `cap` flagged rows, in row order" for one 256-row block of flag[0, n): base = flagged rows before
+// this block (an exclusive scan of the per-block counts); every flagged row whose rank is below cap gets
+// sel[rank] = h0 + row.  Whole blocks call it (blockDim.x == 256).
+// ---------------------------------------------------------------------------------------
+__device__ __forceinline__ void dgr_select_first_256(const int32_t* __restrict__ flag, int base, int64_t n, int64_t cap,
+                                                     int64_t h0, int32_t* __restrict__ sel) {
+  if (base >= cap) return;                             // uniform per block
+  const int64_t h = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  const int f = h < n ? flag[h] : 0;
+  const int pos = base + dgr_block_exclusive_scan_256(f, nullptr);
+  if (f && pos < cap) sel[pos] = (int32_t)(h0 + h);
 }

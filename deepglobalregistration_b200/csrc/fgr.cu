@@ -1,0 +1,513 @@
+// Fast Global Registration (Zhou, Park & Koltun, ECCV 2016) over feature matches: open3d's
+// registration_fast_based_on_feature_matching, restated in oracle/fgr.py (which pins every boundary convention).
+// The caller supplies both feature kNN directions (dgr_knn_top1 / dgr_knn_top1_tc); the rest runs here with no
+// host read and no atomics, so a call gives the same bits on every run:
+//   fgr_stats_kernel    one CTA per cloud: fp64 mean and max |x - mean| in a fixed order
+//   fgr_mutual_kernel   one thread per row of the larger cloud ("first"; the source on a tie): mutual flag
+//   fgr_scan_kernel     exclusive scan of the per-block counts (dgr_block_scan_inplace); [nb] = n_mut
+//   fgr_select_kernel   the mutual list in first-cloud order (dgr_select_first_256, shared with the RANSAC)
+//   per chunk of kFgrChunk tuple trials (grids sized from the host bound 100 min(n_s, n_t)):
+//     fgr_tuple_kernel       one thread per trial: 3 counter-hash draws, the three edge-ratio tests
+//     fgr_tuple_scan_kernel  scan offset by the acceptances so far; marks the chunk dead once K are in
+//     fgr_select_kernel      the first K accepted trials, in trial order
+//   Every kernel of a chunk that starts after the K-th acceptance (or past 100 n_mut) returns at once, and the
+//   workspace is one chunk's flags whatever the trial count.
+//   fgr_solve_kernel    one launch for all iterations: one CTA (a cluster of 8 when the mutual list is long and
+//                       the tuple test is off); J^T J / J^T r reduced in a fixed order, the 6x6 Cholesky on one
+//                       thread, the pose kept in shared memory.
+#include <cooperative_groups.h>
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "common.cuh"
+
+namespace cg = cooperative_groups;
+
+namespace {
+
+constexpr int kFgrThreads = 256;                        // flag / select kernels (dgr_block_exclusive_scan_256)
+constexpr int kFgrStatThreads = 1024;
+constexpr int64_t kFgrChunk = 1 << 18;                  // tuple trials per chunk
+constexpr int kFgrChunkBlocks = (int)(kFgrChunk / kFgrThreads);
+constexpr int kFgrSolveThreads = 512;
+constexpr int kFgrCluster = 8;
+constexpr int64_t kFgrClusterMin = 16384;               // mutual-list bound from which the solver runs on a cluster
+constexpr int kNv = 27;                                 // J^T J upper triangle (21) + J^T r (6)
+
+struct FgrWs {
+  double* stat;      // [2][4] per cloud: mean xyz, max |x - mean|
+  int32_t* mflag;    // [n_first] mutual flag per first-cloud row
+  int32_t* mblk;     // [n_mblk + 1] per-block counts -> exclusive offsets; [n_mblk] = n_mut
+  int32_t* mut;      // [n_min] first-cloud rows of the mutual pairs, ascending
+  int32_t* tflag;    // [kFgrChunk] accepted flag of the current chunk's trials
+  int32_t* tblk;     // [kFgrChunkBlocks + 1]
+  int32_t* tsel;     // [Kc] accepted trial numbers, in order
+  int32_t* tstate;   // [2] accepted so far, current chunk live
+  double* corr;      // [n_corr_max][6] normalised (source, target) points of the correspondences
+};
+
+inline int64_t fgr_words(int64_t n_int32) { return (n_int32 + 1) / 2; }
+
+// K capped by the trial count bound: at most 100 min(n_s, n_t) trials exist
+inline int64_t fgr_kc(int64_t n_min, int64_t K) { return K < 100 * n_min ? K : 100 * n_min; }
+
+inline int64_t fgr_corr_max(int64_t n_min, int64_t K, int tuple_test) {
+  return tuple_test ? 3 * fgr_kc(n_min, K) : n_min;
+}
+
+// workspace size in 8-byte words; carves `base` into the regions when it is not null
+int64_t fgr_layout(int64_t n_src, int64_t n_tgt, int64_t K, int tuple_test, uint64_t* base, FgrWs* w) {
+  const int64_t n_first = n_src > n_tgt ? n_src : n_tgt, n_min = n_src < n_tgt ? n_src : n_tgt;
+  const int64_t n_mblk = (n_first + kFgrThreads - 1) / kFgrThreads;
+  const int64_t t = tuple_test ? 1 : 0;
+  const int64_t sizes[9] = {8, fgr_words(n_first), fgr_words(n_mblk + 1), fgr_words(n_min), t * fgr_words(kFgrChunk),
+                            t * fgr_words(kFgrChunkBlocks + 1), t * fgr_words(fgr_kc(n_min, K)), 1,
+                            6 * fgr_corr_max(n_min, K, tuple_test)};
+  int64_t ofs[9], total = 0;
+  for (int k = 0; k < 9; ++k) { ofs[k] = total; total += sizes[k]; }
+  if (base != nullptr) {
+    w->stat = reinterpret_cast<double*>(base + ofs[0]);
+    w->mflag = reinterpret_cast<int32_t*>(base + ofs[1]);
+    w->mblk = reinterpret_cast<int32_t*>(base + ofs[2]);
+    w->mut = reinterpret_cast<int32_t*>(base + ofs[3]);
+    w->tflag = reinterpret_cast<int32_t*>(base + ofs[4]);
+    w->tblk = reinterpret_cast<int32_t*>(base + ofs[5]);
+    w->tsel = reinterpret_cast<int32_t*>(base + ofs[6]);
+    w->tstate = reinterpret_cast<int32_t*>(base + ofs[7]);
+    w->corr = reinterpret_cast<double*>(base + ofs[8]);
+  }
+  return total;
+}
+
+// the normalisation of oracle/fgr.py::normalise: x -> (x - mean) / scale
+struct FgrFrame {
+  double ms[3], mt[3];
+  double s;          // largest |x - mean| over both clouds (1 when both clouds are a single point)
+  double scale;      // s, or 1 with use_absolute_scale
+};
+
+__device__ __forceinline__ FgrFrame fgr_frame(const double* __restrict__ stat, int absolute) {
+  FgrFrame f;
+  for (int c = 0; c < 3; ++c) { f.ms[c] = stat[c]; f.mt[c] = stat[4 + c]; }
+  const double s = fmax(stat[3], stat[7]);
+  f.s = s > 0.0 ? s : 1.0;
+  f.scale = absolute ? 1.0 : f.s;
+  return f;
+}
+
+__device__ __forceinline__ void fgr_point(const float* __restrict__ x, int64_t i, const double m[3], double scale,
+                                          double p[3]) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) p[c] = __ddiv_rn(__dsub_rn((double)__ldg(x + 3 * i + c), m[c]), scale);
+}
+
+// |a - b| as numpy evaluates it: sqrt((dx dx + dy dy) + dz dz), no contraction
+__device__ __forceinline__ double fgr_dist(const double a[3], const double b[3]) {
+  const double dx = __dsub_rn(a[0], b[0]), dy = __dsub_rn(a[1], b[1]), dz = __dsub_rn(a[2], b[2]);
+  return sqrt(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)));
+}
+
+// (source row, target row) of the mutual pair whose first-cloud row is f
+__device__ __forceinline__ void fgr_pair(int32_t f, int swapped, const int32_t* __restrict__ nn_st,
+                                         const int32_t* __restrict__ nn_ts, int32_t& i, int32_t& j) {
+  if (swapped) { j = f; i = __ldg(nn_ts + f); }
+  else { i = f; j = __ldg(nn_st + f); }
+}
+
+__global__ void __launch_bounds__(kFgrStatThreads)
+fgr_stats_kernel(const float* __restrict__ src, int64_t n_src, const float* __restrict__ tgt, int64_t n_tgt,
+                 double* __restrict__ stat, int32_t* __restrict__ tstate) {
+  __shared__ double s_part[kFgrStatThreads / 32][3];
+  __shared__ double s_mean[3];
+  const float* x = blockIdx.x ? tgt : src;
+  const int64_t n = blockIdx.x ? n_tgt : n_src;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (blockIdx.x == 0 && threadIdx.x == 0) { tstate[0] = 0; tstate[1] = 0; }
+  double a[3] = {0.0, 0.0, 0.0};
+  for (int64_t i = threadIdx.x; i < n; i += kFgrStatThreads)
+    for (int c = 0; c < 3; ++c) a[c] += (double)x[3 * i + c];
+  for (int c = 0; c < 3; ++c) {
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) a[c] += __shfl_xor_sync(0xffffffffu, a[c], d);
+    if (lane == 0) s_part[warp][c] = a[c];
+  }
+  __syncthreads();
+  if (threadIdx.x < 3) {
+    double s = 0.0;
+    for (int w = 0; w < kFgrStatThreads / 32; ++w) s += s_part[w][threadIdx.x];
+    s_mean[threadIdx.x] = s / (double)n;
+  }
+  __syncthreads();
+  const double m[3] = {s_mean[0], s_mean[1], s_mean[2]};
+  double mx = 0.0;                                      // a maximum does not depend on the order
+  for (int64_t i = threadIdx.x; i < n; i += kFgrStatThreads) {
+    double p[3];
+    fgr_point(x, i, m, 1.0, p);
+    const double o[3] = {0.0, 0.0, 0.0};
+    mx = fmax(mx, fgr_dist(p, o));
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, d));
+  __syncthreads();
+  if (lane == 0) s_part[warp][0] = mx;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < kFgrStatThreads / 32; ++w) mx = fmax(mx, s_part[w][0]);
+    for (int c = 0; c < 3; ++c) stat[4 * blockIdx.x + c] = m[c];
+    stat[4 * blockIdx.x + 3] = mx;
+  }
+}
+
+__global__ void __launch_bounds__(kFgrThreads)
+fgr_mutual_kernel(const int32_t* __restrict__ nn_first, const int32_t* __restrict__ nn_other, int64_t n_first,
+                  int64_t n_other, int32_t* __restrict__ flag, int32_t* __restrict__ blk) {
+  const int64_t f = (int64_t)blockIdx.x * kFgrThreads + threadIdx.x;
+  int ok = 0;
+  if (f < n_first) {
+    const int32_t j = __ldg(nn_first + f);
+    ok = j >= 0 && j < n_other && __ldg(nn_other + j) == f;
+    flag[f] = ok;
+  }
+  const int cnt = __syncthreads_count(ok);
+  if (threadIdx.x == 0) blk[blockIdx.x] = cnt;
+}
+
+__global__ void __launch_bounds__(1024) fgr_scan_kernel(int32_t* blk, int64_t nb) {
+  const int total = dgr_block_scan_inplace(blk, nb);
+  if (threadIdx.x == 0) blk[nb] = total;
+}
+
+// live (optional): skip the launch's work when *live == 0
+__global__ void __launch_bounds__(kFgrThreads)
+fgr_select_kernel(const int32_t* __restrict__ flag, const int32_t* __restrict__ blk, int64_t n, int64_t cap, int64_t h0,
+                  int32_t* __restrict__ sel, const int32_t* __restrict__ live) {
+  if (live != nullptr && *live == 0) return;            // uniform per launch
+  dgr_select_first_256(flag, blk[blockIdx.x], n, cap, h0, sel);
+}
+
+// trials [h0, h0 + kFgrChunk) of 100 n_mut: trial k draws list positions 3k .. 3k + 2 of the counter hash and is
+// accepted when every edge satisfies l_s tuple_scale < l_t < l_s / tuple_scale on the normalised points
+__global__ void __launch_bounds__(kFgrThreads)
+fgr_tuple_kernel(const float* __restrict__ src, const float* __restrict__ tgt, const int32_t* __restrict__ nn_st,
+                 const int32_t* __restrict__ nn_ts, int swapped, const int32_t* __restrict__ mut,
+                 const int32_t* __restrict__ n_mut_p, const double* __restrict__ stat, int absolute, uint64_t seed,
+                 int64_t h0, double tuple_scale, int64_t Kc, const int32_t* __restrict__ tstate,
+                 int32_t* __restrict__ flag, int32_t* __restrict__ blk) {
+  const int64_t n_mut = *n_mut_p;
+  const int64_t n_trials = n_mut >= 3 ? 100 * n_mut : 0;
+  if (tstate[0] >= Kc || h0 >= n_trials) return;        // uniform per launch: K accepted, or no trial left
+  const int64_t local = (int64_t)blockIdx.x * kFgrThreads + threadIdx.x, k = h0 + local;
+  int ok = 0;
+  if (k < n_trials) {
+    const FgrFrame fr = fgr_frame(stat, absolute);
+    double p[3][3], q[3][3];
+    for (int s = 0; s < 3; ++s) {
+      const uint32_t pos = dgr_counter_pick(seed, 3 * (uint64_t)k + s, (uint32_t)n_mut);
+      int32_t i, j;
+      fgr_pair(__ldg(mut + pos), swapped, nn_st, nn_ts, i, j);
+      fgr_point(src, i, fr.ms, fr.scale, p[s]);
+      fgr_point(tgt, j, fr.mt, fr.scale, q[s]);
+    }
+    ok = 1;
+    for (int e = 0; e < 3; ++e) {
+      const int a = e, b = e == 2 ? 0 : e + 1;
+      const double ls = fgr_dist(p[a], p[b]), lt = fgr_dist(q[a], q[b]);
+      if (!(ls * tuple_scale < lt && lt < ls / tuple_scale)) ok = 0;
+    }
+  }
+  flag[local] = ok;
+  const int cnt = __syncthreads_count(ok);
+  if (threadIdx.x == 0) blk[blockIdx.x] = cnt;
+}
+
+// exclusive offsets of this chunk's blocks, shifted by the acceptances of the earlier chunks
+__global__ void __launch_bounds__(1024)
+fgr_tuple_scan_kernel(int32_t* __restrict__ blk, const int32_t* __restrict__ n_mut_p, int64_t h0, int64_t Kc,
+                      int32_t* __restrict__ tstate) {
+  const int64_t n_mut = *n_mut_p;
+  const int64_t n_trials = n_mut >= 3 ? 100 * n_mut : 0;
+  const int acc = tstate[0];                            // read by every thread before thread 0 rewrites it below
+  const int live = acc < Kc && h0 < n_trials;
+  if (!live) {
+    if (threadIdx.x == 0) tstate[1] = 0;
+    return;
+  }
+  const int total = dgr_block_scan_inplace(blk, kFgrChunkBlocks);
+  for (int b = threadIdx.x; b < kFgrChunkBlocks; b += blockDim.x) blk[b] += acc;
+  if (threadIdx.x == 0) {
+    tstate[0] = acc + total;
+    tstate[1] = 1;
+  }
+}
+
+struct FgrShared {
+  double slots[2][kFgrCluster][kNv];
+  double warp_part[kFgrSolveThreads / 32][kNv];
+  double tot[kNv];
+  double T[12];                                         // target -> source in normalised units, row-major [R | t]
+};
+
+// Sum kNv per-thread doubles over the CTA (CS == 1) or the cluster; every CTA ends with the same sh.tot, summed
+// in the same order (lanes by butterfly, warps in order, CTAs in rank order).
+template <int CS>
+__device__ __forceinline__ void fgr_allreduce(FgrShared& sh, double (&v)[kNv], int& parity) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < kNv; ++k) {
+    double x = v[k];
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) x += __shfl_xor_sync(0xffffffffu, x, d);
+    if (lane == 0) sh.warp_part[warp][k] = x;
+  }
+  __syncthreads();
+  double s = 0.0;
+  if (threadIdx.x < kNv)
+    for (int w = 0; w < kFgrSolveThreads / 32; ++w) s += sh.warp_part[w][threadIdx.x];
+  if constexpr (CS == 1) {
+    if (threadIdx.x < kNv) sh.tot[threadIdx.x] = s;
+  } else {
+    cg::cluster_group cluster = cg::this_cluster();
+    const unsigned rank = cluster.block_rank();
+    if (threadIdx.x < kNv)
+      for (unsigned r = 0; r < CS; ++r) cluster.map_shared_rank(&sh, r)->slots[parity][rank][threadIdx.x] = s;
+    cluster.sync();
+    if (threadIdx.x < kNv) {
+      s = 0.0;
+      for (int r = 0; r < CS; ++r) s += sh.slots[parity][r][threadIdx.x];
+      sh.tot[threadIdx.x] = s;
+    }
+  }
+  __syncthreads();
+  parity ^= 1;
+}
+
+// x = -(A^-1 g) by Cholesky of the symmetric A (upper triangle a[21], row-major); false on a non-positive pivot
+__device__ bool fgr_cholesky_step(const double* a, const double* g, double x[6]) {
+  double L[6][6];
+  int k = 0;
+  double A[6][6];
+  for (int r = 0; r < 6; ++r)
+    for (int c = r; c < 6; ++c) { A[r][c] = a[k]; A[c][r] = a[k]; ++k; }
+  for (int j = 0; j < 6; ++j) {
+    double d = A[j][j];
+    for (int m = 0; m < j; ++m) d -= L[j][m] * L[j][m];
+    if (!(d > 0.0)) return false;
+    L[j][j] = sqrt(d);
+    for (int i = j + 1; i < 6; ++i) {
+      double e = A[i][j];
+      for (int m = 0; m < j; ++m) e -= L[i][m] * L[j][m];
+      L[i][j] = e / L[j][j];
+    }
+  }
+  double y[6];
+  for (int i = 0; i < 6; ++i) {
+    double e = -g[i];
+    for (int m = 0; m < i; ++m) e -= L[i][m] * y[m];
+    y[i] = e / L[i][i];
+  }
+  for (int i = 5; i >= 0; --i) {
+    double e = y[i];
+    for (int m = i + 1; m < 6; ++m) e -= L[m][i] * x[m];
+    x[i] = e / L[i][i];
+  }
+  return true;
+}
+
+template <int CS>
+__global__ void __launch_bounds__(kFgrSolveThreads, 1)
+fgr_solve_kernel(const float* __restrict__ src, const float* __restrict__ tgt, const int32_t* __restrict__ nn_st,
+                 const int32_t* __restrict__ nn_ts, int swapped, const int32_t* __restrict__ mut,
+                 const int32_t* __restrict__ n_mut_p, const int32_t* __restrict__ tsel,
+                 const int32_t* __restrict__ tstate, int64_t Kc, int tuple_test, const double* __restrict__ stat,
+                 int absolute, uint64_t seed, int iteration_number, int decrease_mu, double division_factor,
+                 double max_corr_dist, double* __restrict__ corr, int32_t* __restrict__ corres_out,
+                 double* __restrict__ result) {
+  __shared__ FgrShared sh;
+  unsigned rank = 0;
+  if constexpr (CS > 1) rank = cg::this_cluster().block_rank();
+  const int tid = threadIdx.x;
+  const int64_t n_mut = *n_mut_p;
+  int64_t n_corr, drawn;
+  if (tuple_test) {
+    const int64_t acc = n_mut >= 3 ? min((int64_t)tstate[0], Kc) : 0;
+    n_corr = 3 * acc;
+    drawn = n_mut < 3 ? 0 : ((int64_t)tstate[0] >= Kc ? (int64_t)tsel[Kc - 1] + 1 : 100 * n_mut);
+  } else {
+    n_corr = n_mut;
+    drawn = 0;
+  }
+  const FgrFrame fr = fgr_frame(stat, absolute);
+  // the normalised correspondences, once; a thread later reads exactly the entries it wrote here
+  const int64_t G = (int64_t)CS * kFgrSolveThreads, g0 = (int64_t)rank * kFgrSolveThreads + tid;
+  for (int64_t k = g0; k < n_corr; k += G) {
+    const int64_t pos = tuple_test ? (int64_t)dgr_counter_pick(seed, 3 * (uint64_t)tsel[k / 3] + k % 3, (uint32_t)n_mut)
+                                   : k;
+    int32_t i, j;
+    fgr_pair(mut[pos], swapped, nn_st, nn_ts, i, j);
+    fgr_point(src, i, fr.ms, fr.scale, corr + 6 * k);
+    fgr_point(tgt, j, fr.mt, fr.scale, corr + 6 * k + 3);
+    if (corres_out != nullptr) { corres_out[2 * k] = i; corres_out[2 * k + 1] = j; }
+  }
+  if (tid < 12) sh.T[tid] = (tid % 5 == 0) ? 1.0 : 0.0;
+  __syncthreads();
+  double mu = absolute ? fr.s : 1.0;
+  const int ran = n_corr >= 10;
+  int parity = 0;
+  for (int itr = 0; ran && itr < iteration_number; ++itr) {
+    if (decrease_mu && itr % 4 == 0 && mu > max_corr_dist) mu /= division_factor;
+    double T[12];
+#pragma unroll
+    for (int k = 0; k < 12; ++k) T[k] = sh.T[k];
+    double v[kNv];
+#pragma unroll
+    for (int k = 0; k < kNv; ++k) v[k] = 0.0;
+    for (int64_t k = g0; k < n_corr; k += G) {
+      const double* c = corr + 6 * k;
+      const double p[3] = {c[0], c[1], c[2]};
+      double q[3];
+#pragma unroll
+      for (int r = 0; r < 3; ++r) q[r] = T[4 * r] * c[3] + T[4 * r + 1] * c[4] + T[4 * r + 2] * c[5] + T[4 * r + 3];
+      const double rv[3] = {p[0] - q[0], p[1] - q[1], p[2] - q[2]};
+      const double tmp = mu / (rv[0] * rv[0] + rv[1] * rv[1] + rv[2] * rv[2] + mu);
+      const double w = tmp * tmp;
+      // d(p - (R q + t)) / d(alpha, beta, gamma, t) at the current q, one row per residual component
+      const double J[3][6] = {{0.0, -q[2], q[1], -1.0, 0.0, 0.0},
+                              {q[2], 0.0, -q[0], 0.0, -1.0, 0.0},
+                              {-q[1], q[0], 0.0, 0.0, 0.0, -1.0}};
+#pragma unroll
+      for (int r = 0; r < 3; ++r) {
+        int m = 0;
+#pragma unroll
+        for (int a = 0; a < 6; ++a) {
+#pragma unroll
+          for (int b = a; b < 6; ++b) { v[m] += w * J[r][a] * J[r][b]; ++m; }
+          v[21 + a] += w * J[r][a] * rv[r];
+        }
+      }
+    }
+    fgr_allreduce<CS>(sh, v, parity);
+    if (tid == 0) {
+      double x[6];
+      if (!fgr_cholesky_step(sh.tot, sh.tot + 21, x))
+        for (int k = 0; k < 6; ++k) x[k] = 0.0;
+      // delta = [Rz(gamma) Ry(beta) Rx(alpha) | x[3..6)], composed on the left
+      const double ca = cos(x[0]), sa = sin(x[0]), cb = cos(x[1]), sb = sin(x[1]), cc = cos(x[2]), sc = sin(x[2]);
+      const double Rz[3][3] = {{cc, -sc, 0.0}, {sc, cc, 0.0}, {0.0, 0.0, 1.0}};
+      const double Ry[3][3] = {{cb, 0.0, sb}, {0.0, 1.0, 0.0}, {-sb, 0.0, cb}};
+      const double Rx[3][3] = {{1.0, 0.0, 0.0}, {0.0, ca, -sa}, {0.0, sa, ca}};
+      double Rzy[3][3], D[3][3];
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) Rzy[r][c] = Rz[r][0] * Ry[0][c] + Rz[r][1] * Ry[1][c] + Rz[r][2] * Ry[2][c];
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) D[r][c] = Rzy[r][0] * Rx[0][c] + Rzy[r][1] * Rx[1][c] + Rzy[r][2] * Rx[2][c];
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 4; ++c)
+          sh.T[4 * r + c] = D[r][0] * T[c] + D[r][1] * T[4 + c] + D[r][2] * T[8 + c] + (c == 3 ? x[3 + r] : 0.0);
+    }
+    __syncthreads();
+  }
+  if constexpr (CS > 1) cg::this_cluster().sync();      // nobody exits while peers may still write its slots
+  if (rank != 0 || tid != 0) return;
+  // target -> source in the input frame: [R | -R m_t + scale t + m_s]; the result is its inverse
+  double R[3][3], t[3];
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) R[r][c] = sh.T[4 * r + c];
+    t[r] = -(R[r][0] * fr.mt[0] + R[r][1] * fr.mt[1] + R[r][2] * fr.mt[2]) + fr.scale * sh.T[4 * r + 3] + fr.ms[r];
+  }
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) result[4 * r + c] = R[c][r];
+    result[4 * r + 3] = -(R[0][r] * t[0] + R[1][r] * t[1] + R[2][r] * t[2]);
+  }
+  result[12] = 0; result[13] = 0; result[14] = 0; result[15] = 1;
+  result[16] = (double)n_mut;
+  result[17] = (double)n_corr;
+  result[18] = (double)drawn;
+  result[19] = mu;
+  result[20] = ran;
+  result[21] = swapped;
+  result[22] = 0;
+  result[23] = 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t dgr_fgr_ws_elems(int64_t n_src, int64_t n_tgt, int64_t maximum_tuple_count, int32_t tuple_test,
+                         int64_t* n_elems) {
+  DGR_ARG_CHECK(n_elems != nullptr && n_src >= 0 && n_tgt >= 0 && maximum_tuple_count >= 0, "bad arguments");
+  *n_elems = fgr_layout(n_src, n_tgt, maximum_tuple_count, tuple_test != 0, nullptr, nullptr);
+  return DGR_OK;
+}
+
+int32_t dgr_fgr_feature_matching(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt,
+                                 const int32_t* nn_st, const int32_t* nn_ts, double division_factor,
+                                 int32_t use_absolute_scale, int32_t decrease_mu,
+                                 double maximum_correspondence_distance, int32_t iteration_number,
+                                 double tuple_scale, int64_t maximum_tuple_count, int32_t tuple_test, uint64_t seed,
+                                 uint64_t* ws, int32_t* corres_out, double* result, void* stream) {
+  DGR_ARG_CHECK(src != nullptr && tgt != nullptr && nn_st != nullptr && nn_ts != nullptr && ws != nullptr &&
+                result != nullptr, "null pointer");
+  DGR_ARG_CHECK(n_src >= 1 && n_tgt >= 1, "both clouds need a point");
+  const int64_t n_min = n_src < n_tgt ? n_src : n_tgt, n_first = n_src < n_tgt ? n_tgt : n_src;
+  DGR_ARG_CHECK(n_first < (1ll << 31) && 100 * n_min < (1ll << 31), "point count out of range");
+  DGR_ARG_CHECK(division_factor > 1.0, "division_factor must be > 1");
+  DGR_ARG_CHECK(maximum_correspondence_distance > 0.0, "maximum_correspondence_distance must be positive");
+  DGR_ARG_CHECK(iteration_number >= 0, "iteration_number must be >= 0");
+  DGR_ARG_CHECK(tuple_scale > 0.0 && tuple_scale <= 1.0, "tuple_scale must lie in (0, 1]");
+  DGR_ARG_CHECK(maximum_tuple_count >= 1 && maximum_tuple_count <= (1ll << 30), "maximum_tuple_count out of range");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int tt = tuple_test != 0, absolute = use_absolute_scale != 0, swapped = n_tgt > n_src;
+  FgrWs w;
+  fgr_layout(n_src, n_tgt, maximum_tuple_count, tt, ws, &w);
+  const int64_t Kc = fgr_kc(n_min, maximum_tuple_count);
+  const unsigned n_mblk = dgr_blocks(n_first, kFgrThreads);
+  int launches = 0;
+  fgr_stats_kernel<<<2, kFgrStatThreads, 0, st>>>(src, n_src, tgt, n_tgt, w.stat, w.tstate);
+  fgr_mutual_kernel<<<n_mblk, kFgrThreads, 0, st>>>(swapped ? nn_ts : nn_st, swapped ? nn_st : nn_ts, n_first, n_min,
+                                                    w.mflag, w.mblk);
+  fgr_scan_kernel<<<1, 1024, 0, st>>>(w.mblk, n_mblk);
+  fgr_select_kernel<<<n_mblk, kFgrThreads, 0, st>>>(w.mflag, w.mblk, n_first, n_min, 0, w.mut, nullptr);
+  launches += 4;
+  const int32_t* n_mut = w.mblk + n_mblk;
+  if (tt && n_min >= 3) {
+    for (int64_t h0 = 0; h0 < 100 * n_min; h0 += kFgrChunk) {
+      fgr_tuple_kernel<<<kFgrChunkBlocks, kFgrThreads, 0, st>>>(src, tgt, nn_st, nn_ts, swapped, w.mut, n_mut, w.stat,
+                                                                 absolute, seed, h0, tuple_scale, Kc, w.tstate,
+                                                                 w.tflag, w.tblk);
+      fgr_tuple_scan_kernel<<<1, 1024, 0, st>>>(w.tblk, n_mut, h0, Kc, w.tstate);
+      fgr_select_kernel<<<kFgrChunkBlocks, kFgrThreads, 0, st>>>(w.tflag, w.tblk, kFgrChunk, Kc, h0, w.tsel,
+                                                                  w.tstate + 1);
+      launches += 3;
+    }
+  }
+  const bool clustered = !tt && n_min >= kFgrClusterMin;
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr[1];
+  cfg.gridDim = dim3(clustered ? kFgrCluster : 1);
+  cfg.blockDim = dim3(kFgrSolveThreads);
+  cfg.stream = st;
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = clustered ? kFgrCluster : 1;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = clustered ? 1 : 0;
+  if (clustered)
+    DGR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, fgr_solve_kernel<kFgrCluster>, src, tgt, nn_st, nn_ts, swapped,
+                                      (const int32_t*)w.mut, n_mut, (const int32_t*)w.tsel, (const int32_t*)w.tstate,
+                                      Kc, tt, (const double*)w.stat, absolute, seed, (int)iteration_number,
+                                      (int)(decrease_mu != 0), division_factor, maximum_correspondence_distance,
+                                      w.corr, corres_out, result));
+  else
+    fgr_solve_kernel<1><<<1, kFgrSolveThreads, 0, st>>>(src, tgt, nn_st, nn_ts, swapped, w.mut, n_mut, w.tsel,
+                                                         w.tstate, Kc, tt, w.stat, absolute, seed, iteration_number,
+                                                         decrease_mu != 0, division_factor,
+                                                         maximum_correspondence_distance, w.corr, corres_out, result);
+  launches += 1;
+  dgr_note_launches(launches);
+  DGR_LAUNCH_CHECK();
+  return DGR_OK;
+}
+
+}  // extern "C"

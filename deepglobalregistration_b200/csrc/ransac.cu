@@ -39,8 +39,7 @@ __global__ void ransac_pack_kernel(const float* __restrict__ x, const float* __r
 // slot-th sample of hypothesis h: uniform in [0, n) (with replacement, like open3d's
 // per-iteration uniform_int_distribution draws)
 __device__ __forceinline__ uint32_t ransac_pick(uint64_t seed, uint64_t h, int slot, uint32_t n) {
-  uint64_t z = dgr_mix64(seed + (h * 4 + (uint64_t)slot + 1) * 0x9E3779B97F4A7C15ull);
-  return (uint32_t)(((z >> 32) * (uint64_t)n) >> 32);
+  return dgr_counter_pick(seed, h * 4 + (uint64_t)slot, n);
 }
 
 // Umeyama without scaling: the pose (R, t) minimising sum |R p_j + t - q_j|^2 over 4 pairs, fp64
@@ -334,12 +333,7 @@ __global__ void __launch_bounds__(1024) fm_scan_kernel(int32_t* blk, int64_t n_h
 __global__ void __launch_bounds__(kFmThreads)
 fm_select_kernel(const int32_t* __restrict__ flag, const int32_t* __restrict__ blk, int64_t M, int64_t Vc,
                  int32_t* __restrict__ sel) {
-  const int base = blk[blockIdx.x];
-  if (base >= Vc) return;                              // uniform per block
-  const int64_t h = (int64_t)blockIdx.x * kFmThreads + threadIdx.x;
-  const int f = h < M ? flag[h] : 0;
-  const int pos = base + dgr_block_exclusive_scan_256(f, nullptr);
-  if (f && pos < Vc) sel[pos] = (int32_t)h;
+  dgr_select_first_256(flag, blk[blockIdx.x], M, Vc, 0, sel);
 }
 
 __global__ void __launch_bounds__(kFmThreads, 4)   // <= 64 registers: 32 warps per SM hide the probe latency

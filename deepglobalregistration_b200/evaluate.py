@@ -197,9 +197,10 @@ def main(argv=None):
   ap.add_argument('--success_rte_thresh', type=float, default=0.3, help='m (config.py:127; KITTI: 0.6)')
   ap.add_argument('--success_rre_thresh', type=float, default=15.0, help='deg (config.py:128; KITTI: 5)')
   ap.add_argument('--no_icp', action='store_true')
-  ap.add_argument('--method', choices=('dgr', 'fcgf_ransac'), default='dgr',
+  ap.add_argument('--method', choices=('dgr', 'fcgf_ransac', 'fcgf_fgr'), default='dgr',
                   help='dgr: DeepGlobalRegistration.register; fcgf_ransac: the FCGF + RANSAC baseline on the same '
-                  'checkpoint (core/fcgf_ransac.py)')
+                  'checkpoint (core/fcgf_ransac.py); fcgf_fgr: FCGF + Fast Global Registration with open3d\'s '
+                  'default options (core/fcgf_fgr.py)')
   ap.add_argument('--ransac_max_iteration', type=int, default=80000, help='fcgf_ransac: hypotheses drawn at most')
   ap.add_argument('--ransac_max_validation', type=int, default=1000,
                   help='fcgf_ransac: hypotheses scored (the ones that pass the checkers first)')
@@ -224,6 +225,9 @@ def main(argv=None):
     method = FCGFRansac(dgr)
     method.max_iteration, method.max_validation = args.ransac_max_iteration, args.ransac_max_validation
     method.edge_ratio = args.ransac_edge_ratio
+  elif args.method == 'fcgf_fgr':
+    from .core.fcgf_fgr import FCGFFastGlobal
+    method = FCGFFastGlobal(dgr)
   if args.threed_match_dir:
     pairs = threedmatch_pairs(args.threed_match_dir)
   elif args.kitti_dir:
@@ -244,7 +248,8 @@ def main(argv=None):
   if rank == 0:
     summary = summarize(result)
     print(json.dumps(dict(summary, world_size=world)))          # the summary first: a failing save loses nothing
-    stem, name = ('dgr-b200', 'DGR') if args.method == 'dgr' else ('fcgf-ransac-b200', 'RANSAC')
+    stem, name = {'dgr': ('dgr-b200', 'DGR'), 'fcgf_ransac': ('fcgf-ransac-b200', 'RANSAC'),
+                  'fcgf_fgr': ('fcgf-fgr-b200', 'FGR')}[args.method]
     out = os.path.join(out_dir, f'{stem}-stats.npz')
     np.savez(out, stats=result['stats'][None], names=[name], poses=result['poses'], groups=result['groups'])
     print(json.dumps(dict(summary, world_size=world, saved=out)))

@@ -14,9 +14,15 @@
          max_validation)), the edge-length and distance checkers, every validated hypothesis scored on all source
          points through a voxel hash of the target.
 
+It also carries the call open3d users make when RANSAC is too slow:
+
+  registration_fast_based_on_feature_matching(source, target, source_feature, target_feature, option)
+      -> dgr_knn_top1 both ways + dgr_fgr_feature_matching: Fast Global Registration (mutual matches, tuple
+         test, graduated non-convexity) with FastGlobalRegistrationOption's fields and defaults.
+
 With ``shims.install()`` these are reachable as ``open3d.pipelines.registration`` (and the pre-0.12 alias
 ``open3d.registration``) whenever the real open3d is absent, so the reference's own class runs on this stack
-without a line changed.  There is no CPU path: the functions raise without an sm_100 device.
+without a line changed.  There is no CPU path: the functions raise without an sm_90 device.
 """
 import numpy as np
 import torch
@@ -198,3 +204,67 @@ def registration_ransac_based_on_feature_matching(source, target, source_feature
                                    edge_ratio, check_dist, criteria.max_iteration, criteria.max_validation,
                                    seed=seed).cpu().numpy()
   return RegistrationResult(r[:16], r[16], r[17], r[19])
+
+
+class FastGlobalRegistrationOption:
+  """open3d's option object for Fast Global Registration, with its field names and defaults.  ``seed`` (not an
+  open3d field in every release) makes the tuple test's draws reproducible."""
+
+  def __init__(self, division_factor=1.4, use_absolute_scale=False, decrease_mu=True,
+               maximum_correspondence_distance=0.025, iteration_number=64, tuple_scale=0.95,
+               maximum_tuple_count=1000, tuple_test=True, seed=0):
+    self.division_factor = float(division_factor)
+    self.use_absolute_scale = bool(use_absolute_scale)
+    self.decrease_mu = bool(decrease_mu)
+    self.maximum_correspondence_distance = float(maximum_correspondence_distance)
+    self.iteration_number = int(iteration_number)
+    self.tuple_scale = float(tuple_scale)
+    self.maximum_tuple_count = int(maximum_tuple_count)
+    self.tuple_test = bool(tuple_test)
+    self.seed = int(seed)
+
+  def __repr__(self):
+    return ('FastGlobalRegistrationOption(' + ', '.join(f'{k}={v}' for k, v in vars(self).items()) + ')')
+
+
+def _fgr_option_check(o):
+  if not o.division_factor > 1.0:
+    raise ValueError(f'division_factor must be > 1, got {o.division_factor}')
+  if not o.maximum_correspondence_distance > 0.0:
+    raise ValueError(f'maximum_correspondence_distance must be positive, got {o.maximum_correspondence_distance}')
+  if o.iteration_number < 0:
+    raise ValueError(f'iteration_number must be >= 0, got {o.iteration_number}')
+  if not 0.0 < o.tuple_scale <= 1.0:
+    raise ValueError(f'tuple_scale must lie in (0, 1], got {o.tuple_scale}')
+  if o.maximum_tuple_count < 1:
+    raise ValueError(f'maximum_tuple_count must be >= 1, got {o.maximum_tuple_count}')
+
+
+def registration_fast_based_on_feature_matching(source, target, source_feature, target_feature,
+                                                option=None):
+  """Fast Global Registration (Zhou, Park & Koltun 2016) on feature matches.  Both nearest-feature directions
+  come from dgr_knn_top1 (fp32); dgr_fgr_feature_matching keeps the mutual matches, runs the tuple test and the
+  graduated non-convexity optimiser.  Like open3d's, the result carries the transformation only (fitness 0, no
+  correspondence set)."""
+  option = FastGlobalRegistrationOption() if option is None else option
+  _fgr_option_check(option)
+  fs = np.asarray(source_feature.data, dtype=np.float32).T
+  ft = np.asarray(target_feature.data, dtype=np.float32).T
+  if fs.shape[1] != ft.shape[1]:
+    raise ValueError(f'feature dimensions differ: {fs.shape[1]} vs {ft.shape[1]}')
+  n_s = len(np.asarray(getattr(source, 'points', source)).reshape(-1, 3))
+  n_t = len(np.asarray(getattr(target, 'points', target)).reshape(-1, 3))
+  if len(fs) != n_s or len(ft) != n_t:
+    raise ValueError('one feature per point is required')
+  if n_s == 0 or n_t == 0:
+    return RegistrationResult(np.eye(4))
+  dev = _abi.require_device('cuda')
+  _abi.refresh_stream()
+  src, tgt = _points(source, dev).float().contiguous(), _points(target, dev).float().contiguous()
+  fs_d = torch.from_numpy(np.ascontiguousarray(fs)).to(dev)
+  ft_d = torch.from_numpy(np.ascontiguousarray(ft)).to(dev)
+  r = _abi.fgr_feature_matching(src, tgt, _abi.knn_top1(fs_d, ft_d), _abi.knn_top1(ft_d, fs_d),
+                                option.division_factor, option.use_absolute_scale, option.decrease_mu,
+                                option.maximum_correspondence_distance, option.iteration_number, option.tuple_scale,
+                                option.maximum_tuple_count, option.tuple_test, seed=option.seed).cpu().numpy()
+  return RegistrationResult(r[:16])

@@ -43,7 +43,8 @@ def _open3d_stub():
   """The part of open3d the reference touches on the registration path: demo.py:10-48 (I/O, PointCloud, a no-op
   viewer, backed by io.py) and core/deep_global_registration.py:29-64,317-322 + util/pointcloud.py:15-23
   (pipelines.registration.registration_icp / registration_ransac_based_on_correspondence /
-  registration_ransac_based_on_feature_matching, Feature, utility vectors) backed
+  registration_ransac_based_on_feature_matching, Feature, utility vectors; plus
+  registration_fast_based_on_feature_matching / FastGlobalRegistrationOption for FGR users) backed
   by libdgr_b200 (o3d_registration.py) - so the reference's OWN DeepGlobalRegistration class and demo.py run on
   this stack unmodified.  This package's DeepGlobalRegistration does not go through here: it calls the library."""
   import numpy as np
@@ -65,7 +66,8 @@ def _open3d_stub():
   for name in ('TransformationEstimationPointToPoint', 'ICPConvergenceCriteria', 'RANSACConvergenceCriteria',
                'CorrespondenceCheckerBasedOnDistance', 'CorrespondenceCheckerBasedOnEdgeLength', 'Feature',
                'RegistrationResult', 'registration_icp', 'registration_ransac_based_on_correspondence',
-               'registration_ransac_based_on_feature_matching'):
+               'registration_ransac_based_on_feature_matching', 'FastGlobalRegistrationOption',
+               'registration_fast_based_on_feature_matching'):
     setattr(o3d.pipelines.registration, name, getattr(reg, name))
   o3d.registration = o3d.pipelines.registration          # the pre-0.12 module path
   sys.modules['open3d.pipelines'] = o3d.pipelines

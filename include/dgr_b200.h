@@ -284,6 +284,34 @@ int32_t dgr_ransac_feature_matching(const float* src, int64_t n_src, const float
                                     int64_t max_iteration, int64_t max_validation, uint64_t seed, uint64_t* ws,
                                     double* result, void* stream);
 
+/* ---- Fast Global Registration over feature matches: open3d registration_fast_based_on_feature_matching
+ *      with FastGlobalRegistrationOption (the FGR row of the reference's results) ---------------------- */
+/* nn_st[i] = row of the target feature nearest to source feature i, nn_ts[j] = row of the source feature nearest
+ * to target feature j (dgr_knn_top1 / dgr_knn_top1_tc).  Both clouds are centred on their fp64 means and divided by
+ * s = the largest centred norm (use_absolute_scale: not divided, mu starts at s instead of 1).  Mutual pairs
+ * (nn_ts[nn_st[i]] == i) are listed in the order of the larger cloud's rows (the source's on a tie).  tuple_test:
+ * trials k = 0 .. 100 n_mut - 1 draw 3 list positions with the counter hash (draws 3k .. 3k + 2 of `seed`) and
+ * pass when every edge has l_s tuple_scale < l_t < l_s / tuple_scale; the first maximum_tuple_count that pass
+ * give 3 correspondences each, in order (no trial when n_mut < 3); without tuple_test the correspondences are the
+ * mutual list.  With >= 10 correspondences, iteration_number Gauss-Newton steps on the Geman-McClure objective
+ * sum (mu / (r^2 + mu))^2-weighted |p - T q|^2 move the target onto the source (mu divided by division_factor
+ * when decrease_mu, itr % 4 == 0 and mu > maximum_correspondence_distance; a non-positive Cholesky pivot makes
+ * that step the identity).  All fp64, no host read, the same bits on every run.
+ * ws: dgr_fgr_ws_elems() 8-byte words.  corres_out (optional): int32 (source, target) pairs, room for
+ * tuple_test ? 3 min(maximum_tuple_count, 100 min(n_src, n_tgt)) : min(n_src, n_tgt) of them; the first
+ * result[17] are written.  result: device double[24] = 4x4 pose mapping the source into the target, n_mut,
+ * correspondences used, trials drawn until the maximum_tuple_count-th acceptance (100 n_mut if it is never
+ * reached, 0 without trials), final mu, 1 if the optimiser ran, 1 if the clouds were swapped for the matching
+ * order (n_tgt > n_src), 2 zeros. */
+int32_t dgr_fgr_ws_elems(int64_t n_src, int64_t n_tgt, int64_t maximum_tuple_count, int32_t tuple_test,
+                         int64_t* n_elems);
+int32_t dgr_fgr_feature_matching(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt,
+                                 const int32_t* nn_st, const int32_t* nn_ts, double division_factor,
+                                 int32_t use_absolute_scale, int32_t decrease_mu,
+                                 double maximum_correspondence_distance, int32_t iteration_number,
+                                 double tuple_scale, int64_t maximum_tuple_count, int32_t tuple_test, uint64_t seed,
+                                 uint64_t* ws, int32_t* corres_out, double* result, void* stream);
+
 /* ======================================================================================
  * Round 2: coordinate planning with device-side counts, and the native executor.
  * ====================================================================================== */
