@@ -40,19 +40,10 @@ SIGNATURES = {
     'dgr_scan_ws_elems': [_i64],
     'dgr_hash_find': [_p, _i64, _i32, _p, _p, _p, _i64, _p, _p],
     'dgr_gather_rows_i32': [_p, _p, _i64, _i32, _p, _p],
-    'dgr_stride_coords': [_p, _i64, _i32, _i32, _p, _p],
-    'dgr_bloom_build': [_p, _i64, _p, _i64, _p],
-    'dgr_kernel_map_table': [_p, _i64, _i32, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p, _p, _p],
-    'dgr_kmap_ws_elems': [_i32, _i64],
-    'dgr_kernel_map_count': [_p, _i32, _i64, _p, _i32, _p, _p, _p],
-    'dgr_kernel_map_fill': [_p, _i32, _i64, _p, _p, _p, _p],
-    'dgr_kernel_map_tiles': [_p, _i32, _i32, _i32, _i32, _p, _p, _p],
-    'dgr_kernel_map_tiles2': [_p, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _p],
     'dgr_spconv_fwd': [_p, _i32, _p, _i32, _p, _p, _p, _p, _p, _i32, _i32, _i32, _p, _p],
     'dgr_spconv_tc_supported': [_i32, _i32],
     'dgr_pack_weight_tf32': [_p, _i32, _i32, _i32, _p, _p],
     'dgr_spconv_tc_fwd': [_p, _i32, _p, _i32, _p, _p, _p, _p, _p, _i32, _i32, _i32, _p, _p],
-    'dgr_spconv_table_fwd': [_p, _i32, _p, _i32, _p, _i32, _i64, _p, _p, _p, _p],
     'dgr_linear_fwd': [_p, _i32, _p, _i32, _i64, _p, _i32, _p, _i32, _i32, _p, _p],
     'dgr_affine_act': [_p, _i64, _i32, _p, _p, _p, _i32, _p, _p],
     'dgr_cat2': [_p, _i32, _p, _i32, _i64, _p, _p],
@@ -80,10 +71,12 @@ SIGNATURES = {
     'dgr_coarse_scan_elems': [_i64],
     'dgr_coarse_maps': [_p, _i64, _p, _i32, _p, _i32, _p, _p, _p, _i64, _p, _p, _p, _p, _p],
     'dgr_bloom2_build': [_p, _i64, _p, _i64, _p],
+    'dgr_bloom2_words': [_i64],
     'dgr_kmap_mask_words': [_i64],
     'dgr_kmap_cnt_elems': [_i32, _i64],
     'dgr_kmap_probe': [_p, _i64, _p, _i32, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p, _p, _p, _p, _p],
     'dgr_kmap_fill': [_p, _p, _i32, _i64, _p, _i32, _p, _p, _p, _i64, _p, _p, _p, _p],
+    'dgr_kernel_map_tiles': [_p, _i32, _i32, _i32, _i32, _p, _p, _p],
     'dgr_kmap_dense': [_p, _i64, _p, _i32, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p, _i64, _p, _p],
     'dgr_spconv_ones_bits_fwd': [_p, _i32, _p, _i64, _i32, _i64, _p, _p, _p, _p],
     'dgr_spconv_os_supported': [_i32, _i32],
@@ -110,7 +103,7 @@ SIGNATURES = {
     'dgr_pair_tap': [_p, _i32, _p, _p, _p],
 }
 _RESTYPES = {'dgr_coarse_scan_elems': _i64, 'dgr_kmap_mask_words': _i64, 'dgr_kmap_cnt_elems': _i64, 'dgr_ctx_stream': C.c_void_p,
-             'dgr_ctx_profile_read': _i64, 'dgr_last_error': C.c_char_p, 'dgr_knn_tc_ws_elems': _i64, 'dgr_launch_count': _i64, 'dgr_spconv_tc_supported': _i32, 'dgr_scan_ws_elems': _i64, 'dgr_kmap_ws_elems': _i64}
+             'dgr_ctx_profile_read': _i64, 'dgr_last_error': C.c_char_p, 'dgr_knn_tc_ws_elems': _i64, 'dgr_launch_count': _i64, 'dgr_spconv_tc_supported': _i32, 'dgr_scan_ws_elems': _i64, 'dgr_bloom2_words': _i64}
 
 _lib = None
 
@@ -236,24 +229,27 @@ def scratch(name, numel, dtype, device):
 # --------------------------------------------------------------------------- #
 # thin typed wrappers (allocate outputs / workspaces with torch, call the ABI)
 # --------------------------------------------------------------------------- #
-class HashTable:
-  __slots__ = ('keys', 'vals', 'cap', '_bloom')
+def table_cap(n):
+  """Capacity of the table of n keys: a power of two, load factor <= 0.5."""
+  return max(1024, next_pow2(2 * max(int(n), 1)))
 
-  def bloom(self):
-    """(words, n_bits) miss filter, built on first use by a kernel map."""
-    if getattr(self, '_bloom', None) is None:
-      bits = 16 * self.cap
-      words = torch.empty(bits // 32, dtype=torch.int32, device=self.keys.device)
-      call('dgr_bloom_build', ptr(self.keys), self.cap, ptr(words), bits, stream())
-      self._bloom = (words, bits)
-    return self._bloom
+
+class HashTable:
+  __slots__ = ('keys', 'vals', 'cap')
 
   def __init__(self, n, device):
-    self.cap = max(1024, next_pow2(2 * max(int(n), 1)))
+    """An empty table for n keys."""
+    self.cap = table_cap(n)
     self.keys = torch.empty(self.cap, dtype=torch.int64, device=device)
     self.vals = torch.empty(self.cap, dtype=torch.int32, device=device)
-    self._bloom = None
     call('dgr_hash_clear', ptr(self.keys), ptr(self.vals), self.cap, stream())
+
+  @classmethod
+  def wrap(cls, keys, vals, cap):
+    """A table another call has filled (one level of coarse_maps), not cleared."""
+    t = cls.__new__(cls)
+    t.keys, t.vals, t.cap = keys, vals, cap
+    return t
 
 
 def quantize_points(xyz, voxel, batch=0):
@@ -323,14 +319,27 @@ def gather_rows_i32(src, idx, n):
   return out
 
 
-def stride_coords(coords, out_stride):
-  out = torch.empty_like(coords)
-  call('dgr_stride_coords', ptr(coords), coords.shape[0], coords.shape[1], out_stride, ptr(out), stream())
-  return out
+def coarse_maps(fine, spec, strides):
+  """Coordinate maps at up to 4 tensor strides, all derived from the distinct rows `fine` [n, ncols]: level l
+  holds floor(c / s) * s of every cell in the order of its first row in `fine`.  -> (coords int32
+  [L, max(n, 1), ncols] (first n_out[l] rows of level l valid), tables, n_out device int32 [L])."""
+  _chk(fine, torch.int32, 'fine')
+  n, ncols = fine.shape
+  L, nmx, dev = len(strides), max(n, 1), fine.device
+  cap = table_cap(n)               # one capacity for every level: at least 2 n
+  keys = torch.empty(L, cap, dtype=torch.int64, device=dev)
+  vals = torch.empty(L, cap, dtype=torch.int32, device=dev)
+  coords = torch.empty(L, nmx, ncols, dtype=torch.int32, device=dev)
+  n_out = torch.empty(L, dtype=torch.int32, device=dev)
+  slot = scratch('cm_slot', L * nmx, torch.int32, dev)
+  scan = scratch('cm_scan', L * lib().dgr_coarse_scan_elems(nmx), torch.int32, dev)
+  call('dgr_coarse_maps', ptr(fine), n, None, ncols, ptr(spec), L, (C.c_int32 * L)(*strides), ptr(keys), ptr(vals),
+       cap, ptr(coords), ptr(n_out), ptr(slot), ptr(scan), stream())
+  return coords, [HashTable.wrap(keys[l], vals[l], cap) for l in range(L)], n_out
 
 
 class KernelMap:
-  """Neighbour table + (kappa, j)-sorted pair lists + the gather-GEMM-scatter work list."""
+  """(kappa, j)-sorted pair lists + the gather-GEMM-scatter work list (+ the dense neighbour table when kept)."""
   __slots__ = ('K', 'n_in', 'n_out', 'nbr', 'in_idx', 'out_idx', 'kofs', 'kofs_host', 'n_pairs',
                'tile_k', 'tile_start', 'n_tiles', '_paired')
 
@@ -358,26 +367,35 @@ class KernelMap:
 
 
 def kernel_map_begin(out_coords, spec, in_table, n_in, offsets, keep_table=False, slot=0):
-  """First half of a kernel map: neighbour table + bucket counts, all asynchronous.  `slot` selects
-  the scratch buffers so that several maps can be in flight before ONE host read finishes them
-  all (kernel_maps_finish)."""
+  """First half of a kernel map: occupancy bits + bucket offsets (and the dense neighbour table when kept), all
+  asynchronous.  `slot` selects the scratch buffers so that several maps can be in flight before ONE host read
+  finishes them all (kernel_maps_finish)."""
   _chk(out_coords, torch.int32, 'out_coords')
   _chk(offsets, torch.int32, 'offsets')
   dev = out_coords.device
   n_out, ncols = out_coords.shape
   K = offsets.shape[0]
-  if keep_table:
-    nbr = torch.empty(K, max(n_out, 1), dtype=torch.int32, device=dev)
-  else:
-    nbr = scratch(('km_nbr', slot), K * max(n_out, 1), torch.int32, dev).view(K, max(n_out, 1))
-  # the miss filter pays off when most probes miss: many offsets per row (6-D, 5^3, 7^3 kernels)
-  bloom, bloom_bits = in_table.bloom() if K > 27 else (None, 0)
-  ws = scratch(('km_ws', slot), lib().dgr_kmap_ws_elems(K, n_out), torch.int32, dev)
-  call('dgr_kernel_map_table', ptr(out_coords), n_out, ncols, ptr(spec), ptr(in_table.keys),
-       ptr(in_table.vals), in_table.cap, ptr(bloom), bloom_bits, ptr(offsets), K, ptr(nbr), ptr(ws), stream())
+  nmx = max(n_out, 1)
+  bits = scratch(('km_bits', slot), K * lib().dgr_kmap_mask_words(nmx), torch.int32, dev)
+  cnt = scratch(('km_cnt', slot), lib().dgr_kmap_cnt_elems(K, nmx), torch.int32, dev)
   kofs = torch.empty(K + 2, dtype=torch.int32, device=dev)
-  call('dgr_kernel_map_count', ptr(nbr), K, n_out, ptr(ws), 1, ptr(kofs), ptr(spec), stream())
-  return dict(K=K, n_in=n_in, n_out=n_out, nbr=nbr, ws=ws, kofs=kofs, keep=keep_table, dev=dev)
+  meta = scratch('km_meta', 5, torch.int32, dev)          # written by the probe, read by nobody here
+  # the miss filter pays off when most probes miss: many offsets per row (6-D, 5^3, 7^3 kernels)
+  bloom, n_words = None, 0
+  if K > 27:
+    n_words = lib().dgr_bloom2_words(n_in)
+    bloom = scratch('km_bloom', n_words, torch.int32, dev)
+    call('dgr_bloom2_build', ptr(in_table.keys), in_table.cap, ptr(bloom), n_words, stream())
+  table = (ptr(in_table.keys), ptr(in_table.vals), in_table.cap)
+  call('dgr_kmap_probe', ptr(out_coords), n_out, None, ncols, ptr(spec), *table, ptr(bloom), n_words, ptr(offsets), K,
+       ptr(bits), ptr(cnt), ptr(kofs), ptr(meta), stream())
+  nbr = None
+  if keep_table:
+    nbr = torch.empty(K, nmx, dtype=torch.int32, device=dev)
+    call('dgr_kmap_dense', ptr(out_coords), n_out, None, ncols, ptr(spec), *table, ptr(bloom), n_words, ptr(offsets),
+         K, ptr(nbr), nmx, None, stream())
+  return dict(K=K, n_in=n_in, n_out=n_out, out_coords=out_coords, spec=spec, in_table=in_table, offsets=offsets,
+              bits=bits, cnt=cnt, kofs=kofs, nbr=nbr, dev=dev)
 
 
 def kernel_map_finish(pend, kofs_all):
@@ -395,15 +413,17 @@ def kernel_map_finish(pend, kofs_all):
   km.K, km.n_in, km.n_out = K, pend['n_in'], n_out
   km.in_idx = torch.empty(max(P, 1), dtype=torch.int32, device=dev)
   km.out_idx = torch.empty(max(P, 1), dtype=torch.int32, device=dev)
-  if n_out > 0:
-    call('dgr_kernel_map_fill', ptr(pend['nbr']), K, n_out, ptr(pend['ws']), ptr(km.in_idx), ptr(km.out_idx),
-         stream())
   km.tile_k = torch.empty(max(n_tiles, 1), dtype=torch.int32, device=dev)
   km.tile_start = torch.empty(max(n_tiles, 1), dtype=torch.int32, device=dev)
-  call('dgr_kernel_map_tiles', ptr(pend['kofs']), K, TILE_ROWS, n_tiles, 0, ptr(km.tile_k), ptr(km.tile_start),
-       stream())
+  if P > 0:
+    out_coords, t = pend['out_coords'], pend['in_table']
+    call('dgr_kmap_fill', ptr(pend['bits']), ptr(pend['cnt']), K, n_out, ptr(out_coords), out_coords.shape[1],
+         ptr(pend['spec']), ptr(t.keys), ptr(t.vals), t.cap, ptr(pend['offsets']), ptr(km.in_idx), ptr(km.out_idx),
+         stream())
+    call('dgr_kernel_map_tiles', ptr(pend['kofs']), K, TILE_ROWS, n_tiles, 0, ptr(km.tile_k), ptr(km.tile_start),
+         stream())
   km.kofs, km.kofs_host, km.n_pairs, km.n_tiles = pend['kofs'], kofs_host, P, n_tiles
-  km.nbr = pend['nbr'] if pend['keep'] else None
+  km.nbr = pend['nbr']
   km._paired = None
   return km
 
@@ -524,8 +544,8 @@ def spconv_table_fwd(feat, weight, km, cout, scale=None, shift=None):
   _chk(feat, torch.float32, 'feat'); _chk(weight, torch.float32, 'weight')
   assert km.nbr is not None
   out = torch.empty(km.n_out, cout, dtype=torch.float32, device=feat.device)
-  call('dgr_spconv_table_fwd', ptr(feat), feat.shape[1], ptr(weight), cout, ptr(km.nbr), km.K, km.n_out,
-       ptr(scale), ptr(shift), ptr(out), stream())
+  call('dgr_spconv_table_fwd_strided', ptr(feat), feat.shape[1], ptr(weight), cout, ptr(km.nbr), km.K, km.n_out,
+       km.nbr.stride(0), ptr(scale), ptr(shift), ptr(out), stream())
   return out
 
 

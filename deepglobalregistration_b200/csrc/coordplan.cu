@@ -1,19 +1,18 @@
 // Coordinate planning with DEVICE-SIDE row counts: the integer work of one network forward
 // (coarse coordinate maps, kernel maps) enqueued without a single host round trip.
 //
-// The round-1 builders (coords.cu) size every launch from host-side counts, so building the
-// maps of one ResUNet cost one device-to-host read per dependent step (rows of each strided
-// map, pairs of each kernel map).  Here every kernel takes (n_max, n_dev): a host-side upper
-// bound that sizes buffers and grids, and a device pointer to the actual count that the
-// kernels read.  The native executor (exec.cu) enqueues the whole coordinate phase of a
-// network, then reads ONE small meta block (rows per level, pairs / tiles per map, key
-// overflow) and launches the fill + convolution phase.
+// Every kernel takes (n_max, n_dev): a host-side upper bound that sizes buffers and grids,
+// and a device pointer to the actual count that the kernels read (NULL: n_max is the count,
+// as on the operator path of me/coords.py).  The native executor (exec.cu) enqueues the whole
+// coordinate phase of a network, then reads ONE small meta block (rows per level, pairs /
+// tiles per map, key overflow) and launches the fill + convolution phase.
 //
-// Kernel maps no longer go through the dense neighbour table nbr[K][N_out] (150 MB per 6-D
-// map, 99.7 % of it -1): the probe pass stores one BIT per (offset, output row) - a ballot
-// word per (offset, warp of 32 rows), 32x smaller - together with per-(offset, block) hit
-// counts; after an exclusive scan the fill pass walks the set bits, re-probes those (hits
-// only) and writes the (kappa, j)-sorted pair lists, bit-identical to the round-1 builder.
+// Kernel maps do not go through a dense neighbour table nbr[K][N_out] (150 MB per 6-D map,
+// 99.7 % of it -1): the probe pass stores one BIT per (offset, output row) - a ballot word
+// per (offset, warp of 32 rows), 32x smaller - together with per-(offset, block) hit counts;
+// after an exclusive scan the fill pass walks the set bits, re-probes those (hits only) and
+// writes the (kappa, j)-sorted pair lists, bit-identical to the oracle's buckets.  A dense
+// table is built (dgr_kmap_dense) only where a convolution reads one.
 // Misses, 96-99.7 % of all probes of a 6-D map, are answered by a blocked Bloom filter of the
 // input table held in SHARED memory (one 32-bit word holds both bits of a key: one
 // shared-memory load per probe) instead of an L2 round trip.
@@ -457,6 +456,31 @@ kmap_fill_kernel(const uint32_t* __restrict__ bits, int W, int bpk, const int32_
   }
 }
 
+// Work list of a kernel map (one block): bucket k gets ceil(count_k / tile_rows) tiles, rounded up to an even
+// number when `pair` is set (CTA pairs; the last tile may then be empty); tile t covers pairs
+// [tile_start[t], +tile_rows) of bucket tile_k[t].
+__global__ void tiles_kernel(const int32_t* __restrict__ kofs, int K, int tile_rows, int n_tiles, int pair,
+                             int32_t* __restrict__ tile_k, int32_t* __restrict__ tile_start) {
+  extern __shared__ int tofs[];   // K + 1 exclusive tile offsets
+  for (int k = threadIdx.x; k < K; k += blockDim.x) {
+    const int v = (kofs[k + 1] - kofs[k] + tile_rows - 1) / tile_rows;
+    tofs[k] = pair ? (v + 1) & ~1 : v;
+  }
+  __syncthreads();
+  const int total = dgr_block_scan_inplace(tofs, K);
+  if (threadIdx.x == 0) tofs[K] = total;
+  __syncthreads();
+  for (int t = threadIdx.x; t < n_tiles; t += blockDim.x) {
+    int lo = 0, hi = K;   // largest k with tofs[k] <= t (non-empty: tofs[k + 1] > t)
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (tofs[mid] <= t) lo = mid; else hi = mid;
+    }
+    tile_k[t] = lo;
+    tile_start[t] = kofs[lo] + (t - tofs[lo]) * tile_rows;
+  }
+}
+
 }  // namespace
 
 // =========================================================================================
@@ -545,6 +569,14 @@ int32_t dgr_bloom2_build(const uint64_t* keys, int64_t cap, uint32_t* words, int
   dgr_note_launches(1);
   DGR_LAUNCH_CHECK();
   return DGR_OK;
+}
+
+/* Filter size of a table of n_max keys: about 10 bits per key, a power of two in [1024, 16384] words, so that it
+ * fits the 32768-word shared-memory limit of dgr_kmap_probe / dgr_kmap_dense. */
+int64_t dgr_bloom2_words(int64_t n_max) {
+  int64_t words = 1;
+  while (words < (n_max * 10 + 31) / 32) words <<= 1;
+  return words < 1024 ? 1024 : (words > 16384 ? 16384 : words);
 }
 
 /* words per offset of the bit-mask representation (one word per 32 output rows) */
@@ -647,6 +679,17 @@ int32_t dgr_kmap_dense(const int32_t* out_coords, int64_t n_out_max, const int32
         out_coords, n_out_dev, n_out_max, ncols, spec, in_keys, in_vals, (uint64_t)in_cap - 1, nullptr, 1u, offsets, K,
         k_per_block, nullptr, 0, nullptr, 0, nbr, nbr_stride, hit_count);
   }
+  dgr_note_launches(1);
+  DGR_LAUNCH_CHECK();
+  return DGR_OK;
+}
+
+int32_t dgr_kernel_map_tiles(const int32_t* kofs, int32_t K, int32_t tile_rows, int32_t n_tiles, int32_t pair,
+                             int32_t* tile_k, int32_t* tile_start, void* stream) {
+  DGR_ARG_CHECK(tile_rows >= 1, "tile_rows must be positive");
+  if (n_tiles == 0) return DGR_OK;
+  tiles_kernel<<<1, 1024, (K + 1) * sizeof(int), (cudaStream_t)stream>>>(kofs, K, tile_rows, n_tiles, pair, tile_k,
+                                                                        tile_start);
   dgr_note_launches(1);
   DGR_LAUNCH_CHECK();
   return DGR_OK;

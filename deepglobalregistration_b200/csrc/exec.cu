@@ -376,9 +376,7 @@ int32_t plan_begin(dgr_ctx* c, const dgr_net* net, Plan& p) {
   // miss filters for the kernel maps with many offsets per row (6-D: 729)
   const bool use_bloom = p.D > 3;
   if (use_bloom || net->conv1_ks > 3) {
-    int64_t words = next_pow2((n_max * 10 + 31) / 32);
-    if (words < 1024) words = 1024;
-    if (words > 16384) words = 16384;
+    const int64_t words = dgr_bloom2_words(n_max);
     for (int l = 0; l < (use_bloom ? 4 : 1); ++l) {       // 3-D: only the stride-1 table is probed with 5^3 / 7^3 offsets
       DGR_TRY(aalloc(c, words, &p.lv[l].bloom));
       p.lv[l].n_bloom = words;

@@ -5,8 +5,8 @@
 //                         kernel offset, input rows gathered with 16-byte cp.async into
 //                         shared memory, fp32 FFMA register tiles, vectorised
 //                         red.global.add.v4.f32 scatter.
-//   dgr_spconv_table_fwd  output-stationary kernel for conv1 (cin <= 8): walks the dense
-//                         neighbour table, weights in shared memory, fused BatchNorm.
+//   dgr_spconv_table_fwd_strided  output-stationary kernel for conv1 (cin <= 8): walks the
+//                         dense neighbour table, weights in shared memory, fused BatchNorm.
 //   dgr_linear_fwd        1x1 convolutions with fused concat / bias / ReLU / L2-normalise.
 //   dgr_affine_act, dgr_cat2, dgr_l2_normalize   elementwise layers.
 //
@@ -546,7 +546,7 @@ int32_t dgr_spconv_table_fwd_strided(const float* in_feat, int32_t cin, const fl
     spconv_table_kernel<16><<<blocks, kThreads, smem, st>>>(in_feat, cin, weight, nbr, K, n_out, nbr_stride, scale,
                                                            shift, out);
   else {
-    dgr_set_error("dgr_spconv_table_fwd: cout must be 16, 32 or 64 (got %d)", cout);
+    dgr_set_error("dgr_spconv_table_fwd_strided: cout must be 16, 32 or 64 (got %d)", cout);
     return DGR_ERR_ARG;
   }
   dgr_note_launches(1);
@@ -554,15 +554,9 @@ int32_t dgr_spconv_table_fwd_strided(const float* in_feat, int32_t cin, const fl
   return DGR_OK;
 }
 
-int32_t dgr_spconv_table_fwd(const float* in_feat, int32_t cin, const float* weight, int32_t cout,
-                             const int32_t* nbr, int32_t K, int64_t n_out, const float* scale,
-                             const float* shift, float* out, void* stream) {
-  return dgr_spconv_table_fwd_strided(in_feat, cin, weight, cout, nbr, K, n_out, n_out, scale, shift, out, stream);
-}
-
 // conv1 with one all-ones input channel from the kernel map's occupancy masks (dgr_kmap_probe's `bits`):
 //   out[j, :] = (sum over kappa with bit (kappa, j) set of weight[kappa, 0, :]) * scale + shift.
-// Same summation order over kappa as dgr_spconv_table_fwd on an all-ones input (bit-identical result).
+// Same summation order over kappa as dgr_spconv_table_fwd_strided on an all-ones input (bit-identical result).
 int32_t dgr_spconv_ones_bits_fwd(const float* weight, int32_t cout, const uint32_t* bits, int64_t mask_words, int32_t K,
                                  int64_t n_out, const float* scale, const float* shift, float* out, void* stream) {
   DGR_ARG_CHECK((scale == nullptr) == (shift == nullptr), "scale and shift go together");

@@ -184,7 +184,7 @@ int32_t dgr_spconv_os_supported(int32_t cin, int32_t cout) {
 
 // Output-stationary tensor-core convolution with the fused layer epilogue:
 //   out[j, :] = act((sum_kappa in_feat[nbr[kappa * nbr_stride + j], :] @ W[kappa]) * scale + shift + residual[j, :])
-// nbr: dense neighbour table (dgr_kmap_dense / dgr_kernel_map_table; -1 = no neighbour), weight_t: the packed TF32
+// nbr: dense neighbour table (dgr_kmap_dense; -1 = no neighbour), weight_t: the packed TF32
 // hi | lo slabs of dgr_pack_weight_tf32 (3xTF32, fp32-accurate).  scale / shift / residual may be NULL; `out` need
 // not be initialised and must not alias in_feat (it may alias nothing that is read).  Deterministic.
 int32_t dgr_spconv_os_fwd(const float* in_feat, int32_t cin, const float* weight_t, int32_t cout, const int32_t* nbr,

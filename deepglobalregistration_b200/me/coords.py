@@ -98,34 +98,28 @@ class CoordinateManager:
   def _map(self, stride):
     if stride not in self._maps:
       assert stride % 2 == 0 and stride > 1, f'no coordinate map at stride {stride}'
-      fine = self._map(stride // 2)
-      floored = _abi.stride_coords(fine.coords, stride)
-      table, sel, _, cnt = _abi.unique_first(floored, self.spec)
-      n = _abi.read_count(cnt)
-      self._maps[stride] = _Map(_abi.gather_rows_i32(floored, sel, n), table, n)
+      self._build_maps([stride])
     return self._maps[stride]
+
+  def _build_maps(self, strides):
+    """Coordinate maps at up to 4 `strides` with one host read, all derived from the stride-1 rows (floor(c / s) * s
+    composes, and ranking cells by their first stride-1 row reproduces the cascaded first-occurrence order)."""
+    coords, tables, n_out = _abi.coarse_maps(self._maps[1].coords, self.spec, strides)
+    *counts, overflow = torch.cat([n_out, self.spec[1:2]]).cpu().tolist()
+    _abi.D2H_BYTES += 4 * (len(strides) + 1)
+    if overflow:
+      raise _abi.DgrError('coordinate extent does not fit a 63-bit packed key')
+    for l, (s, n) in enumerate(zip(strides, counts)):
+      self._maps[s] = _Map(coords[l, :n], tables[l], n)
 
   def prepare(self, strides, maps):
     """Build every missing coordinate map of `strides` and every missing kernel map of `maps`
     ((s_in, conv_stride, kernel_size) triples) with TWO host reads in total instead of one per map:
-    all strided maps are derived from the stride-1 rows directly (floor(c / s) * s composes, and
-    ranking cells by their first stride-1 row reproduces the cascaded first-occurrence order), all
-    neighbour tables and bucket counts are enqueued before the single read that sizes them."""
-    base = self._maps[1]
+    all strided maps come from one read, all kernel-map probes are enqueued before the single read
+    that sizes their pair lists."""
     todo = [s for s in strides if s not in self._maps]
     if todo:
-      built = []
-      for s in todo:
-        floored = _abi.stride_coords(base.coords, s)
-        table, sel, _, cnt = _abi.unique_first(floored, self.spec)
-        built.append((s, floored, table, sel, cnt))
-      counts = torch.cat([b[4] for b in built]).cpu().tolist()
-      _abi.D2H_BYTES += 8 * len(built)
-      for i, (s, floored, table, sel, _) in enumerate(built):
-        n, overflow = counts[2 * i], counts[2 * i + 1]
-        if overflow:
-          raise _abi.DgrError('coordinate extent does not fit a 63-bit packed key')
-        self._maps[s] = _Map(_abi.gather_rows_i32(floored, sel, n), table, n)
+      self._build_maps(todo)
     pending, keys = [], []
     for slot, (s_in, conv_stride, ksize) in enumerate(maps):
       ck = (s_in, s_in * conv_stride, ksize)

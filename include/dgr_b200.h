@@ -99,49 +99,6 @@ int32_t dgr_hash_find(const int32_t* coords, int64_t n, int32_t ncols, const dgr
 int32_t dgr_gather_rows_i32(const int32_t* src, const int32_t* idx, int64_t n, int32_t ncols,
                             int32_t* out, void* stream);
 
-/* ---- strided coordinate maps: ME stride-2 convolution output map
- *      (model/resunet.py:461-507 conv2/conv3/conv4) --------------------------------- */
-/* out[r, 0] = in[r, 0]; out[r, c] = floor_div(in[r, c], out_stride) * out_stride. */
-int32_t dgr_stride_coords(const int32_t* coords, int64_t n, int32_t ncols, int32_t out_stride,
-                          int32_t* out, void* stream);
-
-/* ---- kernel maps: ME kernel_map for KernelGenerator(kernel_size, HYPER_CUBE)
- *      (model/residual_block.py:31-44,56-80) ----------------------------------------- */
-/* nbr[kappa * n_out + j] = row i of the input map with C_in[i] == C_out[j] + offsets[kappa]
- * or -1.  offsets is a DEVICE int32 [K, ncols-1] matrix (already scaled by the input
- * tensor stride), kappa enumerates axis 0 fastest.  block_cnt (optional, dgr_kmap_ws_elems
- * int32, zeroed by the call) receives the per-(kappa, 2048-row block) hit counts so that
- * dgr_kernel_map_count(counts_ready = 1) need not read the table again. */
-/* Optional miss filter of a table: bloom[bloom_bits / 32] words, one hashed bit per stored key
- * (bloom_bits a power of two, 16 x capacity recommended).  With it, dgr_kernel_map_table
- * answers most misses (99.7 % of the probes of a 6-D map) from L1. */
-int32_t dgr_bloom_build(const uint64_t* keys, int64_t cap, uint32_t* bloom, int64_t bloom_bits, void* stream);
-int32_t dgr_kernel_map_table(const int32_t* out_coords, int64_t n_out, int32_t ncols,
-                             const dgr_keyspec_t* spec, const uint64_t* in_keys,
-                             const int32_t* in_vals, int64_t in_cap, const uint32_t* bloom,
-                             int64_t bloom_bits, const int32_t* offsets, int32_t K, int32_t* nbr,
-                             int32_t* block_cnt, void* stream);
-/* Pair lists sorted by (kappa, j): two calls around one host read of kofs (kofs[K] = P).
- *   count: kofs[K+2] (device int32): exclusive offsets of every bucket, then the key-overflow
- *          flag of `spec` (may be NULL) so the same host read validates the keys; block_ws
- *          workspace of dgr_kmap_ws_elems(K, n_out) int32;
- *   fill : in_idx[P], out_idx[P]. */
-int64_t dgr_kmap_ws_elems(int32_t K, int64_t n_out);
-int32_t dgr_kernel_map_count(const int32_t* nbr, int32_t K, int64_t n_out, int32_t* block_ws,
-                             int32_t counts_ready, int32_t* kofs, const dgr_keyspec_t* spec, void* stream);
-int32_t dgr_kernel_map_fill(const int32_t* nbr, int32_t K, int64_t n_out, const int32_t* block_ws,
-                            int32_t* in_idx, int32_t* out_idx, void* stream);
-/* Work list of the gather-GEMM-scatter kernel: tile t covers pairs
- * [tile_start[t], min(tile_start[t] + tile_rows, kofs[tile_k[t] + 1])) of bucket tile_k[t].
- * n_tiles = sum_k ceil(count_k / tile_rows) is computed by the caller from kofs.  pair != 0
- * rounds every offset's tile count up to even (the extra tile is empty); the convolutions skip
- * empty tiles, so either list serves them. */
-int32_t dgr_kernel_map_tiles(const int32_t* kofs, int32_t K, int32_t tile_rows, int32_t n_tiles, int32_t pair,
-                             int32_t* tile_k, int32_t* tile_start, void* stream);
-/* Both lists (pair = 0 and pair = 1) in one launch. */
-int32_t dgr_kernel_map_tiles2(const int32_t* kofs, int32_t K, int32_t tile_rows, int32_t n_tiles, int32_t n_tiles_paired,
-                              int32_t* tile_k, int32_t* tile_start, int32_t* ptile_k, int32_t* ptile_start, void* stream);
-
 /* ---- sparse convolution forward: ME.MinkowskiConvolution / ConvolutionTranspose
  *      (model/residual_block.py:38-44,72-80; graph model/resunet.py:598-649) ---------- */
 /* out[out_idx[p], :] += in[in_idx[p], :] @ W[kappa(p)]   for all pairs p.
@@ -168,12 +125,6 @@ int32_t dgr_spconv_tc_fwd(const float* in_feat, int32_t cin, const float* weight
                           const int32_t* in_idx, const int32_t* out_idx, const int32_t* kofs,
                           const int32_t* tile_k, const int32_t* tile_start, int32_t n_tiles,
                           int32_t tile_rows, int32_t passes, float* out, void* stream);
-/* Output-stationary variant for few input channels (conv1: cin == 1): reads the dense
- * neighbour table, no atomics, optional fused per-channel affine (eval BatchNorm):
- *   out[j, :] = (sum_kappa in[nbr[kappa, j], :] @ W[kappa]) * scale + shift. */
-int32_t dgr_spconv_table_fwd(const float* in_feat, int32_t cin, const float* weight, int32_t cout,
-                             const int32_t* nbr, int32_t K, int64_t n_out, const float* scale,
-                             const float* shift, float* out, void* stream);
 /* kernel_size == 1 convolution (conv1_tr / final, model/resunet.py:578-596):
  *   out = act((concat(a, b) @ W[ca+cb, cout]) + bias), b may be NULL (cb = 0): fuses ME.cat.
  * relu != 0 applies ReLU; normalize != 0 divides every row by (||row||_2 + 1e-8)
@@ -316,8 +267,9 @@ int32_t dgr_fgr_feature_matching(const float* src, int64_t n_src, const float* t
  * Round 2: coordinate planning with device-side counts, and the native executor.
  * ====================================================================================== */
 
-/* Output-stationary conv1 kernel reading a neighbour table whose rows are nbr_stride apart
- * (dgr_spconv_table_fwd is the nbr_stride == n_out case). */
+/* Output-stationary variant of dgr_spconv_fwd for few input channels (conv1: cin <= 8): reads the dense
+ * neighbour table (rows nbr_stride apart), no atomics, optional fused per-channel affine (eval BatchNorm):
+ *   out[j, :] = (sum_kappa in[nbr[kappa * nbr_stride + j], :] @ W[kappa]) * scale + shift. */
 int32_t dgr_spconv_table_fwd_strided(const float* in_feat, int32_t cin, const float* weight, int32_t cout,
                                      const int32_t* nbr, int32_t K, int64_t n_out, int64_t nbr_stride,
                                      const float* scale, const float* shift, float* out, void* stream);
@@ -382,9 +334,15 @@ int32_t dgr_coarse_maps(const int32_t* fine, int64_t n_max, const int32_t* n_dev
                         const dgr_keyspec_t* spec, int32_t n_levels, const int32_t* strides, uint64_t* keys,
                         int32_t* vals, int64_t cap, int32_t* coords_out, int32_t* n_out, int32_t* slot_ws,
                         int32_t* scan_ws, void* stream);
-/* Blocked Bloom filter of a table (both bits of a key in one 32-bit word); n_words a power of two. */
+/* Blocked Bloom filter of a table (both bits of a key in one 32-bit word); n_words a power of two.  Kernel maps
+ * with many offsets per row (K > 27: 6-D maps, 5^3 / 7^3 kernels) miss on most probes and use one.
+ * dgr_bloom2_words(n_max): the filter size for a table of n_max keys (about 10 bits per key, 1024..16384 words). */
 int32_t dgr_bloom2_build(const uint64_t* keys, int64_t cap, uint32_t* words, int64_t n_words, void* stream);
-/* Kernel map, phase 1: bits[K][W] (W = dgr_kmap_mask_words(n_out_max)) holds one bit per (offset, output row),
+int64_t dgr_bloom2_words(int64_t n_max);
+/* Kernel map of KernelGenerator(kernel_size, HYPER_CUBE) (model/residual_block.py:31-44,56-80): the pairs
+ * (i, j) with C_in[i] == C_out[j] + offsets[kappa], sorted by (kappa, j).  offsets is a DEVICE int32
+ * [K, ncols-1] matrix (already scaled by the input tensor stride), kappa enumerates axis 0 fastest.
+ * Phase 1: bits[K][W] (W = dgr_kmap_mask_words(n_out_max)) holds one bit per (offset, output row),
  * block_cnt (dgr_kmap_cnt_elems ints) the exclusive-scanned per-(offset, 256-word block) pair counts,
  * kofs[K + 2] the bucket offsets + key-overflow flag, meta[5] = (pairs P, 128-row tiles, tiles with an even
  * count per offset, non-empty offsets, key overflow).  bloom_words (optional, <= 32768 words) is copied to
@@ -396,11 +354,18 @@ int32_t dgr_kmap_probe(const int32_t* out_coords, int64_t n_out_max, const int32
                        const uint32_t* bloom_words, int64_t n_bloom_words, const int32_t* offsets, int32_t K,
                        uint32_t* bits, int32_t* block_cnt, int32_t* kofs, int32_t* meta, void* stream);
 /* Kernel map, phase 2 (after the caller has read P from meta): in_idx[P], out_idx[P] sorted by (kappa, j),
- * bit-identical to dgr_kernel_map_fill. */
+ * the same lists as the oracle's buckets (oracle/sparse_ops.py). */
 int32_t dgr_kmap_fill(const uint32_t* bits, const int32_t* block_cnt, int32_t K, int64_t n_out_max,
                       const int32_t* out_coords, int32_t ncols, const dgr_keyspec_t* spec, const uint64_t* in_keys,
                       const int32_t* in_vals, int64_t in_cap, const int32_t* offsets, int32_t* in_idx,
                       int32_t* out_idx, void* stream);
+/* Work list of the gather-GEMM-scatter kernel: tile t covers pairs
+ * [tile_start[t], min(tile_start[t] + tile_rows, kofs[tile_k[t] + 1])) of bucket tile_k[t].
+ * n_tiles = sum_k ceil(count_k / tile_rows) (meta[1] of dgr_kmap_probe).  pair != 0 rounds every offset's tile
+ * count up to even (meta[2]; the extra tile is empty); the convolutions skip empty tiles, so either list serves
+ * them. */
+int32_t dgr_kernel_map_tiles(const int32_t* kofs, int32_t K, int32_t tile_rows, int32_t n_tiles, int32_t pair,
+                             int32_t* tile_k, int32_t* tile_start, void* stream);
 /* Dense neighbour table nbr[kappa * nbr_stride + j] (-1 = no neighbour) with a device-side row count;
  * bloom_words optional as in dgr_kmap_probe; hit_count (optional device int32, zeroed by the call) receives
  * the number of pairs P. */

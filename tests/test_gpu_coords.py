@@ -95,12 +95,18 @@ def test_strided_maps_bit_exact(abi, D):
   c = np.unique(g.integers(-40, 40, size=(6000, D)), axis=0)
   c = c[g.permutation(len(c))]
   coords = np.concatenate([np.zeros((len(c), 1), np.int64), c], 1).astype(np.int32)
-  man = _manager(abi, coords)
+  lazy = _manager(abi, coords)                  # one map per _map() call
+  planned = _manager(abi, coords)
+  planned.prepare([2, 4, 8], [])                # all three from one call
   cur = coords
   for s in (2, 4, 8):
     want, _ = so.stride_coords(cur, s)
-    got = man.coordinates(CoordinateMapKey(s)).cpu().numpy()
-    assert np.array_equal(got, want), f'stride {s}'
+    for man in (lazy, planned):
+      got = man.coordinates(CoordinateMapKey(s)).cpu().numpy()
+      assert np.array_equal(got, want), f'stride {s}'
+      # the table maps every coarse coordinate to its row
+      rows = abi.hash_find(torch.from_numpy(want).cuda(), man.spec, man._maps[s].table).cpu().numpy()
+      assert np.array_equal(rows, np.arange(len(want))), f'stride {s}'
     cur = want
 
 
@@ -120,6 +126,12 @@ def _check_kmap(km, buckets):
     assert kofs[k] <= s < e
     covered[s:e] += 1
   assert (covered[:km.n_pairs] == 1).all()
+  if km.nbr is not None:
+    # the dense neighbour table kept for the conv1 table kernel: nbr[kappa, j] = i of every pair, otherwise -1
+    want = np.full((len(buckets), km.n_out), -1, np.int32)
+    for kap, (wi, wj) in enumerate(buckets):
+      want[kap, wj] = wi
+    assert np.array_equal(km.nbr.cpu().numpy(), want)
 
 
 @pytest.mark.parametrize('D,ks', [(3, 3), (3, 5), (3, 7), (6, 3)])
@@ -132,6 +144,7 @@ def test_kernel_maps_bit_exact(abi, D, ks):
   coords = np.concatenate([np.zeros((len(c), 1), np.int64), c], 1).astype(np.int32)
   man = _manager(abi, coords)
   _, km = man.kernel_map(CoordinateMapKey(1), 1, ks)
+  assert (km.nbr is not None) == (D == 3 and ks > 3)
   _check_kmap(km, so.kernel_map(coords, coords, so.kernel_offsets(ks, D, 1)))
   if ks == 3:
     # stride-2 map and its transposed use, then the 3^D map on the coarse level

@@ -1,5 +1,5 @@
 """Round-2 native layer: coordinate planning with device-side counts (csrc/coordplan.cu) and the native
-executor (csrc/exec.cu) against the round-1 operator path and the CPU oracle.
+executor (csrc/exec.cu) against the operator path and the CPU oracle.
 
 Integer work is bit-exact (coarse maps, kernel-map pair lists, voxel selection); floating point within the
 stated tolerances (atomic scatter-add order differs between runs: 2e-5 relative)."""
@@ -106,15 +106,32 @@ def _new_kmap(abi, out_coords, n_out_max, n_out_dev, spec, table, offsets, bloom
   return kofs.cpu().numpy(), in_idx[:P].cpu().numpy(), out_idx[:P].cpu().numpy(), m
 
 
+def _bucket_offsets(buckets):
+  return np.concatenate([[0], np.cumsum([len(b[0]) for b in buckets])])
+
+
+def _dense_table(buckets, n_out):
+  """nbr[kappa, j] = i for every pair of bucket kappa, otherwise -1."""
+  nbr = np.full((len(buckets), n_out), -1, np.int32)
+  for kap, (i, j) in enumerate(buckets):
+    nbr[kap, j] = i
+  return nbr
+
+
 @pytest.mark.parametrize('D,ks,n,ext,bloom', [(3, 3, 9000, 16, False), (3, 5, 3000, 9, False), (6, 3, 6000, 3, True),
                                               (6, 3, 6000, 3, False), (3, 3, 30, 2, False)])
-def test_kernel_map_bits_equal_round1_builder(abi, D, ks, n, ext, bloom):
-  from deepglobalregistration_b200.me.coords import CoordinateMapKey, kernel_offsets
+def test_kernel_map_bits_equal_oracle_buckets(abi, D, ks, n, ext, bloom):
+  from deepglobalregistration_b200.me.coords import kernel_offsets
   coords = _cloud(D, n, ext, seed=ks + n)
   ct = torch.from_numpy(coords).cuda().contiguous()
   man, spec, table = _spec_and_table(abi, ct)
-  _, km = man.kernel_map(CoordinateMapKey(1), 1, ks)
   offs = kernel_offsets(ks, D, 1, torch.device('cuda'))
+  buckets = so.kernel_map(coords, coords, so.kernel_offsets(ks, D, 1))
+  want_kofs = _bucket_offsets(buckets)
+  counts = np.diff(want_kofs)
+  tiles = (counts + 127) // 128
+  want_i = np.concatenate([b[0] for b in buckets])
+  want_j = np.concatenate([b[1] for b in buckets])
   nreal = len(coords)
   for extra in (0, 1500):
     n_max = nreal + extra
@@ -122,15 +139,11 @@ def test_kernel_map_bits_equal_round1_builder(abi, D, ks, n, ext, bloom):
     n_dev = torch.tensor([nreal], dtype=torch.int32, device='cuda')
     kofs, ii, jj, meta = _new_kmap(abi, oc, n_max, n_dev, spec, table, offs, bloom)
     K = ks ** D
-    assert np.array_equal(kofs[:K + 1], km.kofs_host)
-    assert meta[0] == km.n_pairs and meta[1] == km.n_tiles and meta[4] == 0
-    assert meta[3] == int((np.diff(km.kofs_host) > 0).sum())
-    assert np.array_equal(ii, km.in_idx[:km.n_pairs].cpu().numpy())
-    assert np.array_equal(jj, km.out_idx[:km.n_pairs].cpu().numpy())
-  # and against the oracle's buckets
-  buckets = so.kernel_map(coords, coords, so.kernel_offsets(ks, D, 1))
-  assert np.array_equal(ii, np.concatenate([b[0] for b in buckets]))
-  assert np.array_equal(jj, np.concatenate([b[1] for b in buckets]))
+    assert np.array_equal(kofs[:K + 1], want_kofs)
+    assert meta[0] == want_kofs[-1] and meta[1] == tiles.sum() and meta[2] == ((tiles + 1) // 2 * 2).sum()
+    assert meta[3] == int((counts > 0).sum()) and meta[4] == 0
+    assert np.array_equal(ii, want_i)
+    assert np.array_equal(jj, want_j)
 
 
 def test_strided_kernel_map_and_dense_table(abi):
@@ -143,19 +156,24 @@ def test_strided_kernel_map_and_dense_table(abi):
   offs = kernel_offsets(3, 3, 1, torch.device('cuda'))
   n2 = coarse.shape[0]
   kofs, ii, jj, meta = _new_kmap(abi, coarse, n2, None, spec, table, offs, False)
-  assert np.array_equal(kofs[:28], km.kofs_host) and np.array_equal(ii, km.in_idx[:km.n_pairs].cpu().numpy())
+  down = so.kernel_map(coords, coarse.cpu().numpy(), so.kernel_offsets(3, 3, 1))
+  assert np.array_equal(kofs[:28], _bucket_offsets(down)) and np.array_equal(kofs[:28], km.kofs_host)
+  assert np.array_equal(ii, np.concatenate([b[0] for b in down]))
+  assert np.array_equal(jj, np.concatenate([b[1] for b in down]))
+  assert np.array_equal(ii, km.in_idx[:km.n_pairs].cpu().numpy())
   assert np.array_equal(jj, km.out_idx[:km.n_pairs].cpu().numpy())
   # dense table with a row stride and a device count
-  _, km7 = man.kernel_map(CoordinateMapKey(1), 1, 7)
   offs7 = kernel_offsets(7, 3, 1, torch.device('cuda'))
   n = len(coords)
+  b7 = so.kernel_map(coords, coords, so.kernel_offsets(7, 3, 1))
+  want = torch.from_numpy(_dense_table(b7, n)).cuda()
   stride = n + 100
   nbr = torch.full((343, stride), -5, dtype=torch.int32, device='cuda')
   n_dev = torch.tensor([n], dtype=torch.int32, device='cuda')
   padded = _padded(coords, 100)
   abi.call('dgr_kmap_dense', abi.ptr(padded), n + 100, abi.ptr(n_dev), 4, abi.ptr(spec), abi.ptr(table.keys),
            abi.ptr(table.vals), table.cap, None, 0, abi.ptr(offs7), 343, abi.ptr(nbr), stride, None, abi.stream())
-  assert torch.equal(nbr[:, :n], km7.nbr) and bool((nbr[:, n:] == -5).all())
+  assert torch.equal(nbr[:, :n], want) and bool((nbr[:, n:] == -5).all())
   # with the shared-memory miss filter
   words = torch.empty(2048, dtype=torch.int32, device='cuda')
   abi.call('dgr_bloom2_build', abi.ptr(table.keys), table.cap, abi.ptr(words), 2048, abi.stream())
@@ -164,8 +182,8 @@ def test_strided_kernel_map_and_dense_table(abi):
   abi.call('dgr_kmap_dense', abi.ptr(padded), n + 100, abi.ptr(n_dev), 4, abi.ptr(spec), abi.ptr(table.keys),
            abi.ptr(table.vals), table.cap, abi.ptr(words), 2048, abi.ptr(offs7), 343, abi.ptr(nbr2), stride, abi.ptr(hits),
            abi.stream())
-  assert torch.equal(nbr2[:, :n], km7.nbr) and bool((nbr2[:, n:] == -5).all())
-  assert int(hits) == km7.n_pairs
+  assert torch.equal(nbr2[:, :n], want) and bool((nbr2[:, n:] == -5).all())
+  assert int(hits) == sum(len(b[0]) for b in b7)
 
 
 @pytest.fixture(scope='module')

@@ -1,6 +1,6 @@
-"""Repeat the round-1 and the round-2 kernel-map builders on one cloud and compare every run with the first
-(and the two builders with each other, and bucket kappa with its mirror K-1-kappa): a race shows up as a run
-that differs.  Usage: python tools/kmap_determinism.py [reps]   (also meant to run under compute-sanitizer)."""
+"""Build the same kernel map repeatedly on one cloud and compare every run with the first (and bucket kappa with its
+mirror K-1-kappa, which holds the same number of pairs): a race shows up as a run that differs.
+Usage: python tools/kmap_determinism.py [reps]"""
 import os
 import sys
 
@@ -8,8 +8,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 
-from deepglobalregistration_b200 import _abi as abi
-from deepglobalregistration_b200.me.coords import CoordinateManager, CoordinateMapKey, kernel_offsets
+from deepglobalregistration_b200.me.coords import CoordinateManager, CoordinateMapKey
 
 reps = int(sys.argv[1]) if len(sys.argv) > 1 else 5
 g = np.random.default_rng(3 + 9000)
@@ -17,38 +16,17 @@ c = np.unique(g.integers(-16, 16, size=(9000, 3)), axis=0)
 c = c[g.permutation(len(c))]
 coords = np.concatenate([np.zeros((len(c), 1), np.int64), c], 1).astype(np.int32)
 ct = torch.from_numpy(coords).cuda().contiguous()
-n = len(coords)
-offs = kernel_offsets(3, 3, 1, torch.device('cuda'))
 ok = True
-first_old = first_new = None
+first = None
 for r in range(reps):
   man = CoordinateManager(ct, assume_unique=True)
-  table, spec = man._maps[1].table, man.spec
   _, km = man.kernel_map(CoordinateMapKey(1), 1, 3)
-  old = (km.kofs_host.copy(), km.in_idx[:km.n_pairs].cpu().numpy(), km.out_idx[:km.n_pairs].cpu().numpy())
-  K = 27
-  W = abi.lib().dgr_kmap_mask_words(n)
-  bits = torch.empty(K * W, dtype=torch.int32, device='cuda')
-  cnt = torch.empty(abi.lib().dgr_kmap_cnt_elems(K, n), dtype=torch.int32, device='cuda')
-  kofs = torch.empty(K + 2, dtype=torch.int32, device='cuda')
-  meta = torch.empty(5, dtype=torch.int32, device='cuda')
-  abi.call('dgr_kmap_probe', abi.ptr(ct), n, None, 4, abi.ptr(spec), abi.ptr(table.keys), abi.ptr(table.vals), table.cap,
-           None, 0, abi.ptr(offs), K, abi.ptr(bits), abi.ptr(cnt), abi.ptr(kofs), abi.ptr(meta), abi.stream())
-  P = int(meta.cpu()[0])
-  ii = torch.empty(max(P, 1), dtype=torch.int32, device='cuda')
-  jj = torch.empty(max(P, 1), dtype=torch.int32, device='cuda')
-  abi.call('dgr_kmap_fill', abi.ptr(bits), abi.ptr(cnt), K, n, abi.ptr(ct), 4, abi.ptr(spec), abi.ptr(table.keys),
-           abi.ptr(table.vals), table.cap, abi.ptr(offs), abi.ptr(ii), abi.ptr(jj), abi.stream())
-  torch.cuda.synchronize()
-  new = (kofs.cpu().numpy()[:K + 1], ii[:P].cpu().numpy(), jj[:P].cpu().numpy())
-  cnt_old, cnt_new = np.diff(old[0]), np.diff(new[0])
-  sym_old, sym_new = bool(np.array_equal(cnt_old, cnt_old[::-1])), bool(np.array_equal(cnt_new, cnt_new[::-1]))
-  same = all(np.array_equal(a, b) for a, b in zip(old, new))
-  print(f'rep {r}: P old {old[0][-1]} new {new[0][-1]} builders equal {same} mirror-symmetric old {sym_old} new {sym_new}',
-        flush=True)
-  if first_old is None:
-    first_old, first_new = old, new
-  else:
-    ok &= all(np.array_equal(a, b) for a, b in zip(old, first_old)) and all(np.array_equal(a, b) for a, b in zip(new, first_new))
-  ok &= same and sym_old and sym_new
+  run = (km.kofs_host.copy(), km.in_idx[:km.n_pairs].cpu().numpy(), km.out_idx[:km.n_pairs].cpu().numpy(),
+         km.tile_k[:km.n_tiles].cpu().numpy(), km.tile_start[:km.n_tiles].cpu().numpy())
+  counts = np.diff(run[0])
+  sym = bool(np.array_equal(counts, counts[::-1]))
+  same = first is None or all(np.array_equal(a, b) for a, b in zip(run, first))
+  print(f'rep {r}: P {run[0][-1]} equal to run 0 {same} mirror-symmetric {sym}', flush=True)
+  first = first or run
+  ok &= same and sym
 print('DETERMINISM', 'PASS' if ok else 'FAIL')
