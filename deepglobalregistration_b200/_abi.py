@@ -55,6 +55,9 @@ SIGNATURES = {
     'dgr_inlier_coords': [_p, _p, _p, _i64, _p, _p],
     'dgr_sigmoid_clip_sum': [_p, _i64, _f32, _p, _p, _p],
     'dgr_icp_point_to_point': [_p, _i64, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _p, _i32, _f64, _f64, _p, _p, _p],
+    'dgr_estimate_normals': [_p, _i64, _p, _p, _p, _i64, _i32, _f64, _f64, _i32, _p, _p, _p, _p],
+    'dgr_icp_plane_ws_elems': [_i64, _p],
+    'dgr_icp_point_to_plane': [_p, _i64, _p, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _p, _i32, _f64, _f64, _p, _p, _p],
     'dgr_ransac_ws_elems': [_i64, _i64, _p],
     'dgr_ransac_correspondence': [_p, _p, _p, _p, _i64, _f64, _i64, C.c_uint64, _p, _p, _p],
     'dgr_ransac_fm_ws_elems': [_i64, _i64, _i64, _p],
@@ -646,6 +649,59 @@ def icp_point_to_point(src, tgt, tgt_manager, voxel, max_dist, T_init, max_iter=
   call('dgr_icp_point_to_point', ptr(src), src.shape[0], ptr(tgt), ptr(tgt_manager.spec), ptr(m.table.keys),
        ptr(m.table.vals), m.table.cap, int(batch), float(voxel), float(max_dist), ptr(T_init), int(max_iter),
        float(rel_fitness), float(rel_rmse), ptr(state), ptr(res), stream())
+  return res
+
+
+MAX_NN = 64            # dgr_estimate_normals' bound on the neighbours per point
+
+
+def _hash_of(manager_or_table):
+  """(spec, table) of a CoordinateManager (its stride-1 table) or of a (spec, table) pair."""
+  if hasattr(manager_or_table, '_maps'):
+    return manager_or_table.spec, manager_or_table._maps[1].table
+  spec, table = manager_or_table
+  return spec, table
+
+
+def estimate_normals(xyz, manager_or_table, cell, radius, max_nn, prev=None, return_counts=False, batch=0):
+  """Normals of xyz (CUDA float32 [n, 3]) from its neighbours strictly within `radius`, at most `max_nn` (<= 64) of
+  them by (d^2, row), searched through the cloud's own voxel hash at `cell` (a CoordinateManager preprocess() built,
+  or (spec, table) of a dgr_unique_first table; one point per cell, batch column `batch`).  prev: CUDA float32
+  [n, 3] normals to orient against.  -> float32 [n, 3] (and the int32 [n] counts within the radius)."""
+  _chk(xyz, torch.float32, 'xyz')
+  if prev is not None:
+    _chk(prev, torch.float32, 'prev')
+    if prev.shape != xyz.shape:
+      raise DgrError('prev must hold one normal per point')
+  spec, table = _hash_of(manager_or_table)
+  n = xyz.shape[0]
+  normals = torch.empty(n, 3, dtype=torch.float32, device=xyz.device)
+  counts = torch.empty(max(n, 1), dtype=torch.int32, device=xyz.device)[:n]
+  call('dgr_estimate_normals', ptr(xyz), n, ptr(spec), ptr(table.keys), ptr(table.vals), table.cap, int(batch),
+       float(cell), float(radius), int(max_nn), ptr(prev), ptr(normals), ptr(counts), stream())
+  return (normals, counts) if return_counts else normals
+
+
+def icp_point_to_plane(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter=30, rel_fitness=1e-6,
+                       rel_rmse=1e-6, batch=0):
+  """Point-to-plane ICP (open3d's TransformationEstimationPointToPlane, default criteria) of src onto tgt through
+  tgt's voxel hash; arguments as icp_point_to_point plus tgt_normals (CUDA float32 [n_tgt, 3]); tgt_manager may
+  also be a (spec, table) pair.  -> device double [20] (pose 16, fitness, inlier RMSE, iterations,
+  correspondences)."""
+  _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt'); _chk(tgt_normals, torch.float32, 'tgt_normals')
+  if tgt_normals.shape != tgt.shape:
+    raise DgrError('tgt_normals must hold one normal per target point')
+  dev = src.device
+  spec, table = _hash_of(tgt_manager)
+  if not (isinstance(T_init, torch.Tensor) and T_init.is_cuda and T_init.numel() == 12):
+    T_init = torch.as_tensor(T_init, dtype=torch.float64).reshape(4, 4)[:3].contiguous().to(dev)
+  words = C.c_int64(0)
+  call('dgr_icp_plane_ws_elems', src.shape[0], C.byref(words))
+  ws = scratch('icp_plane', words.value, torch.float64, dev)
+  res = torch.empty(20, dtype=torch.float64, device=dev)
+  call('dgr_icp_point_to_plane', ptr(src), src.shape[0], ptr(tgt), ptr(tgt_normals), ptr(spec), ptr(table.keys),
+       ptr(table.vals), table.cap, int(batch), float(voxel), float(max_dist), ptr(T_init), int(max_iter),
+       float(rel_fitness), float(rel_rmse), ptr(ws), ptr(res), stream())
   return res
 
 

@@ -20,6 +20,7 @@
 #include <stdint.h>
 
 #include "common.cuh"
+#include "kabsch.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -281,38 +282,6 @@ __device__ __forceinline__ void fgr_allreduce(FgrShared& sh, double (&v)[kNv], i
   parity ^= 1;
 }
 
-// x = -(A^-1 g) by Cholesky of the symmetric A (upper triangle a[21], row-major); false on a non-positive pivot
-__device__ bool fgr_cholesky_step(const double* a, const double* g, double x[6]) {
-  double L[6][6];
-  int k = 0;
-  double A[6][6];
-  for (int r = 0; r < 6; ++r)
-    for (int c = r; c < 6; ++c) { A[r][c] = a[k]; A[c][r] = a[k]; ++k; }
-  for (int j = 0; j < 6; ++j) {
-    double d = A[j][j];
-    for (int m = 0; m < j; ++m) d -= L[j][m] * L[j][m];
-    if (!(d > 0.0)) return false;
-    L[j][j] = sqrt(d);
-    for (int i = j + 1; i < 6; ++i) {
-      double e = A[i][j];
-      for (int m = 0; m < j; ++m) e -= L[i][m] * L[j][m];
-      L[i][j] = e / L[j][j];
-    }
-  }
-  double y[6];
-  for (int i = 0; i < 6; ++i) {
-    double e = -g[i];
-    for (int m = 0; m < i; ++m) e -= L[i][m] * y[m];
-    y[i] = e / L[i][i];
-  }
-  for (int i = 5; i >= 0; --i) {
-    double e = y[i];
-    for (int m = i + 1; m < 6; ++m) e -= L[m][i] * x[m];
-    x[i] = e / L[i][i];
-  }
-  return true;
-}
-
 template <int CS>
 __global__ void __launch_bounds__(kFgrSolveThreads, 1)
 fgr_solve_kernel(const float* __restrict__ src, const float* __restrict__ tgt, const int32_t* __restrict__ nn_st,
@@ -388,21 +357,9 @@ fgr_solve_kernel(const float* __restrict__ src, const float* __restrict__ tgt, c
     fgr_allreduce<CS>(sh, v, parity);
     if (tid == 0) {
       double x[6];
-      if (!fgr_cholesky_step(sh.tot, sh.tot + 21, x))
+      if (!cholesky6_step(sh.tot, sh.tot + 21, x))
         for (int k = 0; k < 6; ++k) x[k] = 0.0;
-      // delta = [Rz(gamma) Ry(beta) Rx(alpha) | x[3..6)], composed on the left
-      const double ca = cos(x[0]), sa = sin(x[0]), cb = cos(x[1]), sb = sin(x[1]), cc = cos(x[2]), sc = sin(x[2]);
-      const double Rz[3][3] = {{cc, -sc, 0.0}, {sc, cc, 0.0}, {0.0, 0.0, 1.0}};
-      const double Ry[3][3] = {{cb, 0.0, sb}, {0.0, 1.0, 0.0}, {-sb, 0.0, cb}};
-      const double Rx[3][3] = {{1.0, 0.0, 0.0}, {0.0, ca, -sa}, {0.0, sa, ca}};
-      double Rzy[3][3], D[3][3];
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) Rzy[r][c] = Rz[r][0] * Ry[0][c] + Rz[r][1] * Ry[1][c] + Rz[r][2] * Ry[2][c];
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) D[r][c] = Rzy[r][0] * Rx[0][c] + Rzy[r][1] * Rx[1][c] + Rzy[r][2] * Rx[2][c];
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 4; ++c)
-          sh.T[4 * r + c] = D[r][0] * T[c] + D[r][1] * T[4 + c] + D[r][2] * T[8 + c] + (c == 3 ? x[3 + r] : 0.0);
+      zyx_update_left(x, T, sh.T);                      // delta = [Rz(gamma) Ry(beta) Rx(alpha) | x[3..6)], on the left
     }
     __syncthreads();
   }

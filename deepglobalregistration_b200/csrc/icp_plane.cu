@@ -1,0 +1,393 @@
+// Normal estimation and point-to-plane ICP: open3d 0.10's EstimateNormals(KDTreeSearchParamHybrid(radius, max_nn))
+// and RegistrationICP with TransformationEstimationPointToPlane, restated in oracle/normals.py and oracle/icp.py
+// (which pin every boundary convention).  Both search the cloud's own voxel hash (a dgr_unique_first table with at
+// most one point per cell): the (2 reach + 1)^3 cells around a point, reach = ceil(radius / cell) <= 4, 8 lanes per
+// point as in dgr_voxel_nearest8.  No atomics: every sum has a fixed order, so a call gives the same bits on every
+// run.
+//   normals_kernel           8 lanes per point, one probe pass: count and fp64 cumulants of the offsets p_j - p_i of
+//                            the rows with |p_j - p_i|^2 < radius^2; a point with <= max_nn of them gets its normal
+//   normals_select_kernel    a warp per point with more than max_nn: the in-radius rows again, in cell order, into
+//                            shared memory; the max_nn smallest (d^2, row) keys by rank; their cumulants
+//   icp_plane_match_kernel   nearest target row within max_dist (dgr_voxel_nearest8); J = [s x n, n], r = (s - q).n;
+//                            the 21 + 6 normal-equation sums, the count and sum d^2 as per-block partials
+//   icp_plane_update_kernel  the partials reduced in block order, open3d's stopping rule, the 6x6 Cholesky step
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "common.cuh"
+#include "kabsch.cuh"
+
+namespace {
+
+constexpr int kNormThreads = 256;
+constexpr int kSelWarps = 4;                            // normals_select_kernel: warps (points) per block
+constexpr int kMaxNN = 64;
+constexpr int kPlaneThreads = 256;
+constexpr int kPlaneMaxBlocks = 2368;
+constexpr int kPlaneNv = 29;                            // J^T J upper triangle (21), J^T r (6), count, sum d^2
+constexpr int kPlaneStride = 32;                        // doubles per block partial
+constexpr int kPlaneState = 32;                         // doubles of IcpPlaneState (static_assert below)
+
+// The cell probe of dgr_voxel_nearest8: row in cell c of the block around cell c3, or -1
+__device__ __forceinline__ int32_t cell_row(int c, int side, int reach, const int c3[3], int32_t batch,
+                                            const dgr_keyspec_t& s, const uint64_t* __restrict__ keys,
+                                            const int32_t* __restrict__ vals, uint64_t mask) {
+  const int dx = c % side - reach, dy = (c / side) % side - reach, dz = c / (side * side) - reach;
+  const int32_t row[4] = {batch, c3[0] + dx, c3[1] + dy, c3[2] + dz};
+  bool inside = true;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const long long d = (long long)row[q] - s.lo[q];
+    inside = inside && d >= 0 && d < (1ll << s.bits[q]);
+  }
+  if (!inside) return -1;
+  return dgr_hash_lookup(keys, vals, mask, dgr_pack_key(row, s));
+}
+
+// offset e = p_j - p_i and d2 = |e|^2 evaluated as numpy does ((ex ex + ey ey) + ez ez, no contraction), so that
+// the strict radius test and the (d^2, row) order agree with the oracle bit for bit
+__device__ __forceinline__ double offset_d2(const float* __restrict__ xyz, int32_t j, const double p[3], double e[3]) {
+#pragma unroll
+  for (int a = 0; a < 3; ++a) e[a] = __dsub_rn((double)__ldg(xyz + 3 * (int64_t)j + a), p[a]);
+  return __dadd_rn(__dadd_rn(__dmul_rn(e[0], e[0]), __dmul_rn(e[1], e[1])), __dmul_rn(e[2], e[2]));
+}
+
+// m[0..3) += e, m[3..9) += e e^T (xx, xy, xz, yy, yz, zz)
+__device__ __forceinline__ void add_cumulants(double m[9], const double e[3]) {
+  m[0] += e[0]; m[1] += e[1]; m[2] += e[2];
+  m[3] += e[0] * e[0]; m[4] += e[0] * e[1]; m[5] += e[0] * e[2];
+  m[6] += e[1] * e[1]; m[7] += e[1] * e[2]; m[8] += e[2] * e[2];
+}
+
+// open3d's ComputeNormal on the cumulant sums of n neighbours: C = E[e e^T] - mu mu^T, the eigenvector of the
+// smallest eigenvalue (one-sided Jacobi, kabsch.cuh; the first on a tie); (0, 0, 1) for n < 3 or C == 0.
+// Sign: the largest-magnitude component made positive (the first on a tie) - a fixed rule, not open3d's - then,
+// with previous normals, flipped when it points against the previous one (open3d's rule).
+__device__ void store_normal(const double m[9], int n, const float* __restrict__ prev, int64_t i,
+                             float* __restrict__ normals) {
+  double nv[3] = {0.0, 0.0, 1.0};
+  if (n >= 3) {
+    const double inv = 1.0 / (double)n;
+    const double mu[3] = {m[0] * inv, m[1] * inv, m[2] * inv};
+    const double cxx = m[3] * inv - mu[0] * mu[0], cxy = m[4] * inv - mu[0] * mu[1], cxz = m[5] * inv - mu[0] * mu[2];
+    const double cyy = m[6] * inv - mu[1] * mu[1], cyz = m[7] * inv - mu[1] * mu[2], czz = m[8] * inv - mu[2] * mu[2];
+    if (cxx != 0.0 || cxy != 0.0 || cxz != 0.0 || cyy != 0.0 || cyz != 0.0 || czz != 0.0) {
+      const double C[3][3] = {{cxx, cxy, cxz}, {cxy, cyy, cyz}, {cxz, cyz, czz}};
+      double A[3][3], V[3][3], sig[3];
+      jacobi_svd3(C, A, V, sig);
+      int k = 0;
+      if (sig[1] < sig[k]) k = 1;
+      if (sig[2] < sig[k]) k = 2;
+      for (int a = 0; a < 3; ++a) nv[a] = V[a][k];
+      int big = 0;
+      if (fabs(nv[1]) > fabs(nv[big])) big = 1;
+      if (fabs(nv[2]) > fabs(nv[big])) big = 2;
+      if (nv[big] < 0.0)
+        for (int a = 0; a < 3; ++a) nv[a] = -nv[a];
+    }
+  }
+  if (prev != nullptr) {
+    const double d = nv[0] * (double)prev[3 * i] + nv[1] * (double)prev[3 * i + 1] + nv[2] * (double)prev[3 * i + 2];
+    if (d < 0.0)
+      for (int a = 0; a < 3; ++a) nv[a] = -nv[a];
+  }
+  for (int a = 0; a < 3; ++a) normals[3 * i + a] = (float)nv[a];
+}
+
+__global__ void __launch_bounds__(kNormThreads)
+normals_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspec_t* __restrict__ spec_p,
+               const uint64_t* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask, int32_t batch,
+               double cell, int reach, double r2, int max_nn, const float* __restrict__ prev,
+               float* __restrict__ normals, int32_t* __restrict__ counts) {
+  const dgr_keyspec_t s = *spec_p;
+  const int64_t i0 = ((int64_t)blockIdx.x * kNormThreads + threadIdx.x) >> 3;
+  const int sub = threadIdx.x & 7;
+  const bool have = i0 < n;                             // whole warps stay for the shuffles
+  const int64_t i = have ? i0 : 0;
+  const double p[3] = {(double)xyz[3 * i], (double)xyz[3 * i + 1], (double)xyz[3 * i + 2]};
+  const int side = 2 * reach + 1, n_cells = side * side * side;
+  int c3[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) c3[a] = (int)floor(p[a] / cell);
+  int cnt = 0;
+  double m[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+  for (int c = sub; c < n_cells && have; c += 8) {
+    const int32_t j = cell_row(c, side, reach, c3, batch, s, keys, vals, mask);
+    if (j < 0) continue;
+    double e[3];
+    if (offset_d2(xyz, j, p, e) < r2) {
+      ++cnt;
+      add_cumulants(m, e);
+    }
+  }
+#pragma unroll
+  for (int d = 1; d < 8; d <<= 1) {                     // fixed butterfly within the group of 8
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, d);
+#pragma unroll
+    for (int k = 0; k < 9; ++k) m[k] += __shfl_xor_sync(0xffffffffu, m[k], d);
+  }
+  if (!have || sub != 0) return;
+  counts[i] = cnt;
+  if (cnt <= max_nn) store_normal(m, cnt, prev, i, normals);
+}
+
+// (d2, row) of a before b
+__device__ __forceinline__ bool key_less(double da, int32_t ja, double db, int32_t jb) {
+  return da < db || (da == db && ja < jb);
+}
+
+__global__ void __launch_bounds__(kSelWarps * 32)
+normals_select_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspec_t* __restrict__ spec_p,
+                      const uint64_t* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask,
+                      int32_t batch, double cell, int reach, double r2, int max_nn, const float* __restrict__ prev,
+                      float* __restrict__ normals, const int32_t* __restrict__ counts) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int side = 2 * reach + 1, n_cells = side * side * side;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t i = (int64_t)blockIdx.x * kSelWarps + warp;
+  if (i >= n || counts[i] <= max_nn) return;            // uniform per warp
+  double* kd = reinterpret_cast<double*>(smem_raw) + (size_t)warp * n_cells;
+  int32_t* kj = reinterpret_cast<int32_t*>(reinterpret_cast<double*>(smem_raw) + (size_t)kSelWarps * n_cells) +
+                (size_t)warp * n_cells;
+  const dgr_keyspec_t s = *spec_p;
+  const double p[3] = {(double)xyz[3 * i], (double)xyz[3 * i + 1], (double)xyz[3 * i + 2]};
+  int c3[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) c3[a] = (int)floor(p[a] / cell);
+  // the in-radius rows in cell order (ordered append: ballot + prefix popcount)
+  int m_cnt = 0;
+  for (int c0 = 0; c0 < n_cells; c0 += 32) {
+    const int c = c0 + lane;
+    int32_t j = c < n_cells ? cell_row(c, side, reach, c3, batch, s, keys, vals, mask) : -1;
+    double d2 = 0.0;
+    if (j >= 0) {
+      double e[3];
+      d2 = offset_d2(xyz, j, p, e);
+      if (!(d2 < r2)) j = -1;
+    }
+    const unsigned ball = __ballot_sync(0xffffffffu, j >= 0);
+    if (j >= 0) {
+      const int pos = m_cnt + __popc(ball & ((1u << lane) - 1u));
+      kd[pos] = d2;
+      kj[pos] = j;
+    }
+    m_cnt += __popc(ball);
+  }
+  __syncwarp();
+  // candidate k is kept when fewer than max_nn keys rank before it (keys are distinct: rows are)
+  double mm[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+  for (int k = lane; k < m_cnt; k += 32) {
+    const double dk = kd[k];
+    const int32_t jk = kj[k];
+    int rank = 0;
+    for (int l = 0; l < m_cnt; ++l) rank += key_less(kd[l], kj[l], dk, jk);
+    if (rank < max_nn) {
+      double e[3];
+      offset_d2(xyz, jk, p, e);
+      add_cumulants(mm, e);
+    }
+  }
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1)
+#pragma unroll
+    for (int k = 0; k < 9; ++k) mm[k] += __shfl_xor_sync(0xffffffffu, mm[k], d);
+  if (lane == 0) store_normal(mm, max_nn, prev, i, normals);
+}
+
+// ---------------------------------------------------------------------------------------
+// point-to-plane ICP
+// ---------------------------------------------------------------------------------------
+struct IcpPlaneState {
+  double T[12];          // current pose, row-major [R | t]
+  double prev_fitness, prev_rmse, fitness, rmse, n_corr;
+  int iteration, done;
+};
+
+__global__ void icp_plane_init_kernel(const double* __restrict__ T_init, IcpPlaneState* st) {
+  if (threadIdx.x == 0 && blockIdx.x == 0) {
+    for (int k = 0; k < 12; ++k) st->T[k] = T_init[k];
+    st->prev_fitness = st->prev_rmse = st->fitness = st->rmse = st->n_corr = 0.0;
+    st->iteration = 0;
+    st->done = 0;
+  }
+}
+
+// Lane `sub` of a point's group of 8 owns the sums k = 8 a + sub (a < 4), so a lane keeps 4 accumulators rather
+// than 29.  Per-block partials: part[block][k], summed lanes by butterfly and warps in order.
+__global__ void __launch_bounds__(kPlaneThreads)
+icp_plane_match_kernel(const float* __restrict__ src, int64_t n_src, const float* __restrict__ tgt,
+                       const float* __restrict__ tnorm, const dgr_keyspec_t* __restrict__ spec_p,
+                       const uint64_t* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask,
+                       int32_t batch, double voxel, double max_dist, const IcpPlaneState* __restrict__ st,
+                       double* __restrict__ part) {
+  if (st->done) return;
+  const dgr_keyspec_t s = *spec_p;
+  double T[12];
+#pragma unroll
+  for (int k = 0; k < 12; ++k) T[k] = st->T[k];
+  double acc[4] = {0.0, 0.0, 0.0, 0.0};
+  const int reach = (int)ceil(max_dist / voxel);
+  const int sub = threadIdx.x & 7;
+  const int64_t groups = ((int64_t)gridDim.x * blockDim.x) >> 3;
+  for (int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 3; i0 < ((n_src + groups - 1) / groups) * groups;
+       i0 += groups) {
+    const bool have = i0 < n_src;
+    const int64_t i = have ? i0 : 0;
+    const double x = src[3 * i], y = src[3 * i + 1], z = src[3 * i + 2];
+    const double p[3] = {T[0] * x + T[1] * y + T[2] * z + T[3], T[4] * x + T[5] * y + T[6] * z + T[7],
+                         T[8] * x + T[9] * y + T[10] * z + T[11]};
+    double best = max_dist * max_dist;
+    int best_j;
+    dgr_voxel_nearest8(p, have, sub, tgt, s, keys, vals, mask, batch, voxel, reach, best, best_j);
+    if (have && best_j >= 0) {                          // every lane of the group has the match
+      const int64_t j = best_j;
+      const double q[3] = {tgt[3 * j], tgt[3 * j + 1], tgt[3 * j + 2]};
+      const double nv[3] = {tnorm[3 * j], tnorm[3 * j + 1], tnorm[3 * j + 2]};
+      const double r = (p[0] - q[0]) * nv[0] + (p[1] - q[1]) * nv[1] + (p[2] - q[2]) * nv[2];
+      const double J[6] = {p[1] * nv[2] - p[2] * nv[1], p[2] * nv[0] - p[0] * nv[2], p[0] * nv[1] - p[1] * nv[0],
+                           nv[0], nv[1], nv[2]};
+      int k = 0;
+#pragma unroll
+      for (int a = 0; a < 6; ++a)
+#pragma unroll
+        for (int b = a; b < 6; ++b) {
+          if ((k & 7) == sub) acc[k >> 3] += J[a] * J[b];
+          ++k;
+        }
+#pragma unroll
+      for (int a = 0; a < 6; ++a) {
+        if (((21 + a) & 7) == sub) acc[(21 + a) >> 3] += J[a] * r;
+      }
+      if (sub == (27 & 7)) acc[27 >> 3] += 1.0;
+      if (sub == (28 & 7)) acc[28 >> 3] += best;
+    }
+  }
+  __shared__ double red[kPlaneThreads / 32][kPlaneStride];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int a = 0; a < 4; ++a) {
+    double v = acc[a];
+    v += __shfl_xor_sync(0xffffffffu, v, 8);            // the 4 groups of the warp, same sub
+    v += __shfl_xor_sync(0xffffffffu, v, 16);
+    if (lane < 8) red[warp][8 * a + lane] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < kPlaneNv) {
+    double v = 0.0;
+    for (int w = 0; w < kPlaneThreads / 32; ++w) v += red[w][threadIdx.x];
+    part[(int64_t)blockIdx.x * kPlaneStride + threadIdx.x] = v;
+  }
+}
+
+// one block of kPlaneNv warps: warp k sums partial k over the blocks (lane-strided, then butterfly)
+__global__ void __launch_bounds__(kPlaneNv * 32)
+icp_plane_update_kernel(IcpPlaneState* st, const double* __restrict__ part, int n_blocks, int64_t n_src, int max_iter,
+                        double rel_fitness, double rel_rmse, double* __restrict__ result) {
+  __shared__ double tot[kPlaneStride];
+  const bool live = !st->done;                          // uniform per launch
+  if (live) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double v = 0.0;
+    for (int b = lane; b < n_blocks; b += 32) v += part[(int64_t)b * kPlaneStride + warp];
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+    if (lane == 0) tot[warp] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  if (live) {
+    const double n = tot[27];
+    double fitness, rmse;
+    const bool stop = icp_stop_rule(*st, n, tot[28], n_src, max_iter, rel_fitness, rel_rmse, fitness, rmse);
+    const int k = st->iteration;
+    st->fitness = fitness;
+    st->rmse = rmse;
+    st->n_corr = n;
+    if (stop) {
+      st->done = 1;
+    } else {
+      double x[6], T[12];
+      if (!cholesky6_step(tot, tot + 21, x))            // singular J^T J (no match, a single plane): identity
+        for (int q = 0; q < 6; ++q) x[q] = 0.0;
+      for (int q = 0; q < 12; ++q) T[q] = st->T[q];
+      zyx_update_left(x, T, st->T);
+      st->prev_fitness = fitness;
+      st->prev_rmse = rmse;
+      st->iteration = k + 1;
+    }
+  }
+  for (int q = 0; q < 12; ++q) result[q] = st->T[q];
+  result[12] = 0.0; result[13] = 0.0; result[14] = 0.0; result[15] = 1.0;
+  result[16] = st->fitness;
+  result[17] = st->rmse;
+  result[18] = (double)st->iteration;
+  result[19] = st->n_corr;
+}
+
+inline int plane_blocks(int64_t n_src) {
+  unsigned blocks = dgr_blocks(n_src * 8, kPlaneThreads);   // 8 lanes per source point
+  return blocks > (unsigned)kPlaneMaxBlocks ? kPlaneMaxBlocks : (int)blocks;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t dgr_estimate_normals(const float* xyz, int64_t n, const dgr_keyspec_t* spec, const uint64_t* keys,
+                             const int32_t* vals, int64_t cap, int32_t batch, double cell, double radius,
+                             int32_t max_nn, const float* prev, float* normals, int32_t* counts, void* stream) {
+  DGR_ARG_CHECK(n >= 0 && n < (1ll << 31), "point count out of range");
+  DGR_ARG_CHECK(n == 0 || (xyz != nullptr && spec != nullptr && keys != nullptr && vals != nullptr &&
+                           normals != nullptr && counts != nullptr), "null pointer");
+  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
+  DGR_ARG_CHECK(cell > 0 && radius > 0, "cell and radius must be positive");
+  DGR_ARG_CHECK(radius / cell <= 4.0, "search radius above 4 cells is not supported");
+  DGR_ARG_CHECK(max_nn >= 1 && max_nn <= kMaxNN, "max_nn must lie in [1, 64]");
+  if (n == 0) return DGR_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int reach = (int)ceil(radius / cell);
+  const int side = 2 * reach + 1, n_cells = side * side * side;
+  const double r2 = radius * radius;
+  normals_kernel<<<dgr_blocks(n * 8, kNormThreads), kNormThreads, 0, st>>>(
+      xyz, n, spec, keys, vals, (uint64_t)cap - 1, batch, cell, reach, r2, max_nn, prev, normals, counts);
+  const size_t smem = (size_t)kSelWarps * n_cells * (sizeof(double) + sizeof(int32_t));   // <= 35 KB
+  normals_select_kernel<<<dgr_blocks(n, kSelWarps), kSelWarps * 32, smem, st>>>(
+      xyz, n, spec, keys, vals, (uint64_t)cap - 1, batch, cell, reach, r2, max_nn, prev, normals, counts);
+  dgr_note_launches(2);
+  DGR_LAUNCH_CHECK();
+  return DGR_OK;
+}
+
+int32_t dgr_icp_plane_ws_elems(int64_t n_src, int64_t* n_elems) {
+  DGR_ARG_CHECK(n_elems != nullptr && n_src >= 0, "bad arguments");
+  *n_elems = kPlaneState + (int64_t)plane_blocks(n_src) * kPlaneStride;
+  return DGR_OK;
+}
+
+int32_t dgr_icp_point_to_plane(const float* src, int64_t n_src, const float* tgt, const float* tgt_normals,
+                               const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap,
+                               int32_t batch, double voxel, double max_dist, const double* T_init, int32_t max_iter,
+                               double rel_fitness, double rel_rmse, double* ws, double* result, void* stream) {
+  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
+  DGR_ARG_CHECK(voxel > 0 && max_dist > 0 && max_iter >= 0, "bad ICP parameters");
+  DGR_ARG_CHECK(max_dist / voxel <= 4.0, "search radius above 4 voxels is not supported");
+  DGR_ARG_CHECK(n_src >= 0 && n_src < (1ll << 31), "point count out of range");
+  DGR_ARG_CHECK(T_init != nullptr && ws != nullptr && result != nullptr && spec != nullptr, "null pointer");
+  static_assert(sizeof(IcpPlaneState) <= kPlaneState * sizeof(double), "state workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  IcpPlaneState* state = reinterpret_cast<IcpPlaneState*>(ws);
+  double* part = ws + kPlaneState;
+  const int blocks = plane_blocks(n_src);
+  icp_plane_init_kernel<<<1, 32, 0, st>>>(T_init, state);
+  for (int k = 0; k <= max_iter; ++k) {
+    icp_plane_match_kernel<<<blocks, kPlaneThreads, 0, st>>>(src, n_src, tgt, tgt_normals, spec, keys, vals,
+                                                             (uint64_t)cap - 1, batch, voxel, max_dist, state, part);
+    icp_plane_update_kernel<<<1, kPlaneNv * 32, 0, st>>>(state, part, blocks, n_src, max_iter, rel_fitness, rel_rmse,
+                                                         result);
+  }
+  dgr_note_launches(1 + 2 * (max_iter + 1));
+  DGR_LAUNCH_CHECK();
+  return DGR_OK;
+}
+
+}  // extern "C"

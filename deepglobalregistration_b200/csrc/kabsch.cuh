@@ -1,4 +1,5 @@
-// Shared by registration.cu (weighted Procrustes, ICP) and ransac.cu (4-point hypotheses).
+// Small fp64 solvers shared by registration.cu (weighted Procrustes, ICP), ransac.cu (4-point hypotheses), fgr.cu
+// (Gauss-Newton steps) and icp_plane.cu (normals, point-to-plane steps).
 #pragma once
 
 // ---------------------------------------------------------------------------------------
@@ -10,8 +11,10 @@ __device__ inline double det3(const double m[3][3]) {
          m[0][2] * (m[1][0] * m[2][1] - m[1][1] * m[2][0]);
 }
 
-__device__ inline void kabsch_rotation(const double S[3][3], double R[3][3]) {
-  double A[3][3], V[3][3];
+// One-sided Jacobi sweeps on S: on return A = S V has orthogonal columns, V is orthogonal and sig[j] = |A[:, j]|
+// (the singular values, unsorted).  For a symmetric positive semi-definite S the columns of V are its eigenvectors
+// and sig its eigenvalues.
+__device__ __forceinline__ void jacobi_svd3(const double S[3][3], double A[3][3], double V[3][3], double sig[3]) {
   for (int i = 0; i < 3; ++i)
     for (int j = 0; j < 3; ++j) {
       A[i][j] = S[i][j];
@@ -43,8 +46,12 @@ __device__ inline void kabsch_rotation(const double S[3][3], double R[3][3]) {
       }
     if (!rotated) break;
   }
-  double sig[3];
   for (int j = 0; j < 3; ++j) sig[j] = sqrt(A[0][j] * A[0][j] + A[1][j] * A[1][j] + A[2][j] * A[2][j]);
+}
+
+__device__ inline void kabsch_rotation(const double S[3][3], double R[3][3]) {
+  double A[3][3], V[3][3], sig[3];
+  jacobi_svd3(S, A, V, sig);
   int ord[3] = {0, 1, 2};   // descending singular values
   for (int a = 0; a < 2; ++a)
     for (int b = a + 1; b < 3; ++b)
@@ -84,3 +91,70 @@ __device__ inline void kabsch_rotation(const double S[3][3], double R[3][3]) {
       R[i][j] = U[i][0] * W[j][0] + U[i][1] * W[j][1] + sgn * U[i][2] * W[j][2];
 }
 
+// ---------------------------------------------------------------------------------------
+// 6-DoF Gauss-Newton step (FGR, point-to-plane ICP)
+// ---------------------------------------------------------------------------------------
+// x = -(A^-1 g) by Cholesky of the symmetric A (upper triangle a[21], row-major); false on a non-positive pivot
+__device__ inline bool cholesky6_step(const double* a, const double* g, double x[6]) {
+  double L[6][6];
+  int k = 0;
+  double A[6][6];
+  for (int r = 0; r < 6; ++r)
+    for (int c = r; c < 6; ++c) { A[r][c] = a[k]; A[c][r] = a[k]; ++k; }
+  for (int j = 0; j < 6; ++j) {
+    double d = A[j][j];
+    for (int m = 0; m < j; ++m) d -= L[j][m] * L[j][m];
+    if (!(d > 0.0)) return false;
+    L[j][j] = sqrt(d);
+    for (int i = j + 1; i < 6; ++i) {
+      double e = A[i][j];
+      for (int m = 0; m < j; ++m) e -= L[i][m] * L[j][m];
+      L[i][j] = e / L[j][j];
+    }
+  }
+  double y[6];
+  for (int i = 0; i < 6; ++i) {
+    double e = -g[i];
+    for (int m = 0; m < i; ++m) e -= L[i][m] * y[m];
+    y[i] = e / L[i][i];
+  }
+  for (int i = 5; i >= 0; --i) {
+    double e = y[i];
+    for (int m = i + 1; m < 6; ++m) e -= L[m][i] * x[m];
+    x[i] = e / L[i][i];
+  }
+  return true;
+}
+
+// Tn = [Rz(x[2]) Ry(x[1]) Rx(x[0]) | x[3..6)] T, poses row-major [R | t] (open3d's TransformVector6dToMatrix4d)
+__device__ __forceinline__ void zyx_update_left(const double x[6], const double T[12], double* Tn) {
+  const double ca = cos(x[0]), sa = sin(x[0]), cb = cos(x[1]), sb = sin(x[1]), cc = cos(x[2]), sc = sin(x[2]);
+  const double Rz[3][3] = {{cc, -sc, 0.0}, {sc, cc, 0.0}, {0.0, 0.0, 1.0}};
+  const double Ry[3][3] = {{cb, 0.0, sb}, {0.0, 1.0, 0.0}, {-sb, 0.0, cb}};
+  const double Rx[3][3] = {{1.0, 0.0, 0.0}, {0.0, ca, -sa}, {0.0, sa, ca}};
+  double Rzy[3][3], D[3][3];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) Rzy[r][c] = Rz[r][0] * Ry[0][c] + Rz[r][1] * Ry[1][c] + Rz[r][2] * Ry[2][c];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) D[r][c] = Rzy[r][0] * Rx[0][c] + Rzy[r][1] * Rx[1][c] + Rzy[r][2] * Rx[2][c];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 4; ++c)
+      Tn[4 * r + c] = D[r][0] * T[c] + D[r][1] * T[4 + c] + D[r][2] * T[8 + c] + (c == 3 ? x[3 + r] : 0.0);
+}
+
+// ---------------------------------------------------------------------------------------
+// open3d's RegistrationICP stopping rule (both estimation methods): fitness and inlier RMSE of the correspondences
+// found at step k = st.iteration (n of them, squared Euclidean distances summing to sum_d2); the loop stops when both changed by
+// less than the tolerances since step k - 1, or at k = max_iter
+// ---------------------------------------------------------------------------------------
+template <class State>
+__device__ __forceinline__ bool icp_stop_rule(const State& st, double n, const double& sum_d2, int64_t n_src, int max_iter,
+                                              double rel_fitness, double rel_rmse, double& fitness, double& rmse) {
+  fitness = n_src > 0 ? n / (double)n_src : 0.0;
+  rmse = n > 0 ? sqrt(sum_d2 / n) : 0.0;
+  const int k = st.iteration;
+  bool stop = false;
+  if (k > 0 && fabs(st.prev_fitness - fitness) < rel_fitness && fabs(st.prev_rmse - rmse) < rel_rmse) stop = true;
+  if (k >= max_iter) stop = true;
+  return stop;
+}

@@ -516,12 +516,9 @@ __global__ void icp_update_kernel(IcpState* st, int64_t n_src, int max_iter, dou
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   if (!st->done) {
     const double n = st->sums[0];
-    const double fitness = n_src > 0 ? n / (double)n_src : 0.0;
-    const double rmse = n > 0 ? sqrt(st->sums[1] / n) : 0.0;
+    double fitness, rmse;
+    const bool stop = icp_stop_rule(*st, n, st->sums[1], n_src, max_iter, rel_fitness, rel_rmse, fitness, rmse);
     const int k = st->iteration;
-    bool stop = false;
-    if (k > 0 && fabs(st->prev_fitness - fitness) < rel_fitness && fabs(st->prev_rmse - rmse) < rel_rmse) stop = true;
-    if (k >= max_iter) stop = true;
     st->fitness = fitness;
     st->rmse = rmse;
     if (stop) {

@@ -11,7 +11,10 @@ numpy only, nothing here touches the GPU path:
 
 ``PointCloud`` is the small part of ``open3d.geometry.PointCloud`` the reference's demo and
 ``DeepGlobalRegistration.preprocess`` (core/deep_global_registration.py:143-148) rely on:
-``.points``, ``.transform(T)``, ``estimate_normals()`` (accepted, not needed by the path).
+``.points``, ``.normals``, ``.transform(T)`` and ``estimate_normals``.  With no argument
+``estimate_normals()`` does nothing (demo.py calls it for display only); with
+``KDTreeSearchParamHybrid(radius, max_nn)`` (util/pointcloud.py:60) it computes the normals on the GPU -
+the one call here that leaves the host, through a lazy import of o3d_registration.
 """
 import os
 import re
@@ -56,10 +59,23 @@ class PointCloud:
     if T.shape != (4, 4):
       raise ValueError('transform expects a 4x4 matrix')
     self._points = self._points @ T[:3, :3].T + T[:3, 3]
+    if self.normals is not None:
+      self.normals = np.asarray(self.normals, dtype=np.float64) @ T[:3, :3].T
     return self
 
-  def estimate_normals(self, *args, **kwargs):
-    """demo.py:35,37 calls this for visualisation; registration does not use normals."""
+  def has_normals(self):
+    return self.normals is not None
+
+  def estimate_normals(self, search_param=None, fast_normal_computation=True):
+    """``estimate_normals()`` is a no-op (demo.py:35,37 calls it for display; open3d's default there is
+    KDTreeSearchParamKNN(30), an unbounded search the voxel-hash kernel cannot do).
+    ``estimate_normals(KDTreeSearchParamHybrid(radius, max_nn))`` computes the normals on the GPU
+    (o3d_registration.estimate_normals; max_nn <= 64) into ``normals`` (float64 [N, 3]); existing normals orient
+    the new ones, as in open3d.  KDTreeSearchParamKNN / KDTreeSearchParamRadius raise NotImplementedError."""
+    if search_param is None:
+      return self
+    from .o3d_registration import estimate_normals
+    self.normals = estimate_normals(self._points, search_param, prev=self.normals)
     return self
 
   def __repr__(self):

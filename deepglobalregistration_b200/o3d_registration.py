@@ -14,7 +14,9 @@
          max_validation)), the edge-length and distance checkers, every validated hypothesis scored on all source
          points through a voxel hash of the target.
 
-It also carries the call open3d users make when RANSAC is too slow:
+It also carries the calls open3d users make beyond DGR's own: point-to-plane ICP (``registration_icp`` with
+``TransformationEstimationPointToPlane``, -> dgr_icp_point_to_plane) on target normals from
+``PointCloud.estimate_normals(KDTreeSearchParamHybrid(radius, max_nn))`` (-> dgr_estimate_normals), and
 
   registration_fast_based_on_feature_matching(source, target, source_feature, target_feature, option)
       -> dgr_knn_top1 both ways + dgr_fgr_feature_matching: Fast Global Registration (mutual matches, tuple
@@ -35,6 +37,65 @@ class TransformationEstimationPointToPoint:
     if with_scaling:
       raise NotImplementedError('with_scaling=True is not used by DGR and not built')
     self.with_scaling = False
+
+
+class TransformationEstimationPointToPlane:
+  def __init__(self, kernel=None):
+    if kernel is not None:
+      raise NotImplementedError('robust kernels (the open3d >= 0.12 form) are not built')
+    self.kernel = None
+
+
+class KDTreeSearchParamHybrid:
+  """Neighbours within `radius`, at most `max_nn` of them: what estimate_normals searches on the GPU."""
+
+  def __init__(self, radius, max_nn):
+    self.radius, self.max_nn = float(radius), int(max_nn)
+
+
+class KDTreeSearchParamKNN:
+  """open3d's unbounded k-nearest search: accepted as a name, not built (the voxel-hash search needs a radius)."""
+
+  def __init__(self, knn=30):
+    self.knn = int(knn)
+
+
+class KDTreeSearchParamRadius:
+  """open3d's radius search without a neighbour bound: accepted as a name, not built."""
+
+  def __init__(self, radius):
+    self.radius = float(radius)
+
+
+def _hybrid_check(search_param):
+  if isinstance(search_param, (KDTreeSearchParamKNN, KDTreeSearchParamRadius)):
+    raise NotImplementedError(f'{type(search_param).__name__}: only KDTreeSearchParamHybrid(radius, max_nn) is built '
+                              '(a bounded radius the voxel hash can search)')
+  if not isinstance(search_param, KDTreeSearchParamHybrid):
+    raise TypeError(f'expected KDTreeSearchParamHybrid, got {type(search_param).__name__}')
+  if not search_param.radius > 0.0:
+    raise ValueError(f'radius must be positive, got {search_param.radius}')
+  if not 1 <= search_param.max_nn <= _abi.MAX_NN:
+    raise ValueError(f'max_nn must lie in [1, {_abi.MAX_NN}], got {search_param.max_nn}')
+
+
+def estimate_normals(points, search_param, prev=None):
+  """Normals of points [N, 3] (float64 [N, 3], as open3d stores them) from KDTreeSearchParamHybrid neighbours,
+  through a voxel hash of the cloud (dgr_estimate_normals); prev [N, 3]: the normals to orient against."""
+  _hybrid_check(search_param)
+  pts = np.asarray(points, dtype=np.float64).reshape(-1, 3)
+  if prev is not None and np.asarray(prev).shape != pts.shape:
+    raise ValueError('previous normals must hold one row per point')
+  if len(pts) == 0:
+    return np.zeros((0, 3))
+  dev = _abi.require_device('cuda')
+  _abi.refresh_stream()
+  p64 = torch.from_numpy(np.ascontiguousarray(pts)).to(dev)
+  cell, spec, table = _target_hash(p64, search_param.radius)
+  prev_d = None if prev is None else torch.from_numpy(np.ascontiguousarray(prev, dtype=np.float32)).to(dev)
+  nrm = _abi.estimate_normals(p64.float().contiguous(), (spec, table), cell, search_param.radius, search_param.max_nn,
+                              prev=prev_d)
+  return nrm.cpu().numpy().astype(np.float64)
 
 
 class ICPConvergenceCriteria:
@@ -95,9 +156,9 @@ def _points(pcd, device):
 
 
 def _target_hash(tgt64, max_dist):
-  """Voxel hash of the target with at most one point per cell (what the ICP kernel searches): cell =
+  """Voxel hash of the target with at most one point per cell (what the ICP and normal kernels search): cell =
   max_dist / 2 as in DGR (voxelised clouds, radius 2 voxels); a cloud with several points per cell gets finer
-  cells up to the kernel's reach of 4."""
+  cells up to the kernels' reach of 4."""
   from .me.coords import KEY_MARGIN
   for div in (2.0, 3.0, 4.0):
     cell = max_dist / div
@@ -111,13 +172,18 @@ def _target_hash(tgt64, max_dist):
 
 
 def registration_icp(source, target, max_correspondence_distance, init=None, estimation_method=None, criteria=None):
+  """Point-to-point (the default, what DGR calls) or point-to-plane ICP; point-to-plane needs target normals
+  (``target.estimate_normals(KDTreeSearchParamHybrid(radius, max_nn))``)."""
+  plane = isinstance(estimation_method, TransformationEstimationPointToPlane)
+  if not (plane or estimation_method is None or isinstance(estimation_method, TransformationEstimationPointToPoint)):
+    raise NotImplementedError('only point-to-point and point-to-plane ICP are built')
+  tgt_normals = getattr(target, 'normals', None) if plane else None
+  if plane and tgt_normals is None:
+    raise RuntimeError('TransformationEstimationPointToPlane needs target normals: call '
+                       'target.estimate_normals(KDTreeSearchParamHybrid(radius, max_nn)) first')
   dev = _abi.require_device('cuda')
   _abi.refresh_stream()
   criteria = criteria or ICPConvergenceCriteria()
-  if isinstance(estimation_method, TransformationEstimationPointToPoint) or estimation_method is None:
-    pass
-  else:
-    raise NotImplementedError('only point-to-point ICP is built (what DGR calls)')
   src64, tgt64 = _points(source, dev), _points(target, dev)
   T0 = np.eye(4) if init is None else np.asarray(init, dtype=np.float64).reshape(4, 4)
   if len(src64) == 0 or len(tgt64) == 0:
@@ -125,6 +191,14 @@ def registration_icp(source, target, max_correspondence_distance, init=None, est
   cell, spec, table = _target_hash(tgt64, float(max_correspondence_distance))
   src, tgt = src64.float().contiguous(), tgt64.float().contiguous()
   T12 = torch.from_numpy(np.ascontiguousarray(T0[:3])).to(dev)
+  if plane:
+    nrm = np.asarray(tgt_normals, dtype=np.float32).reshape(-1, 3)
+    if len(nrm) != len(tgt):
+      raise RuntimeError('target normals must hold one row per target point')
+    r = _abi.icp_point_to_plane(src, tgt, torch.from_numpy(np.ascontiguousarray(nrm)).to(dev), (spec, table), cell,
+                                float(max_correspondence_distance), T12, int(criteria.max_iteration),
+                                float(criteria.relative_fitness), float(criteria.relative_rmse)).cpu().numpy()
+    return RegistrationResult(r[:16], r[16], r[17], r[19])
   state = torch.empty(64, dtype=torch.float64, device=dev)
   res = torch.empty(20, dtype=torch.float64, device=dev)
   _abi.call('dgr_icp_point_to_point', _abi.ptr(src), src.shape[0], _abi.ptr(tgt), _abi.ptr(spec), _abi.ptr(table.keys),

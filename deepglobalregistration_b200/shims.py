@@ -44,7 +44,8 @@ def _open3d_stub():
   viewer, backed by io.py) and core/deep_global_registration.py:29-64,317-322 + util/pointcloud.py:15-23
   (pipelines.registration.registration_icp / registration_ransac_based_on_correspondence /
   registration_ransac_based_on_feature_matching, Feature, utility vectors; plus
-  registration_fast_based_on_feature_matching / FastGlobalRegistrationOption for FGR users) backed
+  registration_fast_based_on_feature_matching / FastGlobalRegistrationOption for FGR users, and
+  TransformationEstimationPointToPlane with geometry.KDTreeSearchParamHybrid for point-to-plane ICP users) backed
   by libdgr_b200 (o3d_registration.py) - so the reference's OWN DeepGlobalRegistration class and demo.py run on
   this stack unmodified.  This package's DeepGlobalRegistration does not go through here: it calls the library."""
   import numpy as np
@@ -63,7 +64,11 @@ def _open3d_stub():
   from . import o3d_registration as reg
   o3d.pipelines = types.ModuleType('open3d.pipelines')
   o3d.pipelines.registration = types.ModuleType('open3d.pipelines.registration')
-  for name in ('TransformationEstimationPointToPoint', 'ICPConvergenceCriteria', 'RANSACConvergenceCriteria',
+  for name in ('KDTreeSearchParamHybrid', 'KDTreeSearchParamKNN', 'KDTreeSearchParamRadius'):
+    setattr(o3d.geometry, name, getattr(reg, name))
+    setattr(o3d, name, getattr(reg, name))               # the pre-0.10 top-level path (util/pointcloud.py:60)
+  for name in ('TransformationEstimationPointToPoint', 'TransformationEstimationPointToPlane', 'ICPConvergenceCriteria',
+               'RANSACConvergenceCriteria',
                'CorrespondenceCheckerBasedOnDistance', 'CorrespondenceCheckerBasedOnEdgeLength', 'Feature',
                'RegistrationResult', 'registration_icp', 'registration_ransac_based_on_correspondence',
                'registration_ransac_based_on_feature_matching', 'FastGlobalRegistrationOption',

@@ -196,6 +196,32 @@ int32_t dgr_icp_point_to_point(const float* src, int64_t n_src, const float* tgt
                                double rel_fitness, double rel_rmse, double* state_ws, double* result,
                                void* stream);
 
+/* ---- Normal estimation and point-to-plane ICP: open3d 0.10 EstimateNormals(KDTreeSearchParamHybrid(radius, max_nn))
+ *      and registration_icp with TransformationEstimationPointToPlane (the ICP (Point-to-plane) row of the
+ *      reference's results; util/pointcloud.py:60, scripts/test_3dmatch.py:72-73) ---------------------------- */
+/* Normals of the cloud xyz[n] through its OWN voxel hash (keys / vals / spec of a dgr_unique_first table at `cell`,
+ * at most one point per cell, rows = rows of xyz, `batch` = its batch column; radius / cell <= 4).  Neighbours of
+ * point i: the rows j with |p_j - p_i|^2 < radius^2 (strict; i itself included), the max_nn (1..64) smallest by
+ * (d^2, row) when more qualify.  Normal: eigenvector of the smallest eigenvalue of E[e e^T] - mu mu^T over the
+ * offsets e = p_j - p_i (fp64 cumulants, one-sided Jacobi); (0, 0, 1) for fewer than 3 neighbours or a zero
+ * covariance.  Sign: largest-magnitude component positive; with prev (optional float [n, 3]) then flipped where it
+ * has a negative dot product with prev[i].  normals: float [n, 3]; counts: int32 [n] = rows within the radius
+ * (before the max_nn truncation).  No atomics, the same bits on every run. */
+int32_t dgr_estimate_normals(const float* xyz, int64_t n, const dgr_keyspec_t* spec, const uint64_t* keys,
+                             const int32_t* vals, int64_t cap, int32_t batch, double cell, double radius,
+                             int32_t max_nn, const float* prev, float* normals, int32_t* counts, void* stream);
+/* Point-to-plane ICP: as dgr_icp_point_to_point (correspondences, stopping rule, fitness and Euclidean inlier RMSE,
+ * result layout), with tgt_normals (float [n_tgt, 3]) and the update of open3d's TransformationEstimationPointToPlane:
+ * r = (s - q).n, J = [s x n, n] over the correspondences (s = current transformed source point), J^T J x = -J^T r by
+ * fp64 Cholesky (a non-positive pivot gives the identity update), T <- [Rz(x2) Ry(x1) Rx(x0) | x3..5] T.  The sums
+ * are per-block partials reduced in block order: the same bits on every run.  No host round trip.
+ * ws: dgr_icp_plane_ws_elems(n_src) doubles. */
+int32_t dgr_icp_plane_ws_elems(int64_t n_src, int64_t* n_elems);
+int32_t dgr_icp_point_to_plane(const float* src, int64_t n_src, const float* tgt, const float* tgt_normals,
+                               const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap,
+                               int32_t batch, double voxel, double max_dist, const double* T_init, int32_t max_iter,
+                               double rel_fitness, double rel_rmse, double* ws, double* result, void* stream);
+
 /* ---- Safeguard RANSAC (SURVEY 8f rank 2): open3d registration_ransac_based_on_correspondence as
  *      called at core/deep_global_registration.py:50-64 (from :302-315) ---------------------- */
 /* Correspondence i pairs x[idx0[i]] with y[idx1[i]] (a null index array means i itself).
