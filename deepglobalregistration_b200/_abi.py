@@ -50,7 +50,7 @@ SIGNATURES = {
     'dgr_l2_normalize': [_p, _i64, _i32, _p, _p],
     'dgr_knn_top1': [_p, _i64, _p, _i64, _i32, _p, _p, _p, _p],
     'dgr_knn_tc_supported': [_i32],
-    'dgr_knn_tc_ws_elems': [_i64, _i64],
+    'dgr_knn_tc_ws_elems': [_i64, _i64, _i32],
     'dgr_knn_top1_tc': [_p, _i64, _p, _i64, _i32, _p, _p, _p, _p, _p],
     'dgr_inlier_coords': [_p, _p, _p, _i64, _p, _p],
     'dgr_sigmoid_clip_sum': [_p, _i64, _f32, _p, _p, _p],
@@ -598,7 +598,7 @@ def knn_top1(f0, f1, return_distance=False, mode=None):
   idx = torch.empty(n0, dtype=torch.int32, device=f0.device)
   dist = torch.empty(n0, dtype=torch.float32, device=f0.device) if return_distance else None
   if mode == 'tc' and lib().dgr_knn_tc_supported(c) and n0 > 0:
-    fws = scratch('knn_fws', lib().dgr_knn_tc_ws_elems(n0, n1), torch.float32, f0.device)
+    fws = scratch('knn_fws', lib().dgr_knn_tc_ws_elems(n0, n1, c), torch.float32, f0.device)
     call('dgr_knn_top1_tc', ptr(f0), n0, ptr(f1), n1, c, ptr(ws), ptr(fws), ptr(idx), ptr(dist), stream())
   else:
     call('dgr_knn_top1', ptr(f0), n0, ptr(f1), n1, c, ptr(ws), ptr(idx), ptr(dist), stream())

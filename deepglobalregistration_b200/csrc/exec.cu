@@ -1018,7 +1018,7 @@ int32_t dgr_pair_register(dgr_ctx_t* c, dgr_net_t* fcgf, dgr_net_t* inlier, cons
   DGR_TRY(aalloc(c, N0, &packed_ws));
   if (dgr_knn_tc_supported(Cf)) {
     float* fws;
-    DGR_TRY(aalloc(c, dgr_knn_tc_ws_elems(N0, N1), &fws));
+    DGR_TRY(aalloc(c, dgr_knn_tc_ws_elems(N0, N1, Cf), &fws));
     DGR_TRY(dgr_knn_top1_tc(F, N0, F + (int64_t)N0 * Cf, N1, Cf, packed_ws, fws, idx1, nullptr, st));
   } else {
     DGR_TRY(dgr_knn_top1(F, N0, F + (int64_t)N0 * Cf, N1, Cf, packed_ws, idx1, nullptr, st));

@@ -156,9 +156,9 @@ int32_t dgr_knn_top1(const float* f0, int64_t n0, const float* f1, int64_t n1, i
 /* Tensor-core variant for c in {32, 64} (dgr_knn_tc_supported): two wgmma (TF32) sweeps
  * find, per row, the candidate columns whose approximate distance is within a proven error
  * bound of the row minimum; only those are evaluated with the exact fp32 arithmetic above.
- * Results are bit-identical to dgr_knn_top1.  ws: dgr_knn_tc_ws_elems(n0, n1) floats. */
+ * Results are bit-identical to dgr_knn_top1.  ws: dgr_knn_tc_ws_elems(n0, n1, c) floats, 16-byte aligned. */
 int32_t dgr_knn_tc_supported(int32_t c);
-int64_t dgr_knn_tc_ws_elems(int64_t n0, int64_t n1);
+int64_t dgr_knn_tc_ws_elems(int64_t n0, int64_t n1, int32_t c);
 int32_t dgr_knn_top1_tc(const float* f0, int64_t n0, const float* f1, int64_t n1, int32_t c,
                         uint64_t* packed_ws, float* ws, int32_t* idx, float* dist, void* stream);
 
