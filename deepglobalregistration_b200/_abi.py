@@ -82,8 +82,6 @@ SIGNATURES = {
     'dgr_kernel_map_tiles': [_p, _i32, _i32, _i32, _i32, _p, _p, _p],
     'dgr_kmap_dense': [_p, _i64, _p, _i32, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p, _i64, _p, _p],
     'dgr_spconv_ones_bits_fwd': [_p, _i32, _p, _i64, _i32, _i64, _p, _p, _p, _p],
-    'dgr_spconv_os_supported': [_i32, _i32],
-    'dgr_spconv_os_fwd': [_p, _i32, _p, _i32, _p, _i64, _i32, _i64, _p, _p, _p, _i32, _p, _p],
     'dgr_spconv_wgrad': [_p, _i32, _p, _i32, _p, _p, _p, _i32, _p, _p],
     'dgr_affine_act_amax': [_p, _i64, _i32, _p, _p, _p, _i32, _p, _p, _p],
     'dgr_absmax_f32': [_p, _i64, _p, _p],
@@ -369,18 +367,19 @@ class KernelMap:
     return t
 
 
-def kernel_map_begin(out_coords, spec, in_table, n_in, offsets, keep_table=False, slot=0):
-  """First half of a kernel map: occupancy bits + bucket offsets (and the dense neighbour table when kept), all
-  asynchronous.  `slot` selects the scratch buffers so that several maps can be in flight before ONE host read
-  finishes them all (kernel_maps_finish)."""
+def kernel_map(out_coords, spec, in_table, n_in, offsets, keep_table=False):
+  """offsets: CUDA int32 [K, D] (scaled by the input tensor stride).  Occupancy bits + bucket offsets (and the
+  dense neighbour table when kept), then ONE host read of the bucket offsets sizes the pair lists and the work
+  list."""
+  global D2H_BYTES
   _chk(out_coords, torch.int32, 'out_coords')
   _chk(offsets, torch.int32, 'offsets')
   dev = out_coords.device
   n_out, ncols = out_coords.shape
   K = offsets.shape[0]
   nmx = max(n_out, 1)
-  bits = scratch(('km_bits', slot), K * lib().dgr_kmap_mask_words(nmx), torch.int32, dev)
-  cnt = scratch(('km_cnt', slot), lib().dgr_kmap_cnt_elems(K, nmx), torch.int32, dev)
+  bits = scratch('km_bits', K * lib().dgr_kmap_mask_words(nmx), torch.int32, dev)
+  cnt = scratch('km_cnt', lib().dgr_kmap_cnt_elems(K, nmx), torch.int32, dev)
   kofs = torch.empty(K + 2, dtype=torch.int32, device=dev)
   meta = scratch('km_meta', 5, torch.int32, dev)          # written by the probe, read by nobody here
   # the miss filter pays off when most probes miss: many offsets per row (6-D, 5^3, 7^3 kernels)
@@ -392,19 +391,13 @@ def kernel_map_begin(out_coords, spec, in_table, n_in, offsets, keep_table=False
   table = (ptr(in_table.keys), ptr(in_table.vals), in_table.cap)
   call('dgr_kmap_probe', ptr(out_coords), n_out, None, ncols, ptr(spec), *table, ptr(bloom), n_words, ptr(offsets), K,
        ptr(bits), ptr(cnt), ptr(kofs), ptr(meta), stream())
-  nbr = None
+  km = KernelMap()
+  km.nbr = None
   if keep_table:
-    nbr = torch.empty(K, nmx, dtype=torch.int32, device=dev)
+    km.nbr = torch.empty(K, nmx, dtype=torch.int32, device=dev)
     call('dgr_kmap_dense', ptr(out_coords), n_out, None, ncols, ptr(spec), *table, ptr(bloom), n_words, ptr(offsets),
-         K, ptr(nbr), nmx, None, stream())
-  return dict(K=K, n_in=n_in, n_out=n_out, out_coords=out_coords, spec=spec, in_table=in_table, offsets=offsets,
-              bits=bits, cnt=cnt, kofs=kofs, nbr=nbr, dev=dev)
-
-
-def kernel_map_finish(pend, kofs_all):
-  """Second half: pair lists and work list, sized from the host copy of the bucket offsets."""
-  global D2H_BYTES
-  K, n_out, dev = pend['K'], pend['n_out'], pend['dev']
+         K, ptr(km.nbr), nmx, None, stream())
+  kofs_all = kofs.cpu().numpy()
   D2H_BYTES += kofs_all.nbytes
   if kofs_all[K + 1] != 0:
     raise DgrError('coordinate extent does not fit a 63-bit packed key')
@@ -412,42 +405,18 @@ def kernel_map_finish(pend, kofs_all):
   P = int(kofs_host[K])
   counts = kofs_host[1:] - kofs_host[:-1]
   n_tiles = int(((counts + TILE_ROWS - 1) // TILE_ROWS).sum())
-  km = KernelMap()
-  km.K, km.n_in, km.n_out = K, pend['n_in'], n_out
+  km.K, km.n_in, km.n_out = K, n_in, n_out
   km.in_idx = torch.empty(max(P, 1), dtype=torch.int32, device=dev)
   km.out_idx = torch.empty(max(P, 1), dtype=torch.int32, device=dev)
   km.tile_k = torch.empty(max(n_tiles, 1), dtype=torch.int32, device=dev)
   km.tile_start = torch.empty(max(n_tiles, 1), dtype=torch.int32, device=dev)
   if P > 0:
-    out_coords, t = pend['out_coords'], pend['in_table']
-    call('dgr_kmap_fill', ptr(pend['bits']), ptr(pend['cnt']), K, n_out, ptr(out_coords), out_coords.shape[1],
-         ptr(pend['spec']), ptr(t.keys), ptr(t.vals), t.cap, ptr(pend['offsets']), ptr(km.in_idx), ptr(km.out_idx),
-         stream())
-    call('dgr_kernel_map_tiles', ptr(pend['kofs']), K, TILE_ROWS, n_tiles, 0, ptr(km.tile_k), ptr(km.tile_start),
-         stream())
-  km.kofs, km.kofs_host, km.n_pairs, km.n_tiles = pend['kofs'], kofs_host, P, n_tiles
-  km.nbr = pend['nbr']
+    call('dgr_kmap_fill', ptr(bits), ptr(cnt), K, n_out, ptr(out_coords), ncols, ptr(spec), *table, ptr(offsets),
+         ptr(km.in_idx), ptr(km.out_idx), stream())
+    call('dgr_kernel_map_tiles', ptr(kofs), K, TILE_ROWS, n_tiles, 0, ptr(km.tile_k), ptr(km.tile_start), stream())
+  km.kofs, km.kofs_host, km.n_pairs, km.n_tiles = kofs, kofs_host, P, n_tiles
   km._paired = None
   return km
-
-
-def kernel_maps_finish(pending):
-  """Finish several begun kernel maps with a single device-to-host read."""
-  if not pending:
-    return []
-  host = torch.cat([p['kofs'] for p in pending]).cpu().numpy() if len(pending) > 1 else \
-      pending[0]['kofs'].cpu().numpy()
-  out, ofs = [], 0
-  for p in pending:
-    n = p['K'] + 2
-    out.append(kernel_map_finish(p, host[ofs:ofs + n]))
-    ofs += n
-  return out
-
-
-def kernel_map(out_coords, spec, in_table, n_in, offsets, keep_table=False):
-  """offsets: CUDA int32 [K, D] (scaled by the input tensor stride).  One host read."""
-  return kernel_maps_finish([kernel_map_begin(out_coords, spec, in_table, n_in, offsets, keep_table)])[0]
 
 
 def spconv_fwd(feat, weight, km, out, relu_in=False):
@@ -530,16 +499,6 @@ def spconv_tc_f16_fwd(feat, weight, km, out, amax=None):
     call('dgr_absmax_f32', ptr(feat), feat.numel(), ptr(amax), stream())
   call('dgr_spconv_tc_f16_fwd', ptr(feat), cin, ptr(packed), cout, ptr(km.in_idx), ptr(km.out_idx), ptr(km.kofs),
        ptr(km.tile_k), ptr(km.tile_start), km.n_tiles, TILE_ROWS, ptr(amax), ptr(wscale), ptr(out), stream())
-  return out
-
-
-def spconv_os_fwd(feat, weight_t, nbr, cout, scale=None, shift=None, residual=None, relu=False):
-  """Output-stationary tensor-core convolution with the fused epilogue; nbr: dense table [K, n_out] int32."""
-  _chk(feat, torch.float32, 'feat'); _chk(weight_t, torch.float32, 'weight_t'); _chk(nbr, torch.int32, 'nbr')
-  K, n_out = nbr.shape
-  out = torch.empty(n_out, cout, dtype=torch.float32, device=feat.device)
-  call('dgr_spconv_os_fwd', ptr(feat), feat.shape[1], ptr(weight_t), cout, ptr(nbr), nbr.stride(0), K, n_out,
-       ptr(scale), ptr(shift), ptr(residual), int(relu), ptr(out), stream())
   return out
 
 

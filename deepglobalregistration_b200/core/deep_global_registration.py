@@ -16,7 +16,6 @@ import threading
 import time
 
 from .. import _abi, native, shims
-from ..me import SparseTensor
 from ..me.coords import CoordinateManager, KEY_MARGIN
 from ..model import load_model
 from ..util.timer import Timer
@@ -69,9 +68,9 @@ class DeepGlobalRegistration:
         conv1_kernel_size=nc['inlier_conv1_kernel_size'], normalize_feature=False, D=6)
     self._pinned = {}
     # native executor (csrc/exec.cu): one C call per pair; built lazily, rebuilt when the weights change
-    self.use_native = os.environ.get('DGR_NATIVE', '1') != '0'
     self._native_nets = None
     self._native_ctx = []
+    self._stage_ctx = None          # the stage methods' own context: they never overwrite a register() call's taps
     self._last_ctx = None
     self._last_sel_value = None
     self._log('=> loading finished')
@@ -144,20 +143,30 @@ class DeepGlobalRegistration:
     feats = torch.ones(npts, 1, device=self.device)
     return xyz_sel, coords, feats
 
+  def _stage_forward(self, net, coords, feats=None, unique=False):
+    """`net` (a native.Net) over coords CUDA int32 [n, D+1] and feats float32 [n, in_channels] (None = ones) on the
+    stage context.  The executor assumes distinct rows and cannot detect duplicates, so rows not known to be
+    distinct (from preprocess(), which attaches `_dgr_manager`, or `unique`) are checked first."""
+    _abi.refresh_stream()
+    coords = coords.to(self.device, torch.int32).contiguous()
+    if not unique and getattr(coords, '_dgr_manager', None) is None:
+      CoordinateManager(coords)         # raises ValueError on duplicate rows
+    if feats is not None:
+      feats = feats.to(self.device, torch.float32).contiguous()
+    if self._stage_ctx is None:
+      self._stage_ctx = native.Context(self.device)
+    return net.forward(self._stage_ctx, coords, feats)
+
   def fcgf_feature_extraction(self, feats, coords):
     """Step 1: FCGF feature per voxel."""
-    sinput = SparseTensor(feats, coordinates=coords, device=self.device)
-    return self.fcgf_model.forward_fused(sinput).F
+    return self._stage_forward(self.native_networks()[0], coords, feats)
 
   def fcgf_feature_extraction_pair(self, coords0, coords1):
     """Both clouds of a pair in ONE sparse tensor (batch indices 0 / 1): the hash keys carry the
     batch column, so neighbourhoods never cross clouds and the features equal two separate
     forward passes - at half the launches and host synchronisations."""
     n0 = coords0.shape[0]
-    coords = torch.cat((coords0, coords1), 0)
-    coords._dgr_manager = CoordinateManager(coords, assume_unique=True)   # two unique sets, batch 0 / 1
-    feats = torch.ones(coords.shape[0], 1, device=self.device)
-    F = self.fcgf_model.forward_fused(SparseTensor(feats, coordinates=coords, device=self.device)).F
+    F = self._stage_forward(self.native_networks()[0], torch.cat((coords0, coords1), 0), unique=True)
     return F[:n0], F[n0:]
 
   def fcgf_feature_matching(self, feats0, feats1):
@@ -184,8 +193,7 @@ class DeepGlobalRegistration:
 
   def inlier_prediction(self, inlier_feats, coords):
     """Step 4: inlier logit per correspondence."""
-    sinput = SparseTensor(inlier_feats, coordinates=coords, device=self.device)
-    return self.inlier_model.forward_fused(sinput).F
+    return self._stage_forward(self.native_networks()[1], coords, inlier_feats)
 
   def safeguard_registration(self, pcd0, pcd1, idx0, idx1, feats0, feats1, distance_threshold,
                              num_iterations):
@@ -242,8 +250,8 @@ class DeepGlobalRegistration:
     return self._native_ctx[k]
 
   def _native_ok(self):
-    return (self.use_native and self.config.inlier_feature_type == 'ones' and
-            self.safeguard_method == 'correspondence' and hasattr(self.fcgf_model, 'CHANNELS'))
+    return (self.config.inlier_feature_type == 'ones' and self.safeguard_method == 'correspondence' and
+            hasattr(self.fcgf_model, 'CHANNELS'))
 
   @staticmethod
   def _points(pcd):
@@ -335,8 +343,8 @@ class DeepGlobalRegistration:
     return results
 
   def register_stagewise(self, xyz0, xyz1, inlier_thr=0.00):
-    """The same algorithm driven stage by stage from Python through the operator-level C ABI (round 1's
-    path): every inlier feature type, and the reference's own stage methods, go through here."""
+    """The same algorithm driven stage by stage from Python: the reference's own stage methods, with both
+    networks on the native executor.  Every inlier feature type goes through here."""
     self.reg_timer.tic()
     _abi.refresh_stream()
     with torch.no_grad():
@@ -349,16 +357,13 @@ class DeepGlobalRegistration:
 
       idx1 = _abi.knn_top1(fcgf_feats0, fcgf_feats1)              # int32 [N0]
       inlier_coords = _abi.inlier_coords(coords0, coords1, idx1)    # int32 [N0, 7]
-      feat_type = self.config.inlier_feature_type
-      if feat_type == 'ones':
-        inlier_feats = torch.ones((len(idx1), 1), device=self.device)
-      else:
+      inlier_feats = None                                           # 'ones'
+      if self.config.inlier_feature_type != 'ones':
         corres_idx0 = torch.arange(len(idx1), device=self.device)
         inlier_feats = self.inlier_feature_generation(xyz0, xyz1, coords0, coords1, fcgf_feats0,
                                                       fcgf_feats1, corres_idx0, idx1.long())
       # rows are distinct by construction (idx0 = arange over unique voxels)
-      inlier_coords._dgr_manager = CoordinateManager(inlier_coords, assume_unique=True)
-      logit = self.inlier_prediction(inlier_feats.contiguous(), coords=inlier_coords)
+      logit = self._stage_forward(self.native_networks()[1], inlier_coords, inlier_feats, unique=True)
       weights, wsum_dev = _abi.sigmoid_clip_sum(logit, self.clip_weight_thresh)
       # Procrustes + refinement are launched before the weight-sum gate is known (0.6 ms of GPU
       # time in the rare safeguard case) so that gate and pose come back in ONE host read

@@ -44,7 +44,6 @@ constexpr int kMetaPerMap = 5;
 constexpr int kKeyMargin = 32;        // spare cells around the bounding box (7^3 kernels, stride-8 flooring)
 
 bool tc_f16_enabled();
-bool tc_os_enabled();
 int tc_f16_min_cout();
 
 #define DGR_TRY(expr)                 \
@@ -208,7 +207,6 @@ struct dgr_net {
   const float* final_b = nullptr;
   std::vector<float*> owned;
   int device = 0;
-  bool os_level[4] = {false, false, false, false};   // stride-1 3^3 layers of level l run output-stationary
 };
 
 namespace {
@@ -305,7 +303,7 @@ struct Level {
 
 struct KMap {
   int lin = 0, lout = 0, ksize = 3, K = 27;
-  bool dense = false;        // dense neighbour table instead of pair lists (conv1 table kernel, output-stationary layers)
+  bool dense = false;        // dense neighbour table instead of pair lists (conv1 table kernel)
   bool bits_only = false;    // occupancy masks only: conv1 of a network whose single input channel is all ones
   int64_t W = 0;             // mask words per offset
   const int32_t* offsets = nullptr;
@@ -330,7 +328,7 @@ struct Plan {
   bool input_ones = false;   // the network input is one channel of ones (FCGF / inlier 'ones'): conv1 needs occupancy only
 };
 
-bool conv1_uses_table(const dgr_net* net) {
+bool conv1_table_kernel(const dgr_net* net) {
   return net->D == 3 && net->conv1_ks > 3 && net->in_ch <= 8 && (net->C[1] == 16 || net->C[1] == 32 || net->C[1] == 64);
 }
 
@@ -393,16 +391,13 @@ int32_t plan_begin(dgr_ctx* c, const dgr_net* net, Plan& p) {
     for (int a = 0; a < p.D; ++a) m.K *= ksize;
     return p.n_maps++;
   };
-  // 3-D network: the stride-1 3^3 layers run output-stationary over a dense neighbour table (spconv_os.cu); the
-  // stride-1 map at level 0 keeps its pair lists when conv1 (one input channel, fp32 kernel) shares it
-  for (int l = 0; l < 4; ++l)
-    p.map_same[l] = add_map(l, l, 3, net->os_level[l]);
+  for (int l = 0; l < 4; ++l) p.map_same[l] = add_map(l, l, 3, false);
   for (int l = 0; l < 3; ++l) p.map_down[l] = add_map(l, l + 1, 3, false);
   if (net->conv1_ks == 3) {
     p.map_conv1 = p.map_same[0];
   } else {
-    const bool bits_only = conv1_uses_table(net) && p.input_ones && net->in_ch == 1;
-    p.map_conv1 = add_map(0, 0, net->conv1_ks, conv1_uses_table(net) && !bits_only);
+    const bool bits_only = conv1_table_kernel(net) && p.input_ones && net->in_ch == 1;
+    p.map_conv1 = add_map(0, 0, net->conv1_ks, conv1_table_kernel(net) && !bits_only);
     p.maps[p.map_conv1].bits_only = bits_only;
   }
   for (int i = 0; i < p.n_maps; ++i) {
@@ -475,7 +470,6 @@ struct LayerExec {
   bool transposed;
   int n_in, n_out;
   bool table;     // conv1: output-stationary fp32 table kernel (few input channels)
-  bool os;        // output-stationary tensor-core kernel with the fused epilogue
   bool bits;      // conv1 on an all-ones input from the occupancy masks
 };
 
@@ -483,13 +477,6 @@ bool tc_f16_enabled() {
   static const bool v = [] {
     const char* e = getenv("DGR_TC_F16");
     return e ? atoi(e) != 0 : true;
-  }();
-  return v;
-}
-bool tc_os_enabled() {
-  static const bool v = [] {
-    const char* e = getenv("DGR_TC_OS");      // output-stationary kernel for the 3-D stride-1 layers: opt-in (measured
-    return e ? atoi(e) != 0 : false;          // slower than the pair-list kernel, see DESIGN.md)
   }();
   return v;
 }
@@ -501,7 +488,7 @@ int tc_f16_min_cout() {
   return v;
 }
 
-int32_t run_conv(dgr_ctx* c, const LayerExec& L, const float* feat, const float* residual, int relu, float* out) {
+int32_t run_conv(dgr_ctx* c, const LayerExec& L, const float* feat, float* out) {
   void* st = c->stream;
   const Conv& cv = *L.conv;
   const KMap& m = *L.map;
@@ -523,10 +510,6 @@ int32_t run_conv(dgr_ctx* c, const LayerExec& L, const float* feat, const float*
     DGR_TRY(dgr_spconv_table_fwd_strided(feat, cv.cin, cv.w, cv.cout, m.nbr, m.K, L.n_out, m.nbr_stride, cv.scale,
                                          cv.shift, out, st));
     rec.kind = 2;
-  } else if (L.os) {
-    DGR_TRY(dgr_spconv_os_fwd(feat, cv.cin, cv.packed, cv.cout, m.nbr, m.nbr_stride, m.K, L.n_out, cv.scale, cv.shift,
-                              residual, relu, out, st));
-    rec.kind = 3;
   } else {
     const int32_t* in_idx = L.transposed ? m.out_idx : m.in_idx;
     const int32_t* out_idx = L.transposed ? m.in_idx : m.out_idx;
@@ -563,41 +546,39 @@ int32_t run_conv(dgr_ctx* c, const LayerExec& L, const float* feat, const float*
   return DGR_OK;
 }
 
-// Port of ResUNet2.forward_fused: eval-BatchNorm folded to scale/shift applied together with the residual
-// add and ReLU in one pass after each scatter-add convolution; ME.cat fused into the consuming 1x1
-// convolution; ReLU + bias + L2-normalise fused into the 1x1 epilogues.  (model/resunet.py:598-649)
+// ResUNet2.forward of the reference (model/resunet.py:598-649) with fused epilogues: eval-BatchNorm folded to
+// scale/shift applied together with the residual add and ReLU in one pass after each scatter-add convolution;
+// ME.cat fused into the consuming 1x1 convolution; ReLU + bias + L2-normalise fused into the 1x1 epilogues.
+// The ReLUs after each block are idempotent (the block already ends in ReLU) and are dropped.
 int32_t run_network(dgr_ctx* c, const dgr_net* net, Plan& p, const float* feats_in, float* out) {
   void* st = c->stream;
   std::vector<LayerExec> layers;
   const int n[4] = {p.lv[0].n, p.lv[1].n, p.lv[2].n, p.lv[3].n};
   for (int s = 0; s < 4; ++s) {
     const KMap* m = s == 0 ? &p.maps[p.map_conv1] : &p.maps[p.map_down[s - 1]];
-    const bool os = net->os_level[s];
-    layers.push_back({&net->enc[s], m, false, s == 0 ? n[0] : n[s - 1], n[s], s == 0 && m->dense && m != &p.maps[p.map_same[0]], false,
-                      s == 0 && m->bits_only});
-    layers.push_back({&net->eb1[s], &p.maps[p.map_same[s]], false, n[s], n[s], false, os, false});
-    layers.push_back({&net->eb2[s], &p.maps[p.map_same[s]], false, n[s], n[s], false, os, false});
+    layers.push_back({&net->enc[s], m, false, s == 0 ? n[0] : n[s - 1], n[s], s == 0 && m->dense, s == 0 && m->bits_only});
+    layers.push_back({&net->eb1[s], &p.maps[p.map_same[s]], false, n[s], n[s], false, false});
+    layers.push_back({&net->eb2[s], &p.maps[p.map_same[s]], false, n[s], n[s], false, false});
   }
   for (int d = 0; d < 3; ++d) {
     const int lo = 2 - d;       // output level index
-    const bool os = net->os_level[lo];
-    layers.push_back({&net->dec[d], &p.maps[p.map_down[lo]], true, n[lo + 1], n[lo], false, false, false});
-    layers.push_back({&net->db1[d], &p.maps[p.map_same[lo]], false, n[lo], n[lo], false, os, false});
-    layers.push_back({&net->db2[d], &p.maps[p.map_same[lo]], false, n[lo], n[lo], false, os, false});
+    layers.push_back({&net->dec[d], &p.maps[p.map_down[lo]], true, n[lo + 1], n[lo], false, false});
+    layers.push_back({&net->db1[d], &p.maps[p.map_same[lo]], false, n[lo], n[lo], false, false});
+    layers.push_back({&net->db2[d], &p.maps[p.map_same[lo]], false, n[lo], n[lo], false, false});
   }
   // one slab for every convolution output, zero-filled once (the scatter-add kernels accumulate)
-  // (output-stationary layers write every row themselves: their outputs live outside the zeroed slab)
-  int64_t total = 0, total_os = 0;
-  for (auto& L : layers) (L.table || L.os || L.bits ? total_os : total) += (int64_t)L.n_out * L.conv->cout;
-  float *slab, *slab_os;
+  // (the conv1 table / bits kernels write every row themselves: their outputs live outside the zeroed slab)
+  int64_t total = 0, total_direct = 0;
+  for (auto& L : layers) (L.table || L.bits ? total_direct : total) += (int64_t)L.n_out * L.conv->cout;
+  float *slab, *slab_direct;
   DGR_TRY(aalloc(c, total, &slab));
-  DGR_TRY(aalloc(c, total_os, &slab_os));
+  DGR_TRY(aalloc(c, total_direct, &slab_direct));
   if (total > 0) DGR_CUDA_CHECK(cudaMemsetAsync(slab, 0, (size_t)total * sizeof(float), c->stream));
-  int64_t ofs = 0, ofs_os = 0;
+  int64_t ofs = 0, ofs_direct = 0;
   auto take = [&](const LayerExec& L) {
-    const bool direct = L.table || L.os || L.bits;
-    float* b = direct ? slab_os + ofs_os : slab + ofs;
-    (direct ? ofs_os : ofs) += (int64_t)L.n_out * L.conv->cout;
+    const bool direct = L.table || L.bits;
+    float* b = direct ? slab_direct + ofs_direct : slab + ofs;
+    (direct ? ofs_direct : ofs) += (int64_t)L.n_out * L.conv->cout;
     return b;
   };
   // max |activation| of every elementwise-pass output, reduced in that pass: the 3xFP16 layers read their
@@ -610,8 +591,8 @@ int32_t run_network(dgr_ctx* c, const dgr_net* net, Plan& p, const float* feats_
   auto conv_bn = [&](const LayerExec& L, const float* feat, const float* residual, int relu, bool want_amax,
                      float** res) -> int32_t {
     float* o = take(L);
-    DGR_TRY(run_conv(c, L, feat, residual, relu, o));
-    if (!L.table && !L.os && !L.bits) {
+    DGR_TRY(run_conv(c, L, feat, o));
+    if (!L.table && !L.bits) {
       float* slot = (want_amax && L.conv->cout % 4 == 0) ? amax_slots + n_slots++ : nullptr;
       DGR_TRY(dgr_affine_act_amax(o, L.n_out, L.conv->cout, L.conv->scale, L.conv->shift, residual, relu, o, slot, st));
       if (slot != nullptr) c->amax_of[o] = slot;
@@ -811,12 +792,11 @@ int32_t dgr_net_create(int32_t device, int32_t D, int32_t in_ch, int32_t out_ch,
   int k3 = 1, k1 = 1;
   for (int a = 0; a < D; ++a) { k3 *= 3; k1 *= conv1_ks; }
   int pi = 0;
-  // os: a stride-1 3^3 layer of the 3-D network, run by the output-stationary kernel (3xTF32 slabs)
-  auto set_conv = [&](Conv& cv, int cin, int cout, int ksize, int K, bool os) -> int32_t {
+  auto set_conv = [&](Conv& cv, int cin, int cout, int ksize, int K) -> int32_t {
     cv.w = params[pi++]; cv.scale = params[pi++]; cv.shift = params[pi++];
     cv.cin = cin; cv.cout = cout; cv.ksize = ksize; cv.K = K;
     cv.tc = dgr_spconv_tc_supported(cin, cout) != 0;
-    cv.f16 = cv.tc && !os && tc_f16_enabled() && cout >= tc_f16_min_cout() &&
+    cv.f16 = cv.tc && tc_f16_enabled() && cout >= tc_f16_min_cout() &&
              dgr_spconv_tc_f16_supported(cin, cout) != 0;
     if (cv.f16) {
       DGR_CUDA_CHECK(cudaMalloc(&cv.packed16, (size_t)4 * K * cin * cout));
@@ -832,25 +812,18 @@ int32_t dgr_net_create(int32_t device, int32_t D, int32_t in_ch, int32_t out_ch,
     return DGR_OK;
   };
   const int enc_in[4] = {in_ch, C[1], C[2], C[3]};
-  const int dec_lvl_ch[4] = {T[2], T[3], T[4], 0};      // decoder block channels at level 0, 1, 2 (none at level 3)
-  for (int l = 0; l < 4; ++l)
-    net->os_level[l] = D == 3 && tc_os_enabled() && !(l == 0 && conv1_ks == 3) &&
-                       dgr_spconv_os_supported(C[l + 1], C[l + 1]) &&
-                       (l == 3 || dgr_spconv_os_supported(dec_lvl_ch[l], dec_lvl_ch[l]));
   int32_t rc = DGR_OK;
   for (int s = 0; s < 4 && rc == DGR_OK; ++s) {
-    const bool os = net->os_level[s];
-    rc = set_conv(net->enc[s], enc_in[s], C[s + 1], s == 0 ? conv1_ks : 3, s == 0 ? k1 : k3, false);
-    if (rc == DGR_OK) rc = set_conv(net->eb1[s], C[s + 1], C[s + 1], 3, k3, os);
-    if (rc == DGR_OK) rc = set_conv(net->eb2[s], C[s + 1], C[s + 1], 3, k3, os);
+    rc = set_conv(net->enc[s], enc_in[s], C[s + 1], s == 0 ? conv1_ks : 3, s == 0 ? k1 : k3);
+    if (rc == DGR_OK) rc = set_conv(net->eb1[s], C[s + 1], C[s + 1], 3, k3);
+    if (rc == DGR_OK) rc = set_conv(net->eb2[s], C[s + 1], C[s + 1], 3, k3);
   }
   const int dec_in[3] = {C[4], C[3] + T[4], C[2] + T[3]};
   const int dec_out[3] = {T[4], T[3], T[2]};
   for (int d = 0; d < 3 && rc == DGR_OK; ++d) {
-    const bool os = net->os_level[2 - d];
-    rc = set_conv(net->dec[d], dec_in[d], dec_out[d], 3, k3, false);
-    if (rc == DGR_OK) rc = set_conv(net->db1[d], dec_out[d], dec_out[d], 3, k3, os);
-    if (rc == DGR_OK) rc = set_conv(net->db2[d], dec_out[d], dec_out[d], 3, k3, os);
+    rc = set_conv(net->dec[d], dec_in[d], dec_out[d], 3, k3);
+    if (rc == DGR_OK) rc = set_conv(net->db1[d], dec_out[d], dec_out[d], 3, k3);
+    if (rc == DGR_OK) rc = set_conv(net->db2[d], dec_out[d], dec_out[d], 3, k3);
   }
   if (rc != DGR_OK) {
     for (auto p : net->owned) cudaFree(p);

@@ -96,42 +96,17 @@ class CoordinateManager:
     return self._map(key.stride).coords
 
   def _map(self, stride):
+    """Coordinate map at `stride`, derived from the stride-1 rows with one host read (floor(c / s) * s composes,
+    and ranking cells by their first stride-1 row reproduces the cascaded first-occurrence order)."""
     if stride not in self._maps:
       assert stride % 2 == 0 and stride > 1, f'no coordinate map at stride {stride}'
-      self._build_maps([stride])
+      coords, tables, n_out = _abi.coarse_maps(self._maps[1].coords, self.spec, [stride])
+      n, overflow = torch.cat([n_out, self.spec[1:2]]).cpu().tolist()
+      _abi.D2H_BYTES += 8
+      if overflow:
+        raise _abi.DgrError('coordinate extent does not fit a 63-bit packed key')
+      self._maps[stride] = _Map(coords[0, :n], tables[0], n)
     return self._maps[stride]
-
-  def _build_maps(self, strides):
-    """Coordinate maps at up to 4 `strides` with one host read, all derived from the stride-1 rows (floor(c / s) * s
-    composes, and ranking cells by their first stride-1 row reproduces the cascaded first-occurrence order)."""
-    coords, tables, n_out = _abi.coarse_maps(self._maps[1].coords, self.spec, strides)
-    *counts, overflow = torch.cat([n_out, self.spec[1:2]]).cpu().tolist()
-    _abi.D2H_BYTES += 4 * (len(strides) + 1)
-    if overflow:
-      raise _abi.DgrError('coordinate extent does not fit a 63-bit packed key')
-    for l, (s, n) in enumerate(zip(strides, counts)):
-      self._maps[s] = _Map(coords[l, :n], tables[l], n)
-
-  def prepare(self, strides, maps):
-    """Build every missing coordinate map of `strides` and every missing kernel map of `maps`
-    ((s_in, conv_stride, kernel_size) triples) with TWO host reads in total instead of one per map:
-    all strided maps come from one read, all kernel-map probes are enqueued before the single read
-    that sizes their pair lists."""
-    todo = [s for s in strides if s not in self._maps]
-    if todo:
-      self._build_maps(todo)
-    pending, keys = [], []
-    for slot, (s_in, conv_stride, ksize) in enumerate(maps):
-      ck = (s_in, s_in * conv_stride, ksize)
-      if ck in self._kmaps or ck in keys:
-        continue
-      m_in, m_out = self._map(s_in), self._map(s_in * conv_stride)
-      keep = self.D == 3 and conv_stride == 1 and ksize > 3
-      pending.append(_abi.kernel_map_begin(m_out.coords, self.spec, m_in.table, m_in.n, self._offs(ksize, s_in),
-                                           keep_table=keep, slot=slot + 1))
-      keys.append(ck)
-    for ck, km in zip(keys, _abi.kernel_maps_finish(pending)):
-      self._kmaps[ck] = km
 
   def _offs(self, kernel_size, stride):
     k = (kernel_size, self.D, stride, self.device)

@@ -5,16 +5,11 @@ Same constructor signature, attribute names (hence state-dict keys) and forward 
 the reference's ``ResUNet2`` (model/resunet.py:419-665, blocks from
 model/residual_block.py:83-134, norms from model/common.py:11-13), so a checkpoint written
 by the reference loads with ``load_state_dict`` unchanged.  The layers are declared from a
-table instead of the reference's spelled-out constructor, and ``forward`` has two
-executions of the same graph:
-
-  * ``forward``        the operator-by-operator path through the ME-shaped modules;
-  * ``forward_fused``  the production path: eval-BatchNorm folded to scale/shift and applied
-                       together with the residual add and ReLU in one pass, ME.cat fused
-                       into the consuming 1x1 convolution, ReLU+bias+L2-normalise fused
-                       into the 1x1 epilogues.
+table instead of the reference's spelled-out constructor.  ``forward`` is the
+operator-by-operator path through the ME-shaped modules (autograd, BatchNorm calibration);
+inference with fused epilogues runs the same graph on the native executor
+(``native.Net``, csrc/exec.cu).
 """
-import torch
 import torch.nn as nn
 
 from .. import _abi
@@ -119,88 +114,6 @@ class ResUNet2(ME.MinkowskiNetwork):
       return ME.SparseTensor(_abi.l2_normalize(out.F), coordinate_map_key=out.coordinate_map_key,
                              coordinate_manager=out.coordinate_manager)
     return out
-
-  # ---------------------------------------------------------------------------------------
-  def _conv_bn(self, feat, conv_mod, norm_mod, km, out, residual=None, relu=False):
-    """sparse conv -> (BN scale/shift [+ residual] [+ ReLU]) in one elementwise pass.
-    `out` is a pre-zeroed [n_out, cout] buffer (or None for the output-stationary conv1)."""
-    scale, shift = norm_mod.folded()
-    if out is None:
-      return _abi.spconv_table_fwd(feat, conv_mod.kernel.detach(), km, conv_mod.out_channels, scale, shift)
-    ME.sparse_conv(feat, conv_mod, km, out)
-    return _abi.affine_act(out, scale=scale, shift=shift, residual=residual, relu=relu, out=out)
-
-  def _uses_table(self, conv_mod, km):
-    return km.nbr is not None and conv_mod.in_channels <= 8 and conv_mod.out_channels in (16, 32, 64)
-
-  def _plan(self, man, key):
-    """All coordinate maps and kernel maps of the network, built up front: this is where every
-    host synchronisation of the forward pass happens (one bucket-offset read per map); the
-    convolution phase that follows is launch-only.  Returns the layers in execution order as
-    (conv module, norm module, kernel map, role) with the total size of their outputs."""
-    s0 = key.stride
-    man.prepare([2 * s0, 4 * s0, 8 * s0],
-                [(s0, 1, self.conv1.kernel_size), (s0, 1, 3), (s0, 2, 3), (2 * s0, 1, 3), (2 * s0, 2, 3),
-                 (4 * s0, 1, 3), (4 * s0, 2, 3), (8 * s0, 1, 3)])
-    layers = []
-    for l in (1, 2, 3, 4):
-      cm = getattr(self, f'conv{l}')
-      key_out, km = man.kernel_map(key, cm.stride, cm.kernel_size)
-      layers.append((cm, getattr(self, f'norm{l}'), km, 'conv'))
-      _, km3 = man.kernel_map(key_out, 1, 3)
-      blk = getattr(self, f'block{l}')
-      layers += [(blk.conv1, blk.norm1, km3, 'b1'), (blk.conv2, blk.norm2, km3, 'b2')]
-      key = key_out
-    for l in (4, 3, 2):
-      cm = getattr(self, f'conv{l}_tr')
-      key_out, km = man.transpose_kernel_map(key, cm.stride, cm.kernel_size)
-      layers.append((cm, getattr(self, f'norm{l}_tr'), km, 'conv'))
-      _, km3 = man.kernel_map(key_out, 1, 3)
-      blk = getattr(self, f'block{l}_tr')
-      layers += [(blk.conv1, blk.norm1, km3, 'b1'), (blk.conv2, blk.norm2, km3, 'b2')]
-      key = key_out
-    total = sum(km.n_out * cm.out_channels for cm, _, km, _ in layers if not self._uses_table(cm, km))
-    return layers, total, key
-
-  def forward_fused(self, x):
-    """Same graph, fused epilogues.  The ReLUs after each block are idempotent (the block
-    already ends in ReLU) and are dropped.  Phase 1 builds every kernel map (all host syncs);
-    phase 2 zero-fills ONE slab holding every convolution output and launches the layers
-    back to back."""
-    man = x.coordinate_manager
-    layers, total, key_final = self._plan(man, x.coordinate_map_key)
-    slab = _abi.scratch(('conv_out', id(self)), max(total, 1), torch.float32, x.device)
-    slab.zero_()
-    ofs = 0
-
-    def take(cm, km):
-      nonlocal ofs
-      if self._uses_table(cm, km):
-        return None
-      n = km.n_out * cm.out_channels
-      buf = slab[ofs:ofs + n].view(km.n_out, cm.out_channels)
-      ofs += n
-      return buf
-
-    feat, skips, block_in, level = x.F, [], None, 0
-    it = iter(layers)
-    for stage in range(7):          # 4 encoder levels, then 3 decoder levels
-      cm, nm, km, _ = next(it)
-      feat = self._conv_bn(feat, cm, nm, km, take(cm, km))
-      c1, n1, km3, _ = next(it)
-      c2, n2, _, _ = next(it)
-      h = self._conv_bn(feat, c1, n1, km3, take(c1, km3), relu=True)
-      feat = self._conv_bn(h, c2, n2, km3, take(c2, km3), residual=feat, relu=True)
-      if stage < 4:
-        skips.append(feat)            # out_s1, out_s2, out_s4, out_s8
-      elif stage < 6:
-        # decoder levels 4 and 3 feed a 3^D transposed conv: materialise ME.cat(decoder, skip)
-        feat = _abi.cat2(feat, skips[2 - (stage - 4)])
-    # conv1_tr reads (decoder, skip) directly: ME.cat fused into the 1x1 convolution
-    h = _abi.linear_fwd(feat, self.conv1_tr.kernel.detach(), None, b=skips[0], relu=True)
-    out = _abi.linear_fwd(h, self.final.kernel.detach(), self.final.bias.detach().reshape(-1).contiguous(),
-                          normalize=bool(self.normalize_feature))
-    return ME.SparseTensor(out, coordinate_map_key=key_final, coordinate_manager=man)
 
 
 class ResUNetBN2(ResUNet2):

@@ -134,9 +134,13 @@ class Net:
     """coords CUDA int32 [n, D+1] (distinct rows), feats [n, in_channels] or None (= ones) -> [n, out]."""
     _abi._chk(coords, torch.int32, 'coords')
     n = coords.shape[0]
-    out = torch.empty(n, self.out_channels, dtype=torch.float32, device=coords.device)
+    if coords.shape != (n, self.D + 1):
+      raise _abi.DgrError(f'coords must be [n, {self.D + 1}], got {list(coords.shape)}')
     if feats is not None:
       _abi._chk(feats, torch.float32, 'feats')
+      if feats.shape != (n, self.in_channels):
+        raise _abi.DgrError(f'feats must be [{n}, {self.in_channels}], got {list(feats.shape)}')
+    out = torch.empty(n, self.out_channels, dtype=torch.float32, device=coords.device)
     # inputs may have been produced on torch's current stream
     torch.cuda.current_stream(coords.device).synchronize()
     _abi.call('dgr_net_forward', ctx.handle, self.handle, _abi.ptr(coords), n, _abi.ptr(feats), _abi.ptr(out))

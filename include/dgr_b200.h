@@ -400,18 +400,6 @@ int32_t dgr_kmap_dense(const int32_t* out_coords, int64_t n_out_max, const int32
                        const uint32_t* bloom_words, int64_t n_bloom_words, const int32_t* offsets, int32_t K,
                        int32_t* nbr, int64_t nbr_stride, int32_t* hit_count, void* stream);
 
-/* ---- output-stationary tensor-core convolution with the fused layer epilogue (csrc/spconv_os.cu) ----------
- * For stride-1 layers whose neighbour table is dense enough (3^3 kernels of the 3-D network, ~64 % occupied):
- *   out[j, :] = act((sum_kappa in_feat[nbr[kappa * nbr_stride + j], :] @ W[kappa]) * scale + shift + residual[j, :])
- * tile = 128 output rows, accumulator in registers across all offsets, 3xTF32 from the packed slabs of
- * dgr_pack_weight_tf32; every output row is written once with plain stores (no atomics, no pre-zeroed buffer,
- * deterministic); eval BatchNorm (model/common.py:13), the residual add and ReLU of BasicBlockBase.forward
- * (model/residual_block.py:118-134) ride in the epilogue.  scale / shift / residual may be NULL. */
-int32_t dgr_spconv_os_supported(int32_t cin, int32_t cout);          /* both % 32 == 0, cout <= 256 */
-int32_t dgr_spconv_os_fwd(const float* in_feat, int32_t cin, const float* weight_t, int32_t cout, const int32_t* nbr,
-                          int64_t nbr_stride, int32_t K, int64_t n_out, const float* scale, const float* shift,
-                          const float* residual, int32_t relu, float* out, void* stream);
-
 /* ---- native executor (csrc/exec.cu) ------------------------------------------------------
  * A context owns a stream (or uses the one given), a grow-only device arena and pinned staging; calls
  * on one context are serialised by the caller, different contexts may be driven from different host

@@ -89,23 +89,23 @@ def _manager(abi, coords_np):
 
 
 @pytest.mark.parametrize('D', [3, 6])
-def test_strided_maps_bit_exact(abi, D):
+def test_strided_and_coarse_maps_bit_exact(abi, D):
   from deepglobalregistration_b200.me.coords import CoordinateMapKey
   g = np.random.default_rng(D)
   c = np.unique(g.integers(-40, 40, size=(6000, D)), axis=0)
   c = c[g.permutation(len(c))]
   coords = np.concatenate([np.zeros((len(c), 1), np.int64), c], 1).astype(np.int32)
-  lazy = _manager(abi, coords)                  # one map per _map() call
-  planned = _manager(abi, coords)
-  planned.prepare([2, 4, 8], [])                # all three from one call
+  man = _manager(abi, coords)                   # one map per _map() call
+  # all three levels from one call, as the executor builds them (dgr_coarse_maps)
+  multi, tables, n_out = abi.coarse_maps(man.coordinates(CoordinateMapKey(1)), man.spec, [2, 4, 8])
+  n_out = n_out.cpu().tolist()
   cur = coords
-  for s in (2, 4, 8):
+  for l, s in enumerate((2, 4, 8)):
     want, _ = so.stride_coords(cur, s)
-    for man in (lazy, planned):
-      got = man.coordinates(CoordinateMapKey(s)).cpu().numpy()
-      assert np.array_equal(got, want), f'stride {s}'
+    for got, table in ((man.coordinates(CoordinateMapKey(s)), man._maps[s].table), (multi[l, :n_out[l]], tables[l])):
+      assert np.array_equal(got.cpu().numpy(), want), f'stride {s}'
       # the table maps every coarse coordinate to its row
-      rows = abi.hash_find(torch.from_numpy(want).cuda(), man.spec, man._maps[s].table).cpu().numpy()
+      rows = abi.hash_find(torch.from_numpy(want).cuda(), man.spec, table).cpu().numpy()
       assert np.array_equal(rows, np.arange(len(want))), f'stride {s}'
     cur = want
 

@@ -195,8 +195,8 @@ def dgr():
   return d, state
 
 
-@pytest.mark.parametrize('which,ks', [('fcgf', 7), ('fcgf', 5), ('fcgf', 3), ('inlier', 3)])
-def test_net_forward_matches_operator_path(abi, dgr, which, ks):
+@pytest.mark.parametrize('which,ks', [('fcgf', 7), ('fcgf', 5), ('fcgf', 3), ('inlier', 3), ('inlier_coords', 3)])
+def test_native_net_forward_matches_operator_path(abi, dgr, which, ks):
   from deepglobalregistration_b200 import native
   from deepglobalregistration_b200 import me as ME
   from deepglobalregistration_b200.model import load_model
@@ -207,22 +207,32 @@ def test_net_forward_matches_operator_path(abi, dgr, which, ks):
     model.load_state_dict(sd)
     model = model.cuda().eval()
     coords = _cloud(3, 7000, 12, seed=ks, batch2=True)
-  else:
+  elif which == 'inlier':
     model = d.inlier_model
     coords = _cloud(6, 5000, 3, seed=9)
+  else:                     # the 'coords' inlier feature type: six input channels, cos of both points
+    model = load_model('ResUNetBN2C')(6, 1, bn_momentum=0.05, conv1_kernel_size=ks, normalize_feature=False, D=6)
+    model.load_state_dict(syn.resunet_state_dict(12, 6, 1, ks, 6))
+    model = model.cuda().eval()
+    coords = _cloud(6, 5000, 3, seed=10)
   ct = torch.from_numpy(coords).cuda().contiguous()
-  feats = torch.ones(len(coords), 1, device='cuda')
+  g = torch.Generator().manual_seed(ks)
+  feats = torch.ones(len(coords), 1) if model.conv1.in_channels == 1 else torch.cos(3 * torch.randn(len(coords), 6, generator=g))
+  feats = feats.cuda().contiguous()
   with torch.no_grad():
-    want = model.forward_fused(ME.SparseTensor(feats, coordinates=ct, device='cuda')).F
+    want = model(ME.SparseTensor(feats, coordinates=ct, device='cuda')).F
   net = native.Net(model, 'cuda')
   ctx = native.Context('cuda')
-  got = net.forward(ctx, ct)
   scale = float(want.abs().max())
-  assert float((got - want).abs().max()) <= 2e-5 * (1 + scale)
+  if model.conv1.in_channels == 1:
+    got = net.forward(ctx, ct)
+    assert float((got - want).abs().max()) <= 2e-5 * (1 + scale)
   got2 = net.forward(ctx, ct, feats)                     # explicit features, second call on a warm arena
   assert float((got2 - want).abs().max()) <= 2e-5 * (1 + scale)
   st = ctx.stats()
   assert st['host_reads'] == 1
+  with pytest.raises(abi.DgrError):
+    net.forward(ctx, ct, torch.ones(len(coords), model.conv1.in_channels + 1, device='cuda'))
   net.close(); ctx.close()
 
 
@@ -265,6 +275,50 @@ def test_pair_register_native_vs_stagewise_vs_oracle(abi, dgr):
   te, re = syn.rte_rre(T_i, T_oi)
   assert te <= 1e-3 and re <= 1e-3, (te, re)
   d.use_icp = False
+
+
+def test_register_stagewise_coords_feature_type_vs_oracle(abi):
+  """The 'coords' inlier feature type (six input channels: cos of both points) runs stage by stage."""
+  from oracle import pipeline as op
+  from deepglobalregistration_b200.core.deep_global_registration import DeepGlobalRegistration
+  state = syn.make_checkpoint(0, inlier_feature_type='coords')
+  d = DeepGlobalRegistration(types.SimpleNamespace(weights=state, clip_weight_thresh=0.05, verbose=False))
+  d.use_icp = False
+  xyz0, xyz1, _ = syn.room_pair(2, n_raw=20000, extent=(1.8, 1.5, 1.25))
+  T_o, taps = op.register(state, xyz0, xyz1)
+  T = d.register_stagewise(xyz0, xyz1)
+  assert d.last_branch == taps['branch'] == 'procrustes'
+  te, re = syn.rte_rre(T, T_o)
+  assert te <= 1e-3 and re <= 1e-3, (te, re)
+
+
+def test_stage_methods_leave_the_taps_of_register(dgr):
+  """The stage methods run on a context of their own: a call after register() keeps its taps."""
+  d, _ = dgr
+  xyz0, xyz1, _ = syn.room_pair(4, n_raw=15000, extent=(1.8, 1.5, 1.25))
+  d.register(xyz0, xyz1)
+  ctx = d._last_ctx
+  sel, F = d._last_sel.clone(), ctx.tap('features')
+  coords, c6 = ctx.tap('coords'), ctx.tap('coords6')
+  F2 = d.fcgf_feature_extraction(torch.ones(len(coords), 1, device='cuda'), coords)
+  d.inlier_prediction(torch.ones(len(c6), 1, device='cuda'), c6)
+  assert d._last_ctx is ctx
+  assert torch.equal(d._last_sel, sel) and torch.equal(ctx.tap('features'), F)
+  assert float((F2 - F).abs().max()) <= 5e-5
+
+
+def test_stage_methods_reject_malformed_input(abi, dgr):
+  d, _ = dgr
+  c = torch.from_numpy(_cloud(3, 500, 8, seed=3)).cuda()
+  dup = torch.cat((c, c[:1]), 0)
+  with pytest.raises(ValueError):
+    d.fcgf_feature_extraction(torch.ones(len(dup), 1, device='cuda'), dup)
+  c6 = torch.from_numpy(_cloud(6, 500, 3, seed=4)).cuda()
+  dup6 = torch.cat((c6, c6[-1:]), 0)
+  with pytest.raises(ValueError):
+    d.inlier_prediction(torch.ones(len(dup6), 1, device='cuda'), dup6)
+  with pytest.raises(abi.DgrError):
+    d.fcgf_feature_extraction(torch.ones(len(c), 2, device='cuda'), c)
 
 
 def test_register_batch_two_in_flight_equals_serial(dgr):
@@ -339,51 +393,6 @@ def test_conv_3xfp16_matches_fp32_and_3xtf32(abi, D, cin, cout, n, ext, scale):
   e32 = float((out32.double() - ref64).abs().max()) / mag
   print(f'D={D} {cin}->{cout} scale {scale}: 3xFP16 err {e16:.2e}, 3xTF32 err {e32:.2e} (relative to max |out|)')
   assert e16 <= 2e-6 and e16 <= 4 * e32 + 2e-7, (e16, e32)
-
-
-@pytest.mark.parametrize('cin,cout,n,ext', [(32, 32, 6000, 11), (64, 64, 3000, 9), (128, 128, 900, 6), (256, 256, 700, 6),
-                                             (64, 32, 150, 3), (32, 96, 5000, 10)])
-def test_output_stationary_conv_with_fused_epilogue(abi, cin, cout, n, ext):
-  """dgr_spconv_os_fwd (tile = 128 output rows, accumulator across all 27 offsets, BatchNorm / residual / ReLU in
-  the epilogue) against the weight-stationary kernel + dgr_affine_act, and against a float64 reference."""
-  from deepglobalregistration_b200.me.coords import CoordinateMapKey, kernel_offsets
-  coords = _cloud(3, n, ext, seed=cin + cout + n)
-  ct = torch.from_numpy(coords).cuda().contiguous()
-  man, spec, table = _spec_and_table(abi, ct)
-  _, km = man.kernel_map(CoordinateMapKey(1), 1, 3)
-  nrow = len(coords)
-  nbr = torch.empty(27, nrow, dtype=torch.int32, device='cuda')
-  offs = kernel_offsets(3, 3, 1, torch.device('cuda'))
-  abi.call('dgr_kmap_dense', abi.ptr(ct), nrow, None, 4, abi.ptr(spec), abi.ptr(table.keys), abi.ptr(table.vals),
-           table.cap, None, 0, abi.ptr(offs), 27, abi.ptr(nbr), nrow, None, abi.stream())
-  g = torch.Generator().manual_seed(n)
-  feat = torch.randn(nrow, cin, generator=g).cuda()
-  W = (torch.randn(27, cin, cout, generator=g) / np.sqrt(cin * 17)).cuda().contiguous()
-  scale = (1 + 0.1 * torch.randn(cout, generator=g)).cuda()
-  shift = (0.1 * torch.randn(cout, generator=g)).cuda()
-  res = torch.randn(nrow, cout, generator=g).cuda()
-  Wt = abi.pack_weight_tf32(W, 27, cin, cout)
-  # float64 reference through the pair lists
-  ref = torch.zeros(nrow, cout, dtype=torch.float64, device='cuda')
-  ii, jj, kofs = km.in_idx[:km.n_pairs].long(), km.out_idx[:km.n_pairs].long(), km.kofs_host
-  for kap in range(27):
-    a, b = int(kofs[kap]), int(kofs[kap + 1])
-    if b > a:
-      ref.index_add_(0, jj[a:b], feat[ii[a:b]].double() @ W[kap].double())
-  for use_affine, use_res, relu in ((True, True, True), (True, False, True), (False, False, False)):
-    want = ref * scale.double() + shift.double() if use_affine else ref.clone()
-    if use_res:
-      want = want + res.double()
-    if relu:
-      want = want.clamp_min(0)
-    got = abi.spconv_os_fwd(feat, Wt, nbr, cout, scale if use_affine else None, shift if use_affine else None,
-                            res if use_res else None, relu)
-    torch.cuda.synchronize()
-    err = float((got.double() - want).abs().max()) / (1 + float(want.abs().max()))
-    assert err <= 3e-5, (use_affine, use_res, relu, err)     # one fp32 accumulator over all 27 x cin products
-    got2 = abi.spconv_os_fwd(feat, Wt, nbr, cout, scale if use_affine else None, shift if use_affine else None,
-                             res if use_res else None, relu)
-    assert torch.equal(got, got2)          # deterministic: no atomics
 
 
 def test_conv1_from_occupancy_masks_equals_table_kernel(abi):

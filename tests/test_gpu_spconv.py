@@ -196,9 +196,18 @@ def _small_pair_cloud(seed=0, n_raw=20000):
   return so.batched_coordinates([coords])
 
 
-@pytest.mark.parametrize('fused', [False, True])
-def test_resunet_fcgf_forward(abi, fused):
-  from deepglobalregistration_b200 import me as ME
+def _forward(model, coords, path):
+  """The network on all-ones input: operator by operator, or on the native executor."""
+  from deepglobalregistration_b200 import me as ME, native
+  ct = torch.from_numpy(coords).cuda().contiguous()
+  if path == 'native':
+    return native.Net(model, 'cuda').forward(native.Context('cuda'), ct)
+  with torch.no_grad():
+    return model(ME.SparseTensor(torch.ones(len(coords), 1), coordinates=ct, device='cuda')).F
+
+
+@pytest.mark.parametrize('path', ['operator', 'native'])
+def test_resunet_fcgf_forward(abi, path):
   from deepglobalregistration_b200.model import load_model
   state = syn.make_checkpoint(0, with_inlier=False)
   coords = _small_pair_cloud()
@@ -207,16 +216,13 @@ def test_resunet_fcgf_forward(abi, fused):
   model = load_model('ResUNetBN2C')(1, 32, bn_momentum=0.05, conv1_kernel_size=7, normalize_feature=True)
   model.load_state_dict(state['state_dict'])
   model = model.cuda().eval()
-  with torch.no_grad():
-    x = ME.SparseTensor(torch.ones(len(coords), 1), coordinates=torch.from_numpy(coords), device='cuda')
-    got = (model.forward_fused(x) if fused else model(x)).F
+  got = _forward(model, coords, path)
   _close(got, want, tol=5e-5, what='FCGF features')
   assert torch.allclose(got.norm(dim=1).cpu(), torch.ones(len(coords)), atol=1e-5)
 
 
-@pytest.mark.parametrize('fused', [False, True])
-def test_resunet_inlier_forward_6d(abi, fused):
-  from deepglobalregistration_b200 import me as ME
+@pytest.mark.parametrize('path', ['operator', 'native'])
+def test_resunet_inlier_forward_6d(abi, path):
   from deepglobalregistration_b200.model import load_model
   sd = syn.resunet_state_dict(5, 1, 1, 3, 6)
   g = np.random.default_rng(0)
@@ -231,7 +237,5 @@ def test_resunet_inlier_forward_6d(abi, fused):
   model = load_model('ResUNetBN2C')(1, 1, bn_momentum=0.05, conv1_kernel_size=3, normalize_feature=False, D=6)
   model.load_state_dict(sd)
   model = model.cuda().eval()
-  with torch.no_grad():
-    x = ME.SparseTensor(torch.ones(n, 1), coordinates=torch.from_numpy(coords6), device='cuda')
-    got = (model.forward_fused(x) if fused else model(x)).F
+  got = _forward(model, coords6, path)
   _close(got, want, tol=5e-5, what='inlier logits')

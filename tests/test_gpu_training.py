@@ -64,7 +64,7 @@ def test_conv_backward_matches_oracle_autograd(D, cin, cout, stride, transpose):
   assert rel(gw, wo.grad) <= 2e-5, rel(gw, wo.grad)
 
 
-def test_training_step_through_the_network():
+def test_training_step_then_native_inference():
   """ResUNetBN2C in train() mode (BatchNorm on batch statistics): loss.backward() reaches every parameter, the
   gradients are finite, running statistics move, and two SGD steps reduce the loss."""
   from deepglobalregistration_b200 import me as ME
@@ -87,11 +87,13 @@ def test_training_step_through_the_network():
     opt.step()
   assert losses[2] < losses[0], losses
   assert not torch.equal(rm0, net.norm1.bn.running_mean)
-  # back to inference: eval() + no_grad() is the forward-only path and matches the fused executor
+  # back to inference: eval() + no_grad() is the forward-only path and matches the native executor
+  from deepglobalregistration_b200 import native
   net.eval()
   with torch.no_grad():
     x = ME.SparseTensor(torch.ones(len(coords), 1), coordinates=coords, device='cuda')
-    a, b = net(x).F, net.forward_fused(x).F
+    a = net(x).F
+  b = native.Net(net, 'cuda').forward(native.Context('cuda'), coords.cuda().contiguous(), x.F)
   assert float((a - b).abs().max()) <= 2e-5 * (1 + float(a.abs().max()))
 
 

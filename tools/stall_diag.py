@@ -5,8 +5,6 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
 from deepglobalregistration_b200 import _abi, synthetic as syn
 from deepglobalregistration_b200.core.deep_global_registration import DeepGlobalRegistration
-from deepglobalregistration_b200.me import SparseTensor
-from deepglobalregistration_b200.me.coords import CoordinateManager
 
 state = syn.make_checkpoint(0)
 dgr = DeepGlobalRegistration(types.SimpleNamespace(weights=state, clip_weight_thresh=0.05, verbose=False))
@@ -29,15 +27,10 @@ for step in range(300):
     with torch.no_grad():
       _abi.refresh_stream()
       x0, c0, _ = dgr.preprocess(a, 0, _batch=0); x1, c1, _ = dgr.preprocess(b, 1, _batch=1); t.append(sync())
-      coords = torch.cat((c0, c1), 0); coords._dgr_manager = CoordinateManager(coords, assume_unique=True)
-      xs = SparseTensor(torch.ones(coords.shape[0], 1, device='cuda'), coordinates=coords, device='cuda')
-      layers, total, kf = dgr.fcgf_model._plan(xs.coordinate_manager, xs.coordinate_map_key); t.append(sync())
-      F = dgr.fcgf_model.forward_fused(xs).F; t.append(sync())
-      idx1 = _abi.knn_top1(F[:len(c0)], F[len(c0):]); t.append(sync())
-      c6 = _abi.inlier_coords(c0, c1, idx1); c6._dgr_manager = CoordinateManager(c6, assume_unique=True)
-      x6 = SparseTensor(torch.ones(len(idx1), 1, device='cuda'), coordinates=c6, device='cuda')
-      dgr.inlier_model._plan(x6.coordinate_manager, x6.coordinate_map_key); t.append(sync())
-      logit = dgr.inlier_model.forward_fused(x6).F; t.append(sync())
+      F0, F1 = dgr.fcgf_feature_extraction_pair(c0, c1); t.append(sync())
+      idx1 = _abi.knn_top1(F0, F1); t.append(sync())
+      c6 = _abi.inlier_coords(c0, c1, idx1)
+      logit = dgr._stage_forward(dgr.native_networks()[1], c6, unique=True); t.append(sync())
       w, ws = _abi.sigmoid_clip_sum(logit, 0.05)
       res = _abi.se3_register(x0, x1, w.reshape(-1), idx1=idx1, quantization_size=0.1, break_threshold_ratio=1e-4).cpu(); t.append(sync())
   rows.append((t[0] - t_begin, [1e3 * (y - x) for x, y in zip(t[:-1], t[1:])]))
@@ -46,7 +39,7 @@ tot = np.array([sum(r[1]) for r in rows])
 print(mode, 'median %.2f mean %.2f max %.1f  n>25ms %d' % (np.median(tot), tot.mean(), tot.max(), (tot > 25).sum()))
 for k in ('num_device_alloc', 'num_device_free', 'num_alloc_retries', 'reserved_bytes.all.current', 'num_sync_all_streams'):
   print(' ', k, st0.get(k), '->', st1.get(k))
-names = ['preproc', 'fcgf_plan', 'fcgf_conv', 'knn', 'inl_plan', 'inl_conv', 'refine+read']
+names = ['preproc', 'fcgf', 'knn', 'inlier', 'refine+read']
 med = np.median(np.array([r[1] for r in rows]), 0) if mode != 'plain' else None
 if med is not None: print('  median per phase', dict(zip(names, np.round(med, 2))))
 for ts, ph in rows:
