@@ -54,10 +54,9 @@ SIGNATURES = {
     'dgr_knn_top1_tc': [_p, _i64, _p, _i64, _i32, _p, _p, _p, _p, _p],
     'dgr_inlier_coords': [_p, _p, _p, _i64, _p, _p],
     'dgr_sigmoid_clip_sum': [_p, _i64, _f32, _p, _p, _p],
-    'dgr_icp_point_to_point': [_p, _i64, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _p, _i32, _f64, _f64, _p, _p, _p],
     'dgr_estimate_normals': [_p, _i64, _p, _p, _p, _i64, _i32, _f64, _f64, _i32, _p, _p, _p, _p],
-    'dgr_icp_plane_ws_elems': [_i64, _p],
-    'dgr_icp_point_to_plane': [_p, _i64, _p, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _p, _i32, _f64, _f64, _p, _p, _p],
+    'dgr_icp_ws_elems': [_i64, _p],
+    'dgr_icp': [_p, _i64, _p, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _p, _i32, _f64, _f64, _p, _p, _p],
     'dgr_ransac_ws_elems': [_i64, _i64, _p],
     'dgr_ransac_correspondence': [_p, _p, _p, _p, _i64, _f64, _i64, C.c_uint64, _p, _p, _p],
     'dgr_ransac_fm_ws_elems': [_i64, _i64, _i64, _p],
@@ -593,24 +592,6 @@ def se3_register(x, y, w, idx1=None, quantization_size=1.0, max_iter=1000, max_b
   return res
 
 
-def icp_point_to_point(src, tgt, tgt_manager, voxel, max_dist, T_init, max_iter=30, rel_fitness=1e-6,
-                       rel_rmse=1e-6, batch=0):
-  """Point-to-point ICP (open3d defaults) of src onto tgt through tgt's voxel hash.
-  src / tgt: CUDA float32 [n, 3]; tgt_manager: the CoordinateManager preprocess() built for tgt;
-  T_init: 4x4 (numpy / tensor) or device double [12].  -> device double [20]."""
-  _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
-  dev = src.device
-  m = tgt_manager._maps[1]
-  if not (isinstance(T_init, torch.Tensor) and T_init.is_cuda and T_init.numel() == 12):
-    T_init = torch.as_tensor(T_init, dtype=torch.float64).reshape(4, 4)[:3].contiguous().to(dev)
-  state = torch.empty(64, dtype=torch.float64, device=dev)
-  res = torch.empty(20, dtype=torch.float64, device=dev)
-  call('dgr_icp_point_to_point', ptr(src), src.shape[0], ptr(tgt), ptr(tgt_manager.spec), ptr(m.table.keys),
-       ptr(m.table.vals), m.table.cap, int(batch), float(voxel), float(max_dist), ptr(T_init), int(max_iter),
-       float(rel_fitness), float(rel_rmse), ptr(state), ptr(res), stream())
-  return res
-
-
 MAX_NN = 64            # dgr_estimate_normals' bound on the neighbours per point
 
 
@@ -641,27 +622,42 @@ def estimate_normals(xyz, manager_or_table, cell, radius, max_nn, prev=None, ret
   return (normals, counts) if return_counts else normals
 
 
-def icp_point_to_plane(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter=30, rel_fitness=1e-6,
-                       rel_rmse=1e-6, batch=0):
-  """Point-to-plane ICP (open3d's TransformationEstimationPointToPlane, default criteria) of src onto tgt through
-  tgt's voxel hash; arguments as icp_point_to_point plus tgt_normals (CUDA float32 [n_tgt, 3]); tgt_manager may
-  also be a (spec, table) pair.  -> device double [20] (pose 16, fitness, inlier RMSE, iterations,
-  correspondences)."""
-  _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt'); _chk(tgt_normals, torch.float32, 'tgt_normals')
-  if tgt_normals.shape != tgt.shape:
-    raise DgrError('tgt_normals must hold one normal per target point')
+def _icp(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter, rel_fitness, rel_rmse, batch):
+  _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
+  if tgt_normals is not None:
+    _chk(tgt_normals, torch.float32, 'tgt_normals')
+    if tgt_normals.shape != tgt.shape:
+      raise DgrError('tgt_normals must hold one normal per target point')
   dev = src.device
   spec, table = _hash_of(tgt_manager)
   if not (isinstance(T_init, torch.Tensor) and T_init.is_cuda and T_init.numel() == 12):
     T_init = torch.as_tensor(T_init, dtype=torch.float64).reshape(4, 4)[:3].contiguous().to(dev)
   words = C.c_int64(0)
-  call('dgr_icp_plane_ws_elems', src.shape[0], C.byref(words))
-  ws = scratch('icp_plane', words.value, torch.float64, dev)
+  call('dgr_icp_ws_elems', src.shape[0], C.byref(words))
+  ws = scratch('icp', words.value, torch.float64, dev)
   res = torch.empty(20, dtype=torch.float64, device=dev)
-  call('dgr_icp_point_to_plane', ptr(src), src.shape[0], ptr(tgt), ptr(tgt_normals), ptr(spec), ptr(table.keys),
-       ptr(table.vals), table.cap, int(batch), float(voxel), float(max_dist), ptr(T_init), int(max_iter),
-       float(rel_fitness), float(rel_rmse), ptr(ws), ptr(res), stream())
+  # ptr() of an empty tgt_normals is 0, which selects point-to-point; without target points neither update has a
+  # correspondence, so both give the same result
+  call('dgr_icp', ptr(src), src.shape[0], ptr(tgt), ptr(tgt_normals), ptr(spec), ptr(table.keys), ptr(table.vals),
+       table.cap, int(batch), float(voxel), float(max_dist), ptr(T_init), int(max_iter), float(rel_fitness),
+       float(rel_rmse), ptr(ws), ptr(res), stream())
   return res
+
+
+def icp_point_to_point(src, tgt, tgt_manager, voxel, max_dist, T_init, max_iter=30, rel_fitness=1e-6,
+                       rel_rmse=1e-6, batch=0):
+  """Point-to-point ICP (open3d defaults) of src onto tgt through tgt's voxel hash.
+  src / tgt: CUDA float32 [n, 3]; tgt_manager: the CoordinateManager preprocess() built for tgt, or (spec, table)
+  of a dgr_unique_first table of tgt at `voxel` (batch column `batch`); T_init: 4x4 (numpy / tensor) or device
+  double [12].  -> device double [20] (pose 16, fitness, inlier RMSE, iterations, correspondences)."""
+  return _icp(src, tgt, None, tgt_manager, voxel, max_dist, T_init, max_iter, rel_fitness, rel_rmse, batch)
+
+
+def icp_point_to_plane(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter=30, rel_fitness=1e-6,
+                       rel_rmse=1e-6, batch=0):
+  """Point-to-plane ICP (open3d's TransformationEstimationPointToPlane, default criteria) of src onto tgt through
+  tgt's voxel hash; arguments as icp_point_to_point plus tgt_normals (CUDA float32 [n_tgt, 3])."""
+  return _icp(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter, rel_fitness, rel_rmse, batch)
 
 
 def ransac_correspondence(x, y, idx0, idx1, max_dist, num_hyp=4000000, seed=0):

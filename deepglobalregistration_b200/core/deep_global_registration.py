@@ -31,7 +31,7 @@ class DeepGlobalRegistration:
     # and the 80000 it passes lands in open3d's confidence slot (clamped to 1 = no early exit).
     self.safeguard_max_iteration = 4000000
     self.safeguard_seed = 0       # open3d draws from std::random_device; here a call is reproducible
-    self.use_icp = True           # as the reference; GPU point-to-point ICP (dgr_icp_point_to_point)
+    self.use_icp = True           # as the reference; GPU point-to-point ICP (dgr_icp)
     self.verbose = getattr(config, 'verbose', True)
     self.feat_timer = Timer()
     self.reg_timer = Timer()

@@ -7,7 +7,7 @@
 
 Voxelise both clouds (the wrapped object's ``preprocess`` and ``voxel_size``; no FCGF) -> point_to_plane: target
 normals from neighbours within 2 voxels, at most 30 (dgr_estimate_normals, util/pointcloud.py:60's setting), through
-cloud 1's voxel table -> ICP from ``init`` through the same table (dgr_icp_point_to_plane / dgr_icp_point_to_point)
+cloud 1's voxel table -> ICP from ``init`` through the same table (dgr_icp, with or without the normals)
 -> one readback.
 """
 import numpy as np

@@ -108,6 +108,23 @@ __device__ __forceinline__ int32_t dgr_hash_lookup(const uint64_t* __restrict__ 
   }
 }
 
+// Row in cell c (0 <= c < side^3, x fastest) of the block of side = 2 reach + 1 cells centred on cell c3, batch
+// column `batch`, or -1 when that cell is empty or outside the key spec's range
+__device__ __forceinline__ int32_t dgr_probe_cell(int c, int side, int reach, const int c3[3], int32_t batch,
+                                                  const dgr_keyspec_t& s, const uint64_t* __restrict__ keys,
+                                                  const int32_t* __restrict__ vals, uint64_t mask) {
+  const int dx = c % side - reach, dy = (c / side) % side - reach, dz = c / (side * side) - reach;
+  const int32_t row[4] = {batch, c3[0] + dx, c3[1] + dy, c3[2] + dz};
+  bool inside = true;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const long long d = (long long)row[q] - s.lo[q];
+    inside = inside && d >= 0 && d < (1ll << s.bits[q]);
+  }
+  if (!inside) return -1;
+  return dgr_hash_lookup(keys, vals, mask, dgr_pack_key(row, s));
+}
+
 // Nearest target row strictly within sqrt(best) of the point p, through a voxel hash holding at most one
 // target point per cell of size `cell` (the cells within `reach` = ceil(radius / cell) of p's cell on every
 // side are the candidates).  8 lanes share one query point: an aligned group of 8 lanes of the warp, lane
@@ -126,16 +143,7 @@ __device__ __forceinline__ void dgr_voxel_nearest8(const double p[3], bool have,
   for (int a = 0; a < 3; ++a) c3[a] = (int)floor(p[a] / cell);
   best_j = -1;
   for (int c = sub; c < n_cells && have; c += 8) {
-    const int dx = c % side - reach, dy = (c / side) % side - reach, dz = c / (side * side) - reach;
-    const int32_t row[4] = {batch, c3[0] + dx, c3[1] + dy, c3[2] + dz};
-    bool inside = true;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const long long d = (long long)row[q] - s.lo[q];
-      inside = inside && d >= 0 && d < (1ll << s.bits[q]);
-    }
-    if (!inside) continue;
-    const int32_t j = dgr_hash_lookup(keys, vals, mask, dgr_pack_key(row, s));
+    const int32_t j = dgr_probe_cell(c, side, reach, c3, batch, s, keys, vals, mask);
     if (j < 0) continue;
     const double ex = p[0] - tgt[3 * (int64_t)j], ey = p[1] - tgt[3 * (int64_t)j + 1],
                  ez = p[2] - tgt[3 * (int64_t)j + 2];

@@ -1040,15 +1040,17 @@ int32_t dgr_pair_register(dgr_ctx_t* c, dgr_net_t* fcgf, dgr_net_t* inlier, cons
   DGR_TRY(dgr_se3_register(xyz, xyz1p, idx1, w, N0, (float)(2 * voxel), 1000, 20, 1e-4f, 0.1f, 0.999f, pack_ws,
                            cnt_ws, se3, st));
   if (use_icp) {
-    double *T12, *state;
+    double *T12, *icp_ws;
+    int64_t icp_words = 0;
+    DGR_TRY(dgr_icp_ws_elems(N0, &icp_words));
     DGR_TRY(aalloc(c, 12, &T12));
-    DGR_TRY(aalloc(c, 64, &state));
+    DGR_TRY(aalloc(c, icp_words, &icp_ws));
     DGR_TRY(aalloc(c, 20, &icp_res));
     pose_to_T12_kernel<<<1, 32, 0, c->stream>>>(se3, T12);
     dgr_note_launches(1);
     // nearest target point through the pair's voxel hash: rows of cloud 1 are rows N0.. of `xyz` (batch 1)
-    DGR_TRY(dgr_icp_point_to_point(xyz, N0, xyz, spec, keys, vals, cap, 1, voxel, 2 * voxel, T12, 30, 1e-6, 1e-6,
-                                   state, icp_res, st));
+    DGR_TRY(dgr_icp(xyz, N0, xyz, nullptr, spec, keys, vals, cap, 1, voxel, 2 * voxel, T12, 30, 1e-6, 1e-6, icp_ws,
+                    icp_res, st));
   }
   mark_stage(c, ranges, 9);                                        // 9: weights + Procrustes + refinement (+ ICP)
   pack_result_kernel<<<1, 64, 0, c->stream>>>(se3, wsum, icp_res, c->res_dev);
@@ -1096,12 +1098,13 @@ int32_t dgr_pair_safeguard(dgr_ctx_t* c, double max_dist, int64_t num_hyp, uint6
   DGR_TRY(dgr_ransac_correspondence(c->pair_xyz, c->pair_xyz + 3 * N0, nullptr, c->pair_idx1, N0, max_dist, num_hyp,
                                     seed, ws, res, st));
   if (use_icp) {
-    double* state;
-    DGR_TRY(aalloc(c, 64, &state));
+    double* icp_ws;
+    int64_t icp_words = 0;
+    DGR_TRY(dgr_icp_ws_elems(N0, &icp_words));
+    DGR_TRY(aalloc(c, icp_words, &icp_ws));
     icp_res = res + 20;
-    DGR_TRY(dgr_icp_point_to_point(c->pair_xyz, N0, c->pair_xyz, c->pair_spec, c->pair_keys, c->pair_vals,
-                                   c->pair_cap, 1, c->pair_voxel, 2 * c->pair_voxel, res, 30, 1e-6, 1e-6, state,
-                                   icp_res, st));
+    DGR_TRY(dgr_icp(c->pair_xyz, N0, c->pair_xyz, nullptr, c->pair_spec, c->pair_keys, c->pair_vals, c->pair_cap, 1,
+                    c->pair_voxel, 2 * c->pair_voxel, res, 30, 1e-6, 1e-6, icp_ws, icp_res, st));
   }
   DGR_CUDA_CHECK(cudaMemcpyAsync(c->res_host, res, 40 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   DGR_CUDA_CHECK(cudaStreamSynchronize(c->stream));

@@ -1,5 +1,5 @@
-// Small fp64 solvers shared by registration.cu (weighted Procrustes, ICP), ransac.cu (4-point hypotheses), fgr.cu
-// (Gauss-Newton steps) and icp_plane.cu (normals, point-to-plane steps).
+// Small fp64 solvers shared by registration.cu (weighted Procrustes), ransac.cu (4-point hypotheses), fgr.cu
+// (Gauss-Newton steps) and icp.cu (normals, ICP steps).
 #pragma once
 
 // ---------------------------------------------------------------------------------------

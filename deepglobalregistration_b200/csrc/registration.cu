@@ -429,133 +429,6 @@ se3_register_kernel(const float* __restrict__ pack, int64_t n, float q, int max_
   cluster.sync();   // nobody exits while peers may still write into its shared memory
 }
 
-
-// ---------------------------------------------------------------------------------------
-// point-to-point ICP (open3d registration_icp as called at core/deep_global_registration.py:
-// 317-322): nearest target point within a radius through the target's voxel hash, Kabsch
-// update in fp64, open3d's convergence rule.  No host round trip: all max_iter + 1
-// (match, update) launch pairs are enqueued up front and turn into no-ops once the
-// device-side `done` flag is set.
-// ---------------------------------------------------------------------------------------
-struct IcpState {
-  double T[12];          // current pose, row-major [R | t]
-  double sums[17];       // n, sum d2, sum p (3), sum q (3), sum q p^T (9)
-  double prev_fitness, prev_rmse, fitness, rmse;
-  int iteration, done;
-};
-
-__global__ void icp_init_kernel(const double* __restrict__ T_init, IcpState* st) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) {
-    for (int k = 0; k < 12; ++k) st->T[k] = T_init[k];
-    for (int k = 0; k < 17; ++k) st->sums[k] = 0.0;
-    st->prev_fitness = st->prev_rmse = st->fitness = st->rmse = 0.0;
-    st->iteration = 0;
-    st->done = 0;
-  }
-}
-
-__global__ void __launch_bounds__(256)
-icp_match_kernel(const float* __restrict__ src, int64_t n_src, const float* __restrict__ tgt,
-                 const dgr_keyspec_t* __restrict__ spec_p, const uint64_t* __restrict__ keys,
-                 const int32_t* __restrict__ vals, uint64_t mask, int32_t batch, double voxel, double max_dist,
-                 IcpState* st) {
-  if (st->done) return;
-  const dgr_keyspec_t s = *spec_p;
-  double T[12];
-#pragma unroll
-  for (int k = 0; k < 12; ++k) T[k] = st->T[k];
-  double acc[17];
-#pragma unroll
-  for (int k = 0; k < 17; ++k) acc[k] = 0.0;
-  const int reach = (int)ceil(max_dist / voxel);     // cells to search on every side (2 for DGR)
-  // 8 lanes share one source point (dgr_voxel_nearest8); lane 0 of the group accumulates the moments
-  const int sub = threadIdx.x & 7;
-  const int64_t groups = ((int64_t)gridDim.x * blockDim.x) >> 3;
-  for (int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 3; i0 < ((n_src + groups - 1) / groups) * groups;
-       i0 += groups) {
-    const bool have = i0 < n_src;                      // whole warps stay in the loop for the shuffles
-    const int64_t i = have ? i0 : 0;
-    const double x = src[3 * i], y = src[3 * i + 1], z = src[3 * i + 2];
-    const double p[3] = {T[0] * x + T[1] * y + T[2] * z + T[3], T[4] * x + T[5] * y + T[6] * z + T[7],
-                         T[8] * x + T[9] * y + T[10] * z + T[11]};
-    double best = max_dist * max_dist;
-    int best_j;
-    dgr_voxel_nearest8(p, have, sub, tgt, s, keys, vals, mask, batch, voxel, reach, best, best_j);
-    if (have && sub == 0 && best_j >= 0) {
-      const double q[3] = {tgt[3 * (int64_t)best_j], tgt[3 * (int64_t)best_j + 1], tgt[3 * (int64_t)best_j + 2]};
-      acc[0] += 1.0;
-      acc[1] += best;
-#pragma unroll
-      for (int a = 0; a < 3; ++a) {
-        acc[2 + a] += p[a];
-        acc[5 + a] += q[a];
-#pragma unroll
-        for (int b = 0; b < 3; ++b) acc[8 + 3 * a + b] += q[a] * p[b];
-      }
-    }
-  }
-  __shared__ double red[8][17];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < 17; ++k) {
-    double v = acc[k];
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
-    if (lane == 0) red[warp][k] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < 17) {
-    double v = 0.0;
-    for (int w = 0; w < 8; ++w) v += red[w][threadIdx.x];
-    if (v != 0.0) atomicAdd(&st->sums[threadIdx.x], v);
-  }
-}
-
-__global__ void icp_update_kernel(IcpState* st, int64_t n_src, int max_iter, double rel_fitness, double rel_rmse,
-                                  double* __restrict__ result) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  if (!st->done) {
-    const double n = st->sums[0];
-    double fitness, rmse;
-    const bool stop = icp_stop_rule(*st, n, st->sums[1], n_src, max_iter, rel_fitness, rel_rmse, fitness, rmse);
-    const int k = st->iteration;
-    st->fitness = fitness;
-    st->rmse = rmse;
-    if (stop) {
-      st->done = 1;
-    } else {
-      double R[3][3] = {{1, 0, 0}, {0, 1, 0}, {0, 0, 1}}, t[3] = {0, 0, 0};
-      if (n > 0) {
-        double mp[3], mq[3], S[3][3];
-        for (int a = 0; a < 3; ++a) { mp[a] = st->sums[2 + a] / n; mq[a] = st->sums[5 + a] / n; }
-        for (int a = 0; a < 3; ++a)
-          for (int b = 0; b < 3; ++b) S[a][b] = st->sums[8 + 3 * a + b] / n - mq[a] * mp[b];
-        kabsch_rotation(S, R);
-        for (int a = 0; a < 3; ++a) t[a] = mq[a] - (R[a][0] * mp[0] + R[a][1] * mp[1] + R[a][2] * mp[2]);
-      }
-      double Tn[12];
-      for (int a = 0; a < 3; ++a) {
-        for (int b = 0; b < 4; ++b) {
-          double v = R[a][0] * st->T[b] + R[a][1] * st->T[4 + b] + R[a][2] * st->T[8 + b];
-          if (b == 3) v += t[a];
-          Tn[4 * a + b] = v;
-        }
-      }
-      for (int q = 0; q < 12; ++q) st->T[q] = Tn[q];
-      st->prev_fitness = fitness;
-      st->prev_rmse = rmse;
-      st->iteration = k + 1;
-      for (int q = 0; q < 17; ++q) st->sums[q] = 0.0;
-    }
-  }
-  for (int q = 0; q < 12; ++q) result[q] = st->T[q];
-  result[12] = 0.0; result[13] = 0.0; result[14] = 0.0; result[15] = 1.0;
-  result[16] = st->fitness;
-  result[17] = st->rmse;
-  result[18] = (double)st->iteration;
-  result[19] = st->sums[0];
-}
-
 }  // namespace
 
 extern "C" {
@@ -599,36 +472,6 @@ int32_t dgr_se3_register(const float* x, const float* y, const int32_t* idx1, co
                                                               max_break_count, break_threshold_ratio,
                                                               lr, gamma, eps, result);
   dgr_note_launches(2);
-  DGR_LAUNCH_CHECK();
-  return DGR_OK;
-}
-
-// Point-to-point ICP with open3d's defaults (what registration_icp(source, target,
-// max_correspondence_distance, init) does at core/deep_global_registration.py:317-322).
-// Nearest neighbours come from the TARGET's voxel hash (keys / vals / spec of the table
-// dgr_unique_first built for the target cloud at `voxel`, rows = rows of tgt).
-// T_init: device double[12] row-major [R | t]; state_ws: 64 doubles; result: device double[20] =
-// 4x4 pose (16), fitness, inlier rmse, iterations, correspondences of the last evaluation.
-int32_t dgr_icp_point_to_point(const float* src, int64_t n_src, const float* tgt, const dgr_keyspec_t* spec,
-                               const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch,
-                               double voxel, double max_dist, const double* T_init, int32_t max_iter,
-                               double rel_fitness, double rel_rmse, double* state_ws, double* result,
-                               void* stream) {
-  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
-  DGR_ARG_CHECK(voxel > 0 && max_dist > 0 && max_iter >= 0, "bad ICP parameters");
-  DGR_ARG_CHECK(max_dist / voxel <= 4.0, "search radius above 4 voxels is not supported");
-  static_assert(sizeof(IcpState) <= 64 * sizeof(double), "state workspace too small");
-  cudaStream_t st = (cudaStream_t)stream;
-  IcpState* state = reinterpret_cast<IcpState*>(state_ws);
-  icp_init_kernel<<<1, 32, 0, st>>>(T_init, state);
-  unsigned blocks = dgr_blocks(n_src * 8, 256);      // 8 lanes per source point
-  if (blocks > 2368) blocks = 2368;
-  for (int k = 0; k <= max_iter; ++k) {
-    icp_match_kernel<<<blocks, 256, 0, st>>>(src, n_src, tgt, spec, keys, vals, (uint64_t)cap - 1, batch, voxel,
-                                             max_dist, state);
-    icp_update_kernel<<<1, 32, 0, st>>>(state, n_src, max_iter, rel_fitness, rel_rmse, result);
-  }
-  dgr_note_launches(1 + 2 * (max_iter + 1));
   DGR_LAUNCH_CHECK();
   return DGR_OK;
 }

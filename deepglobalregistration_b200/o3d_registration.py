@@ -2,7 +2,7 @@
 ``core/deep_global_registration.py`` makes into open3d, with open3d's signatures and result objects:
 
   registration_icp(source, target, max_correspondence_distance, init, ...)             (:317-322)
-      -> dgr_icp_point_to_point: nearest target point through a voxel hash of the target, fp64 Kabsch
+      -> dgr_icp (point-to-point): nearest target point through a voxel hash of the target, fp64 Kabsch
          update, open3d's default stopping rule (relative fitness / RMSE 1e-6, 30 iterations);
   registration_ransac_based_on_correspondence(source, target, corres, ...)              (:50-64)
       -> dgr_ransac_correspondence: criteria.max_iteration four-point hypotheses, each scored on all
@@ -15,7 +15,7 @@
          points through a voxel hash of the target.
 
 It also carries the calls open3d users make beyond DGR's own: point-to-plane ICP (``registration_icp`` with
-``TransformationEstimationPointToPlane``, -> dgr_icp_point_to_plane) on target normals from
+``TransformationEstimationPointToPlane``, -> dgr_icp) on target normals from
 ``PointCloud.estimate_normals(KDTreeSearchParamHybrid(radius, max_nn))`` (-> dgr_estimate_normals), and
 
   registration_fast_based_on_feature_matching(source, target, source_feature, target_feature, option)
@@ -191,20 +191,16 @@ def registration_icp(source, target, max_correspondence_distance, init=None, est
   cell, spec, table = _target_hash(tgt64, float(max_correspondence_distance))
   src, tgt = src64.float().contiguous(), tgt64.float().contiguous()
   T12 = torch.from_numpy(np.ascontiguousarray(T0[:3])).to(dev)
+  args = (float(max_correspondence_distance), T12, int(criteria.max_iteration), float(criteria.relative_fitness),
+          float(criteria.relative_rmse))
   if plane:
     nrm = np.asarray(tgt_normals, dtype=np.float32).reshape(-1, 3)
     if len(nrm) != len(tgt):
       raise RuntimeError('target normals must hold one row per target point')
-    r = _abi.icp_point_to_plane(src, tgt, torch.from_numpy(np.ascontiguousarray(nrm)).to(dev), (spec, table), cell,
-                                float(max_correspondence_distance), T12, int(criteria.max_iteration),
-                                float(criteria.relative_fitness), float(criteria.relative_rmse)).cpu().numpy()
-    return RegistrationResult(r[:16], r[16], r[17], r[19])
-  state = torch.empty(64, dtype=torch.float64, device=dev)
-  res = torch.empty(20, dtype=torch.float64, device=dev)
-  _abi.call('dgr_icp_point_to_point', _abi.ptr(src), src.shape[0], _abi.ptr(tgt), _abi.ptr(spec), _abi.ptr(table.keys),
-            _abi.ptr(table.vals), table.cap, 0, float(cell), float(max_correspondence_distance), _abi.ptr(T12),
-            int(criteria.max_iteration), float(criteria.relative_fitness), float(criteria.relative_rmse),
-            _abi.ptr(state), _abi.ptr(res), _abi.stream())
+    res = _abi.icp_point_to_plane(src, tgt, torch.from_numpy(np.ascontiguousarray(nrm)).to(dev), (spec, table), cell,
+                                  *args)
+  else:
+    res = _abi.icp_point_to_point(src, tgt, (spec, table), cell, *args)
   r = res.cpu().numpy()
   return RegistrationResult(r[:16], r[16], r[17], r[19])
 

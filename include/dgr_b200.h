@@ -182,23 +182,10 @@ int32_t dgr_se3_register(const float* x, const float* y, const int32_t* idx1, co
                          int32_t max_break_count, float break_threshold_ratio, float lr, float gamma,
                          float* pack_ws, int32_t* cnt_ws, float* result, void* stream);
 
-/* ---- ICP fine-tune (SURVEY 8f rank 1): open3d registration_icp point-to-point with default
- *      criteria (core/deep_global_registration.py:317-322) --------------------------------- */
-/* Nearest target point within max_dist through the TARGET cloud's voxel hash (keys / vals / spec
- * of the table dgr_unique_first built at `voxel`; table rows = rows of tgt; `batch` = the batch
- * index those coordinates carry), Kabsch update in fp64, stop when fitness and inlier RMSE both
- * change by less than the tolerances or after max_iter updates.  No host round trip.
- * T_init: device double[12] row-major [R | t]; state_ws: 64 doubles; result: device double[20] =
- * 4x4 pose, fitness, inlier rmse, iterations, correspondences. */
-int32_t dgr_icp_point_to_point(const float* src, int64_t n_src, const float* tgt, const dgr_keyspec_t* spec,
-                               const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch,
-                               double voxel, double max_dist, const double* T_init, int32_t max_iter,
-                               double rel_fitness, double rel_rmse, double* state_ws, double* result,
-                               void* stream);
-
-/* ---- Normal estimation and point-to-plane ICP: open3d 0.10 EstimateNormals(KDTreeSearchParamHybrid(radius, max_nn))
- *      and registration_icp with TransformationEstimationPointToPlane (the ICP (Point-to-plane) row of the
- *      reference's results; util/pointcloud.py:60, scripts/test_3dmatch.py:72-73) ---------------------------- */
+/* ---- Normal estimation and ICP: open3d 0.10 EstimateNormals(KDTreeSearchParamHybrid(radius, max_nn)) and
+ *      registration_icp with default criteria, point-to-point (the ICP fine-tune, SURVEY 8f rank 1,
+ *      core/deep_global_registration.py:317-322) or TransformationEstimationPointToPlane (the ICP (Point-to-plane)
+ *      row of the reference's results; util/pointcloud.py:60, scripts/test_3dmatch.py:72-73) ---------------------- */
 /* Normals of the cloud xyz[n] through its OWN voxel hash (keys / vals / spec of a dgr_unique_first table at `cell`,
  * at most one point per cell, rows = rows of xyz, `batch` = its batch column; radius / cell <= 4).  Neighbours of
  * point i: the rows j with |p_j - p_i|^2 < radius^2 (strict; i itself included), the max_nn (1..64) smallest by
@@ -210,17 +197,22 @@ int32_t dgr_icp_point_to_point(const float* src, int64_t n_src, const float* tgt
 int32_t dgr_estimate_normals(const float* xyz, int64_t n, const dgr_keyspec_t* spec, const uint64_t* keys,
                              const int32_t* vals, int64_t cap, int32_t batch, double cell, double radius,
                              int32_t max_nn, const float* prev, float* normals, int32_t* counts, void* stream);
-/* Point-to-plane ICP: as dgr_icp_point_to_point (correspondences, stopping rule, fitness and Euclidean inlier RMSE,
- * result layout), with tgt_normals (float [n_tgt, 3]) and the update of open3d's TransformationEstimationPointToPlane:
- * r = (s - q).n, J = [s x n, n] over the correspondences (s = current transformed source point), J^T J x = -J^T r by
- * fp64 Cholesky (a non-positive pivot gives the identity update), T <- [Rz(x2) Ry(x1) Rx(x0) | x3..5] T.  The sums
- * are per-block partials reduced in block order: the same bits on every run.  No host round trip.
- * ws: dgr_icp_plane_ws_elems(n_src) doubles. */
-int32_t dgr_icp_plane_ws_elems(int64_t n_src, int64_t* n_elems);
-int32_t dgr_icp_point_to_plane(const float* src, int64_t n_src, const float* tgt, const float* tgt_normals,
-                               const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap,
-                               int32_t batch, double voxel, double max_dist, const double* T_init, int32_t max_iter,
-                               double rel_fitness, double rel_rmse, double* ws, double* result, void* stream);
+/* ICP of src onto tgt.  Correspondences: the nearest target point strictly within max_dist of each transformed
+ * source point s, through the TARGET cloud's voxel hash (keys / vals / spec of the table dgr_unique_first built at
+ * `voxel`; table rows = rows of tgt; `batch` = the batch index those coordinates carry; max_dist / voxel <= 4).
+ * Update, in fp64:
+ *   tgt_normals == NULL: point-to-point, the Kabsch rotation of the correspondences' centred cross-covariance;
+ *   tgt_normals (float [n_tgt, 3]): point-to-plane, r = (s - q).n, J = [s x n, n], J^T J x = -J^T r by Cholesky (a
+ *     non-positive pivot gives the identity update), T <- [Rz(x2) Ry(x1) Rx(x0) | x3..5] T.
+ * Stop when fitness and the Euclidean inlier RMSE both change by less than the tolerances, or after max_iter
+ * updates.  The sums are per-block partials reduced in block order: the same bits on every run.  No host round trip.
+ * T_init: device double[12] row-major [R | t]; ws: dgr_icp_ws_elems(n_src) doubles; result: device double[20] =
+ * 4x4 pose, fitness, inlier rmse, iterations, correspondences. */
+int32_t dgr_icp_ws_elems(int64_t n_src, int64_t* n_elems);
+int32_t dgr_icp(const float* src, int64_t n_src, const float* tgt, const float* tgt_normals, const dgr_keyspec_t* spec,
+                const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch, double voxel, double max_dist,
+                const double* T_init, int32_t max_iter, double rel_fitness, double rel_rmse, double* ws,
+                double* result, void* stream);
 
 /* ---- Safeguard RANSAC (SURVEY 8f rank 2): open3d registration_ransac_based_on_correspondence as
  *      called at core/deep_global_registration.py:50-64 (from :302-315) ---------------------- */

@@ -1,6 +1,6 @@
 """ORACLE (test infrastructure only) - point-to-plane ICP: open3d 0.10's ``registration_icp(source, target,
 max_correspondence_distance, init, TransformationEstimationPointToPlane())`` with the default
-ICPConvergenceCriteria, the GPU's dgr_icp_point_to_plane (csrc/icp_plane.cu).  Target normals come from the caller
+ICPConvergenceCriteria, the GPU's dgr_icp with target normals (csrc/icp.cu).  Target normals come from the caller
 (oracle/normals.py, or the GPU's own, to test this stage alone).
 
 PARITY UNPINNED: open3d is not installable offline, so this restates its published RegistrationICP loop in float64

@@ -3,7 +3,7 @@
 radius 0.1 at scripts/test_3dmatch.py:72-73), i.e. open3d 0.10's EstimateNormals with a hybrid search.
 
 PARITY UNPINNED: open3d is not installable offline, so this restates its published algorithm in float64 and pins
-every boundary convention the GPU kernel (csrc/icp_plane.cu, dgr_estimate_normals) follows:
+every boundary convention the GPU kernel (csrc/icp.cu, dgr_estimate_normals) follows:
 
 * strict radius: neighbours of point i are the rows j with |p_j - p_i|^2 < radius^2 (nanoflann's radius search),
   i itself included; d^2 = (ex ex + ey ey) + ez ez of the offset e = p_j - p_i, evaluated in that order;

@@ -1,4 +1,4 @@
-"""dgr_estimate_normals and dgr_icp_point_to_plane (open3d 0.10's EstimateNormals with KDTreeSearchParamHybrid and
+"""dgr_estimate_normals and dgr_icp (open3d 0.10's EstimateNormals with KDTreeSearchParamHybrid and
 point-to-plane ICP) against oracle/normals.py and oracle/icp_plane.py, the open3d stand-in that calls them, and the
 ICP baselines.  The neighbour sets are compared exactly (both sides evaluate d^2 with the same rounding); the
 cumulant sums and the ICP's normal equations run in a different order on the GPU, so normals and poses are compared
@@ -11,6 +11,7 @@ import pytest
 import torch
 
 from deepglobalregistration_b200 import synthetic as syn
+from oracle import icp as oicp
 from oracle import icp_plane as oip
 from oracle import normals as onm
 from test_gpu_fgr import rotation_angle
@@ -117,6 +118,13 @@ def run_plane(P, Q, nrm, vs, max_dist, T_init, max_iter=30, hashed=None):
                                  max_dist, T_init, max_iter).cpu().numpy()
 
 
+def run_point(P, Q, vs, max_dist, T_init, hashed=None):
+  from deepglobalregistration_b200 import _abi
+  hashed = hashed or cloud_hash(Q, vs)
+  return _abi.icp_point_to_point(_t(P, torch.float32), _t(Q, torch.float32), hashed, vs, max_dist,
+                                 T_init).cpu().numpy()
+
+
 def check_icp(res, P, Q, nrm, max_dist, T_init, max_iter=30):
   T_o, info = oip.icp_point_to_plane(P, Q, nrm.astype(np.float32), max_dist, T_init, max_iter)
   assert (int(res[18]), int(res[19])) == (info['iterations'], info['n_corr']), (res[16:], info)
@@ -149,6 +157,9 @@ def test_reproducible():
   r1 = run_plane(P, Q, nrm, vs, 2 * vs, T_init, hashed=hashed)
   r2 = run_plane(P, Q, nrm, vs, 2 * vs, T_init, hashed=hashed)
   assert np.array_equal(r1, r2)
+  p1 = run_point(P, Q, vs, 2 * vs, T_init, hashed=hashed)
+  p2 = run_point(P, Q, vs, 2 * vs, T_init, hashed=hashed)
+  assert np.array_equal(p1, p2)
 
 
 def test_edge_cases():
@@ -172,9 +183,17 @@ def test_edge_cases():
     assert np.array_equal(T, np.eye(4)), name
   # empty target: an empty table (any key spec)
   spec = cloud_hash(plane, 0.05)[0]
-  res = run_plane(src, empty, empty, 0.05, 0.1, T0, hashed=(spec, _abi.HashTable(1, torch.device('cuda'))))
+  no_target = (spec, _abi.HashTable(1, torch.device('cuda')))
+  res = run_plane(src, empty, empty, 0.05, 0.1, T0, hashed=no_target)
   T, info = check_icp(res, src, empty, empty, 0.1, T0)
   assert np.array_equal(T, np.eye(4)) and res[16] == 0 and int(res[18]) == 1
+  # point-to-point where nothing matches: the identity, fitness 0, open3d's iteration count
+  for name, S, Q, hashed in (('out of range', src + 10.0, plane, None), ('empty source', empty, plane, None),
+                            ('empty target', src, empty, no_target)):
+    res = run_point(S, Q, 0.05, 0.1, T0, hashed=hashed)
+    _, info = oicp.icp_point_to_point(S, Q, 0.1, T0)
+    assert np.array_equal(res[:16].reshape(4, 4), np.eye(4)) and res[16] == 0, name
+    assert (int(res[18]), int(res[19])) == (info['iterations'], info['n_corr']) == (1, 0), name
 
 
 def test_stand_in_reference_call_sequence():
@@ -284,8 +303,7 @@ def test_dgr_pair_size_time():
     ev[1].record()
     r_plane = _abi.icp_point_to_plane(src, tgt, nrm, hashed, vs, 2 * vs, T0)
     ev[2].record()
-    r_point = _abi.icp_point_to_point(src, tgt, types.SimpleNamespace(spec=hashed[0], _maps={1: types.SimpleNamespace(
-        table=hashed[1])}), vs, 2 * vs, T0)
+    r_point = _abi.icp_point_to_point(src, tgt, hashed, vs, 2 * vs, T0)
     ev[3].record()
     torch.cuda.synchronize()
     return [ev[k].elapsed_time(ev[k + 1]) for k in range(3)], r_plane.cpu().numpy(), r_point.cpu().numpy()

@@ -248,7 +248,7 @@ def test_safeguard_branch_known_answer():
 
 
 def test_icp_kernel_vs_oracle():
-  """dgr_icp_point_to_point against the open3d restatement (oracle/icp.py): same pose to 1e-6,
+  """dgr_icp (point-to-point) against the open3d restatement (oracle/icp.py): same pose to 1e-6,
   same fitness / RMSE / iteration count, from a perturbed initial pose."""
   from deepglobalregistration_b200 import _abi
   from deepglobalregistration_b200.core.deep_global_registration import DeepGlobalRegistration
