@@ -6,6 +6,7 @@ module without a built library, or calling into it without an sm_90 device,
 raises.
 """
 import ctypes as C
+import math
 import os
 
 import torch
@@ -65,6 +66,9 @@ SIGNATURES = {
     'dgr_fgr_ws_elems': [_i64, _i64, _i64, _i32, _p],
     'dgr_fgr_feature_matching': [_p, _i64, _p, _i64, _p, _p, _f64, _i32, _i32, _f64, _i32, _f64, _i64, _i32, C.c_uint64,
                                  _p, _p, _p, _p],
+    'dgr_goicp_dt_build': [_p, _i64, _p, _i64, _i32, _f64, _p, _p, _p, _p],
+    'dgr_goicp_ws_elems': [_i64, _i64, _i32, _i64, _i32, _p],
+    'dgr_goicp': [_p, _i64, _p, _i64, _f64, _f64, _i32, _f64, _p, _f64, _p, _f64, _i32, _i32, _i64, _p, _p, _p],
     'dgr_se3_register': [_p, _p, _p, _p, _i64, _f32, _i32, _i32, _f32, _f32, _f32, _p, _p, _p, _p],
     # ---- round 2: coordinate planning with device-side counts (csrc/coordplan.cu) ----
     'dgr_spconv_table_fwd_strided': [_p, _i32, _p, _i32, _p, _i32, _i64, _i64, _p, _p, _p, _p],
@@ -732,3 +736,43 @@ def fgr_feature_matching(src, tgt, nn_st, nn_ts, division_factor=1.4, use_absolu
        int(iteration_number), float(tuple_scale), int(maximum_tuple_count), int(bool(tuple_test)),
        int(seed) & (2**64 - 1), ptr(ws), ptr(corres), ptr(res), stream())
   return (res, corres) if return_correspondences else res
+
+
+GOICP_RESULT = ('E', 'lb_min', 'eps', 'K', 'converged', 'rounds', 'children', 'translation_cubes', 'icp_runs',
+                'inner_overflows', 'pool_high_water', 'scale', 'host_reads')
+
+
+def goicp_distance_transform(tgt, dt_size=300, dt_expand=2.0, src=None):
+  """Go-ICP's distance transform of tgt (CUDA float32 [n, 3]) normalised together with src (at most 1024 points;
+  default: the first 1024 target points).
+  -> (int32 [G, G, G] indexed [z, y, x]: squared distance in cells to the nearest occupied cell, s)."""
+  src = tgt[:1024] if src is None else src
+  _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
+  G, dev = int(dt_size), tgt.device
+  stat = torch.empty(8, dtype=torch.float64, device=dev)
+  y = torch.empty(max(tgt.shape[0], 1), 3, dtype=torch.float32, device=dev)
+  dt = torch.empty(max(G, 1) ** 3, dtype=torch.int32, device=dev)
+  call('dgr_goicp_dt_build', ptr(src), src.shape[0], ptr(tgt), tgt.shape[0], G, float(dt_expand), ptr(stat), ptr(y),
+       ptr(dt), stream())
+  st = stat.cpu().numpy()
+  s = max(st[3], st[7])
+  return dt.reshape(G, G, G), float(s if s > 0 else 1.0)
+
+
+def goicp(src, tgt, mse_thresh=1e-3, trim_fraction=0.0, dt_size=300, dt_expand=2.0, rot_min=(-math.pi,) * 3,
+          rot_width=2 * math.pi, trans_min=(-1.0, -1.0, -1.0), trans_width=2.0, cubes_per_round=64, max_rounds=100000,
+          max_rotation_cubes=1 << 20):
+  """Go-ICP of src (CUDA float32 [n_s <= 1024, 3]) onto tgt (CUDA float32 [n_t, 3]); domains in the normalised frame
+  (both clouds centred, divided by one scale s).  -> device double [32]: 4x4 pose mapping src into tgt, then the
+  fields of GOICP_RESULT."""
+  _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
+  args = (src.shape[0], tgt.shape[0], int(dt_size), int(max_rotation_cubes), int(cubes_per_round))
+  words = C.c_int64(0)
+  call('dgr_goicp_ws_elems', *args, C.byref(words))
+  ws = scratch('goicp', words.value, torch.int64, src.device)
+  res = torch.empty(32, dtype=torch.float64, device=src.device)
+  rmin, tmin = (C.c_double * 3)(*map(float, rot_min)), (C.c_double * 3)(*map(float, trans_min))
+  call('dgr_goicp', ptr(src), src.shape[0], ptr(tgt), tgt.shape[0], float(mse_thresh), float(trim_fraction),
+       int(dt_size), float(dt_expand), rmin, float(rot_width), tmin, float(trans_width), int(cubes_per_round),
+       int(max_rounds), int(max_rotation_cubes), ptr(ws), ptr(res), stream())
+  return res

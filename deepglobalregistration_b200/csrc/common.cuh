@@ -10,6 +10,13 @@
 void dgr_set_error(const char* fmt, ...);
 void dgr_note_launches(int n);   // bookkeeping for dgr_launch_count()
 
+// fgr.cu: one launch of 2 CTAs; stat[4 c .. 4 c + 3] = fp64 mean and largest centred norm of cloud c (source, target)
+void dgr_cloud_stats(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, double* stat, cudaStream_t st);
+// knn.cu: dgr_knn_top1's fp32 brute force, one thread per f0 row; packed[i] = (sqrt(d2 + 1e-7) bits << 32) | row
+// (lowest row on a tie).  One launch, skipped when live != nullptr and *live == 0.
+void dgr_knn_top1_packed(const float* f0, int n0, const float* f1, int n1, int c, uint64_t* packed,
+                         const int32_t* live, cudaStream_t st);
+
 #define DGR_CUDA_CHECK(expr)                                                            \
   do {                                                                                  \
     cudaError_t e__ = (expr);                                                           \

@@ -123,7 +123,7 @@ fgr_stats_kernel(const float* __restrict__ src, int64_t n_src, const float* __re
   const float* x = blockIdx.x ? tgt : src;
   const int64_t n = blockIdx.x ? n_tgt : n_src;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (blockIdx.x == 0 && threadIdx.x == 0) { tstate[0] = 0; tstate[1] = 0; }
+  if (tstate != nullptr && blockIdx.x == 0 && threadIdx.x == 0) { tstate[0] = 0; tstate[1] = 0; }
   double a[3] = {0.0, 0.0, 0.0};
   for (int64_t i = threadIdx.x; i < n; i += kFgrStatThreads)
     for (int c = 0; c < 3; ++c) a[c] += (double)x[3 * i + c];
@@ -387,6 +387,11 @@ fgr_solve_kernel(const float* __restrict__ src, const float* __restrict__ tgt, c
 }
 
 }  // namespace
+
+void dgr_cloud_stats(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, double* stat,
+                     cudaStream_t st) {
+  fgr_stats_kernel<<<2, kFgrStatThreads, 0, st>>>(src, n_src, tgt, n_tgt, stat, nullptr);
+}
 
 extern "C" {
 

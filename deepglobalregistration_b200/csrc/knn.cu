@@ -112,9 +112,11 @@ knn_top1_kernel(const float* __restrict__ f0, int n0, const float* __restrict__ 
 }
 
 // any channel count: one thread per (row, column-split) - correctness path for odd C
+// live (optional): skip the launch's work when *live == 0
 __global__ void knn_top1_generic_kernel(const float* __restrict__ f0, int n0,
                                         const float* __restrict__ f1, int n1, int c,
-                                        unsigned long long* __restrict__ packed) {
+                                        unsigned long long* __restrict__ packed, const int32_t* __restrict__ live) {
+  if (live != nullptr && *live == 0) return;            // uniform per launch
   int row = blockIdx.x * blockDim.x + threadIdx.x;
   if (row >= n0) return;
   float best_s = __int_as_float(0x7f800000), best_d2 = best_s;
@@ -149,6 +151,12 @@ __global__ void knn_unpack_kernel(const unsigned long long* __restrict__ packed,
 
 }  // namespace
 
+void dgr_knn_top1_packed(const float* f0, int n0, const float* f1, int n1, int c, uint64_t* packed,
+                         const int32_t* live, cudaStream_t st) {
+  knn_top1_generic_kernel<<<dgr_blocks(n0, 128), 128, 0, st>>>(f0, n0, f1, n1, c,
+                                                                reinterpret_cast<unsigned long long*>(packed), live);
+}
+
 extern "C" int32_t dgr_knn_top1(const float* f0, int64_t n0, const float* f1, int64_t n1, int32_t c,
                                 uint64_t* packed_ws, int32_t* idx, float* dist, void* stream) {
   DGR_ARG_CHECK(n1 >= 1 || n0 == 0, "F1 must not be empty");
@@ -177,7 +185,7 @@ extern "C" int32_t dgr_knn_top1(const float* f0, int64_t n0, const float* f1, in
     case 32: DGR_LAUNCH_KNN(32); break;
     case 64: DGR_LAUNCH_KNN(64); break;
     default:
-      knn_top1_generic_kernel<<<dgr_blocks(n0, 128), 128, 0, st>>>(f0, (int)n0, f1, (int)n1, c, packed);
+      knn_top1_generic_kernel<<<dgr_blocks(n0, 128), 128, 0, st>>>(f0, (int)n0, f1, (int)n1, c, packed, nullptr);
   }
   knn_unpack_kernel<<<dgr_blocks(n0, kThreads), kThreads, 0, st>>>(packed, n0, idx, dist);
   dgr_note_launches(3);

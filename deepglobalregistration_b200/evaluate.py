@@ -197,12 +197,14 @@ def main(argv=None):
   ap.add_argument('--success_rte_thresh', type=float, default=0.3, help='m (config.py:127; KITTI: 0.6)')
   ap.add_argument('--success_rre_thresh', type=float, default=15.0, help='deg (config.py:128; KITTI: 5)')
   ap.add_argument('--no_icp', action='store_true')
-  ap.add_argument('--method', choices=('dgr', 'fcgf_ransac', 'fcgf_fgr', 'icp_point_to_point', 'icp_point_to_plane'),
+  ap.add_argument('--method', choices=('dgr', 'fcgf_ransac', 'fcgf_fgr', 'icp_point_to_point', 'icp_point_to_plane',
+                                       'goicp'),
                   default='dgr',
                   help='dgr: DeepGlobalRegistration.register; fcgf_ransac: the FCGF + RANSAC baseline on the same '
                   'checkpoint (core/fcgf_ransac.py); fcgf_fgr: FCGF + Fast Global Registration with open3d\'s '
                   'default options (core/fcgf_fgr.py); icp_point_to_point / icp_point_to_plane: ICP from the identity '
-                  'on the checkpoint\'s voxelisation (core/icp_baseline.py)')
+                  'on the checkpoint\'s voxelisation (core/icp_baseline.py); goicp: globally optimal Go-ICP on the same '
+                  'voxelisation (core/goicp.py)')
   ap.add_argument('--ransac_max_iteration', type=int, default=80000, help='fcgf_ransac: hypotheses drawn at most')
   ap.add_argument('--ransac_max_validation', type=int, default=1000,
                   help='fcgf_ransac: hypotheses scored (the ones that pass the checkers first)')
@@ -211,6 +213,10 @@ def main(argv=None):
   ap.add_argument('--icp_max_correspondence_distance', type=float, default=None,
                   help='icp_*: correspondence radius in metres (default 2 voxels, at most 4)')
   ap.add_argument('--icp_max_iteration', type=int, default=30, help='icp_*: ICP updates at most')
+  ap.add_argument('--goicp_mse_thresh', type=float, default=1e-3,
+                  help='goicp: stop when E* - LB < mse_thresh K (normalised units)')
+  ap.add_argument('--goicp_trim_fraction', type=float, default=0.0, help='goicp: share of source points left out')
+  ap.add_argument('--goicp_n_data', type=int, default=1000, help='goicp: source points searched (at most 1024)')
   ap.add_argument('--out_dir', default='.')
   args = ap.parse_args(argv)
 
@@ -236,6 +242,9 @@ def main(argv=None):
   elif args.method in ('icp_point_to_point', 'icp_point_to_plane'):
     from .core.icp_baseline import ICPBaseline
     method = ICPBaseline(dgr, args.method[len('icp_'):], args.icp_max_correspondence_distance, args.icp_max_iteration)
+  elif args.method == 'goicp':
+    from .core.goicp import GoICPBaseline
+    method = GoICPBaseline(dgr, args.goicp_mse_thresh, args.goicp_trim_fraction, args.goicp_n_data)
   if args.threed_match_dir:
     pairs = threedmatch_pairs(args.threed_match_dir)
   elif args.kitti_dir:
@@ -258,7 +267,8 @@ def main(argv=None):
     print(json.dumps(dict(summary, world_size=world)))          # the summary first: a failing save loses nothing
     stem, name = {'dgr': ('dgr-b200', 'DGR'), 'fcgf_ransac': ('fcgf-ransac-b200', 'RANSAC'),
                   'fcgf_fgr': ('fcgf-fgr-b200', 'FGR'), 'icp_point_to_point': ('icp-p2p-b200', 'ICP (Point-to-point)'),
-                  'icp_point_to_plane': ('icp-p2plane-b200', 'ICP (Point-to-plane)')}[args.method]
+                  'icp_point_to_plane': ('icp-p2plane-b200', 'ICP (Point-to-plane)'),
+                  'goicp': ('goicp-b200', 'Go-ICP')}[args.method]
     out = os.path.join(out_dir, f'{stem}-stats.npz')
     np.savez(out, stats=result['stats'][None], names=[name], poses=result['poses'], groups=result['groups'])
     print(json.dumps(dict(summary, world_size=world, saved=out)))

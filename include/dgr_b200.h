@@ -281,6 +281,35 @@ int32_t dgr_fgr_feature_matching(const float* src, int64_t n_src, const float* t
                                  double tuple_scale, int64_t maximum_tuple_count, int32_t tuple_test, uint64_t seed,
                                  uint64_t* ws, int32_t* corres_out, double* result, void* stream);
 
+/* ---- Go-ICP (Yang, Li, Campbell & Jia, TPAMI 2016): globally optimal trimmed ICP by branch and bound (the Go-ICP
+ *      row of the reference's results; oracle/goicp.py is the specification) ------------------------------ */
+/* Normalisation and distance transform.  Both clouds are centred on their fp64 means and divided by s = the larger
+ * largest centred norm (dgr_fgr_feature_matching's statistics): stat = double[8] (source mean, largest norm, target
+ * mean, largest norm), tgt_norm = float [n_tgt, 3] normalised target.  dt = int32 [G][G][G] (x fastest) over
+ * [-e, e]^3, cell size h = 2e/G: the exact squared Euclidean distance in cell units from each cell to the nearest
+ * cell a target point falls in (cell floor((q + e) / h) clamped to the grid); separable exact passes along x, y, z
+ * (Felzenszwalb-Huttenlocher in integers), no atomics.  n_src in [1, 1024], G in [16, 512], e > 0. */
+int32_t dgr_goicp_dt_build(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, int32_t dt_size,
+                           double dt_expand, double* stat, float* tgt_norm, int32_t* dt, void* stream);
+/* Globally optimal registration of src onto tgt (normalised as above) for the trimmed objective
+ * E(R, t) = sum of the K = max(1, floor(n_src (1 - trim_fraction))) smallest squared distance-transform lookups of
+ * R x_i + t (fp32 lookups, fp64 pairwise-tree sums): best-first branch and bound over angle-axis rotation cubes of the
+ * cube (rot_min, rot_width) in rounds of the cubes_per_round smallest (LB, key) pool cubes, each child bounded by two
+ * nested searches over translation cubes of (trans_min, trans_width); trimmed point-to-point ICP (dgr_knn_top1's fp32
+ * correspondences, Kabsch) from the identity and from every child that beats the incumbent.  Stops when the pool is
+ * empty or E* - LB_min < eps = mse_thresh K (converged), after max_rounds rounds, or when a round's children would
+ * overflow max_rotation_cubes (>= 8 cubes_per_round).  One pinned host read per round; the same bits on every run.
+ * ws: dgr_goicp_ws_elems() 8-byte words.  result: device double[32] = 4x4 pose mapping src into tgt, E*, LB_min
+ * (normalised units), eps, K, converged, rounds, rotation children searched, translation cubes evaluated, ICP runs,
+ * inner searches whose pool overflowed, the pool's high-water mark, s, host reads, 3 zeros.  Arguments out of range
+ * are rejected before any device work. */
+int32_t dgr_goicp_ws_elems(int64_t n_src, int64_t n_tgt, int32_t dt_size, int64_t max_rotation_cubes,
+                           int32_t cubes_per_round, int64_t* n_elems);
+int32_t dgr_goicp(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, double mse_thresh,
+                  double trim_fraction, int32_t dt_size, double dt_expand, const double* rot_min, double rot_width,
+                  const double* trans_min, double trans_width, int32_t cubes_per_round, int32_t max_rounds,
+                  int64_t max_rotation_cubes, uint64_t* ws, double* result, void* stream);
+
 /* ======================================================================================
  * Round 2: coordinate planning with device-side counts, and the native executor.
  * ====================================================================================== */
