@@ -69,6 +69,9 @@ SIGNATURES = {
     'dgr_goicp_dt_build': [_p, _i64, _p, _i64, _i32, _f64, _p, _p, _p, _p],
     'dgr_goicp_ws_elems': [_i64, _i64, _i32, _i64, _i32, _p],
     'dgr_goicp': [_p, _i64, _p, _i64, _f64, _f64, _i32, _f64, _p, _f64, _p, _f64, _i32, _i32, _i64, _p, _p, _p],
+    'dgr_super4pcs_ws_elems': [_i64, _i64, _i64, _i32, _i32, _i64, _i64, _i32, _p],
+    'dgr_super4pcs': [_p, _i64, _p, _i64, _i64, _f64, _f64, _f64, _i32, _f64, _i32, _i32, _i64, _i64, _i32, _f64,
+                      C.c_uint64, _p, _p, _p, _p],
     'dgr_se3_register': [_p, _p, _p, _p, _i64, _f32, _i32, _i32, _f32, _f32, _f32, _p, _p, _p, _p],
     # ---- round 2: coordinate planning with device-side counts (csrc/coordplan.cu) ----
     'dgr_spconv_table_fwd_strided': [_p, _i32, _p, _i32, _p, _i32, _i64, _i64, _p, _p, _p, _p],
@@ -776,3 +779,30 @@ def goicp(src, tgt, mse_thresh=1e-3, trim_fraction=0.0, dt_size=300, dt_expand=2
        int(dt_size), float(dt_expand), rmin, float(rot_width), tmin, float(trans_width), int(cubes_per_round),
        int(max_rounds), int(max_rotation_cubes), ptr(ws), ptr(res), stream())
   return res
+
+
+SUPER4PCS_RESULT = ('lcp_fraction', 'lcp', 'bases', 'valid_bases', 'candidates', 'pairs_dropped',
+                    'candidates_dropped', 'best_base', 'best_candidate', 'rounds', 'scale', 'host_reads')
+SUPER4PCS_LOG = ('b1', 'b2', 'b3', 'b4', 'valid', 's1', 's2', 'candidates', 'candidates_dropped', 'verified',
+                 'best_lcp', 'best_candidate')
+
+
+def super4pcs(src, tgt, n_sample_tgt=1024, overlap=0.5, delta=0.1, angle_tol=0.0, dt_size=300, dt_expand=2.0,
+              max_bases=256, bases_per_round=64, max_pairs=262144, max_candidates=65536, verify_per_base=64,
+              terminate_fraction=0.9, seed=0, return_log=False):
+  """Super4PCS of src (CUDA float32 [n_s in 4..1024, 3]) onto tgt (CUDA float32 [n_t, 3]); delta in the clouds' units,
+  angle_tol in radians (0: 2 delta / min(d1, d2) per base).  -> device double [32]: 4x4 pose mapping src into tgt,
+  then the fields of SUPER4PCS_RESULT; with return_log, also the int32 [max_bases, 16] base log (fields
+  SUPER4PCS_LOG, then zeros; -1 rows for bases not run)."""
+  _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
+  words = C.c_int64(0)
+  call('dgr_super4pcs_ws_elems', src.shape[0], tgt.shape[0], int(n_sample_tgt), int(dt_size), int(bases_per_round),
+       int(max_pairs), int(max_candidates), int(verify_per_base), C.byref(words))
+  ws = scratch('super4pcs', words.value, torch.int64, src.device)
+  res = torch.empty(32, dtype=torch.float64, device=src.device)
+  log = torch.empty(max(int(max_bases), 1), 16, dtype=torch.int32, device=src.device) if return_log else None
+  call('dgr_super4pcs', ptr(src), src.shape[0], ptr(tgt), tgt.shape[0], int(n_sample_tgt), float(overlap),
+       float(delta), float(angle_tol), int(dt_size), float(dt_expand), int(max_bases), int(bases_per_round),
+       int(max_pairs), int(max_candidates), int(verify_per_base), float(terminate_fraction),
+       int(seed) & (2**64 - 1), ptr(ws), ptr(log) if return_log else None, ptr(res), stream())
+  return (res, log) if return_log else res

@@ -16,6 +16,10 @@ void dgr_cloud_stats(const float* src, int64_t n_src, const float* tgt, int64_t 
 // (lowest row on a tie).  One launch, skipped when live != nullptr and *live == 0.
 void dgr_knn_top1_packed(const float* f0, int n0, const float* f1, int n1, int c, uint64_t* packed,
                          const int32_t* live, cudaStream_t st);
+// goicp.cu: Go-ICP's normalisation (xn fp64 source, y32 fp32 target; xn may be null) and distance transform
+// (dgr_goicp_dt_build's grid, lookups in goicp_dt.cuh).  Returns the number of launches.
+int dgr_goicp_normalise_dt(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, int G, double e,
+                           double* stat, double* xn, float* y32, int32_t* dt, cudaStream_t st);
 
 #define DGR_CUDA_CHECK(expr)                                                            \
   do {                                                                                  \

@@ -21,6 +21,7 @@
 #include <stdint.h>
 
 #include "common.cuh"
+#include "goicp_dt.cuh"
 #include "kabsch.cuh"
 
 namespace {
@@ -166,27 +167,6 @@ __device__ void rodrigues(const double r[3], double R[9]) {
 // one row of R times x: (R0 x0 + R1 x1) + R2 x2, no contraction
 __device__ __forceinline__ double rot_row(const double* R, const double x[3]) {
   return __dadd_rn(__dadd_rn(__dmul_rn(R[0], x[0]), __dmul_rn(R[1], x[1])), __dmul_rn(R[2], x[2]));
-}
-
-// ---------------------------------------------------------------------------------------
-// distance-transform lookup: cell floor((q + e) / h) clamped to the grid, h sqrt(stored), plus the distance from q
-// to the box [-e, e]^3; every step an IEEE fp32 operation
-// ---------------------------------------------------------------------------------------
-__device__ __forceinline__ int dt_axis(float q, float e32, float h32, int G) {
-  float u = floorf(__fdiv_rn(__fadd_rn(q, e32), h32));
-  u = fminf(fmaxf(u, 0.f), (float)(G - 1));
-  return (int)u;
-}
-
-__device__ __forceinline__ float dt_lookup(const int32_t* __restrict__ dt, int G, float e32, float h32, float qx,
-                                           float qy, float qz) {
-  const int ix = dt_axis(qx, e32, h32, G), iy = dt_axis(qy, e32, h32, G), iz = dt_axis(qz, e32, h32, G);
-  const int v = __ldg(dt + ((int64_t)iz * G + iy) * G + ix);
-  const float D = __fmul_rn(h32, __fsqrt_rn((float)v));
-  const float ox = fmaxf(__fsub_rn(fabsf(qx), e32), 0.f), oy = fmaxf(__fsub_rn(fabsf(qy), e32), 0.f),
-              oz = fmaxf(__fsub_rn(fabsf(qz), e32), 0.f);
-  const float o2 = __fadd_rn(__fadd_rn(__fmul_rn(ox, ox), __fmul_rn(oy, oy)), __fmul_rn(oz, oz));
-  return __fadd_rn(D, __fsqrt_rn(o2));
 }
 
 __device__ __forceinline__ int sk(int i) { return i + (i >> 5); }
@@ -856,6 +836,11 @@ GoHost* pinned_host() {
 }
 
 }  // namespace
+
+int dgr_goicp_normalise_dt(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, int G, double e,
+                           double* stat, double* xn, float* y32, int32_t* dt, cudaStream_t st) {
+  return dt_build(src, n_src, tgt, n_tgt, G, e, stat, xn, y32, dt, st);
+}
 
 extern "C" {
 

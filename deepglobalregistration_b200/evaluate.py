@@ -198,13 +198,14 @@ def main(argv=None):
   ap.add_argument('--success_rre_thresh', type=float, default=15.0, help='deg (config.py:128; KITTI: 5)')
   ap.add_argument('--no_icp', action='store_true')
   ap.add_argument('--method', choices=('dgr', 'fcgf_ransac', 'fcgf_fgr', 'icp_point_to_point', 'icp_point_to_plane',
-                                       'goicp'),
+                                       'goicp', 'super4pcs'),
                   default='dgr',
                   help='dgr: DeepGlobalRegistration.register; fcgf_ransac: the FCGF + RANSAC baseline on the same '
                   'checkpoint (core/fcgf_ransac.py); fcgf_fgr: FCGF + Fast Global Registration with open3d\'s '
                   'default options (core/fcgf_fgr.py); icp_point_to_point / icp_point_to_plane: ICP from the identity '
                   'on the checkpoint\'s voxelisation (core/icp_baseline.py); goicp: globally optimal Go-ICP on the same '
-                  'voxelisation (core/goicp.py)')
+                  'voxelisation (core/goicp.py); super4pcs: 4-point congruent sets on the same voxelisation '
+                  '(core/super4pcs.py)')
   ap.add_argument('--ransac_max_iteration', type=int, default=80000, help='fcgf_ransac: hypotheses drawn at most')
   ap.add_argument('--ransac_max_validation', type=int, default=1000,
                   help='fcgf_ransac: hypotheses scored (the ones that pass the checkers first)')
@@ -217,6 +218,13 @@ def main(argv=None):
                   help='goicp: stop when E* - LB < mse_thresh K (normalised units)')
   ap.add_argument('--goicp_trim_fraction', type=float, default=0.0, help='goicp: share of source points left out')
   ap.add_argument('--goicp_n_data', type=int, default=1000, help='goicp: source points searched (at most 1024)')
+  ap.add_argument('--super4pcs_overlap', type=float, default=0.5,
+                  help='super4pcs: expected overlap; bases span at most overlap x the source diameter')
+  ap.add_argument('--super4pcs_delta', type=float, default=None,
+                  help='super4pcs: congruence and LCP tolerance in metres (default 2 voxels)')
+  ap.add_argument('--super4pcs_sample_size', type=int, default=512,
+                  help='super4pcs: source points (at most 1024); the target sample is twice as many (at most 4096)')
+  ap.add_argument('--super4pcs_max_bases', type=int, default=256, help='super4pcs: bases tried at most')
   ap.add_argument('--out_dir', default='.')
   args = ap.parse_args(argv)
 
@@ -245,6 +253,10 @@ def main(argv=None):
   elif args.method == 'goicp':
     from .core.goicp import GoICPBaseline
     method = GoICPBaseline(dgr, args.goicp_mse_thresh, args.goicp_trim_fraction, args.goicp_n_data)
+  elif args.method == 'super4pcs':
+    from .core.super4pcs import Super4PCSBaseline
+    method = Super4PCSBaseline(dgr, overlap=args.super4pcs_overlap, delta=args.super4pcs_delta,
+                               sample_size=args.super4pcs_sample_size, max_bases=args.super4pcs_max_bases)
   if args.threed_match_dir:
     pairs = threedmatch_pairs(args.threed_match_dir)
   elif args.kitti_dir:
@@ -268,7 +280,7 @@ def main(argv=None):
     stem, name = {'dgr': ('dgr-b200', 'DGR'), 'fcgf_ransac': ('fcgf-ransac-b200', 'RANSAC'),
                   'fcgf_fgr': ('fcgf-fgr-b200', 'FGR'), 'icp_point_to_point': ('icp-p2p-b200', 'ICP (Point-to-point)'),
                   'icp_point_to_plane': ('icp-p2plane-b200', 'ICP (Point-to-plane)'),
-                  'goicp': ('goicp-b200', 'Go-ICP')}[args.method]
+                  'goicp': ('goicp-b200', 'Go-ICP'), 'super4pcs': ('super4pcs-b200', 'Super4PCS')}[args.method]
     out = os.path.join(out_dir, f'{stem}-stats.npz')
     np.savez(out, stats=result['stats'][None], names=[name], poses=result['poses'], groups=result['groups'])
     print(json.dumps(dict(summary, world_size=world, saved=out)))

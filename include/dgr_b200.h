@@ -310,6 +310,33 @@ int32_t dgr_goicp(const float* src, int64_t n_src, const float* tgt, int64_t n_t
                   const double* trans_min, double trans_width, int32_t cubes_per_round, int32_t max_rounds,
                   int64_t max_rotation_cubes, uint64_t* ws, double* result, void* stream);
 
+/* ---- Super4PCS (Mellado, Aiger & Mitra, SGP 2014): 4-point congruent sets scored by their largest common pointset
+ *      (the Super4PCS row of the reference's results; oracle/super4pcs.py is the specification) ------------ */
+/* src (n_src in [4, 1024] rows, sampled by the caller) and the whole tgt are normalised as dgr_goicp's are and the
+ * target's distance transform is built (dt_size, dt_expand as there).  Q = rows floor(k n_tgt / n_sample_tgt) of the
+ * normalised target (n_sample_tgt in [4, 4096], at most n_tgt).  Bases run in rounds of bases_per_round, all rounds
+ * enqueued up front: base b draws 32 triplets from the counter-hash stream of seed, completes the largest into a
+ * coplanar base within D = overlap 2 max|p| and delta / s of its plane; pairs of Q congruent to its two segments
+ * (at most max_pairs each) are joined on their invariant points through a hash of delta-cells, with the angle
+ * filter angle_tol (radians; 0: 2 delta / min(d1, d2)); at most max_candidates congruent sets are fitted by Kabsch,
+ * prefiltered on 64 source rows, and the verify_per_base best are scored on all of src (the LCP: points within
+ * delta of the target through the distance transform).  Stops after max_bases bases or at the end of the first
+ * round whose best LCP is >= terminate_fraction n_src.  delta in the input units.  No host read; the same bits on
+ * every run.  ws: dgr_super4pcs_ws_elems() 8-byte words.  base_log (optional, int32 [max_bases][16]): per base its
+ * 4 source rows, valid, |S1|, |S2|, candidates kept, candidates dropped, candidates verified, best LCP and its
+ * candidate, 4 zeros (-1 rows / best when invalid or not run).  result: device double[32] = 4x4 pose mapping src
+ * into tgt, LCP fraction, LCP count, bases tried, valid bases, candidates, pairs dropped, candidates dropped, the
+ * winning base and candidate (-1: none), rounds, s, host reads (0), 4 zeros.  Arguments out of range are rejected
+ * before any device work. */
+int32_t dgr_super4pcs_ws_elems(int64_t n_src, int64_t n_tgt, int64_t n_sample_tgt, int32_t dt_size,
+                               int32_t bases_per_round, int64_t max_pairs, int64_t max_candidates,
+                               int32_t verify_per_base, int64_t* n_elems);
+int32_t dgr_super4pcs(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, int64_t n_sample_tgt,
+                      double overlap, double delta, double angle_tol, int32_t dt_size, double dt_expand,
+                      int32_t max_bases, int32_t bases_per_round, int64_t max_pairs, int64_t max_candidates,
+                      int32_t verify_per_base, double terminate_fraction, uint64_t seed, uint64_t* ws,
+                      int32_t* base_log, double* result, void* stream);
+
 /* ======================================================================================
  * Round 2: coordinate planning with device-side counts, and the native executor.
  * ====================================================================================== */
