@@ -72,6 +72,10 @@ SIGNATURES = {
     'dgr_super4pcs_ws_elems': [_i64, _i64, _i64, _i32, _i32, _i64, _i64, _i32, _p],
     'dgr_super4pcs': [_p, _i64, _p, _i64, _i64, _f64, _f64, _f64, _i32, _f64, _i32, _i32, _i64, _i64, _i32, _f64,
                       C.c_uint64, _p, _p, _p, _p],
+    'dgr_pointnet_pack': [_p, _p, _p],
+    'dgr_pointnet_forward': [_p, _i64, _p, _p, _i32, _p, _p, _p],
+    'dgr_pointnetlk_ws_elems': [_i64, _i64, _i32, _p],
+    'dgr_pointnetlk': [_p, _i64, _p, _i64, _p, _f64, _i32, _f64, _p, _p, _p, _p, _p],
     'dgr_se3_register': [_p, _p, _p, _p, _i64, _f32, _i32, _i32, _f32, _f32, _f32, _p, _p, _p, _p],
     # ---- round 2: coordinate planning with device-side counts (csrc/coordplan.cu) ----
     'dgr_spconv_table_fwd_strided': [_p, _i32, _p, _i32, _p, _i32, _i64, _i64, _p, _p, _p, _p],
@@ -806,3 +810,73 @@ def super4pcs(src, tgt, n_sample_tgt=1024, overlap=0.5, delta=0.1, angle_tol=0.0
        int(max_pairs), int(max_candidates), int(verify_per_base), float(terminate_fraction),
        int(seed) & (2**64 - 1), ptr(ws), ptr(log) if return_log else None, ptr(res), stream())
   return (res, log) if return_log else res
+
+
+POINTNET_PARAMS = 154368              # DGR_POINTNET_PARAMS
+POINTNET_PACKED_BYTES = 1185792       # DGR_POINTNET_PACKED_BYTES
+POINTNETLK_RESULT = ('iterations', 'last_dx', 'last_r', 'status', 'n_src', 'n_tgt', 'host_reads')
+POINTNETLK_LOG = ('g00', 'g01', 'g02', 'g03', 'g10', 'g11', 'g12', 'g13', 'g20', 'g21', 'g22', 'g23', 'dx_norm',
+                  'r_norm')
+
+
+def pointnet_pack(params):
+  """PointNetLK feature network parameters (CUDA float64 [POINTNET_PARAMS], core/pointnetlk.load_pointnet_weights'
+  order) -> the packed device image (uint8 [POINTNET_PACKED_BYTES]): BatchNorm folded, TF32 hi / lo tiles."""
+  _chk(params, torch.float64, 'params')
+  if params.numel() != POINTNET_PARAMS:
+    raise DgrError(f'params: expected {POINTNET_PARAMS} values, got {params.numel()}')
+  packed = torch.empty(POINTNET_PACKED_BYTES, dtype=torch.uint8, device=params.device)
+  call('dgr_pointnet_pack', ptr(params), ptr(packed), stream())
+  return packed
+
+
+def _chk_packed(packed, device):
+  """packed must be pointnet_pack's image: uint8 [POINTNET_PACKED_BYTES] on `device`, 16-byte aligned (bulk copies)."""
+  _chk(packed, torch.uint8, 'packed')
+  if packed.numel() != POINTNET_PACKED_BYTES or packed.device != device or packed.data_ptr() % 16:
+    raise DgrError(f'packed: expected pointnet_pack\'s {POINTNET_PACKED_BYTES} bytes on {device}, 16-byte aligned; got '
+                   f'{packed.numel()} bytes on {packed.device} at offset {packed.data_ptr() % 16}')
+
+
+def pointnet_forward(points, poses, packed, centre=None):
+  """Max-pooled PointNet features of points (CUDA float32 [n, 3]) under each pose (CUDA float64 [B, 3, 4] or
+  [B, 4, 4]) about centre (CUDA float64 [3]; None: the origin) -> CUDA float32 [B, 1024]."""
+  _chk(points, torch.float32, 'points')
+  if points.dim() != 2 or points.shape[1] != 3:
+    raise DgrError(f'points: expected [n, 3], got {tuple(points.shape)}')
+  if poses.dim() != 3 or tuple(poses.shape[1:]) not in ((3, 4), (4, 4)):
+    raise DgrError(f'poses: expected [B, 3, 4] or [B, 4, 4], got {tuple(poses.shape)}')
+  poses = poses[:, :3, :].contiguous()
+  _chk(poses, torch.float64, 'poses')
+  if centre is not None:
+    _chk(centre, torch.float64, 'centre')
+    if centre.numel() != 3:
+      raise DgrError(f'centre: expected 3 values, got {centre.numel()}')
+  _chk_packed(packed, points.device)
+  out = torch.empty(poses.shape[0], 1024, dtype=torch.float32, device=points.device)
+  call('dgr_pointnet_forward', ptr(points), points.shape[0], ptr(centre), ptr(poses), poses.shape[0], ptr(packed),
+       ptr(out), stream())
+  return out
+
+
+def pointnetlk(src, tgt, packed, delta=1e-2, max_iter=10, xtol=1e-7, return_jacobian=False, return_log=False):
+  """PointNetLK of src onto tgt (CUDA float32 [n, 3] each) with the packed network of pointnet_pack.
+  -> device double [32]: 4x4 pose mapping src into tgt, then the fields of POINTNETLK_RESULT; with return_jacobian,
+  also J (double [1024, 6]); with return_log, also the double [max_iter, 16] iteration log (POINTNETLK_LOG, then
+  zeros; NaN rows for iterations not run)."""
+  _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
+  for name, t in (('src', src), ('tgt', tgt)):
+    if t.dim() != 2 or t.shape[1] != 3:
+      raise DgrError(f'{name}: expected [n, 3], got {tuple(t.shape)}')
+  _chk_packed(packed, src.device)
+  words = C.c_int64(0)
+  call('dgr_pointnetlk_ws_elems', src.shape[0], tgt.shape[0], int(max_iter), C.byref(words))
+  ws = scratch('pointnetlk', words.value, torch.int64, src.device)
+  res = torch.empty(32, dtype=torch.float64, device=src.device)
+  jac = torch.empty(1024, 6, dtype=torch.float64, device=src.device) if return_jacobian else None
+  log = torch.full((max(int(max_iter), 1), 16), float('nan'), dtype=torch.float64, device=src.device) \
+      if return_log else None
+  call('dgr_pointnetlk', ptr(src), src.shape[0], ptr(tgt), tgt.shape[0], ptr(packed), float(delta), int(max_iter),
+       float(xtol), ptr(ws), ptr(jac), ptr(log), ptr(res), stream())
+  out = (res,) + ((jac,) if return_jacobian else ()) + ((log,) if return_log else ())
+  return out if len(out) > 1 else res

@@ -198,14 +198,15 @@ def main(argv=None):
   ap.add_argument('--success_rre_thresh', type=float, default=15.0, help='deg (config.py:128; KITTI: 5)')
   ap.add_argument('--no_icp', action='store_true')
   ap.add_argument('--method', choices=('dgr', 'fcgf_ransac', 'fcgf_fgr', 'icp_point_to_point', 'icp_point_to_plane',
-                                       'goicp', 'super4pcs'),
+                                       'goicp', 'super4pcs', 'pointnetlk'),
                   default='dgr',
                   help='dgr: DeepGlobalRegistration.register; fcgf_ransac: the FCGF + RANSAC baseline on the same '
                   'checkpoint (core/fcgf_ransac.py); fcgf_fgr: FCGF + Fast Global Registration with open3d\'s '
                   'default options (core/fcgf_fgr.py); icp_point_to_point / icp_point_to_plane: ICP from the identity '
                   'on the checkpoint\'s voxelisation (core/icp_baseline.py); goicp: globally optimal Go-ICP on the same '
                   'voxelisation (core/goicp.py); super4pcs: 4-point congruent sets on the same voxelisation '
-                  '(core/super4pcs.py)')
+                  '(core/super4pcs.py); pointnetlk: PointNetLK on the same voxelisation with the network of '
+                  '--pointnetlk_weights (core/pointnetlk.py)')
   ap.add_argument('--ransac_max_iteration', type=int, default=80000, help='fcgf_ransac: hypotheses drawn at most')
   ap.add_argument('--ransac_max_validation', type=int, default=1000,
                   help='fcgf_ransac: hypotheses scored (the ones that pass the checkers first)')
@@ -225,8 +226,13 @@ def main(argv=None):
   ap.add_argument('--super4pcs_sample_size', type=int, default=512,
                   help='super4pcs: source points (at most 1024); the target sample is twice as many (at most 4096)')
   ap.add_argument('--super4pcs_max_bases', type=int, default=256, help='super4pcs: bases tried at most')
+  ap.add_argument('--pointnetlk_weights', default=None,
+                  help='pointnetlk: PointNet_features state dict (required: a random network is no baseline)')
+  ap.add_argument('--pointnetlk_max_iter', type=int, default=10, help='pointnetlk: Lucas-Kanade steps at most')
   ap.add_argument('--out_dir', default='.')
   args = ap.parse_args(argv)
+  if args.method == 'pointnetlk' and not args.pointnetlk_weights:
+    ap.error('--method pointnetlk needs --pointnetlk_weights')
 
   world = int(os.environ.get('WORLD_SIZE', '1'))
   local = int(os.environ.get('LOCAL_RANK', '0'))
@@ -257,6 +263,9 @@ def main(argv=None):
     from .core.super4pcs import Super4PCSBaseline
     method = Super4PCSBaseline(dgr, overlap=args.super4pcs_overlap, delta=args.super4pcs_delta,
                                sample_size=args.super4pcs_sample_size, max_bases=args.super4pcs_max_bases)
+  elif args.method == 'pointnetlk':
+    from .core.pointnetlk import PointNetLKBaseline
+    method = PointNetLKBaseline(dgr, args.pointnetlk_weights, max_iter=args.pointnetlk_max_iter)
   if args.threed_match_dir:
     pairs = threedmatch_pairs(args.threed_match_dir)
   elif args.kitti_dir:
@@ -280,7 +289,8 @@ def main(argv=None):
     stem, name = {'dgr': ('dgr-b200', 'DGR'), 'fcgf_ransac': ('fcgf-ransac-b200', 'RANSAC'),
                   'fcgf_fgr': ('fcgf-fgr-b200', 'FGR'), 'icp_point_to_point': ('icp-p2p-b200', 'ICP (Point-to-point)'),
                   'icp_point_to_plane': ('icp-p2plane-b200', 'ICP (Point-to-plane)'),
-                  'goicp': ('goicp-b200', 'Go-ICP'), 'super4pcs': ('super4pcs-b200', 'Super4PCS')}[args.method]
+                  'goicp': ('goicp-b200', 'Go-ICP'), 'super4pcs': ('super4pcs-b200', 'Super4PCS'),
+                  'pointnetlk': ('pointnetlk-b200', 'PointNetLK')}[args.method]
     out = os.path.join(out_dir, f'{stem}-stats.npz')
     np.savez(out, stats=result['stats'][None], names=[name], poses=result['poses'], groups=result['groups'])
     print(json.dumps(dict(summary, world_size=world, saved=out)))

@@ -15,7 +15,7 @@ import torch.distributed as dist
 
 RESULT_WIDTH = 20
 BRANCH_CODE = {'procrustes': 0.0, 'safeguard': 1.0, 'ransac': 2.0, 'fgr': 3.0, 'icp': 4.0, 'icp_plane': 5.0,
-               'goicp': 6.0, 'super4pcs': 7.0, None: -1.0}
+               'goicp': 6.0, 'super4pcs': 7.0, 'pointnetlk': 8.0, None: -1.0}
 
 
 def shard_indices(n_pairs, rank, world):

@@ -242,6 +242,67 @@ def resunet_state_dict(seed, in_channels, out_channels, conv1_kernel_size, D,
   return sd
 
 
+POINTNET_WIDTHS = ((3, 64), (64, 64), (64, 64), (64, 128), (128, 1024))
+POINTNET_MODULES = (('h1.0', 'h1.1'), ('h1.3', 'h1.4'), ('h2.0', 'h2.1'), ('h2.3', 'h2.4'), ('h2.6', 'h2.7'))
+
+
+def _pointnet_layer(sd, conv, bn, W, b, gamma, beta, mean, var):
+  cout, cin = W.shape
+  sd[conv + '.weight'] = torch.as_tensor(W, dtype=torch.float32).reshape(cout, cin, 1)
+  sd[conv + '.bias'] = torch.as_tensor(b, dtype=torch.float32)
+  sd[bn + '.weight'] = torch.as_tensor(gamma, dtype=torch.float32)
+  sd[bn + '.bias'] = torch.as_tensor(beta, dtype=torch.float32)
+  sd[bn + '.running_mean'] = torch.as_tensor(mean, dtype=torch.float32)
+  sd[bn + '.running_var'] = torch.as_tensor(var, dtype=torch.float32)
+  sd[bn + '.num_batches_tracked'] = torch.tensor(1, dtype=torch.long)
+
+
+def pointnetlk_state_dict(seed):
+  """Seeded PointNet_features state dict in the published PointNetLK layout (Conv1d weights [cout, cin, 1]):
+  torch's default Conv1d init (uniform within 1 / sqrt(cin)) and BatchNorm statistics perturbed by up to 0.1, as
+  ``resunet_state_dict`` does.  A random network: no trained weights exist offline."""
+  g = torch.Generator().manual_seed(seed)
+  sd = {}
+  for (conv, bn), (cin, cout) in zip(POINTNET_MODULES, POINTNET_WIDTHS):
+    bound = 1.0 / math.sqrt(cin)
+    u = lambda: torch.rand(cout, generator=g) * 0.2 - 0.1
+    W = (torch.rand(cout, cin, generator=g) * 2 - 1) * bound
+    b = (torch.rand(cout, generator=g) * 2 - 1) * bound
+    _pointnet_layer(sd, conv, bn, W, b, 1.0 + u(), u(), u(), 1.0 + u())
+  return sd
+
+
+def fibonacci_sphere(n):
+  """n unit directions spread evenly over the sphere (the golden-angle spiral)."""
+  k = np.arange(n) + 0.5
+  z = 1.0 - 2.0 * k / n
+  r = np.sqrt(1.0 - z * z)
+  phi = math.pi * (3.0 - math.sqrt(5.0)) * k
+  return np.stack([r * np.cos(phi), r * np.sin(phi), z], 1)
+
+
+def pointnetlk_support_state_dict(carry=8.0, offset=10.0):
+  """PointNet_features state dict whose features are the support function of the (centred) cloud, shifted:
+  phi_k(P) = max_p a_k . p + offset for the 1024 Fibonacci-sphere directions a_k, up to the fp32 rounding of the
+  weights (the BatchNorms are identities: gamma = sqrt(1 + eps), beta = mean = 0, var = 1).  Layers 1-4 carry x + carry, y + carry, z + carry through three identity channels (carry larger
+  than any |coordinate|, so no ReLU clips them; the other channels are 0); layer 5 maps them to a_k . q + offset
+  (offset larger than any |q|, so no ReLU clips).  A pose-sensitive descriptor with a known meaning."""
+  sd = {}
+  for l, ((conv, bn), (cin, cout)) in enumerate(zip(POINTNET_MODULES, POINTNET_WIDTHS)):
+    W = np.zeros((cout, cin))
+    b = np.zeros(cout)
+    if l < 4:
+      W[:3, :3] = np.eye(3)
+      b[:3] = carry if l == 0 else 0.0
+    else:
+      A = fibonacci_sphere(cout)
+      W[:, :3] = A
+      b[:] = offset - carry * A.sum(1)
+    _pointnet_layer(sd, conv, bn, W, b, np.full(cout, math.sqrt(1.0 + 1e-5)), np.zeros(cout), np.zeros(cout),
+                    np.ones(cout))
+  return sd
+
+
 def make_checkpoint(seed=0, voxel_size=0.05, feat_conv1_kernel_size=7, feat_model_n_out=32,
                     inlier_conv1_kernel_size=3, inlier_feature_type='ones',
                     channels=CHANNELS, tr_channels=TR_CHANNELS, with_inlier=True):

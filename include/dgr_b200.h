@@ -337,6 +337,40 @@ int32_t dgr_super4pcs(const float* src, int64_t n_src, const float* tgt, int64_t
                       int32_t verify_per_base, double terminate_fraction, uint64_t seed, uint64_t* ws,
                       int32_t* base_log, double* result, void* stream);
 
+/* ---- PointNetLK (Aoki, Goforth, Srivatsan & Lucey, CVPR 2019): a PointNet feature under an inverse-compositional
+ *      Lucas-Kanade loop (the PointNetLK row of the reference's results; oracle/pointnetlk.py is the specification) */
+/* The network phi: five 1x1 layers 3 -> 64 -> 64 -> 64 -> 128 -> 1024, each conv + eval-mode BatchNorm (eps 1e-5)
+ * + ReLU, then the max over points of each of the 1024 channels (every feature >= +0).  params: device double
+ * [DGR_POINTNET_PARAMS], per layer W [cout][cin], conv bias, BN weight, BN bias, running mean, running var.
+ * dgr_pointnet_pack folds each BN into its layer in fp64, rounds to fp32 once and lays layers 2-5 out as TF32 hi / lo
+ * tiles in shared-memory image order: packed = DGR_POINTNET_PACKED_BYTES device bytes (16-byte aligned), once per
+ * checkpoint. */
+#define DGR_POINTNET_PARAMS 154368
+#define DGR_POINTNET_PACKED_BYTES 1185792
+int32_t dgr_pointnet_pack(const double* params, void* packed, void* stream);
+/* features (float [n_poses][1024]) = phi(R_b (p - c) + t_b) for poses (device double [n_poses][12], row-major
+ * [R | t]) about the centre c (device double[3]; NULL: the origin).  Each input point is computed in fp64 from the
+ * fp32 point, c and the pose, d = p - c, ((R0 d0 + R1 d1) + R2 d2) + t without contraction, and rounded to fp32 once; the layers run as 3xTF32 tensor-core products (fp32-accurate).  The max is
+ * exact, so every run gives the same bits.  A NaN input point makes every feature of its pose NaN (the ReLUs and the
+ * max keep NaN).  n in [1, 2^31 - 128], n_poses in [1, 65535]. */
+int32_t dgr_pointnet_forward(const float* points, int64_t n, const double* centre, const double* poses, int32_t n_poses,
+                             const void* packed, float* features, void* stream);
+/* PointNetLK of src onto tgt (template T = tgt, source S = src).  Both clouds are centred on their fp64 means
+ * (dgr_fgr_feature_matching's statistics).  J[:, i] = (phi(T) - phi(exp(-delta e_i) T)) / delta (one 7-pose forward),
+ * H = J^T J; a non-positive pivot of H's Cholesky factorisation ends the call with status 1 and g = I.  Then for
+ * k < max_iter: r = phi(g S) - phi(T), dx = -H^-1 J^T r; stop when |dx| < xtol (iterations = k + 1), otherwise
+ * g <- exp(dx) g, with exp the SE(3) exponential of the twist (rotation first).  The pose is
+ * translate(mean_T) g translate(-mean_S).  J, H, the solve, exp and the pose are fp64, reduced in a fixed order; no
+ * host read, the same bits on every run.  ws: dgr_pointnetlk_ws_elems() 8-byte words.  jac_out (optional): double
+ * [1024][6].  log (optional, double [max_iter][16]): per iteration run, g before the step (12), |dx|, |r|, 2 zeros
+ * (rows of iterations not run are left as they were).  result: device double[32] = 4x4 pose mapping src into tgt,
+ * iterations, last |dx|, last |r|, status (0 ok, 1 singular H), n_src, n_tgt, host reads (0), 9 zeros.  delta > 0,
+ * max_iter in [1, 1000], xtol >= 0; arguments out of range are rejected before any device work. */
+int32_t dgr_pointnetlk_ws_elems(int64_t n_src, int64_t n_tgt, int32_t max_iter, int64_t* n_elems);
+int32_t dgr_pointnetlk(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, const void* packed,
+                       double delta, int32_t max_iter, double xtol, uint64_t* ws, double* jac_out, double* log,
+                       double* result, void* stream);
+
 /* ======================================================================================
  * Round 2: coordinate planning with device-side counts, and the native executor.
  * ====================================================================================== */
