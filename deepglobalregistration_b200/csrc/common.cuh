@@ -1,5 +1,6 @@
 // Shared helpers of libdgr_b200 (sm_90a only).
 #pragma once
+#include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -10,16 +11,10 @@
 void dgr_set_error(const char* fmt, ...);
 void dgr_note_launches(int n);   // bookkeeping for dgr_launch_count()
 
-// fgr.cu: one launch of 2 CTAs; stat[4 c .. 4 c + 3] = fp64 mean and largest centred norm of cloud c (source, target)
-void dgr_cloud_stats(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, double* stat, cudaStream_t st);
 // knn.cu: dgr_knn_top1's fp32 brute force, one thread per f0 row; packed[i] = (sqrt(d2 + 1e-7) bits << 32) | row
 // (lowest row on a tie).  One launch, skipped when live != nullptr and *live == 0.
 void dgr_knn_top1_packed(const float* f0, int n0, const float* f1, int n1, int c, uint64_t* packed,
                          const int32_t* live, cudaStream_t st);
-// goicp.cu: Go-ICP's normalisation (xn fp64 source, y32 fp32 target; xn may be null) and distance transform
-// (dgr_goicp_dt_build's grid, lookups in goicp_dt.cuh).  Returns the number of launches.
-int dgr_goicp_normalise_dt(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, int G, double e,
-                           double* stat, double* xn, float* y32, int32_t* dt, cudaStream_t st);
 
 #define DGR_CUDA_CHECK(expr)                                                            \
   do {                                                                                  \
@@ -211,10 +206,12 @@ __device__ __forceinline__ int dgr_block_scan_inplace(int32_t* cnt, int64_t nb) 
 }
 
 // ---------------------------------------------------------------------------------------
-// block-wide exclusive scan of one int per thread (blockDim.x == 256)
+// block-wide exclusive scan of one int per thread (blockDim.x == BS).  The warp totals stay in shared memory until
+// the caller's next __syncthreads, so two calls need one between them.
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ int dgr_block_exclusive_scan_256(int v, int* total) {
-  __shared__ int warp_sums[8];
+template <int BS>
+__device__ __forceinline__ int dgr_block_exclusive_scan(int v, int* total) {
+  __shared__ int warp_sums[BS / 32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   int inc = v;
 #pragma unroll
@@ -226,26 +223,96 @@ __device__ __forceinline__ int dgr_block_exclusive_scan_256(int v, int* total) {
   __syncthreads();
   int base = 0, tot = 0;
 #pragma unroll
-  for (int w = 0; w < 8; ++w) {
+  for (int w = 0; w < BS / 32; ++w) {
     int s = warp_sums[w];
     if (w < warp) base += s;
     tot += s;
   }
-  __syncthreads();
   if (total) *total = tot;
   return base + inc - v;
 }
 
 // ---------------------------------------------------------------------------------------
-// "the first `cap` flagged rows, in row order" for one 256-row block of flag[0, n): base = flagged rows before
-// this block (an exclusive scan of the per-block counts); every flagged row whose rank is below cap gets
-// sel[rank] = h0 + row.  Whole blocks call it (blockDim.x == 256).
+// coords.cu: the count scan and the ordered selection shared by the unique-coordinate pass, FGR and the RANSAC
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ void dgr_select_first_256(const int32_t* __restrict__ flag, int base, int64_t n, int64_t cap,
-                                                     int64_t h0, int32_t* __restrict__ sel) {
-  if (base >= cap) return;                             // uniform per block
-  const int64_t h = (int64_t)blockIdx.x * 256 + threadIdx.x;
-  const int f = h < n ? flag[h] : 0;
-  const int pos = base + dgr_block_exclusive_scan_256(f, nullptr);
-  if (f && pos < cap) sel[pos] = (int32_t)(h0 + h);
+// exclusive scan in place of the per-block counts cnt[0, nb) with one block; cnt[nb] = the total
+void dgr_scan_counts(int32_t* cnt, int64_t nb, cudaStream_t st);
+// The first `cap` flagged rows of flag[0, n), in row order: sel[rank] = h0 + row, one 256-row block per count of
+// blk (scanned by dgr_scan_counts).  live (optional): the launch does nothing when *live == 0.
+void dgr_select_first(const int32_t* flag, const int32_t* blk, int64_t n, int64_t cap, int64_t h0, int32_t* sel,
+                      const int32_t* live, cudaStream_t st);
+
+// ---------------------------------------------------------------------------------------
+// Fixed-order fp64 sums.  Each value's lanes are added by xor butterfly (16, 8, 4, 2, 1), then the BS / 32 warp
+// partials from warp 0 upward starting at +0.0 (so a sum of -0.0 terms is +0.0); the oracles restate this order.
+// ---------------------------------------------------------------------------------------
+// Sum N per-thread values over a block of BS threads.  Thread k < N returns the sum of value k, every other thread
+// +0.0.  part: shared [BS / 32][>= N], rewritten by the next call only after a __syncthreads.  Whole blocks call it.
+template <int BS, int N, int W>
+__device__ __forceinline__ double dgr_block_sum(const double (&v)[N], double (*part)[W]) {
+  static_assert(N <= W, "partial rows too narrow");
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < N; ++k) {
+    double x = v[k];
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) x += __shfl_xor_sync(0xffffffffu, x, d);
+    if (lane == 0) part[warp][k] = x;
+  }
+  __syncthreads();
+  double s = 0.0;
+  if (threadIdx.x < N)
+    for (int w = 0; w < BS / 32; ++w) s += part[w][threadIdx.x];
+  return s;
 }
+
+// Shared memory of dgr_allreduce for up to W values, BS threads and clusters of up to CS CTAs; embedded as the first
+// member of a kernel's shared struct.
+template <int W, int BS, int CS>
+struct DgrReduceShared {
+  double slots[2][CS][W];                               // per-CTA sums, double-buffered by the caller's parity
+  double part[BS / 32][W];
+  double tot[W];
+};
+
+// Sum N per-thread values over the CTA (CS == 1) or its cluster of CS CTAs: dgr_block_sum, then the CTA sums in rank
+// order through distributed shared memory.  Every CTA ends with the same sh.tot[0, N); parity alternates the slots
+// so that consecutive calls need one cluster barrier each.
+template <int CS, int N, int W, int BS, int CSMAX>
+__device__ __forceinline__ void dgr_allreduce(DgrReduceShared<W, BS, CSMAX>& sh, const double (&v)[N], int& parity) {
+  static_assert(CS <= CSMAX, "cluster larger than the slots");
+  double s = dgr_block_sum<BS>(v, sh.part);
+  if constexpr (CS == 1) {
+    if (threadIdx.x < N) sh.tot[threadIdx.x] = s;
+  } else {
+    cooperative_groups::cluster_group cluster = cooperative_groups::this_cluster();
+    const unsigned rank = cluster.block_rank();
+    if (threadIdx.x < N)
+      for (unsigned r = 0; r < CS; ++r) cluster.map_shared_rank(&sh, r)->slots[parity][rank][threadIdx.x] = s;
+    cluster.sync();
+    if (threadIdx.x < N) {
+      s = 0.0;
+      for (int r = 0; r < CS; ++r) s += sh.slots[parity][r][threadIdx.x];
+      sh.tot[threadIdx.x] = s;
+    }
+  }
+  __syncthreads();
+  parity ^= 1;
+}
+
+// ---------------------------------------------------------------------------------------
+// Workspace carving: regions of 8-byte words handed out in order.  With a null base it only counts the words, so one
+// layout function gives both the size a dgr_*_ws_elems reports and the regions.
+// ---------------------------------------------------------------------------------------
+struct DgrCarver {
+  uint64_t* base;
+  int64_t words = 0;
+  explicit DgrCarver(void* b) : base(static_cast<uint64_t*>(b)) {}
+  // n elements of T, rounded up to whole words
+  template <class T>
+  T* take(int64_t n) {
+    T* p = base != nullptr ? reinterpret_cast<T*>(base + words) : nullptr;
+    words += (n * (int64_t)sizeof(T) + 7) / 8;
+    return p;
+  }
+};

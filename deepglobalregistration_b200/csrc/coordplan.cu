@@ -191,7 +191,7 @@ __global__ void coarse_scatter_kernel(const int32_t* __restrict__ fine, const in
     sl[e] = (r < n) ? a.slot[l][r] : -1;
     c += (sl[e] >= 0);
   }
-  int pos = a.scan[l][blockIdx.x] + dgr_block_exclusive_scan_256(c, nullptr);
+  int pos = a.scan[l][blockIdx.x] + dgr_block_exclusive_scan<256>(c, nullptr);
   const int stride = a.stride[l];
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
@@ -434,7 +434,7 @@ kmap_fill_kernel(const uint32_t* __restrict__ bits, int W, int bpk, const int32_
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const int w_own = blockIdx.x * kCntWords + t;
   const uint32_t m_own = w_own < W ? bits[(int64_t)kappa * W + w_own] : 0u;
-  const int excl = dgr_block_exclusive_scan_256(__popc(m_own), nullptr);
+  const int excl = dgr_block_exclusive_scan<256>(__popc(m_own), nullptr);
   s_mask[t] = m_own;
   s_base[t] = base + excl;
   __syncthreads();

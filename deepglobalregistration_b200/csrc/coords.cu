@@ -156,10 +156,21 @@ __global__ void block_count_kernel(const int32_t* __restrict__ flag, int64_t n, 
   }
 }
 
-// single-block exclusive scan in place over nb entries; entry nb receives the total.
-__global__ void scan_kernel(int32_t* cnt, int64_t nb) {
+__global__ void __launch_bounds__(1024) scan_counts_kernel(int32_t* cnt, int64_t nb) {
   const int total = dgr_block_scan_inplace(cnt, nb);
   if (threadIdx.x == 0) cnt[nb] = total;
+}
+
+__global__ void __launch_bounds__(256)
+select_first_kernel(const int32_t* __restrict__ flag, const int32_t* __restrict__ blk, int64_t n, int64_t cap,
+                    int64_t h0, int32_t* __restrict__ sel, const int32_t* __restrict__ live) {
+  if (live != nullptr && *live == 0) return;            // uniform per launch
+  const int base = blk[blockIdx.x];
+  if (base >= cap) return;                              // uniform per block
+  const int64_t h = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  const int f = h < n ? flag[h] : 0;
+  const int pos = base + dgr_block_exclusive_scan<256>(f, nullptr);
+  if (f && pos < cap) sel[pos] = (int32_t)(h0 + h);
 }
 
 // rank winners: sel[rank] = row, table value <- rank
@@ -174,7 +185,7 @@ __global__ void unique_scatter_kernel(const int32_t* __restrict__ flag, const in
     f[e] = (i < n) ? flag[i] : 0;
     c += f[e];
   }
-  int pos = block_ofs[blockIdx.x] + dgr_block_exclusive_scan_256(c, nullptr);
+  int pos = block_ofs[blockIdx.x] + dgr_block_exclusive_scan<kThreads>(c, nullptr);
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
     if (f[e]) {
@@ -223,6 +234,13 @@ __global__ void gather_rows_kernel(const int32_t* __restrict__ src, const int32_
 }
 
 }  // namespace
+
+void dgr_scan_counts(int32_t* cnt, int64_t nb, cudaStream_t st) { scan_counts_kernel<<<1, 1024, 0, st>>>(cnt, nb); }
+
+void dgr_select_first(const int32_t* flag, const int32_t* blk, int64_t n, int64_t cap, int64_t h0, int32_t* sel,
+                      const int32_t* live, cudaStream_t st) {
+  select_first_kernel<<<dgr_blocks(n, 256), 256, 0, st>>>(flag, blk, n, cap, h0, sel, live);
+}
 
 // =========================================================================================
 // C ABI
@@ -298,7 +316,7 @@ int32_t dgr_unique_first(const int32_t* coords, int64_t n, int32_t ncols, const 
                                                                    mask, slot_ws);
   winner_flag_kernel<<<dgr_blocks(n, kThreads), kThreads, 0, st>>>(slot_ws, vals, n, rank_ws);
   block_count_kernel<<<nb, kThreads, 0, st>>>(rank_ws, n, scan_ws);
-  scan_kernel<<<1, 1024, 0, st>>>(scan_ws, nb);
+  dgr_scan_counts(scan_ws, nb, st);
   unique_scatter_kernel<<<nb, kThreads, 0, st>>>(rank_ws, slot_ws, n, scan_ws, sel, vals);
   inverse_kernel<<<dgr_blocks(n, kThreads), kThreads, 0, st>>>(slot_ws, vals, n, inverse);
   copy_total_kernel<<<1, 1, 0, st>>>(scan_ws + nb, spec, n_unique);

@@ -2,14 +2,14 @@
 // registration_fast_based_on_feature_matching, restated in oracle/fgr.py (which pins every boundary convention).
 // The caller supplies both feature kNN directions (dgr_knn_top1 / dgr_knn_top1_tc); the rest runs here with no
 // host read and no atomics, so a call gives the same bits on every run:
-//   fgr_stats_kernel    one CTA per cloud: fp64 mean and max |x - mean| in a fixed order
+//   dgr_cloud_stats     one CTA per cloud: fp64 mean and max |x - mean| in a fixed order (frame.cu)
 //   fgr_mutual_kernel   one thread per row of the larger cloud ("first"; the source on a tie): mutual flag
-//   fgr_scan_kernel     exclusive scan of the per-block counts (dgr_block_scan_inplace); [nb] = n_mut
-//   fgr_select_kernel   the mutual list in first-cloud order (dgr_select_first_256, shared with the RANSAC)
+//   dgr_scan_counts     exclusive scan of the per-block counts (coords.cu); [nb] = n_mut
+//   dgr_select_first    the mutual list in first-cloud order (coords.cu, shared with the RANSAC)
 //   per chunk of kFgrChunk tuple trials (grids sized from the host bound 100 min(n_s, n_t)):
 //     fgr_tuple_kernel       one thread per trial: 3 counter-hash draws, the three edge-ratio tests
 //     fgr_tuple_scan_kernel  scan offset by the acceptances so far; marks the chunk dead once K are in
-//     fgr_select_kernel      the first K accepted trials, in trial order
+//     dgr_select_first       the first K accepted trials, in trial order
 //   Every kernel of a chunk that starts after the K-th acceptance (or past 100 n_mut) returns at once, and the
 //   workspace is one chunk's flags whatever the trial count.
 //   fgr_solve_kernel    one launch for all iterations: one CTA (a cluster of 8 when the mutual list is long and
@@ -20,14 +20,14 @@
 #include <stdint.h>
 
 #include "common.cuh"
+#include "frame.cuh"
 #include "kabsch.cuh"
 
 namespace cg = cooperative_groups;
 
 namespace {
 
-constexpr int kFgrThreads = 256;                        // flag / select kernels (dgr_block_exclusive_scan_256)
-constexpr int kFgrStatThreads = 1024;
+constexpr int kFgrThreads = 256;                        // flag kernels (dgr_select_first's blocks)
 constexpr int64_t kFgrChunk = 1 << 18;                  // tuple trials per chunk
 constexpr int kFgrChunkBlocks = (int)(kFgrChunk / kFgrThreads);
 constexpr int kFgrSolveThreads = 512;
@@ -47,8 +47,6 @@ struct FgrWs {
   double* corr;      // [n_corr_max][6] normalised (source, target) points of the correspondences
 };
 
-inline int64_t fgr_words(int64_t n_int32) { return (n_int32 + 1) / 2; }
-
 // K capped by the trial count bound: at most 100 min(n_s, n_t) trials exist
 inline int64_t fgr_kc(int64_t n_min, int64_t K) { return K < 100 * n_min ? K : 100 * n_min; }
 
@@ -61,23 +59,19 @@ int64_t fgr_layout(int64_t n_src, int64_t n_tgt, int64_t K, int tuple_test, uint
   const int64_t n_first = n_src > n_tgt ? n_src : n_tgt, n_min = n_src < n_tgt ? n_src : n_tgt;
   const int64_t n_mblk = (n_first + kFgrThreads - 1) / kFgrThreads;
   const int64_t t = tuple_test ? 1 : 0;
-  const int64_t sizes[9] = {8, fgr_words(n_first), fgr_words(n_mblk + 1), fgr_words(n_min), t * fgr_words(kFgrChunk),
-                            t * fgr_words(kFgrChunkBlocks + 1), t * fgr_words(fgr_kc(n_min, K)), 1,
-                            6 * fgr_corr_max(n_min, K, tuple_test)};
-  int64_t ofs[9], total = 0;
-  for (int k = 0; k < 9; ++k) { ofs[k] = total; total += sizes[k]; }
-  if (base != nullptr) {
-    w->stat = reinterpret_cast<double*>(base + ofs[0]);
-    w->mflag = reinterpret_cast<int32_t*>(base + ofs[1]);
-    w->mblk = reinterpret_cast<int32_t*>(base + ofs[2]);
-    w->mut = reinterpret_cast<int32_t*>(base + ofs[3]);
-    w->tflag = reinterpret_cast<int32_t*>(base + ofs[4]);
-    w->tblk = reinterpret_cast<int32_t*>(base + ofs[5]);
-    w->tsel = reinterpret_cast<int32_t*>(base + ofs[6]);
-    w->tstate = reinterpret_cast<int32_t*>(base + ofs[7]);
-    w->corr = reinterpret_cast<double*>(base + ofs[8]);
-  }
-  return total;
+  DgrCarver c(base);
+  FgrWs r;
+  r.stat = c.take<double>(8);
+  r.mflag = c.take<int32_t>(n_first);
+  r.mblk = c.take<int32_t>(n_mblk + 1);
+  r.mut = c.take<int32_t>(n_min);
+  r.tflag = c.take<int32_t>(t * kFgrChunk);
+  r.tblk = c.take<int32_t>(t * (kFgrChunkBlocks + 1));
+  r.tsel = c.take<int32_t>(t * fgr_kc(n_min, K));
+  r.tstate = c.take<int32_t>(2);
+  r.corr = c.take<double>(6 * fgr_corr_max(n_min, K, tuple_test));
+  if (w != nullptr) *w = r;
+  return c.words;
 }
 
 // the normalisation of oracle/fgr.py::normalise: x -> (x - mean) / scale
@@ -90,22 +84,9 @@ struct FgrFrame {
 __device__ __forceinline__ FgrFrame fgr_frame(const double* __restrict__ stat, int absolute) {
   FgrFrame f;
   for (int c = 0; c < 3; ++c) { f.ms[c] = stat[c]; f.mt[c] = stat[4 + c]; }
-  const double s = fmax(stat[3], stat[7]);
-  f.s = s > 0.0 ? s : 1.0;
+  f.s = dgr_frame_scale(stat);
   f.scale = absolute ? 1.0 : f.s;
   return f;
-}
-
-__device__ __forceinline__ void fgr_point(const float* __restrict__ x, int64_t i, const double m[3], double scale,
-                                          double p[3]) {
-#pragma unroll
-  for (int c = 0; c < 3; ++c) p[c] = __ddiv_rn(__dsub_rn((double)__ldg(x + 3 * i + c), m[c]), scale);
-}
-
-// |a - b| as numpy evaluates it: sqrt((dx dx + dy dy) + dz dz), no contraction
-__device__ __forceinline__ double fgr_dist(const double a[3], const double b[3]) {
-  const double dx = __dsub_rn(a[0], b[0]), dy = __dsub_rn(a[1], b[1]), dz = __dsub_rn(a[2], b[2]);
-  return sqrt(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)));
 }
 
 // (source row, target row) of the mutual pair whose first-cloud row is f
@@ -115,54 +96,11 @@ __device__ __forceinline__ void fgr_pair(int32_t f, int swapped, const int32_t* 
   else { i = f; j = __ldg(nn_st + f); }
 }
 
-__global__ void __launch_bounds__(kFgrStatThreads)
-fgr_stats_kernel(const float* __restrict__ src, int64_t n_src, const float* __restrict__ tgt, int64_t n_tgt,
-                 double* __restrict__ stat, int32_t* __restrict__ tstate) {
-  __shared__ double s_part[kFgrStatThreads / 32][3];
-  __shared__ double s_mean[3];
-  const float* x = blockIdx.x ? tgt : src;
-  const int64_t n = blockIdx.x ? n_tgt : n_src;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (tstate != nullptr && blockIdx.x == 0 && threadIdx.x == 0) { tstate[0] = 0; tstate[1] = 0; }
-  double a[3] = {0.0, 0.0, 0.0};
-  for (int64_t i = threadIdx.x; i < n; i += kFgrStatThreads)
-    for (int c = 0; c < 3; ++c) a[c] += (double)x[3 * i + c];
-  for (int c = 0; c < 3; ++c) {
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) a[c] += __shfl_xor_sync(0xffffffffu, a[c], d);
-    if (lane == 0) s_part[warp][c] = a[c];
-  }
-  __syncthreads();
-  if (threadIdx.x < 3) {
-    double s = 0.0;
-    for (int w = 0; w < kFgrStatThreads / 32; ++w) s += s_part[w][threadIdx.x];
-    s_mean[threadIdx.x] = s / (double)n;
-  }
-  __syncthreads();
-  const double m[3] = {s_mean[0], s_mean[1], s_mean[2]};
-  double mx = 0.0;                                      // a maximum does not depend on the order
-  for (int64_t i = threadIdx.x; i < n; i += kFgrStatThreads) {
-    double p[3];
-    fgr_point(x, i, m, 1.0, p);
-    const double o[3] = {0.0, 0.0, 0.0};
-    mx = fmax(mx, fgr_dist(p, o));
-  }
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, d));
-  __syncthreads();
-  if (lane == 0) s_part[warp][0] = mx;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < kFgrStatThreads / 32; ++w) mx = fmax(mx, s_part[w][0]);
-    for (int c = 0; c < 3; ++c) stat[4 * blockIdx.x + c] = m[c];
-    stat[4 * blockIdx.x + 3] = mx;
-  }
-}
-
 __global__ void __launch_bounds__(kFgrThreads)
 fgr_mutual_kernel(const int32_t* __restrict__ nn_first, const int32_t* __restrict__ nn_other, int64_t n_first,
-                  int64_t n_other, int32_t* __restrict__ flag, int32_t* __restrict__ blk) {
+                  int64_t n_other, int32_t* __restrict__ flag, int32_t* __restrict__ blk, int32_t* __restrict__ tstate) {
   const int64_t f = (int64_t)blockIdx.x * kFgrThreads + threadIdx.x;
+  if (f == 0) { tstate[0] = 0; tstate[1] = 0; }     // no trial accepted yet, for the tuple chunks that follow
   int ok = 0;
   if (f < n_first) {
     const int32_t j = __ldg(nn_first + f);
@@ -171,19 +109,6 @@ fgr_mutual_kernel(const int32_t* __restrict__ nn_first, const int32_t* __restric
   }
   const int cnt = __syncthreads_count(ok);
   if (threadIdx.x == 0) blk[blockIdx.x] = cnt;
-}
-
-__global__ void __launch_bounds__(1024) fgr_scan_kernel(int32_t* blk, int64_t nb) {
-  const int total = dgr_block_scan_inplace(blk, nb);
-  if (threadIdx.x == 0) blk[nb] = total;
-}
-
-// live (optional): skip the launch's work when *live == 0
-__global__ void __launch_bounds__(kFgrThreads)
-fgr_select_kernel(const int32_t* __restrict__ flag, const int32_t* __restrict__ blk, int64_t n, int64_t cap, int64_t h0,
-                  int32_t* __restrict__ sel, const int32_t* __restrict__ live) {
-  if (live != nullptr && *live == 0) return;            // uniform per launch
-  dgr_select_first_256(flag, blk[blockIdx.x], n, cap, h0, sel);
 }
 
 // trials [h0, h0 + kFgrChunk) of 100 n_mut: trial k draws list positions 3k .. 3k + 2 of the counter hash and is
@@ -206,13 +131,13 @@ fgr_tuple_kernel(const float* __restrict__ src, const float* __restrict__ tgt, c
       const uint32_t pos = dgr_counter_pick(seed, 3 * (uint64_t)k + s, (uint32_t)n_mut);
       int32_t i, j;
       fgr_pair(__ldg(mut + pos), swapped, nn_st, nn_ts, i, j);
-      fgr_point(src, i, fr.ms, fr.scale, p[s]);
-      fgr_point(tgt, j, fr.mt, fr.scale, q[s]);
+      dgr_frame_point(src, i, fr.ms, fr.scale, p[s]);
+      dgr_frame_point(tgt, j, fr.mt, fr.scale, q[s]);
     }
     ok = 1;
     for (int e = 0; e < 3; ++e) {
       const int a = e, b = e == 2 ? 0 : e + 1;
-      const double ls = fgr_dist(p[a], p[b]), lt = fgr_dist(q[a], q[b]);
+      const double ls = dgr_dist3(p[a], p[b]), lt = dgr_dist3(q[a], q[b]);
       if (!(ls * tuple_scale < lt && lt < ls / tuple_scale)) ok = 0;
     }
   }
@@ -242,45 +167,9 @@ fgr_tuple_scan_kernel(int32_t* __restrict__ blk, const int32_t* __restrict__ n_m
 }
 
 struct FgrShared {
-  double slots[2][kFgrCluster][kNv];
-  double warp_part[kFgrSolveThreads / 32][kNv];
-  double tot[kNv];
+  DgrReduceShared<kNv, kFgrSolveThreads, kFgrCluster> red;
   double T[12];                                         // target -> source in normalised units, row-major [R | t]
 };
-
-// Sum kNv per-thread doubles over the CTA (CS == 1) or the cluster; every CTA ends with the same sh.tot, summed
-// in the same order (lanes by butterfly, warps in order, CTAs in rank order).
-template <int CS>
-__device__ __forceinline__ void fgr_allreduce(FgrShared& sh, double (&v)[kNv], int& parity) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < kNv; ++k) {
-    double x = v[k];
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) x += __shfl_xor_sync(0xffffffffu, x, d);
-    if (lane == 0) sh.warp_part[warp][k] = x;
-  }
-  __syncthreads();
-  double s = 0.0;
-  if (threadIdx.x < kNv)
-    for (int w = 0; w < kFgrSolveThreads / 32; ++w) s += sh.warp_part[w][threadIdx.x];
-  if constexpr (CS == 1) {
-    if (threadIdx.x < kNv) sh.tot[threadIdx.x] = s;
-  } else {
-    cg::cluster_group cluster = cg::this_cluster();
-    const unsigned rank = cluster.block_rank();
-    if (threadIdx.x < kNv)
-      for (unsigned r = 0; r < CS; ++r) cluster.map_shared_rank(&sh, r)->slots[parity][rank][threadIdx.x] = s;
-    cluster.sync();
-    if (threadIdx.x < kNv) {
-      s = 0.0;
-      for (int r = 0; r < CS; ++r) s += sh.slots[parity][r][threadIdx.x];
-      sh.tot[threadIdx.x] = s;
-    }
-  }
-  __syncthreads();
-  parity ^= 1;
-}
 
 template <int CS>
 __global__ void __launch_bounds__(kFgrSolveThreads, 1)
@@ -313,8 +202,8 @@ fgr_solve_kernel(const float* __restrict__ src, const float* __restrict__ tgt, c
                                    : k;
     int32_t i, j;
     fgr_pair(mut[pos], swapped, nn_st, nn_ts, i, j);
-    fgr_point(src, i, fr.ms, fr.scale, corr + 6 * k);
-    fgr_point(tgt, j, fr.mt, fr.scale, corr + 6 * k + 3);
+    dgr_frame_point(src, i, fr.ms, fr.scale, corr + 6 * k);
+    dgr_frame_point(tgt, j, fr.mt, fr.scale, corr + 6 * k + 3);
     if (corres_out != nullptr) { corres_out[2 * k] = i; corres_out[2 * k + 1] = j; }
   }
   if (tid < 12) sh.T[tid] = (tid % 5 == 0) ? 1.0 : 0.0;
@@ -354,10 +243,10 @@ fgr_solve_kernel(const float* __restrict__ src, const float* __restrict__ tgt, c
         }
       }
     }
-    fgr_allreduce<CS>(sh, v, parity);
+    dgr_allreduce<CS>(sh.red, v, parity);
     if (tid == 0) {
       double x[6];
-      if (!cholesky6_step(sh.tot, sh.tot + 21, x))
+      if (!cholesky6_step(sh.red.tot, sh.red.tot + 21, x))
         for (int k = 0; k < 6; ++k) x[k] = 0.0;
       zyx_update_left(x, T, sh.T);                      // delta = [Rz(gamma) Ry(beta) Rx(alpha) | x[3..6)], on the left
     }
@@ -387,11 +276,6 @@ fgr_solve_kernel(const float* __restrict__ src, const float* __restrict__ tgt, c
 }
 
 }  // namespace
-
-void dgr_cloud_stats(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, double* stat,
-                     cudaStream_t st) {
-  fgr_stats_kernel<<<2, kFgrStatThreads, 0, st>>>(src, n_src, tgt, n_tgt, stat, nullptr);
-}
 
 extern "C" {
 
@@ -425,11 +309,11 @@ int32_t dgr_fgr_feature_matching(const float* src, int64_t n_src, const float* t
   const int64_t Kc = fgr_kc(n_min, maximum_tuple_count);
   const unsigned n_mblk = dgr_blocks(n_first, kFgrThreads);
   int launches = 0;
-  fgr_stats_kernel<<<2, kFgrStatThreads, 0, st>>>(src, n_src, tgt, n_tgt, w.stat, w.tstate);
+  dgr_cloud_stats(src, n_src, tgt, n_tgt, w.stat, st);
   fgr_mutual_kernel<<<n_mblk, kFgrThreads, 0, st>>>(swapped ? nn_ts : nn_st, swapped ? nn_st : nn_ts, n_first, n_min,
-                                                    w.mflag, w.mblk);
-  fgr_scan_kernel<<<1, 1024, 0, st>>>(w.mblk, n_mblk);
-  fgr_select_kernel<<<n_mblk, kFgrThreads, 0, st>>>(w.mflag, w.mblk, n_first, n_min, 0, w.mut, nullptr);
+                                                    w.mflag, w.mblk, w.tstate);
+  dgr_scan_counts(w.mblk, n_mblk, st);
+  dgr_select_first(w.mflag, w.mblk, n_first, n_min, 0, w.mut, nullptr, st);
   launches += 4;
   const int32_t* n_mut = w.mblk + n_mblk;
   if (tt && n_min >= 3) {
@@ -438,8 +322,7 @@ int32_t dgr_fgr_feature_matching(const float* src, int64_t n_src, const float* t
                                                                  absolute, seed, h0, tuple_scale, Kc, w.tstate,
                                                                  w.tflag, w.tblk);
       fgr_tuple_scan_kernel<<<1, 1024, 0, st>>>(w.tblk, n_mut, h0, Kc, w.tstate);
-      fgr_select_kernel<<<kFgrChunkBlocks, kFgrThreads, 0, st>>>(w.tflag, w.tblk, kFgrChunk, Kc, h0, w.tsel,
-                                                                  w.tstate + 1);
+      dgr_select_first(w.tflag, w.tblk, kFgrChunk, Kc, h0, w.tsel, w.tstate + 1, st);
       launches += 3;
     }
   }

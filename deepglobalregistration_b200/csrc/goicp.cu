@@ -3,10 +3,8 @@
 // transform of the target, with trimmed ICP proposing incumbents.  oracle/goicp.py restates every step (the
 // specification); every bound is an fp32 lookup summed in fp64 over a fixed pairwise tree, so a bound has the same
 // bits here and in numpy.
-//   goicp_normalise_kernel  both clouds centred on their fp64 means (dgr_cloud_stats, fgr.cu) and divided by s
-//   dt_fill / dt_occupy     G^3 grid over [-e, e]^3: 0 in every cell a target point falls in (clamped), "far" elsewhere
-//   dt_line_x_kernel        exact 1-D squared distance to the nearest occupied cell along x, one line per thread
-//   dt_fh_kernel            the Felzenszwalb-Huttenlocher lower envelope along y, then z, in integer arithmetic
+//   dgr_normalise_dt        both clouds centred on their fp64 means and divided by s, and the target's G^3 distance
+//                           transform over [-e, e]^3 (frame.cu)
 //   per round (one pinned host read before it):
 //     goicp_round_kernel     one CTA per rotation child of the B smallest pool cubes: rotated source and gamma_r in
 //                            shared memory; the upper-bound and the lower-bound inner search over translation cubes,
@@ -21,20 +19,18 @@
 #include <stdint.h>
 
 #include "common.cuh"
-#include "goicp_dt.cuh"
+#include "frame.cuh"
 #include "kabsch.cuh"
 
 namespace {
 
-constexpr int kMaxSrc = 1024;
+constexpr int kMaxSrc = kGoicpMaxSrc;
 constexpr int kRoundThreads = 256;                       // 8 warps: one per translation child
 constexpr int kInnerCap = 1536;                          // translation cubes in a CTA's shared-memory pool
 constexpr int kMaxLevel = 19;                            // 3 x 19-bit cube coordinates + the level in a 64-bit key
 constexpr int kMaxB = 512;                               // cubes per round: 8 B children sort in one CTA
 constexpr int kIcpIters = 30;
 constexpr int kIcpThreads = 1024;
-constexpr int kDtFar = 0x3fffffff;
-constexpr int kDtMaxG = 512;
 constexpr int kSkew = kMaxSrc + kMaxSrc / 32;            // a term buffer, skewed so lane l reading [32 l, 32 l + 32) is
                                                          // conflict-free
 constexpr double kSqrt3 = 1.7320508075688772;            // the double nearest sqrt(3)
@@ -92,30 +88,25 @@ struct GoWs {
   uint64_t* ckey;
 };
 
-inline int64_t words(int64_t n_4byte) { return (n_4byte + 1) / 2; }
-
 int64_t goicp_layout(int64_t n_s, int64_t n_t, int64_t G, int64_t cap, int64_t B, uint64_t* base, GoWs* w) {
-  const int64_t sizes[13] = {kStateWords, 8, 3 * n_s, words(3 * n_s), words(3 * n_t), n_s, words(G * G * G),
-                             cap, cap, cap, cap, 8 * 8 * B, 2 * 8 * B};
-  int64_t ofs[13], total = 0;
-  for (int k = 0; k < 13; ++k) { ofs[k] = total; total += sizes[k]; }
-  if (base != nullptr) {
-    w->st = reinterpret_cast<GoState*>(base + ofs[0]);
-    w->stat = reinterpret_cast<double*>(base + ofs[1]);
-    w->xn = reinterpret_cast<double*>(base + ofs[2]);
-    w->p32 = reinterpret_cast<float*>(base + ofs[3]);
-    w->y32 = reinterpret_cast<float*>(base + ofs[4]);
-    w->packed = base + ofs[5];
-    w->dt = reinterpret_cast<int32_t*>(base + ofs[6]);
-    w->pool_lb[0] = reinterpret_cast<double*>(base + ofs[7]);
-    w->pool_key[0] = base + ofs[8];
-    w->pool_lb[1] = reinterpret_cast<double*>(base + ofs[9]);
-    w->pool_key[1] = base + ofs[10];
-    w->child = reinterpret_cast<ChildRec*>(base + ofs[11]);
-    w->clb = reinterpret_cast<double*>(base + ofs[12]);
-    w->ckey = base + ofs[12] + 8 * B;
+  DgrCarver c(base);
+  GoWs r;
+  r.st = reinterpret_cast<GoState*>(c.take<uint64_t>(kStateWords));
+  r.stat = c.take<double>(8);
+  r.xn = c.take<double>(3 * n_s);
+  r.p32 = c.take<float>(3 * n_s);
+  r.y32 = c.take<float>(3 * n_t);
+  r.packed = c.take<uint64_t>(n_s);
+  r.dt = c.take<int32_t>(G * G * G);
+  for (int k = 0; k < 2; ++k) {
+    r.pool_lb[k] = c.take<double>(cap);
+    r.pool_key[k] = c.take<uint64_t>(cap);
   }
-  return total;
+  r.child = c.take<ChildRec>(8 * B);
+  r.clb = c.take<double>(8 * B);
+  r.ckey = c.take<uint64_t>(8 * B);
+  if (w != nullptr) *w = r;
+  return c.words;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -493,11 +484,11 @@ goicp_icp_step_kernel(GoParams P, const uint64_t* __restrict__ packed, GoState* 
   if (!st->icp_live) return;                            // uniform per launch
   __shared__ double sd[kMaxSrc];
   __shared__ int si[kMaxSrc];
-  __shared__ double red[kIcpThreads / 32];
+  __shared__ double red[kIcpThreads / 32][1];
   __shared__ double tot[16];
   __shared__ double sT[12];
   __shared__ int s_live;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   double T[12];
   for (int q = 0; q < 12; ++q) T[q] = st->icpT[q];
   if (tid < P.n_s) {
@@ -536,16 +527,9 @@ goicp_icp_step_kernel(GoParams P, const uint64_t* __restrict__ packed, GoState* 
     d2 = sd[tid];
   }
   for (int k = 0; k < 16; ++k) {
-    double v = k == 0 ? d2 : k < 4 ? x[k - 1] : k < 7 ? y[k - 4] : y[(k - 7) / 3] * x[(k - 7) % 3];
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
-    if (lane == 0) red[warp] = v;
-    __syncthreads();
-    if (tid == 0) {
-      double s = 0.0;
-      for (int w = 0; w < kIcpThreads / 32; ++w) s += red[w];
-      tot[k] = s;
-    }
+    const double v[1] = {k == 0 ? d2 : k < 4 ? x[k - 1] : k < 7 ? y[k - 4] : y[(k - 7) / 3] * x[(k - 7) % 3]};
+    const double s = dgr_block_sum<kIcpThreads>(v, red);
+    if (tid == 0) tot[k] = s;
     __syncthreads();
   }
   if (tid == 0) {
@@ -695,15 +679,10 @@ __global__ void goicp_merge_kernel(const double* __restrict__ alb, const uint64_
 __global__ void goicp_result_kernel(const GoState* __restrict__ st, const double* __restrict__ stat, int K, double eps,
                                     int converged, int rounds, int host_reads, double* __restrict__ result) {
   if (threadIdx.x != 0) return;
-  const double s0 = fmax(stat[3], stat[7]), s = s0 > 0.0 ? s0 : 1.0;
+  const double s = dgr_frame_scale(stat);
   const double* T = st->T;
-  // normalised y = R x + t with x = (X - m_s) / s, y = (Y - m_t) / s  =>  Y = R X + (m_t + s t - R m_s)
-  for (int a = 0; a < 3; ++a) {
-    for (int b = 0; b < 3; ++b) result[4 * a + b] = T[4 * a + b];
-    result[4 * a + 3] = stat[4 + a] + s * T[4 * a + 3] -
-                        (T[4 * a] * stat[0] + T[4 * a + 1] * stat[1] + T[4 * a + 2] * stat[2]);
-  }
-  result[12] = 0.0; result[13] = 0.0; result[14] = 0.0; result[15] = 1.0;
+  const double R[9] = {T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10]}, t[3] = {T[3], T[7], T[11]};
+  dgr_frame_pose(R, t, stat, s, result);
   result[16] = st->h.E;
   result[17] = st->h.pool_n == 0 ? st->h.E : st->h.lb_min;
   result[18] = eps;
@@ -720,113 +699,6 @@ __global__ void goicp_result_kernel(const GoState* __restrict__ st, const double
   result[29] = 0.0; result[30] = 0.0; result[31] = 0.0;
 }
 
-// ---------------------------------------------------------------------------------------
-// normalisation and the distance transform
-// ---------------------------------------------------------------------------------------
-__global__ void goicp_normalise_kernel(const float* __restrict__ src, int64_t n_s, const float* __restrict__ tgt,
-                                       int64_t n_t, const double* __restrict__ stat, double* __restrict__ xn,
-                                       float* __restrict__ y32) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const double s0 = fmax(stat[3], stat[7]), s = s0 > 0.0 ? s0 : 1.0;
-  if (xn != nullptr && i < n_s)
-    for (int a = 0; a < 3; ++a) xn[3 * i + a] = __ddiv_rn(__dsub_rn((double)src[3 * i + a], stat[a]), s);
-  if (i < n_t)
-    for (int a = 0; a < 3; ++a)
-      y32[3 * i + a] = __double2float_rn(__ddiv_rn(__dsub_rn((double)tgt[3 * i + a], stat[4 + a]), s));
-}
-
-__global__ void dt_fill_kernel(int32_t* __restrict__ dt, int64_t n) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) dt[i] = kDtFar;
-}
-
-__global__ void dt_occupy_kernel(const float* __restrict__ y32, int64_t n_t, int G, float e32, float h32,
-                                 int32_t* __restrict__ dt) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_t) return;
-  const int ix = dt_axis(y32[3 * i], e32, h32, G), iy = dt_axis(y32[3 * i + 1], e32, h32, G),
-            iz = dt_axis(y32[3 * i + 2], e32, h32, G);
-  dt[((int64_t)iz * G + iy) * G + ix] = 0;                 // idempotent
-}
-
-// along x: squared distance to the nearest occupied cell of the line (far when there is none)
-__global__ void dt_line_x_kernel(int32_t* __restrict__ dt, int G) {
-  const int64_t line = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (line >= (int64_t)G * G) return;
-  int32_t* r = dt + line * G;
-  int last = -1;
-  for (int x = 0; x < G; ++x) {                           // forward: distance to the last occupied cell
-    if (r[x] == 0) last = x;
-    r[x] = last >= 0 ? x - last : kDtFar;
-  }
-  int next = -1;
-  for (int x = G - 1; x >= 0; --x) {
-    int d = r[x];
-    if (d == 0) next = x;
-    if (next >= 0 && next - x < d) d = next - x;
-    r[x] = d < kDtFar ? d * d : kDtFar;
-  }
-}
-
-// lines along y (pass_z = 0) or z (pass_z = 1): d[q] = min_p (q - p)^2 + f[p] by the lower envelope of the
-// parabolas of the finite f[p]; intersections compared by cross-multiplication in int64
-__global__ void __launch_bounds__(128) dt_fh_kernel(int32_t* __restrict__ dt, int G, int pass_z) {
-  const int64_t line = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (line >= (int64_t)G * G) return;
-  const int64_t GG = (int64_t)G * G;
-  const int64_t base = pass_z ? line : (line / G) * GG + line % G, stride = pass_z ? GG : G;
-  int16_t v[kDtMaxG];
-  int32_t fv[kDtMaxG];
-  int m = 0;
-  for (int q = 0; q < G; ++q) {
-    const int32_t f = dt[base + q * stride];
-    if (f >= kDtFar) continue;
-    while (m >= 2) {
-      const int64_t a = v[m - 2], b = v[m - 1];
-      const int64_t hb = (int64_t)fv[m - 1] + b * b;
-      const int64_t n1 = ((int64_t)f + (int64_t)q * q) - hb, d1 = 2 * (q - b);
-      const int64_t n2 = hb - ((int64_t)fv[m - 2] + a * a), d2 = 2 * (b - a);
-      if (n1 * d2 <= n2 * d1) --m; else break;
-    }
-    v[m] = (int16_t)q;
-    fv[m] = f;
-    ++m;
-  }
-  if (m == 0) return;
-  int k = 0;
-  for (int q = 0; q < G; ++q) {
-    while (k + 1 < m) {
-      const int dn = (q - v[k + 1]) * (q - v[k + 1]) + fv[k + 1], dc = (q - v[k]) * (q - v[k]) + fv[k];
-      if (dn <= dc) ++k; else break;
-    }
-    dt[base + q * stride] = (q - v[k]) * (q - v[k]) + fv[k];
-  }
-}
-
-int32_t dt_check(int64_t n_src, int64_t n_tgt, int32_t G, double e) {
-  DGR_ARG_CHECK(n_src >= 1 && n_src <= kMaxSrc, "n_src must lie in [1, 1024]");
-  DGR_ARG_CHECK(n_tgt >= 1 && n_tgt < (1ll << 31), "n_tgt must lie in [1, 2^31)");
-  DGR_ARG_CHECK(G >= 16 && G <= kDtMaxG, "dt_size must lie in [16, 512]");
-  DGR_ARG_CHECK(e > 0.0 && isfinite(e), "dt_expand must be positive");
-  return DGR_OK;
-}
-
-// normalisation + distance transform; xn may be null
-int dt_build(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, int G, double e, double* stat,
-             double* xn, float* y32, int32_t* dt, cudaStream_t st) {
-  const float e32 = (float)e, h32 = (float)(2.0 * e / G);
-  const int64_t cells = (int64_t)G * G * G, lines = (int64_t)G * G;
-  dgr_cloud_stats(src, n_src, tgt, n_tgt, stat, st);
-  goicp_normalise_kernel<<<dgr_blocks(n_src > n_tgt ? n_src : n_tgt, 256), 256, 0, st>>>(src, n_src, tgt, n_tgt, stat,
-                                                                                          xn, y32);
-  dt_fill_kernel<<<dgr_blocks(cells, 256), 256, 0, st>>>(dt, cells);
-  dt_occupy_kernel<<<dgr_blocks(n_tgt, 256), 256, 0, st>>>(y32, n_tgt, G, e32, h32, dt);
-  dt_line_x_kernel<<<dgr_blocks(lines, 128), 128, 0, st>>>(dt, G);
-  dt_fh_kernel<<<dgr_blocks(lines, 128), 128, 0, st>>>(dt, G, 0);
-  dt_fh_kernel<<<dgr_blocks(lines, 128), 128, 0, st>>>(dt, G, 1);
-  return 7;
-}
-
 // the per-round host read: pinned, one per host thread
 GoHost* pinned_host() {
   static thread_local GoHost* p = nullptr;
@@ -837,24 +709,7 @@ GoHost* pinned_host() {
 
 }  // namespace
 
-int dgr_goicp_normalise_dt(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, int G, double e,
-                           double* stat, double* xn, float* y32, int32_t* dt, cudaStream_t st) {
-  return dt_build(src, n_src, tgt, n_tgt, G, e, stat, xn, y32, dt, st);
-}
-
 extern "C" {
-
-int32_t dgr_goicp_dt_build(const float* src, int64_t n_src, const float* tgt, int64_t n_tgt, int32_t dt_size,
-                           double dt_expand, double* stat, float* tgt_norm, int32_t* dt, void* stream) {
-  DGR_ARG_CHECK(src != nullptr && tgt != nullptr && stat != nullptr && tgt_norm != nullptr && dt != nullptr,
-                "null pointer");
-  const int32_t r = dt_check(n_src, n_tgt, dt_size, dt_expand);
-  if (r != DGR_OK) return r;
-  dgr_note_launches(dt_build(src, n_src, tgt, n_tgt, dt_size, dt_expand, stat, nullptr, tgt_norm, dt,
-                             (cudaStream_t)stream));
-  DGR_LAUNCH_CHECK();
-  return DGR_OK;
-}
 
 int32_t dgr_goicp_ws_elems(int64_t n_src, int64_t n_tgt, int32_t dt_size, int64_t max_rotation_cubes,
                            int32_t cubes_per_round, int64_t* n_elems) {
@@ -870,7 +725,7 @@ int32_t dgr_goicp(const float* src, int64_t n_src, const float* tgt, int64_t n_t
                   int64_t max_rotation_cubes, uint64_t* ws, double* result, void* stream) {
   DGR_ARG_CHECK(src != nullptr && tgt != nullptr && rot_min != nullptr && trans_min != nullptr && ws != nullptr &&
                 result != nullptr, "null pointer");
-  const int32_t r = dt_check(n_src, n_tgt, dt_size, dt_expand);
+  const int32_t r = dgr_goicp_dt_check(n_src, n_tgt, dt_size, dt_expand);
   if (r != DGR_OK) return r;
   DGR_ARG_CHECK(trim_fraction >= 0.0 && trim_fraction < 1.0, "trim_fraction must lie in [0, 1)");
   DGR_ARG_CHECK(mse_thresh > 0.0 && isfinite(mse_thresh), "mse_thresh must be positive");
@@ -902,7 +757,7 @@ int32_t dgr_goicp(const float* src, int64_t n_src, const float* tgt, int64_t n_t
   P.rw = rot_width;
   P.tw = trans_width;
 
-  int launches = dt_build(src, n_src, tgt, n_tgt, dt_size, dt_expand, w.stat, w.xn, w.y32, w.dt, st);
+  int launches = dgr_normalise_dt(src, n_src, tgt, n_tgt, dt_size, dt_expand, w.stat, w.xn, w.y32, w.dt, st);
   GoState* S = w.st;
   const auto icp = [&]() {
     for (int k = 0; k < kIcpIters; ++k) {

@@ -372,6 +372,16 @@ inline int icp_blocks(int64_t n_src) {
   return blocks > (unsigned)kIcpMaxBlocks ? kIcpMaxBlocks : (int)blocks;
 }
 
+// workspace size in 8-byte words; carves `base` into the state and the per-block partials when it is not null
+int64_t icp_layout(int64_t n_src, double* base, IcpState** state, double** part) {
+  static_assert(sizeof(IcpState) <= kIcpState * sizeof(double), "state workspace too small");
+  DgrCarver c(base);
+  IcpState* s = reinterpret_cast<IcpState*>(c.take<double>(kIcpState));
+  double* p = c.take<double>((int64_t)icp_blocks(n_src) * kIcpStride);
+  if (state != nullptr) { *state = s; *part = p; }
+  return c.words;
+}
+
 }  // namespace
 
 extern "C" {
@@ -403,7 +413,7 @@ int32_t dgr_estimate_normals(const float* xyz, int64_t n, const dgr_keyspec_t* s
 
 int32_t dgr_icp_ws_elems(int64_t n_src, int64_t* n_elems) {
   DGR_ARG_CHECK(n_elems != nullptr && n_src >= 0, "bad arguments");
-  *n_elems = kIcpState + (int64_t)icp_blocks(n_src) * kIcpStride;
+  *n_elems = icp_layout(n_src, nullptr, nullptr, nullptr);
   return DGR_OK;
 }
 
@@ -416,10 +426,10 @@ int32_t dgr_icp(const float* src, int64_t n_src, const float* tgt, const float* 
   DGR_ARG_CHECK(max_dist / voxel <= 4.0, "search radius above 4 voxels is not supported");
   DGR_ARG_CHECK(n_src >= 0 && n_src < (1ll << 31), "point count out of range");
   DGR_ARG_CHECK(T_init != nullptr && ws != nullptr && result != nullptr && spec != nullptr, "null pointer");
-  static_assert(sizeof(IcpState) <= kIcpState * sizeof(double), "state workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
-  IcpState* state = reinterpret_cast<IcpState*>(ws);
-  double* part = ws + kIcpState;
+  IcpState* state;
+  double* part;
+  icp_layout(n_src, ws, &state, &part);
   const int blocks = icp_blocks(n_src);
   const auto iterate = [&](auto estimator) {
     using E = decltype(estimator);

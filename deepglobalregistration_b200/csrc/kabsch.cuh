@@ -1,5 +1,6 @@
-// Small fp64 solvers shared by registration.cu (weighted Procrustes), ransac.cu (4-point hypotheses), fgr.cu
-// (Gauss-Newton steps) and icp.cu (normals, ICP steps).
+// Small fp64 solvers shared by registration.cu (weighted Procrustes), ransac.cu (4-point hypotheses), fgr.cu and
+// pointnetlk.cu (Gauss-Newton / Lucas-Kanade steps), icp.cu (normals, ICP steps), goicp.cu (trimmed ICP) and
+// super4pcs.cu (congruent-set fits).
 #pragma once
 
 // ---------------------------------------------------------------------------------------

@@ -23,6 +23,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "frame.cuh"
 #include "kabsch.cuh"
 #include "tc_common.cuh"
 
@@ -301,18 +302,16 @@ struct LkWs {
 };
 
 int64_t lk_layout(uint64_t* base, LkWs* w) {
-  const int64_t sizes[6] = {8, 84, (int64_t)(sizeof(LkState) + 7) / 8, 7 * kF / 2, kF / 2, 6 * kF};
-  int64_t ofs[6], total = 0;
-  for (int k = 0; k < 6; ++k) { ofs[k] = total; total += sizes[k]; }
-  if (base != nullptr) {
-    w->stat = reinterpret_cast<double*>(base + ofs[0]);
-    w->jposes = reinterpret_cast<double*>(base + ofs[1]);
-    w->st = reinterpret_cast<LkState*>(base + ofs[2]);
-    w->fj = reinterpret_cast<unsigned*>(base + ofs[3]);
-    w->f = reinterpret_cast<unsigned*>(base + ofs[4]);
-    w->J = reinterpret_cast<double*>(base + ofs[5]);
-  }
-  return total;
+  DgrCarver c(base);
+  LkWs r;
+  r.stat = c.take<double>(8);
+  r.jposes = c.take<double>(7 * 12);
+  r.st = c.take<LkState>(1);
+  r.fj = c.take<unsigned>(7 * kF);
+  r.f = c.take<unsigned>(kF);
+  r.J = c.take<double>(6 * kF);
+  if (w != nullptr) *w = r;
+  return c.words;
 }
 
 // SE(3) exponential of xi = (omega, v): [R | t] row-major, R = I + A W + B W^2, t = (I + B W + C W^2) v
@@ -344,7 +343,8 @@ __device__ void se3_exp(const double xi[6], double E[12]) {
   }
 }
 
-// fixed-order sum of one double per thread over a 1024-thread block; valid in every thread
+// fixed-order sum of one double per thread over a 1024-thread block (dgr_block_sum's order); valid in every thread,
+// which keeps lk_step_kernel's single-thread tail within its 64 registers
 __device__ double block_sum_1024(double v, double* red) {
   for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;

@@ -189,7 +189,7 @@ ransac_final_kernel(const float4* __restrict__ src, const float4* __restrict__ t
   __syncthreads();
   key = s_key[0];
   hyp = s_hyp[0];
-  double cnt = 0, err = 0;
+  double ce[2] = {0, 0};                                  // inlier count, sum d^2
   if (key != 0) {
     for (uint32_t i = tid; i < n; i += blockDim.x) {
       float4 a = src[i], b = tgt[i];
@@ -197,18 +197,12 @@ ransac_final_kernel(const float4* __restrict__ src, const float4* __restrict__ t
       double dy = s_T[4] * a.x + s_T[5] * a.y + s_T[6] * a.z + s_T[7] - b.y;
       double dz = s_T[8] * a.x + s_T[9] * a.y + s_T[10] * a.z + s_T[11] - b.z;
       double d2 = dx * dx + dy * dy + dz * dz;
-      if (sqrt(d2) < max_dist) { cnt += 1.0; err += d2; }
+      if (sqrt(d2) < max_dist) { ce[0] += 1.0; ce[1] += d2; }
     }
   }
-  for (int d = 16; d > 0; d >>= 1) {
-    cnt += __shfl_xor_sync(0xffffffffu, cnt, d);
-    err += __shfl_xor_sync(0xffffffffu, err, d);
-  }
-  if ((tid & 31) == 0) { s_red[tid >> 5][0] = cnt; s_red[tid >> 5][1] = err; }
-  __syncthreads();
+  const double cnt = dgr_block_sum<1024>(ce, s_red);
+  const double err = __shfl_down_sync(0xffffffffu, cnt, 1);    // thread 1's sum
   if (tid == 0) {
-    cnt = 0; err = 0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { cnt += s_red[w][0]; err += s_red[w][1]; }
     for (int k = 0; k < 12; ++k) result[k] = s_T[k];
     result[12] = 0; result[13] = 0; result[14] = 0; result[15] = 1;
     result[16] = n ? cnt / (double)n : 0.0;                 // fitness
@@ -223,6 +217,27 @@ inline uint32_t ransac_blocks(int64_t num_hyp) {
   return (uint32_t)((num_hyp + per_block - 1) / per_block);
 }
 
+struct RansacWs {
+  float4* src;                 // [n_corr] packed correspondences
+  float4* tgt;
+  unsigned long long* blk_key; // [n_blk] best key and hypothesis per evaluation block
+  unsigned long long* blk_hyp;
+};
+
+// workspace size in 8-byte words; carves `base` into the regions when it is not null
+int64_t ransac_layout(int64_t n_corr, int64_t num_hyp, uint64_t* base, RansacWs* w) {
+  const int64_t n_blk = ransac_blocks(num_hyp);
+  DgrCarver c(base);
+  RansacWs r;
+  r.src = c.take<float4>(n_corr);
+  r.tgt = c.take<float4>(n_corr);
+  r.blk_key = c.take<unsigned long long>(n_blk);
+  r.blk_hyp = c.take<unsigned long long>(n_blk);
+  c.take<uint64_t>(2);                                  // 2 unused words, part of the size reported since the start
+  if (w != nullptr) *w = r;
+  return c.words;
+}
+
 // ---------------------------------------------------------------------------------------
 // Feature-matching RANSAC: open3d 0.10's registration_ransac_based_on_feature_matching as the reference
 // calls it (core/deep_global_registration.py:29-47), restated in oracle/ransac_fm.py.  Hypothesis h draws
@@ -231,8 +246,8 @@ inline uint32_t ransac_blocks(int64_t num_hyp) {
 // pass every checker are scored on ALL source points (nearest target point strictly within max_dist of
 // R s + t, through the target's voxel hash).  Five launches, no host read:
 //   fm_hypothesis_kernel  one thread per hypothesis: draw, edge checker, fit, distance checker -> flag, pose
-//   fm_scan_kernel        exclusive scan of the per-block validated counts (the coordplan.cu pattern)
-//   fm_select_kernel      the first V validated hypothesis numbers, in hypothesis order
+//   dgr_scan_counts       exclusive scan of the per-block validated counts (coords.cu)
+//   dgr_select_first      the first V validated hypothesis numbers, in hypothesis order (coords.cu)
 //   fm_score_kernel       (selected hypothesis x 1024-point chunk) per block, 8 lanes per point
 //                         (dgr_voxel_nearest8, shared with the ICP); fixed-order block partials
 //   fm_final_kernel       partials summed in chunk order, best by (count, smaller sum d^2, lower h)
@@ -251,24 +266,20 @@ struct FmWs {
   double* part;       // [Vc][n_chunk][2] (matched, sum d^2) per scoring block
 };
 
-inline int64_t fm_words(int64_t n_int32) { return (n_int32 + 1) / 2; }
-
 // workspace size in 8-byte words; carves `base` into the regions when it is not null
 int64_t fm_layout(int64_t n_src, int64_t M, int64_t V, uint64_t* base, FmWs* w) {
   const int64_t Vc = V < M ? V : M;
   const int64_t n_hblk = (M + kFmThreads - 1) / kFmThreads;
   const int64_t n_chunk = (n_src + kFmChunk - 1) / kFmChunk;
-  const int64_t sizes[5] = {12 * M, fm_words(M), fm_words(n_hblk + 1), fm_words(Vc), 2 * Vc * n_chunk};
-  int64_t ofs[5], total = 0;
-  for (int k = 0; k < 5; ++k) { ofs[k] = total; total += sizes[k]; }
-  if (base != nullptr) {
-    w->pose = reinterpret_cast<double*>(base + ofs[0]);
-    w->flag = reinterpret_cast<int32_t*>(base + ofs[1]);
-    w->blk = reinterpret_cast<int32_t*>(base + ofs[2]);
-    w->sel = reinterpret_cast<int32_t*>(base + ofs[3]);
-    w->part = reinterpret_cast<double*>(base + ofs[4]);
-  }
-  return total;
+  DgrCarver c(base);
+  FmWs r;
+  r.pose = c.take<double>(12 * M);
+  r.flag = c.take<int32_t>(M);
+  r.blk = c.take<int32_t>(n_hblk + 1);
+  r.sel = c.take<int32_t>(Vc);
+  r.part = c.take<double>(2 * Vc * n_chunk);
+  if (w != nullptr) *w = r;
+  return c.words;
 }
 
 __global__ void __launch_bounds__(kFmThreads)
@@ -323,17 +334,6 @@ fm_hypothesis_kernel(const float* __restrict__ src, uint32_t n_src, const float*
   }
   const int cnt = __syncthreads_count(ok);
   if (threadIdx.x == 0) blk_cnt[blockIdx.x] = cnt;
-}
-
-__global__ void __launch_bounds__(1024) fm_scan_kernel(int32_t* blk, int64_t n_hblk) {
-  const int total = dgr_block_scan_inplace(blk, n_hblk);
-  if (threadIdx.x == 0) blk[n_hblk] = total;
-}
-
-__global__ void __launch_bounds__(kFmThreads)
-fm_select_kernel(const int32_t* __restrict__ flag, const int32_t* __restrict__ blk, int64_t M, int64_t Vc,
-                 int32_t* __restrict__ sel) {
-  dgr_select_first_256(flag, blk[blockIdx.x], M, Vc, 0, sel);
 }
 
 __global__ void __launch_bounds__(kFmThreads, 4)   // <= 64 registers: 32 warps per SM hide the probe latency
@@ -441,7 +441,7 @@ extern "C" {
 
 int32_t dgr_ransac_ws_elems(int64_t n_corr, int64_t num_hyp, int64_t* n_elems) {
   DGR_ARG_CHECK(n_elems != nullptr && n_corr >= 0 && num_hyp >= 0, "bad arguments");
-  *n_elems = 4 * n_corr + 2 * (int64_t)ransac_blocks(num_hyp) + 2;
+  *n_elems = ransac_layout(n_corr, num_hyp, nullptr, nullptr);
   return DGR_OK;
 }
 
@@ -453,15 +453,13 @@ int32_t dgr_ransac_correspondence(const float* x, const float* y, const int32_t*
   DGR_ARG_CHECK(num_hyp >= 1 && num_hyp <= (1ll << 40), "hypothesis count out of range");
   DGR_ARG_CHECK(max_dist > 0, "max_dist must be positive");
   cudaStream_t st = (cudaStream_t)stream;
-  float4* src = reinterpret_cast<float4*>(ws);
-  float4* tgt = src + n_corr;
-  unsigned long long* blk_key = reinterpret_cast<unsigned long long*>(tgt + n_corr);
+  RansacWs w;
+  ransac_layout(n_corr, num_hyp, ws, &w);
   const uint32_t n_blk = ransac_blocks(num_hyp);
-  unsigned long long* blk_hyp = blk_key + n_blk;
-  ransac_pack_kernel<<<dgr_blocks(n_corr, 256), 256, 0, st>>>(x, y, idx0, idx1, n_corr, src, tgt);
-  ransac_eval_kernel<<<n_blk, kRansacThreads, 0, st>>>(src, tgt, (uint32_t)n_corr, seed, (uint64_t)num_hyp,
-                                                       (float)(max_dist * max_dist), blk_key, blk_hyp);
-  ransac_final_kernel<<<1, 1024, 0, st>>>(src, tgt, (uint32_t)n_corr, seed, blk_key, blk_hyp, n_blk, max_dist,
+  ransac_pack_kernel<<<dgr_blocks(n_corr, 256), 256, 0, st>>>(x, y, idx0, idx1, n_corr, w.src, w.tgt);
+  ransac_eval_kernel<<<n_blk, kRansacThreads, 0, st>>>(w.src, w.tgt, (uint32_t)n_corr, seed, (uint64_t)num_hyp,
+                                                       (float)(max_dist * max_dist), w.blk_key, w.blk_hyp);
+  ransac_final_kernel<<<1, 1024, 0, st>>>(w.src, w.tgt, (uint32_t)n_corr, seed, w.blk_key, w.blk_hyp, n_blk, max_dist,
                                           result);
   dgr_note_launches(3);
   DGR_LAUNCH_CHECK();
@@ -496,8 +494,8 @@ int32_t dgr_ransac_feature_matching(const float* src, int64_t n_src, const float
   const int64_t n_chunk = (n_src + kFmChunk - 1) / kFmChunk;
   fm_hypothesis_kernel<<<n_hblk, kFmThreads, 0, st>>>(src, (uint32_t)n_src, tgt, nn, seed, max_iteration, edge_ratio,
                                                       check_dist, w.pose, w.flag, w.blk);
-  fm_scan_kernel<<<1, 1024, 0, st>>>(w.blk, n_hblk);
-  fm_select_kernel<<<n_hblk, kFmThreads, 0, st>>>(w.flag, w.blk, max_iteration, Vc, w.sel);
+  dgr_scan_counts(w.blk, n_hblk, st);
+  dgr_select_first(w.flag, w.blk, max_iteration, Vc, 0, w.sel, nullptr, st);
   fm_score_kernel<<<dim3((unsigned)Vc, (unsigned)n_chunk), kFmThreads, 0, st>>>(
       src, n_src, tgt, spec, keys, vals, (uint64_t)cap - 1, batch, cell, max_dist, w.pose, w.sel, w.blk + n_hblk, Vc,
       w.part);

@@ -148,45 +148,11 @@ __device__ void rot6d_backward(const Rot6dCache& c, const float G[9], float g[6]
 // the cluster kernel
 // ---------------------------------------------------------------------------------------
 struct RegShared {
-  double slots[2][kClusterSize][kMaxVals];
-  double warp_part[kRegThreads / 32][kMaxVals];
-  double tot[kMaxVals];
+  DgrReduceShared<kMaxVals, kRegThreads, kClusterSize> red;   // the per-iteration sums over the cluster
   float params[16];   // R (9) + t (3)
   int counts[kClusterSize];
   int flags[4];
 };
-
-// Sum `nv` per-thread doubles over the whole cluster.  Result in sh.tot[0..nv) of every CTA.
-template <int NV>
-__device__ __forceinline__ void cluster_allreduce(cg::cluster_group& cluster, RegShared& sh,
-                                                  double (&v)[NV], int& parity) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < NV; ++k) {
-    double x = v[k];
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) x += __shfl_xor_sync(0xffffffffu, x, d);
-    if (lane == 0) sh.warp_part[warp][k] = x;
-  }
-  __syncthreads();
-  const unsigned rank = cluster.block_rank();
-  if (threadIdx.x < NV) {
-    double s = 0.0;
-    for (int w = 0; w < kRegThreads / 32; ++w) s += sh.warp_part[w][threadIdx.x];
-    for (unsigned r = 0; r < kClusterSize; ++r) {
-      RegShared* remote = cluster.map_shared_rank(&sh, r);
-      remote->slots[parity][rank][threadIdx.x] = s;
-    }
-  }
-  cluster.sync();
-  if (threadIdx.x < NV) {
-    double s = 0.0;
-    for (int r = 0; r < kClusterSize; ++r) s += sh.slots[parity][r][threadIdx.x];
-    sh.tot[threadIdx.x] = s;
-  }
-  __syncthreads();
-  parity ^= 1;
-}
 
 __global__ void __cluster_dims__(kClusterSize, 1, 1) __launch_bounds__(kRegThreads, 1)
 se3_register_kernel(const float* __restrict__ pack, int64_t n, float q, int max_iter,
@@ -211,24 +177,9 @@ se3_register_kernel(const float* __restrict__ pack, int64_t n, float q, int max_
     int64_t i = base + tid;
     float wv = (i < hi) ? pack[6 * n + i] : 0.f;
     int act = (wv != 0.f) ? 1 : 0;
-    // block exclusive scan of `act`
-    int inc = act;
-    const int lane = tid & 31, warp = tid >> 5;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      int t = __shfl_up_sync(0xffffffffu, inc, d);
-      if (lane >= d) inc += t;
-    }
-    __shared__ int wsum[kRegThreads / 32];
-    if (lane == 31) wsum[warp] = inc;
-    __syncthreads();
-    int wbase = 0, tot = 0;
-    for (int k = 0; k < kRegThreads / 32; ++k) {
-      int s = wsum[k];
-      if (k < warp) wbase += s;
-      tot += s;
-    }
-    int pos = s_count + wbase + inc - act;
+    int tot;
+    const int excl = dgr_block_exclusive_scan<kRegThreads>(act, &tot);
+    const int pos = s_count + excl;
     if (act && pos < kSmemPoints) {
 #pragma unroll
       for (int a = 0; a < 7; ++a) pts[a * kSmemPoints + pos] = pack[a * n + i];
@@ -275,14 +226,14 @@ se3_register_kernel(const float* __restrict__ pack, int64_t n, float q, int max_
       a[4] += w * y[0]; a[5] += w * y[1]; a[6] += w * y[2];
     }
     for (int k = 0; k < 7; ++k) v[k] = (double)a[k];
-    cluster_allreduce<7>(cluster, sh, v, parity);
+    dgr_allreduce<kClusterSize>(sh.red, v, parity);
   }
-  const double W1 = sh.tot[0];
+  const double W1 = sh.red.tot[0];
   const float wden = (float)W1 + eps;
   float mux[3], muy[3];
   for (int k = 0; k < 3; ++k) {
-    mux[k] = (float)(sh.tot[1 + k] / (double)wden);
-    muy[k] = (float)(sh.tot[4 + k] / (double)wden);
+    mux[k] = (float)(sh.red.tot[1 + k] / (double)wden);
+    muy[k] = (float)(sh.red.tot[4 + k] / (double)wden);
   }
   __syncthreads();
   // ---- second moments Sxy = sum wn (y - muy)(x - mux)^T -------------------------------------
@@ -301,12 +252,12 @@ se3_register_kernel(const float* __restrict__ pack, int64_t n, float q, int max_
     }
     double v[9];
     for (int k = 0; k < 9; ++k) v[k] = (double)a[k];
-    cluster_allreduce<9>(cluster, sh, v, parity);
+    dgr_allreduce<kClusterSize>(sh.red, v, parity);
   }
   if (tid == 0) {
     double S[3][3], R[3][3];
     for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) S[r][c] = (double)(float)sh.tot[3 * r + c];   // fp32 Sxy, as the reference
+      for (int c = 0; c < 3; ++c) S[r][c] = (double)(float)sh.red.tot[3 * r + c];   // fp32 Sxy, as the reference
     if (m_total > 0) {
       kabsch_rotation(S, R);
     } else {
@@ -379,17 +330,17 @@ se3_register_kernel(const float* __restrict__ pack, int64_t n, float q, int max_
     double v[13];
 #pragma unroll
     for (int k = 0; k < 13; ++k) v[k] = (double)a[k];
-    cluster_allreduce<13>(cluster, sh, v, parity);
+    dgr_allreduce<kClusterSize>(sh.red, v, parity);
     // every thread evaluates the stop rule on identical data so the cluster stays in lock step
     const double w1 = W1;   // weights are >= 0: sum w == sum |w|
-    loss = (float)(sh.tot[0] / w1);
+    loss = (float)(sh.red.tot[0] / w1);
     if (it == 0) loss_prev = loss;   // the reference evaluates loss_prev on the initial pose
     if (loss < 1e-7f) break;
     if (tid == 0) {
       float G[9], grad[9];
-      for (int k = 0; k < 9; ++k) G[k] = (float)(sh.tot[4 + k] / w1);
+      for (int k = 0; k < 9; ++k) G[k] = (float)(sh.red.tot[4 + k] / w1);
       rot6d_backward(cache, G, grad);
-      for (int k = 0; k < 3; ++k) grad[6 + k] = (float)(sh.tot[1 + k] / w1);
+      for (int k = 0; k < 3; ++k) grad[6 + k] = (float)(sh.red.tot[1 + k] / w1);
       b1t *= 0.9;
       b2t *= 0.999;
       const float step_size = (float)(lr / (1.0 - b1t));

@@ -5,13 +5,13 @@
 // geometry is fp64 in the oracle's operation order with no contraction, so the counts have the same bits here and
 // in numpy.  Every round of B bases is enqueued up front; each kernel returns at once when the device `done` flag
 // is set, so the only host read is the caller's read of the result.
-//   dgr_goicp_normalise_dt   Go-ICP's normalisation and distance transform (goicp.cu)
+//   dgr_normalise_dt         the normalised frame and the target's distance transform, as Go-ICP's (frame.cu)
 //   s4_init_kernel           state, the target sample Q (fp64), r = max |p|, D, delta; base log cleared
 //   per round:
 //     s4_base_kernel         a warp per base: 32 counter-hash triplets (a lane each), the fourth point (lanes over rows)
 //     s4_pair_count_kernel   a (base, tile of kTileRows rows of Q x Q) per CTA: |S1|, |S2| of the tile
 //     s4_pair_scan_kernel    the tile counts of each base scanned (dgr_block_scan_inplace); the join's hash cleared
-//     s4_pair_scatter_kernel the pairs of a tile in row-major order (dgr_block_exclusive_scan_256), capped
+//     s4_pair_scatter_kernel the pairs of a tile in row-major order (dgr_block_exclusive_scan), capped
 //     s4_hash_*_kernel       e2 of every S2 pair bucketed by its delta-grid cell: counts, scan, placement
 //     s4_join_count_kernel   a thread per S1 pair: the S2 pairs in the 27 cells around e1 meeting every predicate
 //     s4_join_scan_kernel    per-pair counts scanned in int64: candidate offsets in (i, j) order, saturated at the cap
@@ -27,7 +27,7 @@
 #include <stdint.h>
 
 #include "common.cuh"
-#include "goicp_dt.cuh"
+#include "frame.cuh"
 #include "kabsch.cuh"
 
 namespace {
@@ -57,7 +57,6 @@ struct BaseRec {
   int64_t ncand_raw;
   int32_t valid, n1, n2, m1, m2, ncand, nver;
 };
-constexpr int kRecWords = (int)((sizeof(BaseRec) + 7) / 8);
 
 struct S4Params {
   const double* xn;      // [n_s][3]
@@ -200,7 +199,7 @@ s4_init_kernel(S4Params P, const double* __restrict__ stat, const float* __restr
   __syncthreads();
   if (threadIdx.x == 0) {
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) m = fmax(m, red[w]);
-    const double s0 = fmax(stat[3], stat[7]), s = s0 > 0.0 ? s0 : 1.0;
+    const double s = dgr_frame_scale(stat);
     st->s = s;
     st->delta = __ddiv_rn(P.delta_m, s);
     st->d32 = __double2float_rn(st->delta);
@@ -386,8 +385,10 @@ __global__ void __launch_bounds__(256) s4_pair_scatter_kernel(S4Params P) {
     int u = 0, v = 0, t1, t2;
     bool f1, f2;
     pair_flags(P, R, e0 + threadIdx.x, nelem, u0, u, v, f1, f2);
-    const int p1 = o1 + dgr_block_exclusive_scan_256(f1, &t1);
-    const int p2 = o2 + dgr_block_exclusive_scan_256(f2, &t2);
+    const int p1 = o1 + dgr_block_exclusive_scan<256>(f1, &t1);
+    __syncthreads();
+    const int p2 = o2 + dgr_block_exclusive_scan<256>(f2, &t2);
+    __syncthreads();
     if (f1 && p1 < P.cap) S1[p1] = make_int2(u, v);
     if (f2 && p2 < P.cap) S2[p2] = make_int2(u, v);
     o1 += t1;
@@ -603,9 +604,11 @@ __global__ void __launch_bounds__(256) s4_select_kernel(S4Params P) {
     const int c = k < R.ncand ? pc[k] : -1;
     const int eq = c == cut, gt = c > cut;
     int teq, tsel;
-    const int req = carry_eq + dgr_block_exclusive_scan_256(eq, &teq);
+    const int req = carry_eq + dgr_block_exclusive_scan<256>(eq, &teq);
+    __syncthreads();
     const int take = gt || (eq && req < need);
-    const int pos = carry_sel + dgr_block_exclusive_scan_256(take, &tsel);
+    const int pos = carry_sel + dgr_block_exclusive_scan<256>(take, &tsel);
+    __syncthreads();
     if (take) sel[pos] = k;
     carry_eq += teq;
     carry_sel += tsel;
@@ -682,13 +685,7 @@ __global__ void s4_result_kernel(const S4State* __restrict__ st, const double* _
                                  double* __restrict__ result) {
   if (threadIdx.x != 0) return;
   const double s = st->s;
-  // normalised y = R x + t with x = (X - m_s) / s, y = (Y - m_t) / s  =>  Y = R X + (m_t + s t - R m_s)
-  for (int a = 0; a < 3; ++a) {
-    for (int c = 0; c < 3; ++c) result[4 * a + c] = st->R[3 * a + c];
-    result[4 * a + 3] = stat[4 + a] + s * st->t[a] -
-                        (st->R[3 * a] * stat[0] + st->R[3 * a + 1] * stat[1] + st->R[3 * a + 2] * stat[2]);
-  }
-  result[12] = 0.0; result[13] = 0.0; result[14] = 0.0; result[15] = 1.0;
+  dgr_frame_pose(st->R, st->t, stat, s, result);
   const int lcp = max(st->best_lcp, 0);
   result[16] = (double)lcp / n_s;
   result[17] = lcp;
@@ -708,8 +705,6 @@ __global__ void s4_result_kernel(const S4State* __restrict__ st, const double* _
 // ---------------------------------------------------------------------------------------
 // workspace
 // ---------------------------------------------------------------------------------------
-inline int64_t words(int64_t n_4byte) { return (n_4byte + 1) / 2; }
-
 int64_t hash_buckets(int64_t cap) {
   int64_t H = 1;
   while (H < 2 * cap) H <<= 1;
@@ -726,35 +721,32 @@ struct S4Ws {
 int64_t s4_layout(int64_t n_s, int64_t n_t, int64_t n_q, int64_t G, int64_t B, int64_t cap, int64_t maxc, int64_t V,
                   uint64_t* base, S4Ws* w, S4Params* P) {
   const int64_t tiles = (n_q + kTileRows - 1) / kTileRows, H = hash_buckets(cap);
-  const int64_t sizes[17] = {kStateWords, 8, 3 * n_s, words(3 * n_t), words(G * G * G), 3 * n_q, B * kRecWords,
-                             words(2 * B * tiles), 2 * B * cap, words(B * (H + 1)), words(B * H), words(B * cap),
-                             words(B * cap), B * maxc, words(B * maxc), words(B * V), words(B * V)};
-  int64_t ofs[17], total = 0;
-  for (int k = 0; k < 17; ++k) { ofs[k] = total; total += sizes[k]; }
-  if (base != nullptr) {
-    P->st = reinterpret_cast<S4State*>(base + ofs[0]);
-    w->stat = reinterpret_cast<double*>(base + ofs[1]);
-    w->xn = reinterpret_cast<double*>(base + ofs[2]);
-    w->y32 = reinterpret_cast<float*>(base + ofs[3]);
-    w->dt = reinterpret_cast<int32_t*>(base + ofs[4]);
-    P->xn = w->xn;
-    P->dt = w->dt;
-    P->q = reinterpret_cast<double*>(base + ofs[5]);
-    P->rec = reinterpret_cast<BaseRec*>(base + ofs[6]);
-    P->cnt = reinterpret_cast<int32_t*>(base + ofs[7]);
-    P->pairs = reinterpret_cast<int2*>(base + ofs[8]);
-    P->hcnt = reinterpret_cast<int32_t*>(base + ofs[9]);
-    P->hcur = reinterpret_cast<int32_t*>(base + ofs[10]);
-    P->ent = reinterpret_cast<int32_t*>(base + ofs[11]);
-    P->jc = reinterpret_cast<int32_t*>(base + ofs[12]);
-    P->cand = reinterpret_cast<int2*>(base + ofs[13]);
-    P->pcnt = reinterpret_cast<int32_t*>(base + ofs[14]);
-    P->sel = reinterpret_cast<int32_t*>(base + ofs[15]);
-    P->lcp = reinterpret_cast<int32_t*>(base + ofs[16]);
-    P->tiles = (int)tiles;
-    P->H = H;
-  }
-  return total;
+  DgrCarver c(base);
+  S4Ws ws;
+  S4Params p;
+  p.st = reinterpret_cast<S4State*>(c.take<uint64_t>(kStateWords));
+  ws.stat = c.take<double>(8);
+  ws.xn = c.take<double>(3 * n_s);
+  ws.y32 = c.take<float>(3 * n_t);
+  ws.dt = c.take<int32_t>(G * G * G);
+  p.xn = ws.xn;
+  p.dt = ws.dt;
+  p.q = c.take<double>(3 * n_q);
+  p.rec = c.take<BaseRec>(B);
+  p.cnt = c.take<int32_t>(2 * B * tiles);
+  p.pairs = c.take<int2>(2 * B * cap);
+  p.hcnt = c.take<int32_t>(B * (H + 1));
+  p.hcur = c.take<int32_t>(B * H);
+  p.ent = c.take<int32_t>(B * cap);
+  p.jc = c.take<int32_t>(B * cap);
+  p.cand = c.take<int2>(B * maxc);
+  p.pcnt = c.take<int32_t>(B * maxc);
+  p.sel = c.take<int32_t>(B * V);
+  p.lcp = c.take<int32_t>(B * V);
+  p.tiles = (int)tiles;
+  p.H = H;
+  if (w != nullptr) { *w = ws; *P = p; }
+  return c.words;
 }
 
 int32_t s4_check(int64_t n_src, int64_t n_tgt, int64_t n_q, double overlap, double delta, double angle_tol,
@@ -820,7 +812,7 @@ int32_t dgr_super4pcs(const float* src, int64_t n_src, const float* tgt, int64_t
   P.seed = seed;
   P.log = base_log;
 
-  int launches = dgr_goicp_normalise_dt(src, n_src, tgt, n_tgt, dt_size, dt_expand, w.stat, w.xn, w.y32, w.dt, st);
+  int launches = dgr_normalise_dt(src, n_src, tgt, n_tgt, dt_size, dt_expand, w.stat, w.xn, w.y32, w.dt, st);
   s4_init_kernel<<<1, 1024, 0, st>>>(P, w.stat, w.y32, n_tgt, max_bases);
   ++launches;
   DGR_LAUNCH_CHECK();
