@@ -16,6 +16,7 @@ LIB_PATH = os.path.join(_HERE, 'libdgr_b200.so')
 
 MAX_COLS = 8
 TILE_ROWS = 128
+KEY_MARGIN = 32     # spare cells around the bounding box: covers 7^3 kernels and stride-8 flooring
 
 
 class KeySpec(C.Structure):
@@ -37,7 +38,7 @@ SIGNATURES = {
     'dgr_coords_minmax': [_p, _i64, _i32, _p, _p],
     'dgr_keyspec_build': [_p, _i32, _i32, _p, _p],
     'dgr_hash_clear': [_p, _p, _i64, _p],
-    'dgr_unique_first': [_p, _i64, _i32, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _p, _p],
+    'dgr_unique_first': [_p, _i64, _i32, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _p],
     'dgr_scan_ws_elems': [_i64],
     'dgr_hash_find': [_p, _i64, _i32, _p, _p, _p, _i64, _p, _p],
     'dgr_gather_rows_i32': [_p, _p, _i64, _i32, _p, _p],
@@ -81,7 +82,6 @@ SIGNATURES = {
     'dgr_spconv_table_fwd_strided': [_p, _i32, _p, _i32, _p, _i32, _i64, _i64, _p, _p, _p, _p],
     'dgr_compact_voxel_pair': [_p, _p, _p, _i64, _i64, _p, _i32, _p, _i32, _p, _p, _p, _p],
     'dgr_table_build_unique': [_p, _i64, _p, _i32, _p, _p, _p, _i64, _p],
-    'dgr_coarse_scan_elems': [_i64],
     'dgr_coarse_maps': [_p, _i64, _p, _i32, _p, _i32, _p, _p, _p, _i64, _p, _p, _p, _p, _p],
     'dgr_bloom2_build': [_p, _i64, _p, _i64, _p],
     'dgr_bloom2_words': [_i64],
@@ -113,7 +113,7 @@ SIGNATURES = {
     'dgr_pair_safeguard': [_p, _f64, _i64, C.c_uint64, _i32, _p],
     'dgr_pair_tap': [_p, _i32, _p, _p, _p],
 }
-_RESTYPES = {'dgr_coarse_scan_elems': _i64, 'dgr_kmap_mask_words': _i64, 'dgr_kmap_cnt_elems': _i64, 'dgr_ctx_stream': C.c_void_p,
+_RESTYPES = {'dgr_kmap_mask_words': _i64, 'dgr_kmap_cnt_elems': _i64, 'dgr_ctx_stream': C.c_void_p,
              'dgr_ctx_profile_read': _i64, 'dgr_last_error': C.c_char_p, 'dgr_knn_tc_ws_elems': _i64, 'dgr_launch_count': _i64, 'dgr_spconv_tc_supported': _i32, 'dgr_scan_ws_elems': _i64, 'dgr_bloom2_words': _i64}
 
 _lib = None
@@ -282,7 +282,7 @@ def coords_minmax(coords):
   return minmax
 
 
-def keyspec_build(minmax, ncols, margin=32):
+def keyspec_build(minmax, ncols, margin=KEY_MARGIN):
   spec = torch.empty(KEYSPEC_INTS, dtype=torch.int32, device=minmax.device)
   call('dgr_keyspec_build', ptr(minmax), ncols, margin, ptr(spec), stream())
   return spec
@@ -299,10 +299,9 @@ def unique_first(coords, spec):
   inverse = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
   cnt = torch.zeros(2, dtype=torch.int32, device=dev)
   slot = scratch('uf_slot', max(n, 1), torch.int32, dev)
-  rank = scratch('uf_rank', max(n, 1), torch.int32, dev)
   scan = scratch('uf_scan', lib().dgr_scan_ws_elems(n), torch.int32, dev)
   call('dgr_unique_first', ptr(coords), n, ncols, ptr(spec), ptr(table.keys), ptr(table.vals), table.cap,
-       ptr(sel), ptr(inverse), ptr(cnt), ptr(slot), ptr(rank), ptr(scan), stream())
+       ptr(sel), ptr(inverse), ptr(cnt), ptr(slot), ptr(scan), stream())
   return table, sel, inverse, cnt
 
 
@@ -314,6 +313,17 @@ def read_count(cnt):
   if overflow:
     raise DgrError('coordinate extent does not fit a 63-bit packed key')
   return n
+
+
+def voxelise(xyz, voxel, batch=0):
+  """The first point of every voxel of xyz CUDA float64/float32 [n, 3]: floor(xyz / voxel) in the input dtype,
+  kept rows ascending, one host read.  -> (raw coords int32 [n, 4], spec, table (voxel key -> index into sel),
+  sel int32 [m], inverse int32 [n], m); raises on key overflow."""
+  raw, minmax = quantize_points(xyz, voxel, batch)
+  spec = keyspec_build(minmax, 4)
+  table, sel, inverse, cnt = unique_first(raw, spec)
+  n = read_count(cnt)
+  return raw, spec, table, sel[:n], inverse, n
 
 
 def hash_find(coords, spec, table):
@@ -343,7 +353,7 @@ def coarse_maps(fine, spec, strides):
   coords = torch.empty(L, nmx, ncols, dtype=torch.int32, device=dev)
   n_out = torch.empty(L, dtype=torch.int32, device=dev)
   slot = scratch('cm_slot', L * nmx, torch.int32, dev)
-  scan = scratch('cm_scan', L * lib().dgr_coarse_scan_elems(nmx), torch.int32, dev)
+  scan = scratch('cm_scan', L * lib().dgr_scan_ws_elems(nmx), torch.int32, dev)
   call('dgr_coarse_maps', ptr(fine), n, None, ncols, ptr(spec), L, (C.c_int32 * L)(*strides), ptr(keys), ptr(vals),
        cap, ptr(coords), ptr(n_out), ptr(slot), ptr(scan), stream())
   return coords, [HashTable.wrap(keys[l], vals[l], cap) for l in range(L)], n_out

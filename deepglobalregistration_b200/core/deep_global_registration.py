@@ -16,7 +16,7 @@ import threading
 import time
 
 from .. import _abi, native, shims
-from ..me.coords import CoordinateManager, KEY_MARGIN
+from ..me.coords import CoordinateManager
 from ..model import load_model
 from ..util.timer import Timer
 
@@ -130,11 +130,7 @@ class DeepGlobalRegistration:
         dxyz = dxyz.double()
     else:
       dxyz = self._upload(xyz, _slot)
-    raw_coords, minmax = _abi.quantize_points(dxyz, self.voxel_size, batch=_batch)
-    spec = _abi.keyspec_build(minmax, 4, KEY_MARGIN)
-    table, sel, _, cnt = _abi.unique_first(raw_coords, spec)
-    npts = _abi.read_count(cnt)
-    sel = sel[:npts]
+    raw_coords, spec, table, sel, _, npts = _abi.voxelise(dxyz, self.voxel_size, batch=_batch)
     coords = _abi.gather_rows_i32(raw_coords, sel, npts)
     xyz_sel = dxyz[sel.long()].float()
     # the dedup table already maps voxel key -> row of `coords`: hand it to SparseTensor

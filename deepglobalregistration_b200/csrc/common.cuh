@@ -64,6 +64,11 @@ static inline unsigned dgr_blocks(int64_t n, int per_block) {
 // ---------------------------------------------------------------------------------------
 #define DGR_EMPTY_KEY 0xFFFFFFFFFFFFFFFFull
 
+// Row count of a kernel that takes (n_max, n_dev): the device count when given, else the host bound
+__device__ __forceinline__ int dgr_dev_count(const int32_t* n_dev, int64_t n_max) {
+  return n_dev != nullptr ? *n_dev : (int)n_max;
+}
+
 __device__ __forceinline__ uint64_t dgr_pack_key(const int32_t* __restrict__ row,
                                                  const dgr_keyspec_t& s) {
   uint64_t k = 0;

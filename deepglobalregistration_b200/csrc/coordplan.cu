@@ -1,5 +1,6 @@
 // Coordinate planning with DEVICE-SIDE row counts: the integer work of one network forward
-// (coarse coordinate maps, kernel maps) enqueued without a single host round trip.
+// (coarse coordinate maps, kernel maps) enqueued without a single host round trip.  The coarse
+// maps and the table of the input rows come from the first-occurrence pass in coords.cu.
 //
 // Every kernel takes (n_max, n_dev): a host-side upper bound that sizes buffers and grids,
 // and a device pointer to the actual count that the kernels read (NULL: n_max is the count,
@@ -20,40 +21,13 @@
 // Replaces the MinkowskiEngine coordinate manager / kernel-map builder behind
 // model/residual_block.py:31-80 and model/resunet.py:598-649 (reference call sites); the pair
 // list semantics are those frozen in oracle/sparse_ops.py.
-#include <limits.h>
-
 #include "common.cuh"
 
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kScanElems = 2048;      // elements per block in the flag scans of the coarse maps (256 threads x 8)
 constexpr int kCntWords = 256;        // mask words per counted block of a kernel map (one fill block, one word per thread)
 constexpr int kProbeThreads = 512;    // 16 warps = 512 output rows per probe block
-constexpr int kMaxLevels = 4;
-
-__device__ __forceinline__ int dev_count(const int32_t* n_dev, int64_t n_max) {
-  return n_dev != nullptr ? *n_dev : (int)n_max;
-}
-
-__device__ __forceinline__ int floor_to(int v, int stride) {
-  int q = v / stride;
-  if ((v % stride != 0) && (v < 0)) --q;
-  return q * stride;
-}
-
-// key of a row floored to `stride` on the spatial columns (column 0 = batch is kept)
-__device__ __forceinline__ uint64_t pack_key_strided(const int32_t* __restrict__ row, const dgr_keyspec_t& s,
-                                                     int stride) {
-  uint64_t k = 0;
-#pragma unroll
-  for (int i = 0; i < DGR_MAX_COLS; ++i)
-    if (i < s.ncols) {
-      const int v = (i == 0 || stride == 1) ? row[i] : floor_to(row[i], stride);
-      k += (uint64_t)(uint32_t)(v - s.lo[i]) << s.shift[i];
-    }
-  return k;
-}
 
 // ---------------------------------------------------------------------------------------
 // voxel compaction of a scan pair (device count of kept points)
@@ -88,121 +62,6 @@ __global__ void compact_voxels_kernel(const int32_t* __restrict__ raw, const int
       x = (float)xyz1[3 * q]; y = (float)xyz1[3 * q + 1]; z = (float)xyz1[3 * q + 2];
     }
     xyz[3 * i] = x; xyz[3 * i + 1] = y; xyz[3 * i + 2] = z;
-  }
-}
-
-// ---------------------------------------------------------------------------------------
-// hash table of rows known to be distinct (value = row index)
-// ---------------------------------------------------------------------------------------
-__global__ void table_clear_kernel(uint64_t* keys, int32_t* vals, int64_t total) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < total) {
-    keys[i] = DGR_EMPTY_KEY;
-    vals[i] = INT_MAX;
-  }
-}
-
-__global__ void insert_unique_kernel(const int32_t* __restrict__ coords, const int32_t* __restrict__ n_dev,
-                                     int64_t n_max, int ncols, const dgr_keyspec_t* __restrict__ spec_p,
-                                     uint64_t* keys, int32_t* vals, uint64_t mask) {
-  const int n = dev_count(n_dev, n_max);
-  int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= n) return;
-  const dgr_keyspec_t s = *spec_p;
-  const uint32_t sl = dgr_hash_insert(keys, mask, dgr_pack_key(coords + r * ncols, s));
-  atomicMin(vals + sl, (int32_t)r);      // distinct rows: one writer; min keeps duplicates deterministic
-}
-
-// ---------------------------------------------------------------------------------------
-// coarse (strided) coordinate maps of up to kMaxLevels strides in one launch per phase
-// ---------------------------------------------------------------------------------------
-struct CoarseArgs {
-  int n_levels;
-  int stride[kMaxLevels];
-  uint64_t* keys[kMaxLevels];
-  int32_t* vals[kMaxLevels];
-  int32_t* slot[kMaxLevels];
-  int32_t* scan[kMaxLevels];
-  int32_t* coords[kMaxLevels];
-  int32_t* n_out[kMaxLevels];
-};
-
-__global__ void coarse_insert_kernel(const int32_t* __restrict__ fine, const int32_t* __restrict__ n_dev,
-                                     int64_t n_max, int ncols, const dgr_keyspec_t* __restrict__ spec_p,
-                                     uint64_t mask, CoarseArgs a) {
-  const int n = dev_count(n_dev, n_max);
-  const int l = blockIdx.y;
-  int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= n) return;
-  const dgr_keyspec_t s = *spec_p;
-  const uint32_t sl = dgr_hash_insert(a.keys[l], mask, pack_key_strided(fine + r * ncols, s, a.stride[l]));
-  atomicMin(a.vals[l] + sl, (int32_t)r);
-  a.slot[l][r] = (int32_t)sl;
-}
-
-// winners (first fine row of every coarse cell) are marked by keeping slot >= 0, losers get ~slot;
-// per-2048-row block winner counts go to scan[l][block]
-__global__ void coarse_flag_kernel(const int32_t* __restrict__ n_dev, int64_t n_max, CoarseArgs a) {
-  const int n = dev_count(n_dev, n_max);
-  const int l = blockIdx.y;
-  const int64_t start = (int64_t)blockIdx.x * kScanElems;
-  int c = 0;
-#pragma unroll
-  for (int e = 0; e < kScanElems / kThreads; ++e) {
-    const int64_t r = start + e * kThreads + threadIdx.x;
-    if (r < n) {
-      const int sl = a.slot[l][r];
-      const bool win = a.vals[l][sl] == (int32_t)r;
-      if (!win) a.slot[l][r] = ~sl;
-      c += win;
-    }
-  }
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) c += __shfl_xor_sync(0xffffffffu, c, d);
-  __shared__ int ws[kThreads / 32];
-  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int t = 0;
-    for (int w = 0; w < kThreads / 32; ++w) t += ws[w];
-    a.scan[l][blockIdx.x] = t;
-  }
-}
-
-__global__ void coarse_scan_kernel(const int32_t* __restrict__ n_dev, int64_t n_max, CoarseArgs a) {
-  const int n = dev_count(n_dev, n_max);
-  const int l = blockIdx.x;
-  const int64_t nb = (n + kScanElems - 1) / kScanElems;
-  const int total = dgr_block_scan_inplace(a.scan[l], nb);
-  if (threadIdx.x == 0) a.n_out[l][0] = total;
-}
-
-// rank the winners in row order: coarse row `pos` = floor(fine row r); table value <- pos
-__global__ void coarse_scatter_kernel(const int32_t* __restrict__ fine, const int32_t* __restrict__ n_dev,
-                                      int64_t n_max, int ncols, CoarseArgs a) {
-  const int n = dev_count(n_dev, n_max);
-  const int l = blockIdx.y;
-  const int64_t start = (int64_t)blockIdx.x * kScanElems + (int64_t)threadIdx.x * 8;
-  if ((int64_t)blockIdx.x * kScanElems >= n) return;      // uniform per block
-  int sl[8], c = 0;
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const int64_t r = start + e;
-    sl[e] = (r < n) ? a.slot[l][r] : -1;
-    c += (sl[e] >= 0);
-  }
-  int pos = a.scan[l][blockIdx.x] + dgr_block_exclusive_scan<256>(c, nullptr);
-  const int stride = a.stride[l];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    if (sl[e] >= 0) {
-      const int64_t r = start + e;
-      int32_t* dst = a.coords[l] + (int64_t)pos * ncols;
-      dst[0] = fine[r * ncols];
-      for (int col = 1; col < ncols; ++col) dst[col] = floor_to(fine[r * ncols + col], stride);
-      a.vals[l][sl[e]] = pos;
-      ++pos;
-    }
   }
 }
 
@@ -258,7 +117,7 @@ kmap_probe_kernel(const int32_t* __restrict__ out_coords, const int32_t* __restr
   uint32_t* mtile = reinterpret_cast<uint32_t*>(smem_raw + (size_t)k_per_block * 8);       // [kWarps][k_per_block]
   uint16_t* queue = reinterpret_cast<uint16_t*>(mtile + (size_t)kWarps * k_per_block);     // [kWarps][64]
   uint32_t* bloom_s = reinterpret_cast<uint32_t*>(queue + kWarps * 64);                    // [n_bloom_words]
-  const int n_out = dev_count(n_out_dev, n_out_max);
+  const int n_out = dgr_dev_count(n_out_dev, n_out_max);
   const int k0 = blockIdx.y * k_per_block;
   const int kn = min(k_per_block, K - k0);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -505,57 +364,6 @@ int32_t dgr_compact_voxel_pair(const int32_t* raw_coords, const int32_t* sel, co
   else DGR_CV(float, float);
 #undef DGR_CV
   dgr_note_launches(1);
-  DGR_LAUNCH_CHECK();
-  return DGR_OK;
-}
-
-int32_t dgr_table_build_unique(const int32_t* coords, int64_t n_max, const int32_t* n_dev, int32_t ncols,
-                               const dgr_keyspec_t* spec, uint64_t* keys, int32_t* vals, int64_t cap,
-                               void* stream) {
-  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
-  DGR_ARG_CHECK(cap >= 2 * n_max, "capacity must be at least 2 n_max");
-  cudaStream_t st = (cudaStream_t)stream;
-  table_clear_kernel<<<dgr_blocks(cap, kThreads), kThreads, 0, st>>>(keys, vals, cap);
-  if (n_max > 0)
-    insert_unique_kernel<<<dgr_blocks(n_max, kThreads), kThreads, 0, st>>>(coords, n_dev, n_max, ncols, spec, keys,
-                                                                         vals, (uint64_t)cap - 1);
-  dgr_note_launches(n_max > 0 ? 2 : 1);
-  DGR_LAUNCH_CHECK();
-  return DGR_OK;
-}
-
-int64_t dgr_coarse_scan_elems(int64_t n_max) { return (n_max + kScanElems - 1) / kScanElems + 2; }
-
-int32_t dgr_coarse_maps(const int32_t* fine, int64_t n_max, const int32_t* n_dev, int32_t ncols,
-                        const dgr_keyspec_t* spec, int32_t n_levels, const int32_t* strides, uint64_t* keys,
-                        int32_t* vals, int64_t cap, int32_t* coords_out, int32_t* n_out, int32_t* slot_ws,
-                        int32_t* scan_ws, void* stream) {
-  DGR_ARG_CHECK(n_levels >= 1 && n_levels <= kMaxLevels, "1..4 levels per call");
-  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0 && cap >= 2 * n_max, "capacity: power of two >= 2 n_max");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t nmx = n_max > 0 ? n_max : 1;
-  const int64_t scan_elems = dgr_coarse_scan_elems(nmx);
-  CoarseArgs a;
-  a.n_levels = n_levels;
-  for (int l = 0; l < kMaxLevels; ++l) {
-    const int k = l < n_levels ? l : 0;
-    DGR_ARG_CHECK(strides[k] >= 1, "stride must be positive");
-    a.stride[l] = strides[k];
-    a.keys[l] = keys + (int64_t)k * cap;
-    a.vals[l] = vals + (int64_t)k * cap;
-    a.slot[l] = slot_ws + (int64_t)k * nmx;
-    a.scan[l] = scan_ws + (int64_t)k * scan_elems;
-    a.coords[l] = coords_out + (int64_t)k * nmx * ncols;
-    a.n_out[l] = n_out + k;
-  }
-  table_clear_kernel<<<dgr_blocks(cap * n_levels, kThreads), kThreads, 0, st>>>(keys, vals, cap * n_levels);
-  const unsigned nb = dgr_blocks(nmx, kScanElems);
-  coarse_insert_kernel<<<dim3(dgr_blocks(nmx, kThreads), n_levels), kThreads, 0, st>>>(fine, n_dev, n_max, ncols, spec,
-                                                                                      (uint64_t)cap - 1, a);
-  coarse_flag_kernel<<<dim3(nb, n_levels), kThreads, 0, st>>>(n_dev, n_max, a);
-  coarse_scan_kernel<<<n_levels, 1024, 0, st>>>(n_dev, n_max, a);
-  coarse_scatter_kernel<<<dim3(nb, n_levels), kThreads, 0, st>>>(fine, n_dev, n_max, ncols, a);
-  dgr_note_launches(5);
   DGR_LAUNCH_CHECK();
   return DGR_OK;
 }

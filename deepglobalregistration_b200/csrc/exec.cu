@@ -41,7 +41,7 @@ constexpr int kTileRows = 128;
 constexpr int kMetaInts = 256;
 constexpr int kMetaNetBase = 8;       // meta[0..8): pair counts (N, N0, N1, key overflow)
 constexpr int kMetaPerMap = 5;
-constexpr int kKeyMargin = 32;        // spare cells around the bounding box (7^3 kernels, stride-8 flooring)
+constexpr int kKeyMargin = 32;        // spare cells around the bounding box (7^3 kernels, stride-8 flooring); _abi.KEY_MARGIN
 
 bool tc_f16_enabled();
 int tc_f16_min_cout();
@@ -357,7 +357,7 @@ int32_t plan_begin(dgr_ctx* c, const dgr_net* net, Plan& p) {
   DGR_TRY(aalloc(c, 3 * cap, &vals));
   DGR_TRY(aalloc(c, 3 * nmx * ncols, &coords));
   DGR_TRY(aalloc(c, 3 * nmx, &slot));
-  DGR_TRY(aalloc(c, 3 * dgr_coarse_scan_elems(nmx), &scan));
+  DGR_TRY(aalloc(c, 3 * dgr_scan_ws_elems(nmx), &scan));
   const int32_t strides[3] = {2, 4, 8};
   int32_t* n_out_dev = c->meta_dev + p.meta_base + 1;
   DGR_TRY(dgr_coarse_maps(l0.coords, n_max, l0.n_dev, ncols, p.spec, 3, strides, keys, vals, cap, coords, n_out_dev,
@@ -920,7 +920,7 @@ int32_t dgr_pair_register(dgr_ctx_t* c, dgr_net_t* fcgf, dgr_net_t* inlier, cons
     d0 = a;
     d1 = b;
   }
-  int32_t *raw, *minmax, *mm_scratch, *sel, *inverse, *n_unique, *slot_ws, *rank_ws, *scan_ws, *coords;
+  int32_t *raw, *minmax, *mm_scratch, *sel, *inverse, *n_unique, *slot_ws, *scan_ws, *coords;
   dgr_keyspec_t* spec;
   float* xyz;
   DGR_TRY(aalloc(c, n_raw * 4, &raw));
@@ -940,10 +940,9 @@ int32_t dgr_pair_register(dgr_ctx_t* c, dgr_net_t* fcgf, dgr_net_t* inlier, cons
   DGR_TRY(aalloc(c, n_raw, &inverse));
   DGR_TRY(aalloc(c, 2, &n_unique));
   DGR_TRY(aalloc(c, n_raw, &slot_ws));
-  DGR_TRY(aalloc(c, n_raw, &rank_ws));
   DGR_TRY(aalloc(c, dgr_scan_ws_elems(n_raw), &scan_ws));
   DGR_TRY(dgr_hash_clear(keys, vals, cap, st));
-  DGR_TRY(dgr_unique_first(raw, n_raw, 4, spec, keys, vals, cap, sel, inverse, n_unique, slot_ws, rank_ws, scan_ws, st));
+  DGR_TRY(dgr_unique_first(raw, n_raw, 4, spec, keys, vals, cap, sel, inverse, n_unique, slot_ws, scan_ws, st));
   DGR_TRY(aalloc(c, n_raw * 4, &coords));
   DGR_TRY(aalloc(c, n_raw * 3, &xyz));
   DGR_TRY(dgr_compact_voxel_pair(raw, sel, n_unique, n_raw0, n_raw1, d0, is_f64_0, d1, is_f64_1, coords, xyz,

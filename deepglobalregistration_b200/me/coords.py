@@ -4,8 +4,7 @@ import numpy as np
 import torch
 
 from .. import _abi
-
-KEY_MARGIN = 32     # spare cells around the bounding box: covers 7^3 kernels and stride-8 flooring
+from .._abi import KEY_MARGIN
 
 
 class CoordinateMapKey:

@@ -26,11 +26,8 @@ def sparse_quantize(coordinates, features=None, labels=None, ignore_label=-100, 
     c = c.double()
   if c.dtype not in (torch.float32, torch.float64):
     c = c.float()
-  coords, minmax = _abi.quantize_points(c.contiguous(), 1.0)
-  spec = _abi.keyspec_build(minmax, 4, 32)
-  _, sel, inverse, cnt = _abi.unique_first(coords, spec)
-  n = _abi.read_count(cnt)
-  index = sel[:n].long()
+  coords, _, _, sel, inverse, _ = _abi.voxelise(c.contiguous(), 1.0)
+  index = sel.long()
   uniq = coords[index][:, 1:].contiguous()
   conv = (lambda t: t.cpu().numpy()) if is_np else (lambda t: t)
   if return_maps_only:

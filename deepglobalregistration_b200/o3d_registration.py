@@ -159,13 +159,10 @@ def _target_hash(tgt64, max_dist):
   """Voxel hash of the target with at most one point per cell (what the ICP and normal kernels search): cell =
   max_dist / 2 as in DGR (voxelised clouds, radius 2 voxels); a cloud with several points per cell gets finer
   cells up to the kernels' reach of 4."""
-  from .me.coords import KEY_MARGIN
   for div in (2.0, 3.0, 4.0):
     cell = max_dist / div
-    raw, minmax = _abi.quantize_points(tgt64, cell)
-    spec = _abi.keyspec_build(minmax, 4, KEY_MARGIN)
-    table, _, _, cnt = _abi.unique_first(raw, spec)
-    if _abi.read_count(cnt) == tgt64.shape[0]:
+    _, spec, table, _, _, n = _abi.voxelise(tgt64, cell)
+    if n == tgt64.shape[0]:
       return cell, spec, table
   raise NotImplementedError('target has several points within max_correspondence_distance / 4 of each other: '
                             'voxel-downsample it first (DGR always passes voxelised clouds)')

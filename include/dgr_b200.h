@@ -84,12 +84,12 @@ int32_t dgr_hash_clear(uint64_t* keys, int32_t* vals, int64_t cap, void* stream)
  *   sel[0..m)      ascending first-occurrence rows,
  *   inverse[n]     row -> index into sel of its representative,
  *   n_unique[2]    (m, spec->overflow) device int32 - one host read for both,
- * and leaves the table mapping key -> index into sel.  slot_ws[n], rank_ws[n] and
- * scan_ws[dgr_scan_ws_elems(n)] are int32 workspaces. */
+ * and leaves the table (cleared beforehand) mapping key -> index into sel.  slot_ws[n] and
+ * scan_ws[dgr_scan_ws_elems(n)] are int32 workspaces.  The stride-1 case of the
+ * first-occurrence pass behind dgr_coarse_maps (csrc/coords.cu). */
 int32_t dgr_unique_first(const int32_t* coords, int64_t n, int32_t ncols, const dgr_keyspec_t* spec,
                          uint64_t* keys, int32_t* vals, int64_t cap, int32_t* sel, int32_t* inverse,
-                         int32_t* n_unique, int32_t* slot_ws, int32_t* rank_ws, int32_t* scan_ws,
-                         void* stream);
+                         int32_t* n_unique, int32_t* slot_ws, int32_t* scan_ws, void* stream);
 int64_t dgr_scan_ws_elems(int64_t n);
 /* rows[i] -> vals of matching key, or -1. */
 int32_t dgr_hash_find(const int32_t* coords, int64_t n, int32_t ncols, const dgr_keyspec_t* spec,
@@ -419,7 +419,8 @@ int32_t dgr_spconv_tc_f16_fwd(const float* in_feat, int32_t cin, const void* wei
 int32_t dgr_spconv_ones_bits_fwd(const float* weight, int32_t cout, const uint32_t* bits, int64_t mask_words, int32_t K,
                                  int64_t n_out, const float* scale, const float* shift, float* out, void* stream);
 
-/* ---- coordinate planning without host round trips (csrc/coordplan.cu) --------------------
+/* ---- coordinate planning without host round trips (csrc/coordplan.cu; the table and coarse maps
+ *      in csrc/coords.cu, on the first-occurrence pass of dgr_unique_first) --------------------
  * Convention: `n_max` is a host-side upper bound of a row count (sizes buffers and grids), `n_dev` a
  * device int32* holding the actual count (NULL = n_max).  Replaces the MinkowskiEngine coordinate
  * manager behind ME.SparseTensor / MinkowskiConvolution (core/deep_global_registration.py:167,214,
@@ -436,8 +437,7 @@ int32_t dgr_table_build_unique(const int32_t* coords, int64_t n_max, const int32
 /* Coarse maps of `n_levels` (<= 4) tensor strides in one call, all derived from the same fine rows:
  * level l: coords_out[l][n_max][ncols] (first n_out[l] rows valid, ordered by first occurrence among the
  * fine rows), table keys[l][cap] / vals[l][cap] (key -> coarse row), n_out[l] device counts.
- * slot_ws: n_levels * n_max ints; scan_ws: n_levels * dgr_coarse_scan_elems(n_max) ints. */
-int64_t dgr_coarse_scan_elems(int64_t n_max);
+ * slot_ws: n_levels * n_max ints; scan_ws: n_levels * dgr_scan_ws_elems(n_max) ints. */
 int32_t dgr_coarse_maps(const int32_t* fine, int64_t n_max, const int32_t* n_dev, int32_t ncols,
                         const dgr_keyspec_t* spec, int32_t n_levels, const int32_t* strides, uint64_t* keys,
                         int32_t* vals, int64_t cap, int32_t* coords_out, int32_t* n_out, int32_t* slot_ws,

@@ -21,12 +21,7 @@ def _cloud(seed, n, scale=3.0, dtype=np.float64):
 
 
 def _quantize_gpu(abi, xyz, voxel):
-  d = torch.from_numpy(xyz).cuda()
-  coords, minmax = abi.quantize_points(d, voxel)
-  spec = abi.keyspec_build(minmax, 4, 32)
-  table, sel, inv, cnt = abi.unique_first(coords, spec)
-  n = abi.read_count(cnt)
-  return coords, spec, table, sel[:n], inv, n
+  return abi.voxelise(torch.from_numpy(xyz).cuda(), voxel)
 
 
 @pytest.mark.parametrize('dtype', [np.float64, np.float32])
@@ -166,7 +161,5 @@ def test_duplicate_coordinates_rejected(abi):
 
 def test_empty_inputs(abi):
   d = torch.zeros(0, 3, dtype=torch.float64, device='cuda')
-  coords, minmax = abi.quantize_points(d, 0.05)
-  spec = abi.keyspec_build(minmax, 4, 32)
-  _, sel, _, cnt = abi.unique_first(coords, spec)
-  assert abi.read_count(cnt) == 0
+  _, _, _, sel, _, n = abi.voxelise(d, 0.05)
+  assert n == 0 and sel.numel() == 0

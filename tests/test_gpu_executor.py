@@ -46,7 +46,7 @@ def _padded(coords, extra, seed=1):
 
 
 @pytest.mark.parametrize('D,n,ext', [(3, 6000, 14), (6, 5000, 3), (3, 40, 3)])
-def test_coarse_maps_bit_exact(abi, D, n, ext):
+def test_coarse_maps_device_count_bit_exact(abi, D, n, ext):
   coords = _cloud(D, n, ext, seed=D + n, batch2=True)
   nreal = len(coords)
   ct = torch.from_numpy(coords).cuda().contiguous()
@@ -61,7 +61,7 @@ def test_coarse_maps_bit_exact(abi, D, n, ext):
   out = torch.full((L, n_max, ncols), -77, dtype=torch.int32, device='cuda')
   n_out = torch.zeros(L, dtype=torch.int32, device='cuda')
   slot = torch.empty(L * n_max, dtype=torch.int32, device='cuda')
-  scan = torch.empty(L * abi.lib().dgr_coarse_scan_elems(n_max), dtype=torch.int32, device='cuda')
+  scan = torch.empty(L * abi.lib().dgr_scan_ws_elems(n_max), dtype=torch.int32, device='cuda')
   strides = (C.c_int32 * 3)(2, 4, 8)
   abi.call('dgr_coarse_maps', abi.ptr(pad), n_max, abi.ptr(n_dev), ncols, abi.ptr(spec), L, strides, abi.ptr(keys),
            abi.ptr(vals), cap, abi.ptr(out), abi.ptr(n_out), abi.ptr(slot), abi.ptr(scan), abi.stream())

@@ -34,11 +34,8 @@ def voxelise(x, cell):
 def cloud_hash(P, cell):
   """(spec, table) of the cloud's own voxel hash at `cell`, rows = rows of P."""
   from deepglobalregistration_b200 import _abi
-  from deepglobalregistration_b200.me.coords import KEY_MARGIN
-  raw, minmax = _abi.quantize_points(_t(P, torch.float64), cell)
-  spec = _abi.keyspec_build(minmax, 4, KEY_MARGIN)
-  table, _, _, cnt = _abi.unique_first(raw, spec)
-  assert _abi.read_count(cnt) == len(P)
+  _, spec, table, _, _, n = _abi.voxelise(_t(P, torch.float64), cell)
+  assert n == len(P)
   return spec, table
 
 

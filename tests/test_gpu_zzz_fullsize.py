@@ -25,11 +25,8 @@ def cloud(abi):
   from deepglobalregistration_b200.me.coords import CoordinateManager
   xyz = syn.room_scan(0, 250_000)
   d = torch.from_numpy(xyz).cuda()
-  raw, minmax = abi.quantize_points(d, 0.05)
-  spec = abi.keyspec_build(minmax, 4, 32)
-  table, sel, inv, cnt = abi.unique_first(raw, spec)
-  n = abi.read_count(cnt)
-  coords = abi.gather_rows_i32(raw, sel[:n], n)
+  raw, _, _, sel, _, n = abi.voxelise(d, 0.05)
+  coords = abi.gather_rows_i32(raw, sel, n)
   assert 45_000 <= n <= 55_000, n                   # SURVEY 8(d) config 2
   # voxelisation invariants at full size: ascending first occurrences, one row per voxel
   s = sel[:n].cpu().numpy()
