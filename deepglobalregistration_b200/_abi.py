@@ -57,6 +57,8 @@ SIGNATURES = {
     'dgr_inlier_coords': [_p, _p, _p, _i64, _p, _p],
     'dgr_sigmoid_clip_sum': [_p, _i64, _f32, _p, _p, _p],
     'dgr_estimate_normals': [_p, _i64, _p, _p, _p, _i64, _i32, _f64, _f64, _i32, _p, _p, _p, _p],
+    'dgr_fpfh_ws_elems': [_i64, _i32, _p],
+    'dgr_compute_fpfh': [_p, _p, _i64, _p, _p, _p, _i64, _i32, _f64, _f64, _i32, _i32, _p, _p, _p, _p],
     'dgr_icp_ws_elems': [_i64, _p],
     'dgr_icp': [_p, _i64, _p, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _p, _i32, _f64, _f64, _p, _p, _p],
     'dgr_ransac_ws_elems': [_i64, _i64, _p],
@@ -641,6 +643,34 @@ def estimate_normals(xyz, manager_or_table, cell, radius, max_nn, prev=None, ret
   call('dgr_estimate_normals', ptr(xyz), n, ptr(spec), ptr(table.keys), ptr(table.vals), table.cap, int(batch),
        float(cell), float(radius), int(max_nn), ptr(prev), ptr(normals), ptr(counts), stream())
   return (normals, counts) if return_counts else normals
+
+
+FPFH_MAX_NN = 128      # dgr_compute_fpfh's bound on the neighbours per point (the point itself included)
+FPFH_DIM = 33
+
+
+def compute_fpfh(xyz, normals, manager_or_table, cell, radius, max_nn, batch=0, ld=FPFH_DIM, return_counts=False):
+  """FPFH features (open3d 0.10's compute_fpfh_feature) of xyz (CUDA float32 [n, 3]) with normals (CUDA float32
+  [n, 3]) from the neighbours strictly within `radius`, at most `max_nn` (<= 128, the point itself included) by
+  (d^2, row), searched through the cloud's own voxel hash at `cell` (as estimate_normals; radius <= 6 cells).
+  -> float32 [n, ld] (ld >= 33; columns 33 .. ld - 1 are zero, so ld = 64 feeds the tensor-core kNN) (and the int32
+  [n] counts within the radius)."""
+  _chk(xyz, torch.float32, 'xyz')
+  if normals is None:
+    raise DgrError('compute_fpfh needs normals: estimate them first')
+  _chk(normals, torch.float32, 'normals')
+  if normals.shape != xyz.shape:
+    raise DgrError('normals must hold one normal per point')
+  spec, table = _hash_of(manager_or_table)
+  n = xyz.shape[0]
+  words = C.c_int64(0)
+  call('dgr_fpfh_ws_elems', n, int(max_nn), C.byref(words))
+  ws = scratch('fpfh', words.value, torch.int64, xyz.device)
+  out = torch.empty(max(n, 1), max(int(ld), 1), dtype=torch.float32, device=xyz.device)[:n]
+  counts = torch.empty(max(n, 1), dtype=torch.int32, device=xyz.device)[:n]
+  call('dgr_compute_fpfh', ptr(xyz), ptr(normals), n, ptr(spec), ptr(table.keys), ptr(table.vals), table.cap,
+       int(batch), float(cell), float(radius), int(max_nn), int(ld), ptr(ws), ptr(out), ptr(counts), stream())
+  return (out, counts) if return_counts else out
 
 
 def _icp(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter, rel_fitness, rel_rmse, batch):

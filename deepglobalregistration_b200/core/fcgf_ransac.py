@@ -11,7 +11,8 @@ core/deep_global_registration.py:29-47 asks of open3d 0.10) -> optionally point-
 stagewise path does.  The wrapped object's preprocessing, FCGF network, voxel size and ``use_icp`` are
 used as they are: no second checkpoint is loaded.
 
-``FCGFBaseline`` is that skeleton with the search step left to the subclass (core/fcgf_fgr.py uses it too).
+``FCGFBaseline`` is that skeleton with the search step left to the subclass (core/fcgf_fgr.py uses it too) and
+the descriptor in one overridable step, ``_features`` (core/fpfh_baseline.py swaps FCGF for FPFH there).
 """
 import numpy as np
 import torch
@@ -21,7 +22,7 @@ from ..util.timer import Timer
 
 
 class FCGFBaseline:
-  """Voxelise -> FCGF on both clouds in one pass -> ``_search`` (device result whose first 12 entries are the
+  """Voxelise -> ``_features`` (FCGF on both clouds in one pass) -> ``_search`` (device result whose first 12 entries are the
   [R | t] rows of the pose) -> optional ICP from that pose -> one readback."""
   branch = None      # last_branch after a call
   label = None       # name in the timing log line
@@ -40,6 +41,11 @@ class FCGFBaseline:
   def use_icp(self):
     return self.dgr.use_icp
 
+  def _features(self, p0, p1, c0, c1):
+    """-> per-point features (f0, f1) of the voxelised clouds p0 / p1 (coords c0 / c1 from preprocess): FCGF of both
+    in one pass."""
+    return self.dgr.fcgf_feature_extraction_pair(c0, c1)
+
   def _search(self, p0, p1, f0, f1, manager1):
     """-> device double result of the global search; manager1: cloud 1's coordinate manager (voxel hash)."""
     raise NotImplementedError
@@ -57,7 +63,7 @@ class FCGFBaseline:
     with torch.no_grad():
       p0, c0, _ = d.preprocess(xyz0, 0, _batch=0)
       p1, c1, _ = d.preprocess(xyz1, 1, _batch=1)
-      f0, f1 = d.fcgf_feature_extraction_pair(c0, c1)
+      f0, f1 = self._features(p0, p1, c0, c1)
       m = c1._dgr_manager
       res = self._search(p0, p1, f0.contiguous(), f1.contiguous(), m)
       parts = [res]

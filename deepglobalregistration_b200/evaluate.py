@@ -197,21 +197,22 @@ def main(argv=None):
   ap.add_argument('--success_rte_thresh', type=float, default=0.3, help='m (config.py:127; KITTI: 0.6)')
   ap.add_argument('--success_rre_thresh', type=float, default=15.0, help='deg (config.py:128; KITTI: 5)')
   ap.add_argument('--no_icp', action='store_true')
-  ap.add_argument('--method', choices=('dgr', 'fcgf_ransac', 'fcgf_fgr', 'icp_point_to_point', 'icp_point_to_plane',
-                                       'goicp', 'super4pcs', 'pointnetlk'),
+  ap.add_argument('--method', choices=('dgr', 'fcgf_ransac', 'fcgf_fgr', 'fpfh_ransac', 'fpfh_fgr', 'icp_point_to_point',
+                                       'icp_point_to_plane', 'goicp', 'super4pcs', 'pointnetlk'),
                   default='dgr',
                   help='dgr: DeepGlobalRegistration.register; fcgf_ransac: the FCGF + RANSAC baseline on the same '
                   'checkpoint (core/fcgf_ransac.py); fcgf_fgr: FCGF + Fast Global Registration with open3d\'s '
-                  'default options (core/fcgf_fgr.py); icp_point_to_point / icp_point_to_plane: ICP from the identity '
+                  'default options (core/fcgf_fgr.py); fpfh_ransac / fpfh_fgr: the same two searches on FPFH features '
+                  'instead of FCGF (core/fpfh_baseline.py); icp_point_to_point / icp_point_to_plane: ICP from the identity '
                   'on the checkpoint\'s voxelisation (core/icp_baseline.py); goicp: globally optimal Go-ICP on the same '
                   'voxelisation (core/goicp.py); super4pcs: 4-point congruent sets on the same voxelisation '
                   '(core/super4pcs.py); pointnetlk: PointNetLK on the same voxelisation with the network of '
                   '--pointnetlk_weights (core/pointnetlk.py)')
-  ap.add_argument('--ransac_max_iteration', type=int, default=80000, help='fcgf_ransac: hypotheses drawn at most')
+  ap.add_argument('--ransac_max_iteration', type=int, default=80000, help='fcgf_ransac / fpfh_ransac: hypotheses drawn at most')
   ap.add_argument('--ransac_max_validation', type=int, default=1000,
-                  help='fcgf_ransac: hypotheses scored (the ones that pass the checkers first)')
+                  help='fcgf_ransac / fpfh_ransac: hypotheses scored (the ones that pass the checkers first)')
   ap.add_argument('--ransac_edge_ratio', type=float, default=0.0,
-                  help='fcgf_ransac: edge-length checker similarity threshold (open3d uses 0.9); 0 = off')
+                  help='fcgf_ransac / fpfh_ransac: edge-length checker similarity threshold (open3d uses 0.9); 0 = off')
   ap.add_argument('--icp_max_correspondence_distance', type=float, default=None,
                   help='icp_*: correspondence radius in metres (default 2 voxels, at most 4)')
   ap.add_argument('--icp_max_iteration', type=int, default=30, help='icp_*: ICP updates at most')
@@ -245,14 +246,18 @@ def main(argv=None):
   dgr = DeepGlobalRegistration(cfg, device=torch.device('cuda', local))
   dgr.use_icp = not args.no_icp
   method = dgr
-  if args.method == 'fcgf_ransac':
+  if args.method in ('fcgf_ransac', 'fpfh_ransac'):
     from .core.fcgf_ransac import FCGFRansac
-    method = FCGFRansac(dgr)
+    from .core.fpfh_baseline import FPFHRansac
+    method = (FCGFRansac if args.method == 'fcgf_ransac' else FPFHRansac)(dgr)
     method.max_iteration, method.max_validation = args.ransac_max_iteration, args.ransac_max_validation
     method.edge_ratio = args.ransac_edge_ratio
   elif args.method == 'fcgf_fgr':
     from .core.fcgf_fgr import FCGFFastGlobal
     method = FCGFFastGlobal(dgr)
+  elif args.method == 'fpfh_fgr':
+    from .core.fpfh_baseline import FPFHFastGlobal
+    method = FPFHFastGlobal(dgr)
   elif args.method in ('icp_point_to_point', 'icp_point_to_plane'):
     from .core.icp_baseline import ICPBaseline
     method = ICPBaseline(dgr, args.method[len('icp_'):], args.icp_max_correspondence_distance, args.icp_max_iteration)
@@ -287,7 +292,8 @@ def main(argv=None):
     summary = summarize(result)
     print(json.dumps(dict(summary, world_size=world)))          # the summary first: a failing save loses nothing
     stem, name = {'dgr': ('dgr-b200', 'DGR'), 'fcgf_ransac': ('fcgf-ransac-b200', 'RANSAC'),
-                  'fcgf_fgr': ('fcgf-fgr-b200', 'FGR'), 'icp_point_to_point': ('icp-p2p-b200', 'ICP (Point-to-point)'),
+                  'fcgf_fgr': ('fcgf-fgr-b200', 'FGR'), 'fpfh_ransac': ('fpfh-ransac-b200', 'FPFH + RANSAC'),
+                  'fpfh_fgr': ('fpfh-fgr-b200', 'FPFH + FGR'), 'icp_point_to_point': ('icp-p2p-b200', 'ICP (Point-to-point)'),
                   'icp_point_to_plane': ('icp-p2plane-b200', 'ICP (Point-to-plane)'),
                   'goicp': ('goicp-b200', 'Go-ICP'), 'super4pcs': ('super4pcs-b200', 'Super4PCS'),
                   'pointnetlk': ('pointnetlk-b200', 'PointNetLK')}[args.method]

@@ -20,12 +20,17 @@ It also carries the calls open3d users make beyond DGR's own: point-to-plane ICP
 
   registration_fast_based_on_feature_matching(source, target, source_feature, target_feature, option)
       -> dgr_knn_top1 both ways + dgr_fgr_feature_matching: Fast Global Registration (mutual matches, tuple
-         test, graduated non-convexity) with FastGlobalRegistrationOption's fields and defaults.
+         test, graduated non-convexity) with FastGlobalRegistrationOption's fields and defaults;
+  compute_fpfh_feature(input, KDTreeSearchParamHybrid(radius, max_nn))
+      -> dgr_compute_fpfh: FPFH descriptors of a cloud with normals, the features open3d's global-registration
+         recipe feeds to the two searches above.
 
 With ``shims.install()`` these are reachable as ``open3d.pipelines.registration`` (and the pre-0.12 alias
 ``open3d.registration``) whenever the real open3d is absent, so the reference's own class runs on this stack
 without a line changed.  There is no CPU path: the functions raise without an sm_90 device.
 """
+import math
+
 import numpy as np
 import torch
 
@@ -67,7 +72,9 @@ class KDTreeSearchParamRadius:
     self.radius = float(radius)
 
 
-def _hybrid_check(search_param):
+def _hybrid_check(search_param, max_nn=_abi.MAX_NN):
+  """A KDTreeSearchParamHybrid with a positive radius and 1 <= max_nn <= the caller's bound (64 for normals, 128 for
+  FPFH)."""
   if isinstance(search_param, (KDTreeSearchParamKNN, KDTreeSearchParamRadius)):
     raise NotImplementedError(f'{type(search_param).__name__}: only KDTreeSearchParamHybrid(radius, max_nn) is built '
                               '(a bounded radius the voxel hash can search)')
@@ -75,8 +82,8 @@ def _hybrid_check(search_param):
     raise TypeError(f'expected KDTreeSearchParamHybrid, got {type(search_param).__name__}')
   if not search_param.radius > 0.0:
     raise ValueError(f'radius must be positive, got {search_param.radius}')
-  if not 1 <= search_param.max_nn <= _abi.MAX_NN:
-    raise ValueError(f'max_nn must lie in [1, {_abi.MAX_NN}], got {search_param.max_nn}')
+  if not 1 <= search_param.max_nn <= max_nn:
+    raise ValueError(f'max_nn must lie in [1, {max_nn}], got {search_param.max_nn}')
 
 
 def estimate_normals(points, search_param, prev=None):
@@ -155,17 +162,47 @@ def _points(pcd, device):
   return torch.from_numpy(np.ascontiguousarray(pts)).to(device)
 
 
-def _target_hash(tgt64, max_dist):
-  """Voxel hash of the target with at most one point per cell (what the ICP and normal kernels search): cell =
+def _target_hash(tgt64, max_dist, max_reach=4, what='max_correspondence_distance'):
+  """Voxel hash of the target with at most one point per cell (what the ICP, normal and FPFH kernels search): cell =
   max_dist / 2 as in DGR (voxelised clouds, radius 2 voxels); a cloud with several points per cell gets finer
-  cells up to the kernels' reach of 4."""
-  for div in (2.0, 3.0, 4.0):
+  cells up to the kernel's reach (4 for ICP and normals, 6 for FPFH, whose 5-voxel radius needs cell = max_dist / 5).
+  A cell whose quotient max_dist / cell rounds above the reach is widened by one ulp."""
+  for div in range(2, max_reach + 1):
     cell = max_dist / div
+    if math.ceil(max_dist / cell) > max_reach:
+      cell = float(np.nextafter(cell, np.inf))
     _, spec, table, _, _, n = _abi.voxelise(tgt64, cell)
     if n == tgt64.shape[0]:
       return cell, spec, table
-  raise NotImplementedError('target has several points within max_correspondence_distance / 4 of each other: '
+  raise NotImplementedError(f'target has several points within {what} / {max_reach} of each other: '
                             'voxel-downsample it first (DGR always passes voxelised clouds)')
+
+
+def compute_fpfh_feature(input, search_param):
+  """open3d's ``registration.compute_fpfh_feature(pcd, KDTreeSearchParamHybrid(radius, max_nn))``: FPFH features of a
+  cloud with normals, through a voxel hash of the cloud (dgr_compute_fpfh; max_nn <= 128, the point itself
+  included).  -> Feature with data float64 [33, N]."""
+  _hybrid_check(search_param, _abi.FPFH_MAX_NN)
+  pts = np.asarray(getattr(input, 'points', input), dtype=np.float64).reshape(-1, 3)
+  nrm = getattr(input, 'normals', None)
+  if nrm is None:
+    raise RuntimeError('compute_fpfh_feature needs normals: call '
+                       'pcd.estimate_normals(KDTreeSearchParamHybrid(radius, max_nn)) first')
+  nrm = np.asarray(nrm, dtype=np.float32).reshape(-1, 3)
+  if len(nrm) != len(pts):
+    raise RuntimeError('normals must hold one row per point')
+  feature = Feature()
+  feature.resize(_abi.FPFH_DIM, len(pts))
+  if len(pts) == 0:
+    return feature
+  dev = _abi.require_device('cuda')
+  _abi.refresh_stream()
+  p64 = torch.from_numpy(np.ascontiguousarray(pts)).to(dev)
+  cell, spec, table = _target_hash(p64, search_param.radius, max_reach=6, what='the radius')
+  f = _abi.compute_fpfh(p64.float().contiguous(), torch.from_numpy(np.ascontiguousarray(nrm)).to(dev), (spec, table),
+                        cell, search_param.radius, search_param.max_nn)
+  feature.data = f.cpu().numpy().astype(np.float64).T.copy()
+  return feature
 
 
 def registration_icp(source, target, max_correspondence_distance, init=None, estimation_method=None, criteria=None):

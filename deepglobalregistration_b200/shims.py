@@ -44,7 +44,8 @@ def _open3d_stub():
   viewer, backed by io.py) and core/deep_global_registration.py:29-64,317-322 + util/pointcloud.py:15-23
   (pipelines.registration.registration_icp / registration_ransac_based_on_correspondence /
   registration_ransac_based_on_feature_matching, Feature, utility vectors; plus
-  registration_fast_based_on_feature_matching / FastGlobalRegistrationOption for FGR users, and
+  registration_fast_based_on_feature_matching / FastGlobalRegistrationOption / compute_fpfh_feature for FGR and
+  FPFH users, and
   TransformationEstimationPointToPlane with geometry.KDTreeSearchParamHybrid for point-to-plane ICP users) backed
   by libdgr_b200 (o3d_registration.py) - so the reference's OWN DeepGlobalRegistration class and demo.py run on
   this stack unmodified.  This package's DeepGlobalRegistration does not go through here: it calls the library."""
@@ -72,7 +73,7 @@ def _open3d_stub():
                'CorrespondenceCheckerBasedOnDistance', 'CorrespondenceCheckerBasedOnEdgeLength', 'Feature',
                'RegistrationResult', 'registration_icp', 'registration_ransac_based_on_correspondence',
                'registration_ransac_based_on_feature_matching', 'FastGlobalRegistrationOption',
-               'registration_fast_based_on_feature_matching'):
+               'registration_fast_based_on_feature_matching', 'compute_fpfh_feature'):
     setattr(o3d.pipelines.registration, name, getattr(reg, name))
   o3d.registration = o3d.pipelines.registration          # the pre-0.12 module path
   sys.modules['open3d.pipelines'] = o3d.pipelines

@@ -197,6 +197,18 @@ int32_t dgr_se3_register(const float* x, const float* y, const int32_t* idx1, co
 int32_t dgr_estimate_normals(const float* xyz, int64_t n, const dgr_keyspec_t* spec, const uint64_t* keys,
                              const int32_t* vals, int64_t cap, int32_t batch, double cell, double radius,
                              int32_t max_nn, const float* prev, float* normals, int32_t* counts, void* stream);
+/* FPFH features (open3d 0.10 ComputeFPFHFeature(KDTreeSearchParamHybrid(radius, max_nn)); oracle/fpfh.py) of the
+ * cloud xyz[n] with normals[n, 3] (required), through its OWN voxel hash as dgr_estimate_normals searches it
+ * (ceil(radius / cell) <= 6, max_nn 1..128 counting the point itself).  The point itself is dropped from its list;
+ * the pair features and the 33-bin SPFH are fp64, the FPFH's weighted sums and scaling fp64 in a fixed order, rounded
+ * to float once.  out: float [n, ld], ld >= 33, columns 33 .. ld - 1 written as zeros (ld = 64 feeds
+ * dgr_knn_top1_tc); counts: int32 [n] = rows within the radius (the point included, before the max_nn truncation);
+ * ws: dgr_fpfh_ws_elems(n, max_nn) 8-byte words.  No atomics, no host read, the same bits on every run. */
+int32_t dgr_fpfh_ws_elems(int64_t n, int32_t max_nn, int64_t* n_elems);
+int32_t dgr_compute_fpfh(const float* xyz, const float* normals, int64_t n, const dgr_keyspec_t* spec,
+                         const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch, double cell,
+                         double radius, int32_t max_nn, int32_t ld, void* ws, float* out, int32_t* counts,
+                         void* stream);
 /* ICP of src onto tgt.  Correspondences: the nearest target point strictly within max_dist of each transformed
  * source point s, through the TARGET cloud's voxel hash (keys / vals / spec of the table dgr_unique_first built at
  * `voxel`; table rows = rows of tgt; `batch` = the batch index those coordinates carry; max_dist / voxel <= 4).
