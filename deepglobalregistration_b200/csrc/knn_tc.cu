@@ -153,10 +153,6 @@ knn_prep_kernel(const float* __restrict__ f0, int n0, const float* __restrict__ 
   }
 }
 
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-
 // exact reference arithmetic for one (row, column) pair, as in knn.cu
 template <int C>
 __device__ __forceinline__ unsigned long long knn_exact_key(const float* __restrict__ f0, const float* __restrict__ f1,

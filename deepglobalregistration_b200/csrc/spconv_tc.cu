@@ -4,16 +4,20 @@
 // (kappa, j)-sorted pair lists) with the sub-GEMM issued as wgmma.mma_async and the accumulator
 // in registers:
 //
-//   * one CTA = one 128-pair tile of one kernel offset, M = 128 rows (pairs) split over two
-//     warpgroups (64 rows each), N = cout (16..256, padded to 32 / 64 / 128 / 256 with zero weight
-//     rows), K = cin in chunks of one 128-byte swizzle row (32 TF32 or 64 FP16 channels);
-//   * all 256 threads gather the 128 input rows (coalesced 16-byte pieces, 8 lanes per row, the
-//     next chunk in flight while the current one multiplies), split every value into a "hi" part and
-//     a "lo" residual and store both into shared memory in the canonical K-major SWIZZLE_128B layout;
-//     one thread bulk-copies the weight slab of the chunk (TMA engine, completion on an mbarrier);
-//   * each warpgroup issues, per k-step, the three products hi*hi + lo*hi + hi*lo (3xTF32 or
-//     3xFP16, fp32-accurate to ~2^-21 relative) from two shared-memory stages, so the stores of
-//     chunk c+1 overlap the MMAs of chunk c;
+//   * a tile is 128 pairs of one kernel offset: M = 128 rows split over two consumer warpgroups (64 rows
+//     each), N = cout (16..256, padded to 32 / 64 / 128 / 256 with zero weight rows), K = cin in chunks of
+//     one 128-byte swizzle row (32 TF32 or 64 FP16 channels);
+//   * a CTA works through a run of consecutive tiles (spconv_ring::tile_run of them) as three warpgroups:
+//     one producer, two consumers, coupled only by the full / empty mbarriers of a two-stage ring whose
+//     position keeps running across tile boundaries (spconv_ring.h);
+//   * the producer gathers the 128 input rows of a chunk (coalesced 16-byte pieces, 8 lanes per row, the
+//     next chunk - of this tile or the next - in flight while the current one is stored), splits every
+//     value into a "hi" part and a "lo" residual and stores both into shared memory in the canonical
+//     K-major SWIZZLE_128B layout; one of its threads bulk-copies the weight slab of the chunk (TMA engine,
+//     completion on the stage's full barrier).  It also parks the tile's out rows in shared memory.  While
+//     the consumers drain the accumulators of tile t, the first chunks of tile t + 1 are already landing;
+//   * each consumer warpgroup issues, per k-step, the three products hi*hi + lo*hi + hi*lo (3xTF32 or
+//     3xFP16, fp32-accurate to ~2^-21 relative) and hands a stage back once the MMAs that read it retired;
 //   * the epilogue scatter-adds the accumulator fragments with red.global.add.v2.f32.
 //
 // Weights come PRE-SPLIT and PRE-SWIZZLED (dgr_pack_weight_tf32 / dgr_pack_weight_f16, cached per layer
@@ -22,11 +26,13 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "spconv_ring.h"
 #include "tc_common.cuh"
 
 namespace {
 
 using namespace tc;
+using namespace spconv_ring;
 
 #define DGR_TRY_RC(expr)             \
   do {                              \
@@ -34,14 +40,25 @@ using namespace tc;
     if (rc__ != DGR_OK) return rc__; \
   } while (0)
 
-constexpr int kThreadsTC = 256;          // two warpgroups: tile rows 0..63 and 64..127
+constexpr int kConsumerWarps = 8;        // two warpgroups: tile rows 0..63 and 64..127
+constexpr int kProducerThreads = 128;    // the third warpgroup
+constexpr int kThreadsTC = kConsumerWarps * 32 + kProducerThreads;
 constexpr int kTileM = 128;
 constexpr int kChunk = 32;               // TF32 channels per 128-byte row
 constexpr int kATileBytes = kTileM * 128;
-constexpr int kStages = 2;
+constexpr int kGatherRows = kTileM / (kProducerThreads / 8);   // rows per producer thread and chunk
+static_assert(kMaxRun <= 32, "one warp lists the tiles of a run");
+
+struct TileDesc {
+  int kappa, p0, rows;
+};
 
 struct TcShared {
-  unsigned long long full[kStages];     // weight slab of the stage has landed (bulk-copy bytes)
+  unsigned long long full[kStages];     // gathered rows stored and weight slab landed (bulk-copy bytes)
+  unsigned long long empty[kStages];    // every consumer warp has retired the MMAs that read the stage
+  int n_run;                            // non-empty tiles of the run
+  TileDesc tiles[kMaxRun];
+  int out_rows[kIdxSlots][kTileM];      // out row of every pair of a tile, -1 beyond the tile's rows
 };
 
 // shared-memory bytes of spconv_tc_kernel<NT, *>
@@ -49,17 +66,26 @@ constexpr size_t tc_smem_bytes(int nt) {
   return sizeof(TcShared) + 1024 + (size_t)kStages * (2 * kATileBytes + 2 * nt * 128);
 }
 
+// NT >= 128: one CTA per SM, the register file re-divided between producer and consumers (setmaxnreg);
+// narrower accumulators leave room for two CTAs, whose 80 registers the TF32 producer fits and the FP16 one
+// (twice the rows per chunk) does not
+constexpr int tc_min_ctas(int nt, bool f16) { return nt >= 128 || f16 ? 1 : 2; }
+constexpr int kProducerRegs = 104, kConsumerRegs = 200;     // 128 * 104 + 256 * 200 = 384 * 168
+
 // kF16: 3xFP16 instead of 3xTF32 (64 channels per 128-byte stage row; `wt` then holds the fp16 slabs of
-// dgr_pack_weight_f16, amax_in the input tensor's absolute maximum, w_inv_scale the inverse of the weight scale)
+// dgr_pack_weight_f16, amax_in the input tensor's absolute maximum, w_inv_scale the inverse of the weight scale).
+// CTA b owns tiles [b * run, min((b + 1) * run, n_tiles)).
 template <int NT, bool kF16, int kPasses>
-__global__ void __launch_bounds__(kThreadsTC, 1)
+__global__ void __launch_bounds__(kThreadsTC, tc_min_ctas(NT, kF16))
 spconv_tc_kernel(const float* __restrict__ in_feat, int cin, const unsigned char* __restrict__ wt, int cout,
                  const int32_t* __restrict__ in_idx, const int32_t* __restrict__ out_idx,
                  const int32_t* __restrict__ kofs, const int32_t* __restrict__ tile_k,
-                 const int32_t* __restrict__ tile_start, const float* __restrict__ amax_in,
+                 const int32_t* __restrict__ tile_start, int n_tiles, int run, const float* __restrict__ amax_in,
                  const float* __restrict__ w_inv_scale, float* __restrict__ out) {
   constexpr int kCh = kF16 ? 64 : kChunk;        // channels per stage (one 128-byte swizzle row)
   constexpr int kV = kF16 ? 2 : 1;               // float4 loads per (thread, row, chunk)
+  // a producer thread keeps eight float4 in flight: a whole chunk of its rows in TF32, half of them in FP16
+  constexpr int kBatches = kV, kBatchRows = kGatherRows / kBatches;
   constexpr int kBTileBytes = NT * 128;          // B tile in shared memory: rows >= cout stay zero
   constexpr int kStageBytes = 2 * kATileBytes + 2 * kBTileBytes;
   extern __shared__ __align__(16) unsigned char smem_dyn[];
@@ -67,16 +93,18 @@ spconv_tc_kernel(const float* __restrict__ in_feat, int cin, const unsigned char
   // stage buffers start at the next 1024-byte boundary (SWIZZLE_128B atom alignment)
   unsigned char* stage0 = reinterpret_cast<unsigned char*>(
       (reinterpret_cast<uintptr_t>(smem_dyn) + sizeof(TcShared) + 1023) & ~(uintptr_t)1023);
-  const int t = threadIdx.x, wg = t >> 7;
+  // warp index through a shuffle: the compiler then knows it is warp-uniform, as the wgmma paths need
+  const int t = threadIdx.x, warp = __shfl_sync(0xffffffffu, t >> 5, 0), lane = t & 31;
   const int n_chunks = cin / kCh;
   const uint32_t b_tile_bytes = (uint32_t)cout * 128;   // one tile (hi or lo) of the packed slab
   const uint32_t slab_bytes = 2 * b_tile_bytes;
-  const int kappa = tile_k[blockIdx.x];
-  const int p0 = tile_start[blockIdx.x];
-  const int rows = min(kTileM, kofs[kappa + 1] - p0);   // <= 0 for the padding tiles of a paired list
+  const uint32_t full0 = smem_u32(&sh.full[0]), empty0 = smem_u32(&sh.empty[0]);
 
   if (t == 0) {
-    for (int s = 0; s < kStages; ++s) mbar_init(smem_u32(&sh.full[s]), 1);
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(full0 + 8 * s, kProducerThreads + 1);     // every producer thread + the slab's expect-tx arrival
+      mbar_init(empty0 + 8 * s, kConsumerWarps);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (NT > cout) {     // zero the padding rows of every B tile once: the bulk copies never write them
@@ -87,82 +115,155 @@ spconv_tc_kernel(const float* __restrict__ in_feat, int cin, const unsigned char
                                 (cout + (e >> 3)) * 128 + (e & 7) * 16) = make_uint4(0u, 0u, 0u, 0u);
     }
   }
-
-  // gather: 8 lanes cover one 128-byte row; 32 row groups, rows rgrp + 32 i
-  const int piece = t & 7, rgrp = t >> 3;
-  const uint32_t a_off = (uint32_t)(rgrp * 128 + ((piece ^ (rgrp & 7)) << 4));   // + i * 4096
-  int src[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r = i * 32 + rgrp;
-    src[i] = (r < rows) ? __ldg(in_idx + p0 + r) : -1;
+  if (warp == 0) {     // the run's tiles, without the padding tiles (rows <= 0) of a paired list
+    const int tile = blockIdx.x * run + lane;
+    TileDesc d = {0, 0, 0};
+    if (lane < run && tile < n_tiles) {
+      d.kappa = tile_k[tile];
+      d.p0 = tile_start[tile];
+      d.rows = min(kTileM, kofs[d.kappa + 1] - d.p0);
+    }
+    const unsigned live = __ballot_sync(0xffffffffu, d.rows > 0);
+    if (d.rows > 0) sh.tiles[__popc(live & ((1u << lane) - 1u))] = d;
+    if (lane == 0) sh.n_run = __popc(live);
   }
-  float4 v[4][kV];
-  auto load_a = [&](int c) {
+  __syncthreads();     // the last block-wide barrier: the roles split here
+  const int n_run = sh.n_run;
+  if (n_run == 0) return;
+
+  if (warp >= kConsumerWarps) {     // producer warpgroup
+    if (NT >= 128) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    // gather: 8 lanes cover one 128-byte row; 16 row groups, rows rgrp + 16 i
+    const int pt = t - kConsumerWarps * 32, piece = pt & 7, rgrp = pt >> 3;
+    const uint32_t a_off = (uint32_t)(rgrp * 128 + ((piece ^ (rgrp & 7)) << 4));   // + i * 2048
+    const float sx = kF16 ? f16_scale_for(__ldg(amax_in)) : 1.f;
+    // in rows of the thread's kGatherRows rows and the out row of pair `pt`, of run tile ti
+    auto load_idx = [&](int ti, int (&src)[kGatherRows], int& oj) {
+      const TileDesc d = sh.tiles[ti < n_run ? ti : 0];
+      const int rows = ti < n_run ? d.rows : 0;
 #pragma unroll
-    for (int i = 0; i < 4; ++i)
+      for (int i = 0; i < kGatherRows; ++i) {
+        const int r = i * 16 + rgrp;
+        src[i] = r < rows ? __ldg(in_idx + d.p0 + r) : -1;
+      }
+      oj = pt < rows ? __ldg(out_idx + d.p0 + pt) : -1;
+    };
+    int src[kGatherRows], src_next[kGatherRows], oj, oj_next;
+    float4 v[kBatchRows][kV];
+    // rows h * kBatchRows ... of chunk c of the tile `src` belongs to
+    auto load_a = [&](int c, int h) {
 #pragma unroll
-      for (int u = 0; u < kV; ++u)
-        v[i][u] = src[i] >= 0 ? __ldg(reinterpret_cast<const float4*>(in_feat + (size_t)src[i] * cin + c * kCh +
-                                                                       piece * (4 * kV) + 4 * u))
-                              : make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int i = 0; i < kBatchRows; ++i)
+#pragma unroll
+        for (int u = 0; u < kV; ++u) {
+          const int row = src[h * kBatchRows + i];
+          v[i][u] = row >= 0 ? __ldg(reinterpret_cast<const float4*>(in_feat + (size_t)row * cin + c * kCh +
+                                                                      piece * (4 * kV) + 4 * u))
+                             : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+    };
+    load_idx(0, src, oj);
+    load_idx(1, src_next, oj_next);     // indices stay one tile ahead of the rows they address
+    load_a(0, 0);
+    unsigned g = 0;                     // chunks of the run so far: the ring position
+    for (int ti = 0; ti < n_run; ++ti) {
+      const unsigned char* slab = wt + (size_t)sh.tiles[ti].kappa * n_chunks * slab_bytes;
+      for (int c = 0; c < n_chunks; ++c, ++g) {
+        const int s = stage_of(g);
+        unsigned char* a_hi = stage0 + (size_t)s * kStageBytes;
+        unsigned char* a_lo = a_hi + kATileBytes;
+        unsigned char* b_hi = a_lo + kATileBytes;
+        if (g >= kStages) mbar_wait(empty0 + 8 * s, empty_parity(g));
+        if (pt == 0) {
+          const unsigned char* bsrc = slab + (size_t)c * slab_bytes;
+          mbar_arrive_expect_tx(full0 + 8 * s, kPasses == 3 ? slab_bytes : b_tile_bytes);
+          bulk_g2s(smem_u32(b_hi), bsrc, b_tile_bytes, full0 + 8 * s);
+          if (kPasses == 3) bulk_g2s(smem_u32(b_hi + kBTileBytes), bsrc + b_tile_bytes, b_tile_bytes, full0 + 8 * s);
+        }
+        if (c == 0) sh.out_rows[idx_slot(ti)][pt] = oj;
+#pragma unroll
+        for (int h = 0; h < kBatches; ++h) {
+#pragma unroll
+          for (int i = 0; i < kBatchRows; ++i) {
+            const uint32_t off = a_off + (h * kBatchRows + i) * 2048;
+            if (kF16) split_store_f16(v[i][0], v[i][kV - 1], sx, a_hi, a_lo, off);
+            else split_store(v[i][0], a_hi, a_lo, off);
+          }
+          // the next rows - of this chunk, the next chunk or the next tile - are in flight while these multiply
+          if (h + 1 < kBatches) {
+            load_a(c, h + 1);
+          } else if (c + 1 < n_chunks) {
+            load_a(c + 1, 0);
+          } else if (ti + 1 < n_run) {
+#pragma unroll
+            for (int i = 0; i < kGatherRows; ++i) src[i] = src_next[i];
+            oj = oj_next;
+            load_a(0, 0);
+            load_idx(ti + 2, src_next, oj_next);
+          }
+        }
+        fence_proxy_async();
+        mbar_arrive(full0 + 8 * s);
+      }
+    }
+    return;
+  }
+
+  if (NT >= 128) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+  // consumers: thread holds rows r0 and r0 + 8 of the tile, two adjacent columns per 8-column group
+  const int wg = warp >> 2;
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  // kF16: the accumulator holds (sx * x) . (sw * w); both scales are powers of two, undone exactly in the epilogue
+  const float inv = kF16 ? __ldg(w_inv_scale) / f16_scale_for(__ldg(amax_in)) : 1.f;
+  auto release = [&](unsigned gq) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty0 + 8 * stage_of(gq));
   };
-  const float sx = kF16 ? f16_scale_for(__ldg(amax_in)) : 1.f;
-  const unsigned char* slab = wt + (size_t)kappa * n_chunks * slab_bytes;
-
-  float acc[NT / 2];
+  unsigned g = 0;
+  for (int ti = 0; ti < n_run; ++ti) {
+    float acc[NT / 2];
 #pragma unroll
-  for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
-  load_a(0);
-  for (int c = 0; c < n_chunks; ++c) {
-    const int s = c % kStages;
-    const uint32_t ph = (c / kStages) & 1;
-    unsigned char* a_hi = stage0 + (size_t)s * kStageBytes;
-    unsigned char* a_lo = a_hi + kATileBytes;
-    unsigned char* b_hi = a_lo + kATileBytes;
-    // every warpgroup has retired the MMAs of chunk c - kStages (wgmma_wait below): stage s is free
-    __syncthreads();
-    if (t == 0) {
-      const unsigned char* bsrc = slab + (size_t)c * slab_bytes;
-      mbar_arrive_expect_tx(smem_u32(&sh.full[s]), kPasses == 3 ? slab_bytes : b_tile_bytes);
-      bulk_g2s(smem_u32(b_hi), bsrc, b_tile_bytes, smem_u32(&sh.full[s]));
-      if (kPasses == 3) bulk_g2s(smem_u32(b_hi + kBTileBytes), bsrc + b_tile_bytes, b_tile_bytes, smem_u32(&sh.full[s]));
+    for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+    for (int c = 0; c < n_chunks; ++c, ++g) {
+      const uint32_t a_hi = smem_u32(stage0 + (size_t)stage_of(g) * kStageBytes);
+      const uint32_t b_hi = a_hi + 2 * kATileBytes;
+      mbar_wait(full0 + 8 * stage_of(g), full_parity(g));
+      wgmma_fence();
+      const uint32_t a0 = a_hi + wg * (kATileBytes / 2);
+      mma_chunk<NT, kF16, kPasses>(acc, a0, a0 + kATileBytes, b_hi, b_hi + kBTileBytes);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (c > 0) release(g - 1);          // the MMAs of the previous chunk have retired: its stage is free
     }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      if (kF16) split_store_f16(v[i][0], v[i][kV - 1], sx, a_hi, a_lo, a_off + i * 4096);
-      else split_store(v[i][0], a_hi, a_lo, a_off + i * 4096);
-    }
-    if (c + 1 < n_chunks) load_a(c + 1);          // in flight while chunk c multiplies
-    fence_proxy_async();
-    __syncthreads();
-    mbar_wait(smem_u32(&sh.full[s]), ph);
-    wgmma_fence();
-    const uint32_t a0 = smem_u32(a_hi) + wg * (kATileBytes / 2);
-    mma_chunk<NT, kF16, kPasses>(acc, a0, a0 + kATileBytes, smem_u32(b_hi), smem_u32(b_hi) + kBTileBytes);
-    wgmma_commit();
-    wgmma_wait<1>();
-  }
-  wgmma_wait<0>();
-  fence_acc(acc);
+    wgmma_wait<0>();
+    fence_acc(acc);
+    release(g - 1);
 
-  // epilogue: thread holds rows r0 and r0 + 8 of its warpgroup, two adjacent columns per 8-column group
-  // kF16: the accumulator holds (sx * x) . (sw * w); both scales are powers of two, undone exactly here
-  const float inv = kF16 ? __ldg(w_inv_scale) / sx : 1.f;
-  const int lane = t & 31;
-  const int r0 = wg * 64 + ((t >> 5) & 3) * 16 + (lane >> 2);
-  const int j0 = r0 < rows ? out_idx[p0 + r0] : -1;
-  const int j1 = r0 + 8 < rows ? out_idx[p0 + r0 + 8] : -1;
-  float* o0 = out + (size_t)(j0 < 0 ? 0 : j0) * cout;
-  float* o1 = out + (size_t)(j1 < 0 ? 0 : j1) * cout;
+    const int* rows_of = sh.out_rows[idx_slot(ti)];
+    const int j0 = rows_of[r0], j1 = rows_of[r0 + 8];
+    float* o0 = out + (size_t)(j0 < 0 ? 0 : j0) * cout;
+    float* o1 = out + (size_t)(j1 < 0 ? 0 : j1) * cout;
 #pragma unroll
-  for (int i = 0; i < NT / 8; ++i) {
-    const int col = 8 * i + 2 * (lane & 3);
-    if (col < cout) {
-      if (j0 >= 0) red_add_v2(o0 + col, acc[4 * i] * inv, acc[4 * i + 1] * inv);
-      if (j1 >= 0) red_add_v2(o1 + col, acc[4 * i + 2] * inv, acc[4 * i + 3] * inv);
+    for (int i = 0; i < NT / 8; ++i) {
+      const int col = 8 * i + 2 * (lane & 3);
+      if (col < cout) {
+        if (j0 >= 0) red_add_v2(o0 + col, acc[4 * i] * inv, acc[4 * i + 1] * inv);
+        if (j1 >= 0) red_add_v2(o1 + col, acc[4 * i + 2] * inv, acc[4 * i + 3] * inv);
+      }
     }
   }
+}
+
+// CTAs of the kernel a device holds at once (SMs x CTAs per SM); 0 if the query fails
+template <int NT, bool kF16, int kPasses>
+int tc_resident_ctas(size_t smem) {
+  int dev = 0, sms = 0, per_sm = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess ||
+      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, spconv_tc_kernel<NT, kF16, kPasses>, kThreadsTC, smem) !=
+          cudaSuccess)
+    return 0;
+  return sms * per_sm;
 }
 
 // one instantiation per kernel: DGR_ENSURE_SMEM keeps its attribute state per call site
@@ -172,8 +273,15 @@ int32_t launch_spconv_tc(const float* in_feat, int cin, const void* wt, int cout
                          int n_tiles, const float* amax_in, const float* w_inv_scale, float* out, cudaStream_t st) {
   const size_t smem = tc_smem_bytes(NT);
   DGR_ENSURE_SMEM((spconv_tc_kernel<NT, kF16, kPasses>), smem);
-  spconv_tc_kernel<NT, kF16, kPasses><<<n_tiles, kThreadsTC, smem, st>>>(
-      in_feat, cin, (const unsigned char*)wt, cout, in_idx, out_idx, kofs, tile_k, tile_start, amax_in, w_inv_scale, out);
+  static const int resident = tc_resident_ctas<NT, kF16, kPasses>(smem);
+  if (resident <= 0) {
+    dgr_set_error("spconv_tc_kernel does not fit the device");
+    return DGR_ERR_CUDA;
+  }
+  const int run = tile_run(n_tiles, resident);
+  spconv_tc_kernel<NT, kF16, kPasses><<<(n_tiles + run - 1) / run, kThreadsTC, smem, st>>>(
+      in_feat, cin, (const unsigned char*)wt, cout, in_idx, out_idx, kofs, tile_k, tile_start, n_tiles, run, amax_in,
+      w_inv_scale, out);
   dgr_note_launches(1);
   DGR_LAUNCH_CHECK();
   return DGR_OK;
