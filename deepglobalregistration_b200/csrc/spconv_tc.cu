@@ -18,7 +18,9 @@
 //     the consumers drain the accumulators of tile t, the first chunks of tile t + 1 are already landing;
 //   * each consumer warpgroup issues, per k-step, the three products hi*hi + lo*hi + hi*lo (3xTF32 or
 //     3xFP16, fp32-accurate to ~2^-21 relative) and hands a stage back once the MMAs that read it retired;
-//   * the epilogue scatter-adds the accumulator fragments with red.global.add.v2.f32.
+//   * the epilogue scatter-adds the accumulator fragments with red.global.add: NT >= 128 through a per-warp
+//     shared-memory transpose, one 128-byte row segment per 8 lanes (.v4); narrower tiles straight from the
+//     fragment (.v2).
 //
 // Weights come PRE-SPLIT and PRE-SWIZZLED (dgr_pack_weight_tf32 / dgr_pack_weight_f16, cached per layer
 // by the host): per (offset, chunk) one contiguous slab holding the hi tile and the lo tile in
@@ -61,9 +63,17 @@ struct TcShared {
   int out_rows[kIdxSlots][kTileM];      // out row of every pair of a tile, -1 beyond the tile's rows
 };
 
+// NT >= 128 (one CTA per SM, shared memory to spare): the epilogue passes each consumer warp's fragment through a
+// 16-row x 32-column scratch so that one red.global.add.v4 instruction covers four whole 128-byte row segments
+// instead of one 32-byte sector in each of eight rows
+constexpr bool tc_line_epilogue(int nt) { return nt >= 128; }
+constexpr int kScratchLd = 40;                                   // floats per scratch row (32 + 8 against conflicts)
+constexpr int kScratchBytes = 16 * kScratchLd * 4;               // per consumer warp
+
 // shared-memory bytes of spconv_tc_kernel<NT, *>
 constexpr size_t tc_smem_bytes(int nt) {
-  return sizeof(TcShared) + 1024 + (size_t)kStages * (2 * kATileBytes + 2 * nt * 128);
+  return sizeof(TcShared) + 1024 + (size_t)kStages * (2 * kATileBytes + 2 * nt * 128) +
+         (tc_line_epilogue(nt) ? (size_t)kConsumerWarps * kScratchBytes : 0);
 }
 
 // NT >= 128: one CTA per SM, the register file re-divided between producer and consumers (setmaxnreg);
@@ -240,15 +250,45 @@ spconv_tc_kernel(const float* __restrict__ in_feat, int cin, const unsigned char
     release(g - 1);
 
     const int* rows_of = sh.out_rows[idx_slot(ti)];
-    const int j0 = rows_of[r0], j1 = rows_of[r0 + 8];
-    float* o0 = out + (size_t)(j0 < 0 ? 0 : j0) * cout;
-    float* o1 = out + (size_t)(j1 < 0 ? 0 : j1) * cout;
+    if constexpr (tc_line_epilogue(NT)) {
+      // per 32-column block: the warp's 16 x 32 fragment goes to its scratch as rows, then every 8 lanes add one
+      // 128-byte row segment; each element still gets exactly one add of the same value
+      float* scr = reinterpret_cast<float*>(stage0 + (size_t)kStages * kStageBytes + warp * kScratchBytes);
+      const int lr = lane >> 2, lc = 2 * (lane & 3);                 // fragment position in the scratch
+      const int sr = lane >> 3, sc = 4 * (lane & 7);                 // segment position: rows sr + 4 k
+      int js[4];
 #pragma unroll
-    for (int i = 0; i < NT / 8; ++i) {
-      const int col = 8 * i + 2 * (lane & 3);
-      if (col < cout) {
-        if (j0 >= 0) red_add_v2(o0 + col, acc[4 * i] * inv, acc[4 * i + 1] * inv);
-        if (j1 >= 0) red_add_v2(o1 + col, acc[4 * i + 2] * inv, acc[4 * i + 3] * inv);
+      for (int k = 0; k < 4; ++k) js[k] = rows_of[r0 - lr + sr + 4 * k];
+#pragma unroll
+      for (int b = 0; b < NT / 32; ++b) {
+        if (32 * b >= cout) break;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int i = 4 * b + q;
+          *reinterpret_cast<float2*>(scr + lr * kScratchLd + 8 * q + lc) =
+              make_float2(acc[4 * i] * inv, acc[4 * i + 1] * inv);
+          *reinterpret_cast<float2*>(scr + (lr + 8) * kScratchLd + 8 * q + lc) =
+              make_float2(acc[4 * i + 2] * inv, acc[4 * i + 3] * inv);
+        }
+        __syncwarp();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const float4 v = *reinterpret_cast<const float4*>(scr + (sr + 4 * k) * kScratchLd + sc);
+          if (js[k] >= 0 && 32 * b + sc < cout) red_add_v4(out + (size_t)js[k] * cout + 32 * b + sc, v.x, v.y, v.z, v.w);
+        }
+        __syncwarp();     // every lane has read the block before the next one overwrites it
+      }
+    } else {
+      const int j0 = rows_of[r0], j1 = rows_of[r0 + 8];
+      float* o0 = out + (size_t)(j0 < 0 ? 0 : j0) * cout;
+      float* o1 = out + (size_t)(j1 < 0 ? 0 : j1) * cout;
+#pragma unroll
+      for (int i = 0; i < NT / 8; ++i) {
+        const int col = 8 * i + 2 * (lane & 3);
+        if (col < cout) {
+          if (j0 >= 0) red_add_v2(o0 + col, acc[4 * i] * inv, acc[4 * i + 1] * inv);
+          if (j1 >= 0) red_add_v2(o1 + col, acc[4 * i + 2] * inv, acc[4 * i + 3] * inv);
+        }
       }
     }
   }
@@ -397,6 +437,7 @@ int32_t dgr_spconv_tc_fwd(const float* in_feat, int32_t cin, const float* weight
   DGR_ARG_CHECK(tile_rows == kTileM, "tile_rows must be 128");
   DGR_ARG_CHECK(dgr_spconv_tc_supported(cin, cout), "shape not supported by the tensor-core path");
   DGR_ARG_CHECK(passes == 1 || passes == 3, "passes must be 1 or 3");
+  DGR_ARG_CHECK(((uintptr_t)out & 15) == 0, "out must be 16-byte aligned");
   if (n_tiles == 0) return DGR_OK;
   auto launch = passes == 3 ? launch_spconv_tc<false, 3> : launch_spconv_tc<false, 1>;
   return launch(in_feat, cin, weight_t, cout, in_idx, out_idx, kofs, tile_k, tile_start, n_tiles, nullptr, nullptr, out,
@@ -451,6 +492,7 @@ int32_t dgr_spconv_tc_f16_fwd(const float* in_feat, int32_t cin, const void* wei
   DGR_ARG_CHECK(tile_rows == kTileM, "tile_rows must be 128");
   DGR_ARG_CHECK(dgr_spconv_tc_f16_supported(cin, cout), "shape not supported by the 3xFP16 path");
   DGR_ARG_CHECK(amax_in != nullptr && w_scale != nullptr, "scales missing");
+  DGR_ARG_CHECK(((uintptr_t)out & 15) == 0, "out must be 16-byte aligned");
   if (n_tiles == 0) return DGR_OK;
   return launch_spconv_tc<true, 3>(in_feat, cin, weight_h, cout, in_idx, out_idx, kofs, tile_k, tile_start, n_tiles,
                                    amax_in, w_scale, out, (cudaStream_t)stream);

@@ -73,6 +73,11 @@ __device__ __forceinline__ void fence_acc(float (&d)[R]) {
 __device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
+// four element-wise fp32 adds at a 16-byte aligned address
+__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
+  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d)
+               : "memory");
+}
 __device__ __forceinline__ float tf32_round(float x) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
