@@ -9,6 +9,7 @@ import ctypes as C
 import math
 import os
 
+import numpy as np
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -61,6 +62,11 @@ SIGNATURES = {
     'dgr_compute_fpfh': [_p, _p, _i64, _p, _p, _p, _i64, _i32, _f64, _f64, _i32, _i32, _p, _p, _p, _p],
     'dgr_icp_ws_elems': [_i64, _p],
     'dgr_icp': [_p, _i64, _p, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _p, _i32, _f64, _f64, _p, _p, _p],
+    'dgr_information_matrix_ws_elems': [_i64, _p],
+    'dgr_information_matrix': [_p, _i64, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _p, _p, _p, _p],
+    'dgr_pose_graph_ws_elems': [_i64, _i64, _p],
+    'dgr_pose_graph_optimize': [_p, _i64, _p, _p, _p, _p, _p, _i64, _f64, _f64, _f64, _i32, _i32, _f64, _f64, _f64,
+                                _f64, _i32, _f64, _f64, _p, _p, _p, _p, _p, _p],
     'dgr_ransac_ws_elems': [_i64, _i64, _p],
     'dgr_ransac_correspondence': [_p, _p, _p, _p, _i64, _f64, _i64, C.c_uint64, _p, _p, _p],
     'dgr_ransac_fm_ws_elems': [_i64, _i64, _i64, _p],
@@ -709,6 +715,66 @@ def icp_point_to_plane(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_in
   """Point-to-plane ICP (open3d's TransformationEstimationPointToPlane, default criteria) of src onto tgt through
   tgt's voxel hash; arguments as icp_point_to_point plus tgt_normals (CUDA float32 [n_tgt, 3])."""
   return _icp(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter, rel_fitness, rel_rmse, batch)
+
+
+def information_matrix(src, tgt, tgt_manager, cell, max_dist, T, batch=0):
+  """open3d's GetInformationMatrixFromPointClouds: sum of G^T G over the nearest target point q of every transformed
+  source point strictly within max_dist (dgr_icp's search through tgt's voxel hash at `cell`; max_dist <= 4 cells).
+  src / tgt: CUDA float32 [n, 3]; tgt_manager: a CoordinateManager of tgt or (spec, table) of a dgr_unique_first table
+  (batch column `batch`); T: 4x4 mapping src into tgt.  -> device double [37] (6x6 row-major, correspondence count)."""
+  _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
+  spec, table = _hash_of(tgt_manager)
+  T = np.ascontiguousarray(np.asarray(T, dtype=np.float64).reshape(4, 4))
+  words = C.c_int64(0)
+  call('dgr_information_matrix_ws_elems', src.shape[0], C.byref(words))
+  ws = scratch('information', words.value, torch.float64, src.device)
+  out = torch.empty(37, dtype=torch.float64, device=src.device)
+  call('dgr_information_matrix', ptr(src), src.shape[0], ptr(tgt), ptr(spec), ptr(table.keys), ptr(table.vals),
+       table.cap, int(batch), float(cell), float(max_dist), T.ctypes.data_as(C.c_void_p), ptr(ws), ptr(out), stream())
+  return out
+
+
+POSE_GRAPH_MAX_NODES = 256
+POSE_GRAPH_MAX_EDGES = 32640
+POSE_GRAPH_STATS = ('iterations', 'iterations_pruned', 'cost', 'pruned', 'status', 'mu', 'mu_pruned', 'cost_start',
+                    'cost_first_pass', 'factorisations')
+
+
+def pose_graph_optimize(poses, ends, T, info, uncertain, confidence, max_correspondence_distance=0.075,
+                        edge_prune_threshold=0.25, preference_loop_closure=1.0, reference_node=-1, max_iteration=100,
+                        min_relative_increment=1e-6, min_relative_residual_increment=1e-6, min_right_term=1e-6,
+                        min_residual=1e-6, max_iteration_lm=20, upper_scale_factor=2 / 3, lower_scale_factor=1 / 3,
+                        device='cuda'):
+  """open3d's GlobalOptimization with GlobalOptimizationLevenbergMarquardt on the device (one launch, one read).
+  poses [N, 4, 4] mapping each fragment into the world; ends [E, 2] (source, target); T [E, 4, 4] mapping source into
+  target; info [E, 6, 6]; uncertain [E] bool; confidence [E] (the line process an uncertain edge starts from); host
+  arrays.  -> (poses [N, 4, 4], kept [E] bool, line process [E], stats dict)."""
+  poses = np.ascontiguousarray(np.asarray(poses, dtype=np.float64).reshape(-1, 16))
+  n = len(poses)
+  ends = np.ascontiguousarray(np.asarray(ends, dtype=np.int32).reshape(-1, 2))
+  e = len(ends)
+  T = np.ascontiguousarray(np.asarray(T, dtype=np.float64).reshape(e, 16))
+  info = np.ascontiguousarray(np.asarray(info, dtype=np.float64).reshape(e, 36))
+  unc = np.ascontiguousarray(np.asarray(uncertain, dtype=np.int32).reshape(e))
+  conf = np.ascontiguousarray(np.asarray(confidence, dtype=np.float64).reshape(e))
+  dev = require_device(device)
+  words = C.c_int64(0)
+  call('dgr_pose_graph_ws_elems', n, e, C.byref(words))
+  ws = scratch('pose_graph', words.value, torch.int64, dev)
+  out = np.zeros((max(n, 1), 16))
+  kept = np.zeros(max(e, 1), dtype=np.int32)
+  lp = np.zeros(max(e, 1))
+  st = np.zeros(16)
+  vp = lambda a: a.ctypes.data_as(C.c_void_p)
+  call('dgr_pose_graph_optimize', vp(poses), n, vp(ends), vp(T), vp(info), vp(unc), vp(conf), e,
+       float(max_correspondence_distance), float(edge_prune_threshold), float(preference_loop_closure),
+       int(reference_node), int(max_iteration), float(min_relative_increment), float(min_relative_residual_increment),
+       float(min_right_term), float(min_residual), int(max_iteration_lm), float(upper_scale_factor),
+       float(lower_scale_factor), ptr(ws), vp(out), vp(kept), vp(lp), vp(st), refresh_stream())
+  stats = {k: float(st[i]) for i, k in enumerate(POSE_GRAPH_STATS)}
+  for k in ('iterations', 'iterations_pruned', 'pruned', 'status', 'factorisations'):
+    stats[k] = int(stats[k])
+  return out[:n].reshape(n, 4, 4), kept[:e].astype(bool), lp[:e], stats
 
 
 def ransac_correspondence(x, y, idx0, idx1, max_dist, num_hyp=4000000, seed=0):

@@ -181,17 +181,8 @@ def summarize(result):
   return out
 
 
-def main(argv=None):
-  import json
-
-  import torch
-  import torch.distributed as dist
-  ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
-  src = ap.add_mutually_exclusive_group(required=True)
-  src.add_argument('--threed_match_dir', help='3DMatch test tree (scene folders + <scene>-evaluation/gt.log)')
-  src.add_argument('--kitti_dir', help='KITTI odometry root (contains dataset/sequences, dataset/poses); '
-                   'use --success_rte_thresh 0.6 --success_rre_thresh 5 (scripts/test_kitti.py:33-34)')
-  src.add_argument('--pair_list', help='text file: file0 file1 [16 numbers] [group] per line')
+def add_method_arguments(ap):
+  """The flags that choose and configure the pairwise method (shared by this CLI and multiway.py)."""
   ap.add_argument('--weights', required=True)
   ap.add_argument('--clip_weight_thresh', type=float, default=0.05)
   ap.add_argument('--success_rte_thresh', type=float, default=0.3, help='m (config.py:127; KITTI: 0.6)')
@@ -230,20 +221,19 @@ def main(argv=None):
   ap.add_argument('--pointnetlk_weights', default=None,
                   help='pointnetlk: PointNet_features state dict (required: a random network is no baseline)')
   ap.add_argument('--pointnetlk_max_iter', type=int, default=10, help='pointnetlk: Lucas-Kanade steps at most')
-  ap.add_argument('--out_dir', default='.')
-  args = ap.parse_args(argv)
+
+
+def check_method_arguments(ap, args):
   if args.method == 'pointnetlk' and not args.pointnetlk_weights:
     ap.error('--method pointnetlk needs --pointnetlk_weights')
 
-  world = int(os.environ.get('WORLD_SIZE', '1'))
-  local = int(os.environ.get('LOCAL_RANK', '0'))
-  torch.cuda.set_device(local)
-  if world > 1:
-    dist.init_process_group('nccl', device_id=torch.device('cuda', local))
-  rank = dist.get_rank() if world > 1 else 0
+
+def build_method(args, device):
+  """The pairwise method the flags of add_method_arguments name, on `device`: DeepGlobalRegistration itself or a
+  baseline wrapped around it (the baselines share its voxelisation and checkpoint)."""
   from .core.deep_global_registration import DeepGlobalRegistration
   cfg = argparse.Namespace(weights=args.weights, clip_weight_thresh=args.clip_weight_thresh, verbose=False)
-  dgr = DeepGlobalRegistration(cfg, device=torch.device('cuda', local))
+  dgr = DeepGlobalRegistration(cfg, device=device)
   dgr.use_icp = not args.no_icp
   method = dgr
   if args.method in ('fcgf_ransac', 'fpfh_ransac'):
@@ -271,6 +261,32 @@ def main(argv=None):
   elif args.method == 'pointnetlk':
     from .core.pointnetlk import PointNetLKBaseline
     method = PointNetLKBaseline(dgr, args.pointnetlk_weights, max_iter=args.pointnetlk_max_iter)
+  return method
+
+
+def main(argv=None):
+  import json
+
+  import torch
+  import torch.distributed as dist
+  ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+  src = ap.add_mutually_exclusive_group(required=True)
+  src.add_argument('--threed_match_dir', help='3DMatch test tree (scene folders + <scene>-evaluation/gt.log)')
+  src.add_argument('--kitti_dir', help='KITTI odometry root (contains dataset/sequences, dataset/poses); '
+                   'use --success_rte_thresh 0.6 --success_rre_thresh 5 (scripts/test_kitti.py:33-34)')
+  src.add_argument('--pair_list', help='text file: file0 file1 [16 numbers] [group] per line')
+  add_method_arguments(ap)
+  ap.add_argument('--out_dir', default='.')
+  args = ap.parse_args(argv)
+  check_method_arguments(ap, args)
+
+  world = int(os.environ.get('WORLD_SIZE', '1'))
+  local = int(os.environ.get('LOCAL_RANK', '0'))
+  torch.cuda.set_device(local)
+  if world > 1:
+    dist.init_process_group('nccl', device_id=torch.device('cuda', local))
+  rank = dist.get_rank() if world > 1 else 0
+  method = build_method(args, torch.device('cuda', local))
   if args.threed_match_dir:
     pairs = threedmatch_pairs(args.threed_match_dir)
   elif args.kitti_dir:

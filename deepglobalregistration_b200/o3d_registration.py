@@ -23,7 +23,13 @@ It also carries the calls open3d users make beyond DGR's own: point-to-plane ICP
          test, graduated non-convexity) with FastGlobalRegistrationOption's fields and defaults;
   compute_fpfh_feature(input, KDTreeSearchParamHybrid(radius, max_nn))
       -> dgr_compute_fpfh: FPFH descriptors of a cloud with normals, the features open3d's global-registration
-         recipe feeds to the two searches above.
+         recipe feeds to the two searches above;
+  get_information_matrix_from_point_clouds(source, target, max_correspondence_distance, transformation)
+      -> dgr_information_matrix: the 6x6 information matrix of a registered pair;
+  PoseGraph / PoseGraphNode / PoseGraphEdge and global_optimization(pose_graph, method, criteria, option)
+      -> dgr_pose_graph_optimize: multiway registration (Levenberg-Marquardt with line processes, pruning,
+         compensation to the reference node) with GlobalOptimizationConvergenceCriteria's and
+         GlobalOptimizationOption's fields and defaults.
 
 With ``shims.install()`` these are reachable as ``open3d.pipelines.registration`` (and the pre-0.12 alias
 ``open3d.registration``) whenever the real open3d is absent, so the reference's own class runs on this stack
@@ -372,3 +378,148 @@ def registration_fast_based_on_feature_matching(source, target, source_feature, 
                                 option.maximum_correspondence_distance, option.iteration_number, option.tuple_scale,
                                 option.maximum_tuple_count, option.tuple_test, seed=option.seed).cpu().numpy()
   return RegistrationResult(r[:16])
+
+
+def get_information_matrix_from_point_clouds(source, target, max_correspondence_distance, transformation):
+  """open3d's ``get_information_matrix_from_point_clouds``: sum of G^T G over the nearest target point of every
+  transformed source point strictly within the radius (dgr_information_matrix, through a voxel hash of the target as
+  registration_icp searches it).  -> float64 [6, 6]; entry [5, 5] is the correspondence count."""
+  d = float(max_correspondence_distance)
+  if not d > 0.0:
+    raise ValueError(f'max_correspondence_distance must be positive, got {max_correspondence_distance}')
+  T = np.asarray(transformation, dtype=np.float64).reshape(4, 4)
+  if not np.isfinite(T).all():
+    raise ValueError('transformation must be finite')
+  n_s = len(np.asarray(getattr(source, 'points', source)).reshape(-1, 3))
+  n_t = len(np.asarray(getattr(target, 'points', target)).reshape(-1, 3))
+  if n_s == 0 or n_t == 0:
+    return np.zeros((6, 6))
+  dev = _abi.require_device('cuda')
+  _abi.refresh_stream()
+  src64, tgt64 = _points(source, dev), _points(target, dev)
+  cell, spec, table = _target_hash(tgt64, d)
+  out = _abi.information_matrix(src64.float().contiguous(), tgt64.float().contiguous(), (spec, table), cell, d, T)
+  return out.cpu().numpy()[:36].reshape(6, 6).copy()
+
+
+class PoseGraphNode:
+  def __init__(self, pose=None):
+    self.pose = np.eye(4) if pose is None else np.asarray(pose, dtype=np.float64).reshape(4, 4).copy()
+
+  def __repr__(self):
+    return 'PoseGraphNode, access pose to get its current pose.'
+
+
+class PoseGraphEdge:
+  def __init__(self, source_node_id=-1, target_node_id=-1, transformation=None, information=None, uncertain=False,
+               confidence=1.0):
+    self.source_node_id, self.target_node_id = int(source_node_id), int(target_node_id)
+    self.transformation = np.eye(4) if transformation is None else \
+        np.asarray(transformation, dtype=np.float64).reshape(4, 4).copy()
+    self.information = np.eye(6) if information is None else \
+        np.asarray(information, dtype=np.float64).reshape(6, 6).copy()
+    self.uncertain = bool(uncertain)
+    self.confidence = float(confidence)
+
+  def __repr__(self):
+    return (f'PoseGraphEdge from nodes {self.source_node_id} to {self.target_node_id}, access transformation to get '
+            'relative transformation')
+
+
+class PoseGraph:
+  def __init__(self):
+    self.nodes = []
+    self.edges = []
+
+  def __repr__(self):
+    return f'PoseGraph with {len(self.nodes)} nodes and {len(self.edges)} edges.'
+
+
+class GlobalOptimizationLevenbergMarquardt:
+  pass
+
+
+class GlobalOptimizationGaussNewton:
+  """Accepted as a name; global_optimization raises NotImplementedError when it is passed."""
+
+
+class GlobalOptimizationConvergenceCriteria:
+  def __init__(self, max_iteration=100, min_relative_increment=1e-6, min_relative_residual_increment=1e-6,
+               min_right_term=1e-6, min_residual=1e-6, max_iteration_lm=20, upper_scale_factor=2. / 3.,
+               lower_scale_factor=1. / 3.):
+    self.max_iteration = int(max_iteration)
+    self.min_relative_increment = float(min_relative_increment)
+    self.min_relative_residual_increment = float(min_relative_residual_increment)
+    self.min_right_term = float(min_right_term)
+    self.min_residual = float(min_residual)
+    self.max_iteration_lm = int(max_iteration_lm)
+    self.upper_scale_factor = float(upper_scale_factor)
+    self.lower_scale_factor = float(lower_scale_factor)
+
+
+class GlobalOptimizationOption:
+  def __init__(self, max_correspondence_distance=0.075, edge_prune_threshold=0.25, preference_loop_closure=1.0,
+               reference_node=-1):
+    self.max_correspondence_distance = float(max_correspondence_distance)
+    self.edge_prune_threshold = float(edge_prune_threshold)
+    self.preference_loop_closure = float(preference_loop_closure)
+    self.reference_node = int(reference_node)
+
+
+def _pose_graph_arrays(pose_graph, option):
+  """Host arrays of a PoseGraph, every argument checked as the library checks it."""
+  n, m = len(pose_graph.nodes), len(pose_graph.edges)
+  if n == 0:
+    raise ValueError('the pose graph has no node')
+  if n > _abi.POSE_GRAPH_MAX_NODES:
+    raise ValueError(f'{n} nodes: at most {_abi.POSE_GRAPH_MAX_NODES} are supported (a dense solver)')
+  if m > _abi.POSE_GRAPH_MAX_EDGES:
+    raise ValueError(f'{m} edges: at most {_abi.POSE_GRAPH_MAX_EDGES} are supported')
+  if not option.max_correspondence_distance > 0.0:
+    raise ValueError(f'max_correspondence_distance must be positive, got {option.max_correspondence_distance}')
+  if not -1 <= option.reference_node < n:
+    raise ValueError(f'reference_node must lie in [-1, {n}), got {option.reference_node}')
+  poses = np.stack([np.asarray(v.pose, dtype=np.float64).reshape(4, 4) for v in pose_graph.nodes])
+  ends = np.array([[e.source_node_id, e.target_node_id] for e in pose_graph.edges], dtype=np.int64).reshape(m, 2)
+  if m and (ends.min() < 0 or ends.max() >= n):
+    raise ValueError('an edge names a node that is not in the graph')
+  if m and (ends[:, 0] == ends[:, 1]).any():
+    raise ValueError('an edge joins a node to itself')
+  T = np.stack([np.asarray(e.transformation, dtype=np.float64).reshape(4, 4) for e in pose_graph.edges]) if m else \
+      np.zeros((0, 4, 4))
+  info = np.stack([np.asarray(e.information, dtype=np.float64).reshape(6, 6) for e in pose_graph.edges]) if m else \
+      np.zeros((0, 6, 6))
+  unc = np.array([bool(e.uncertain) for e in pose_graph.edges], dtype=bool)
+  conf = np.array([float(e.confidence) for e in pose_graph.edges], dtype=np.float64)
+  for name, a in (('node poses', poses), ('edge transformations', T), ('information matrices', info),
+                  ('confidences', conf)):
+    if not np.isfinite(a).all():
+      raise ValueError(f'{name} must be finite')
+  return poses, ends.astype(np.int32), T, info, unc, conf
+
+
+def global_optimization(pose_graph, method=None, criteria=None, option=None):
+  """open3d's ``global_optimization``: Levenberg-Marquardt on the pose graph with line processes on the uncertain
+  edges, the uncertain edges whose line process ends below option.edge_prune_threshold removed, a second run on the
+  rest, then every pose moved so the reference node keeps its pose (dgr_pose_graph_optimize, one launch).  In place:
+  node poses updated, uncertain edges' confidence set to their final line process, pruned edges removed.  Returns
+  the library's statistics (open3d returns None)."""
+  if isinstance(method, GlobalOptimizationGaussNewton):
+    raise NotImplementedError('GlobalOptimizationGaussNewton is not built; use GlobalOptimizationLevenbergMarquardt')
+  if not (method is None or isinstance(method, GlobalOptimizationLevenbergMarquardt)):
+    raise TypeError(f'expected a global optimisation method, got {type(method).__name__}')
+  criteria = GlobalOptimizationConvergenceCriteria() if criteria is None else criteria
+  option = GlobalOptimizationOption() if option is None else option
+  poses, ends, T, info, unc, conf = _pose_graph_arrays(pose_graph, option)
+  out, kept, lp, stats = _abi.pose_graph_optimize(
+      poses, ends, T, info, unc, conf, option.max_correspondence_distance, option.edge_prune_threshold,
+      option.preference_loop_closure, option.reference_node, criteria.max_iteration, criteria.min_relative_increment,
+      criteria.min_relative_residual_increment, criteria.min_right_term, criteria.min_residual,
+      criteria.max_iteration_lm, criteria.upper_scale_factor, criteria.lower_scale_factor)
+  for node, P in zip(pose_graph.nodes, out):
+    node.pose = P.copy()
+  for edge, l in zip(pose_graph.edges, lp):
+    if edge.uncertain:
+      edge.confidence = float(l)
+  pose_graph.edges = [e for e, k in zip(pose_graph.edges, kept) if k]
+  return stats

@@ -45,7 +45,7 @@ def _open3d_stub():
   (pipelines.registration.registration_icp / registration_ransac_based_on_correspondence /
   registration_ransac_based_on_feature_matching, Feature, utility vectors; plus
   registration_fast_based_on_feature_matching / FastGlobalRegistrationOption / compute_fpfh_feature for FGR and
-  FPFH users, and
+  FPFH users, the pose graph and global_optimization for multiway registration, and
   TransformationEstimationPointToPlane with geometry.KDTreeSearchParamHybrid for point-to-plane ICP users) backed
   by libdgr_b200 (o3d_registration.py) - so the reference's OWN DeepGlobalRegistration class and demo.py run on
   this stack unmodified.  This package's DeepGlobalRegistration does not go through here: it calls the library."""
@@ -73,7 +73,10 @@ def _open3d_stub():
                'CorrespondenceCheckerBasedOnDistance', 'CorrespondenceCheckerBasedOnEdgeLength', 'Feature',
                'RegistrationResult', 'registration_icp', 'registration_ransac_based_on_correspondence',
                'registration_ransac_based_on_feature_matching', 'FastGlobalRegistrationOption',
-               'registration_fast_based_on_feature_matching', 'compute_fpfh_feature'):
+               'registration_fast_based_on_feature_matching', 'compute_fpfh_feature',
+               'get_information_matrix_from_point_clouds', 'PoseGraph', 'PoseGraphNode', 'PoseGraphEdge',
+               'GlobalOptimizationLevenbergMarquardt', 'GlobalOptimizationGaussNewton',
+               'GlobalOptimizationConvergenceCriteria', 'GlobalOptimizationOption', 'global_optimization'):
     setattr(o3d.pipelines.registration, name, getattr(reg, name))
   o3d.registration = o3d.pipelines.registration          # the pre-0.12 module path
   sys.modules['open3d.pipelines'] = o3d.pipelines

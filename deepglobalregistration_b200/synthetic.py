@@ -364,3 +364,101 @@ def feature_matching_pair(seed, n=2000, match_frac=0.3, spacing=0.1, noise=0.003
   wrong = (perm + g.integers(1, n, size=n)) % n
   fs = ft[np.where(ident, perm, wrong)] + g.normal(0, 1e-3, size=(n, dim))
   return P, tgt.astype(np.float32), fs.astype(np.float32), ft.astype(np.float32), T, perm, ident
+
+
+# --------------------------------------------------------------------------- #
+# multiway registration
+# --------------------------------------------------------------------------- #
+def _rot_z(a):
+  c, s = math.cos(a), math.sin(a)
+  return np.array([[c, -s, 0.0], [s, c, 0.0], [0.0, 0.0, 1.0]])
+
+
+def room_fragments(seed, n_frag=6, n_raw=120_000, radius=1.9, extent=(3.6, 3.0, 2.5), loop=(0.7, 0.55),
+                   noise=0.003):
+  """Fragments of one ``room_boxes`` room seen from cameras on a loop inside it.  Camera k sits at angle 2 pi k /
+  n_frag on an ellipse of half-axes `loop` [m] around the room's centre, 1.2 m up, turned by that angle about z (plus
+  a seeded tilt of up to 5 degrees).  Fragment k holds its own surface samples (n_raw over the whole room, seed and k
+  fixing them) within `radius` of camera k, expressed in camera k's frame: consecutive fragments overlap strongly and
+  the last closes the loop onto the first.  -> (clouds [n_frag] float64 [n_k, 3], P [n_frag, 4, 4] mapping each
+  fragment into the room frame)."""
+  boxes = room_boxes(seed, extent)
+  ex = np.asarray(extent, float)
+  rng = np.random.default_rng(30_000 + seed)
+  clouds, poses = [], []
+  for k in range(n_frag):
+    th = 2 * math.pi * k / n_frag
+    cam = np.array([ex[0] / 2 + loop[0] * math.cos(th), ex[1] / 2 + loop[1] * math.sin(th), 1.2])
+    tilt = random_se3(rng, 5.0, 0.0)[:3, :3]
+    P = np.eye(4)
+    P[:3, :3] = _rot_z(th) @ tilt
+    P[:3, 3] = cam
+    pts = _sample_boxes(boxes, n_raw, np.random.default_rng(31_000 + 100 * seed + k), noise)
+    pts = pts[np.linalg.norm(pts - cam, axis=1) < radius]
+    clouds.append((pts - cam) @ P[:3, :3])                # P^-1 x
+    poses.append(P)
+  return clouds, np.stack(poses)
+
+
+def _exp6(x):
+  """[Rz(x2) Ry(x1) Rx(x0) | x3..5] (open3d's TransformVector6dToMatrix4d)."""
+  ca, sa, cb, sb = math.cos(x[0]), math.sin(x[0]), math.cos(x[1]), math.sin(x[1])
+  Ry = np.array([[cb, 0, sb], [0, 1.0, 0], [-sb, 0, cb]])
+  Rx = np.array([[1.0, 0, 0], [0, ca, -sa], [0, sa, ca]])
+  T = np.eye(4)
+  T[:3, :3] = _rot_z(x[2]) @ Ry @ Rx
+  T[:3, 3] = x[3:6]
+  return T
+
+
+def information_from_points(q):
+  """Closed-form information matrix of matched target points q [n, 3]: sum of G^T G, G = [[q]x^T | I]."""
+  q = np.asarray(q, np.float64).reshape(-1, 3)
+  S, Q = q.sum(0), q.T @ q
+  Sx = np.array([[0, -S[2], S[1]], [S[2], 0, -S[0]], [-S[1], S[0], 0]])
+  L = np.zeros((6, 6))
+  L[:3, :3] = np.trace(Q) * np.eye(3) - Q
+  L[:3, 3:], L[3:, :3] = Sx, Sx.T
+  L[3:, 3:] = len(q) * np.eye(3)
+  return L
+
+
+def pose_graph(seed, n_nodes, n_loops, noise=0.01, n_wrong=0, n_corr=(200, 2000)):
+  """A pose graph with known answer.  Ground truth: a random walk of poses (<= 20 deg, <= 0.5 m per step) from the
+  identity.  Edges: odometry (k, k + 1) (certain), then n_loops distinct loop closures (i, j), j > i + 1 (uncertain),
+  each X = P_j^-1 P_i perturbed on the left by Exp(noise * N(0, 1)^6); then n_wrong of the loop closures made grossly
+  wrong (an extra rotation >= 30 deg about a random axis and a shift >= 1 m).  Information matrices: the closed form on
+  n_corr[0]..n_corr[1] points uniform in a 2 m cube.
+  -> dict(poses_gt [n, 4, 4], ends [E, 2], T [E, 4, 4], info [E, 6, 6], uncertain [E], wrong [E])."""
+  rng = np.random.default_rng(40_000 + seed)
+  P = [np.eye(4)]
+  for _ in range(n_nodes - 1):
+    P.append(P[-1] @ random_se3(rng, 20.0, 0.5))
+  P = np.stack(P)
+  cand = [(i, j) for i in range(n_nodes) for j in range(i + 2, n_nodes)]
+  if n_loops > len(cand):
+    raise ValueError(f'{n_loops} loop closures asked, {len(cand)} possible')
+  loops = [cand[k] for k in sorted(rng.choice(len(cand), n_loops, replace=False))] if n_loops else []
+  ends = [(k, k + 1) for k in range(n_nodes - 1)] + loops
+  E = len(ends)
+  unc = np.array([j != i + 1 for i, j in ends], bool)
+  wrong = np.zeros(E, bool)
+  if n_wrong:
+    wrong[np.flatnonzero(unc)[rng.choice(int(unc.sum()), n_wrong, replace=False)]] = True
+  T, info = [], []
+  for e, (i, j) in enumerate(ends):
+    X = _exp6(noise * rng.normal(size=6)) @ np.linalg.inv(P[j]) @ P[i]
+    if wrong[e]:
+      ax = rng.normal(size=3)
+      ax /= np.linalg.norm(ax)
+      ang = math.radians(rng.uniform(30.0, 90.0))
+      K = np.array([[0, -ax[2], ax[1]], [ax[2], 0, -ax[0]], [-ax[1], ax[0], 0]])
+      B = np.eye(4)
+      B[:3, :3] = np.eye(3) + math.sin(ang) * K + (1 - math.cos(ang)) * (K @ K)
+      d = rng.normal(size=3)
+      B[:3, 3] = d / np.linalg.norm(d) * rng.uniform(1.0, 2.0)
+      X = B @ X
+    T.append(X)
+    info.append(information_from_points(rng.uniform(-1.0, 1.0, size=(int(rng.integers(*n_corr)), 3))))
+  return dict(poses_gt=P, ends=np.array(ends, np.int64).reshape(E, 2), T=np.stack(T) if E else np.zeros((0, 4, 4)),
+              info=np.stack(info) if E else np.zeros((0, 6, 6)), uncertain=unc, wrong=wrong)

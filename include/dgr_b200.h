@@ -226,6 +226,45 @@ int32_t dgr_icp(const float* src, int64_t n_src, const float* tgt, const float* 
                 const double* T_init, int32_t max_iter, double rel_fitness, double rel_rmse, double* ws,
                 double* result, void* stream);
 
+/* ---- Multiway registration: open3d's GetInformationMatrixFromPointClouds and GlobalOptimization with
+ *      GlobalOptimizationLevenbergMarquardt (csrc/posegraph.cu; oracle/pose_graph.py) ---------------------- */
+/* Information matrix of the registered pair (src, tgt) under the 4x4 pose T (HOST double[16], row-major, mapping src
+ * into tgt): every source point's nearest target point q strictly within max_dist of T s, through the TARGET's voxel
+ * hash as dgr_icp searches it (max_dist / cell <= 4, lower row on a tie), adds G^T G with
+ * G = [[0, z, -y, 1, 0, 0], [-z, 0, x, 0, 1, 0], [y, -x, 0, 0, 0, 1]], q = (x, y, z).  Computed from the ten sums
+ * n, sum q, sum q q^T in fp64, per-CTA partials added in a fixed order: the same bits on every run.
+ * ws: dgr_information_matrix_ws_elems(n_src) doubles; out: device double[37] = the 6x6 matrix (row-major), n. */
+int32_t dgr_information_matrix_ws_elems(int64_t n_src, int64_t* n_elems);
+int32_t dgr_information_matrix(const float* src, int64_t n_src, const float* tgt, const dgr_keyspec_t* spec,
+                               const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch, double cell,
+                               double max_dist, const double* T, double* ws, double* out, void* stream);
+/* Pose-graph optimisation of Choi, Zhou & Koltun (CVPR 2015) as open3d's GlobalOptimization runs it: a
+ * Levenberg-Marquardt pass over all edges with line processes on the uncertain ones, the uncertain edges whose line
+ * process ends below edge_prune_threshold pruned, a second pass over the rest, then (reference_node >= 0) every pose
+ * moved so that the reference node keeps its input pose.  Node k's pose maps fragment k into the world; edge e =
+ * (ends[2e], ends[2e+1]) = (s, t) with T[e] mapping s into t and information Lambda[e]; the residual is
+ * v(T_e^-1 P_t^-1 P_s) with open3d's linearised 6-vector.  All inputs and outputs are HOST arrays (row-major 4x4
+ * poses [n_nodes][16], T [n_edges][16], info [n_edges][36]); confidence[e] is the line process an uncertain edge
+ * starts from.  Every argument is checked before the device is touched.  One launch on one CTA, no atomics: the same
+ * bits on every run; the call synchronises `stream` and returns after one device-to-host copy.
+ * Outputs: poses_out [n_nodes][16], kept_out [n_edges] (0 = pruned), l_out [n_edges] (final line process; 1 for the
+ * certain edges), stats [DGR_POSE_GRAPH_STATS] = iterations of pass 1, of pass 2, final cost, pruned edges, status
+ * (0, or 1 when a factorisation met a pivot that was not positive: the poses are those of the last accepted step),
+ * mu of pass 1, mu of pass 2, cost at the start of pass 1, cost at the end of pass 1, factorisations, 6 zeros.
+ * ws: dgr_pose_graph_ws_elems(n_nodes, n_edges) 8-byte words (dominated by the dense (6 n_nodes)^2 fp64 matrix). */
+#define DGR_POSE_GRAPH_MAX_NODES 256
+#define DGR_POSE_GRAPH_MAX_EDGES 32640    /* every pair of 256 nodes */
+#define DGR_POSE_GRAPH_STATS 16
+int32_t dgr_pose_graph_ws_elems(int64_t n_nodes, int64_t n_edges, int64_t* n_elems);
+int32_t dgr_pose_graph_optimize(const double* poses, int64_t n_nodes, const int32_t* ends, const double* T,
+                                const double* info, const int32_t* uncertain, const double* confidence,
+                                int64_t n_edges, double max_correspondence_distance, double edge_prune_threshold,
+                                double preference_loop_closure, int32_t reference_node, int32_t max_iteration,
+                                double min_relative_increment, double min_relative_residual_increment,
+                                double min_right_term, double min_residual, int32_t max_iteration_lm,
+                                double upper_scale_factor, double lower_scale_factor, uint64_t* ws, double* poses_out,
+                                int32_t* kept_out, double* l_out, double* stats, void* stream);
+
 /* ---- Safeguard RANSAC (SURVEY 8f rank 2): open3d registration_ransac_based_on_correspondence as
  *      called at core/deep_global_registration.py:50-64 (from :302-315) ---------------------- */
 /* Correspondence i pairs x[idx0[i]] with y[idx1[i]] (a null index array means i itself).
