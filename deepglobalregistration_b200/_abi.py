@@ -67,6 +67,14 @@ SIGNATURES = {
     'dgr_pose_graph_ws_elems': [_i64, _i64, _p],
     'dgr_pose_graph_optimize': [_p, _i64, _p, _p, _p, _p, _p, _i64, _f64, _f64, _f64, _i32, _i32, _f64, _f64, _f64,
                                 _f64, _i32, _f64, _f64, _p, _p, _p, _p, _p, _p],
+    'dgr_tsdf_touch_ws_elems': [_i32, _i32, _i32, _f64, _f64, _p, _p],
+    'dgr_tsdf_touch': [_p, _i32, _i32, _p, _p, _f64, _f64, _i32, _i32, _p, _p, _i64, _p, _i64, _i32, _p, _p, _p, _p],
+    'dgr_tsdf_rehash': [_p, _i32, _p, _p, _i64, _p],
+    'dgr_tsdf_integrate': [_p, _p, _i32, _i32, _p, _p, _f64, _f64, _i32, _p, _p, _i32, _p, _p, _p, _i64, _p],
+    'dgr_tsdf_extract_ws_elems': [_i64, _p],
+    'dgr_tsdf_extract_count': [_p, _i32, _p, _p, _i64, _p, _p, _i32, _p, _p, _p],
+    'dgr_tsdf_extract_write': [_p, _i32, _p, _p, _f64, _p, _p, _p, _p, _p],
+    'dgr_tsdf_mc_tables': [_p, _p],
     'dgr_ransac_ws_elems': [_i64, _i64, _p],
     'dgr_ransac_correspondence': [_p, _p, _p, _p, _i64, _f64, _i64, C.c_uint64, _p, _p, _p],
     'dgr_ransac_fm_ws_elems': [_i64, _i64, _i64, _p],
@@ -986,3 +994,83 @@ def pointnetlk(src, tgt, packed, delta=1e-2, max_iter=10, xtol=1e-7, return_jaco
        float(xtol), ptr(ws), ptr(jac), ptr(log), ptr(res), stream())
   out = (res,) + ((jac,) if return_jacobian else ()) + ((log,) if return_log else ())
   return out if len(out) > 1 else res
+
+
+# --------------------------------------------------------------------------- #
+# RGB-D fusion (csrc/tsdf.cu): the device half of o3d_integration.ScalableTSDFVolume
+# --------------------------------------------------------------------------- #
+TSDF_RES = 16
+
+
+def _host_f64(a, n, name):
+  a = np.ascontiguousarray(np.asarray(a, dtype=np.float64).reshape(-1))
+  if a.size != n:
+    raise DgrError(f'{name}: expected {n} values, got {a.size}')
+  return a
+
+
+def tsdf_touch_ws(width, height, stride, voxel_length, sdf_trunc):
+  """-> (candidate units per frame, workspace words) of dgr_tsdf_touch."""
+  n_cand, words = C.c_int64(0), C.c_int64(0)
+  call('dgr_tsdf_touch_ws_elems', int(width), int(height), int(stride), float(voxel_length), float(sdf_trunc),
+       C.byref(n_cand), C.byref(words))
+  return n_cand.value, words.value
+
+
+def tsdf_touch(depth, intr, pose, voxel_length, sdf_trunc, stride, keys, vals, unit_keys, n_total, touched, counts,
+               ws):
+  """Units touched by the CUDA float32 depth [H, W] from camera_pose `pose` (4x4 host); new ones are appended to the
+  volume (table keys / vals, unit_keys [cap, 3]).  touched / counts (int32 [3]) are written; no host read."""
+  _chk(depth, torch.float32, 'depth')
+  intr = _host_f64(intr, 4, 'intr')
+  pose = _host_f64(np.asarray(pose, dtype=np.float64).reshape(4, 4)[:3], 12, 'pose')
+  call('dgr_tsdf_touch', ptr(depth), depth.shape[1], depth.shape[0], intr.ctypes.data_as(C.c_void_p),
+       pose.ctypes.data_as(C.c_void_p), float(voxel_length), float(sdf_trunc), TSDF_RES, int(stride), ptr(keys),
+       ptr(vals), keys.numel(), ptr(unit_keys), unit_keys.shape[0], int(n_total), ptr(touched), ptr(counts), ptr(ws),
+       stream())
+
+
+def tsdf_rehash(unit_keys, n_total, keys, vals):
+  call('dgr_tsdf_rehash', ptr(unit_keys), int(n_total), ptr(keys), ptr(vals), keys.numel(), stream())
+
+
+def tsdf_integrate(depth, color, intr, extrinsic, voxel_length, sdf_trunc, unit_keys, touched, n_touched, tsdf,
+                   weight, rgb):
+  """Integrate one frame (depth CUDA float32 [H, W], color CUDA uint8 [H, W, 3] or None) into the touched units."""
+  _chk(depth, torch.float32, 'depth')
+  if color is not None:
+    _chk(color, torch.uint8, 'color')
+    if tuple(color.shape) != (depth.shape[0], depth.shape[1], 3):
+      raise DgrError(f'color: expected {(depth.shape[0], depth.shape[1], 3)}, got {tuple(color.shape)}')
+  intr = _host_f64(intr, 4, 'intr')
+  ext = _host_f64(np.asarray(extrinsic, dtype=np.float64).reshape(4, 4)[:3], 12, 'extrinsic')
+  call('dgr_tsdf_integrate', ptr(depth), ptr(color), depth.shape[1], depth.shape[0], intr.ctypes.data_as(C.c_void_p),
+       ext.ctypes.data_as(C.c_void_p), float(voxel_length), float(sdf_trunc), TSDF_RES, ptr(unit_keys), ptr(touched),
+       int(n_touched), ptr(tsdf), ptr(weight), ptr(rgb), tsdf.shape[0], stream())
+
+
+def tsdf_extract(unit_keys, n_units, keys, vals, tsdf, weight, rgb, voxel_length):
+  """Marching cubes over the first n_units slots (one host read).  -> (vertices [nv, 3] f64, colours [nv, 3] f64 or
+  None, triangles [nt, 3] int32), CUDA tensors in canonical order."""
+  dev = tsdf.device
+  words = C.c_int64(0)
+  call('dgr_tsdf_extract_ws_elems', int(n_units), C.byref(words))
+  ws = torch.empty(max(words.value, 1), dtype=torch.int64, device=dev)
+  totals = torch.empty(2, dtype=torch.int32, device=dev)
+  call('dgr_tsdf_extract_count', ptr(unit_keys), int(n_units), ptr(keys), ptr(vals), keys.numel(), ptr(tsdf),
+       ptr(weight), TSDF_RES, ptr(ws), ptr(totals), stream())
+  nv, nt = (int(v) for v in totals.cpu())
+  verts = torch.empty(nv, 3, dtype=torch.float64, device=dev)
+  cols = torch.empty(nv, 3, dtype=torch.float64, device=dev) if rgb is not None else None
+  tris = torch.empty(nt, 3, dtype=torch.int32, device=dev)
+  call('dgr_tsdf_extract_write', ptr(unit_keys), int(n_units), ptr(tsdf), ptr(rgb), float(voxel_length), ptr(ws),
+       ptr(verts), ptr(cols), ptr(tris), stream())
+  return verts, cols, tris
+
+
+def tsdf_mc_tables():
+  """-> (edge_table [256], tri_table [256, 16]) int32 numpy: the library's marching-cubes tables."""
+  edge = np.zeros(256, np.int32)
+  tri = np.zeros((256, 16), np.int32)
+  call('dgr_tsdf_mc_tables', edge.ctypes.data_as(C.c_void_p), tri.ctypes.data_as(C.c_void_p))
+  return edge, tri

@@ -274,3 +274,233 @@ def write_trajectory(filename, poses):
       fh.write(' '.join(str(int(m)) for m in meta) + '\n')
       for row in np.asarray(mat, dtype=np.float64):
         fh.write(' '.join(f'{x:.17g}' for x in row) + '\n')
+
+
+# ------------------------------------------------------------------------------------------
+# PNG (3DMatch raw RGB-D frames) and triangle meshes (fragments fused from them)
+# ------------------------------------------------------------------------------------------
+_PNG_SIG = b'\x89PNG\r\n\x1a\n'
+_PNG_KINDS = {(8, 2): (np.dtype('u1'), 3), (16, 0): (np.dtype('>u2'), 1)}   # (bit depth, colour type) -> (dtype, C)
+
+
+def _png_paeth_row(line, prev, bpp):
+  out, prev = bytearray(line), bytes(prev)
+  for i in range(len(out)):
+    a = out[i - bpp] if i >= bpp else 0
+    b = prev[i]
+    c = prev[i - bpp] if i >= bpp else 0
+    p = a + b - c
+    pa, pb, pc = abs(p - a), abs(p - b), abs(p - c)
+    out[i] = (out[i] + (a if pa <= pb and pa <= pc else b if pb <= pc else c)) & 0xFF
+  return np.frombuffer(bytes(out), np.uint8)
+
+
+def _png_average_row(line, prev, bpp):
+  out, prev = bytearray(line), bytes(prev)
+  for i in range(len(out)):
+    a = out[i - bpp] if i >= bpp else 0
+    out[i] = (out[i] + ((a + prev[i]) >> 1)) & 0xFF
+  return np.frombuffer(bytes(out), np.uint8)
+
+
+def read_png(path):
+  """A non-interlaced 8-bit RGB ([H, W, 3] uint8) or 16-bit greyscale ([H, W] uint16) PNG, the two kinds 3DMatch's
+  raw colour and depth frames use; filters 0-4.  Anything else, a bad CRC or truncated data raises ValueError."""
+  import zlib
+  with open(path, 'rb') as fh:
+    buf = fh.read()
+  if buf[:8] != _PNG_SIG:
+    raise ValueError(f'{path}: not a PNG file')
+  pos, ihdr, idat, ended = 8, None, [], False
+  while pos + 12 <= len(buf):
+    n = int.from_bytes(buf[pos:pos + 4], 'big')
+    kind, data = buf[pos + 4:pos + 8], buf[pos + 8:pos + 8 + n]
+    if len(data) != n or pos + 12 + n > len(buf):
+      raise ValueError(f'{path}: truncated {kind!r} chunk')
+    if zlib.crc32(kind + data) != int.from_bytes(buf[pos + 8 + n:pos + 12 + n], 'big'):
+      raise ValueError(f'{path}: CRC mismatch in {kind!r} chunk')
+    pos += 12 + n
+    if kind == b'IHDR':
+      if n != 13:
+        raise ValueError(f'{path}: bad IHDR')
+      ihdr = data
+    elif kind == b'IDAT':
+      idat.append(data)
+    elif kind == b'IEND':
+      ended = True
+      break
+  if ihdr is None or not ended:
+    raise ValueError(f'{path}: missing IHDR or IEND')
+  W, H = int.from_bytes(ihdr[0:4], 'big'), int.from_bytes(ihdr[4:8], 'big')
+  depth, ctype, comp, filt, interlace = ihdr[8], ihdr[9], ihdr[10], ihdr[11], ihdr[12]
+  if (depth, ctype) not in _PNG_KINDS:
+    raise ValueError(f'{path}: unsupported PNG kind (bit depth {depth}, colour type {ctype}); '
+                     'only 8-bit RGB and 16-bit greyscale are read')
+  if comp != 0 or filt != 0 or interlace != 0 or W == 0 or H == 0:
+    raise ValueError(f'{path}: unsupported PNG (compression {comp}, filter method {filt}, interlace {interlace})')
+  dt, ch = _PNG_KINDS[(depth, ctype)]
+  bpp = ch * dt.itemsize
+  stride = W * bpp
+  try:
+    raw = zlib.decompress(b''.join(idat))
+  except zlib.error as e:
+    raise ValueError(f'{path}: corrupt image data ({e})') from None
+  if len(raw) != H * (stride + 1):
+    raise ValueError(f'{path}: image data has {len(raw)} bytes, expected {H * (stride + 1)}')
+  rows = np.frombuffer(raw, np.uint8).reshape(H, stride + 1)
+  out = np.zeros((H, stride), np.uint8)
+  prev = np.zeros(stride, np.uint8)
+  for r in range(H):
+    f, line = rows[r, 0], rows[r, 1:]
+    if f == 0:
+      cur = line
+    elif f == 1:
+      cur = (np.cumsum(line.reshape(W, bpp), axis=0, dtype=np.uint64) & 0xFF).astype(np.uint8).reshape(-1)
+    elif f == 2:
+      cur = line + prev
+    elif f == 3:
+      cur = _png_average_row(line, prev, bpp)
+    elif f == 4:
+      cur = _png_paeth_row(line, prev, bpp)
+    else:
+      raise ValueError(f'{path}: bad filter type {f} on row {r}')
+    out[r] = cur
+    prev = out[r]
+  img = out.view(dt).reshape(H, W, ch) if ch > 1 else out.view(dt).reshape(H, W)
+  return img.astype(dt.newbyteorder('='))
+
+
+def write_png(path, img, filter_type=1):
+  """Write [H, W, 3] uint8 as 8-bit RGB or [H, W] uint16 as 16-bit greyscale; every row uses `filter_type` (0-4)."""
+  import zlib
+  img = np.asarray(img)
+  if img.dtype == np.uint8 and img.ndim == 3 and img.shape[2] == 3:
+    depth, ctype, data = 8, 2, img
+  elif img.dtype == np.uint16 and img.ndim == 2:
+    depth, ctype, data = 16, 0, img.astype('>u2')
+  else:
+    raise ValueError(f'write_png takes [H, W, 3] uint8 or [H, W] uint16, got {img.dtype} {img.shape}')
+  if filter_type not in range(5):
+    raise ValueError(f'filter_type must be 0..4, got {filter_type}')
+  H, W = img.shape[:2]
+  bpp = data.dtype.itemsize * (3 if ctype == 2 else 1)
+  x = np.ascontiguousarray(data).view(np.uint8).reshape(H, W * bpp).astype(np.int32)
+  a = np.zeros_like(x)
+  a[:, bpp:] = x[:, :-bpp]
+  b = np.zeros_like(x)
+  b[1:] = x[:-1]
+  c = np.zeros_like(x)
+  c[1:, bpp:] = x[:-1, :-bpp]
+  if filter_type == 0:
+    pred = np.zeros_like(x)
+  elif filter_type == 1:
+    pred = a
+  elif filter_type == 2:
+    pred = b
+  elif filter_type == 3:
+    pred = (a + b) >> 1
+  else:
+    p = a + b - c
+    pa, pb, pc = np.abs(p - a), np.abs(p - b), np.abs(p - c)
+    pred = np.where((pa <= pb) & (pa <= pc), a, np.where(pb <= pc, b, c))
+  rows = np.empty((H, W * bpp + 1), np.uint8)
+  rows[:, 0] = filter_type
+  rows[:, 1:] = ((x - pred) & 0xFF).astype(np.uint8)
+
+  def chunk(kind, payload):
+    return len(payload).to_bytes(4, 'big') + kind + payload + zlib.crc32(kind + payload).to_bytes(4, 'big')
+  ihdr = W.to_bytes(4, 'big') + H.to_bytes(4, 'big') + bytes([depth, ctype, 0, 0, 0])
+  with open(path, 'wb') as fh:
+    fh.write(_PNG_SIG + chunk(b'IHDR', ihdr) + chunk(b'IDAT', zlib.compress(rows.tobytes(), 6)) + chunk(b'IEND', b''))
+
+
+class Image:
+  """``open3d.geometry.Image``: an [H, W] or [H, W, C] array; ``np.asarray(img)`` returns it."""
+
+  def __init__(self, data=None):
+    self.data = np.ascontiguousarray(np.zeros((0, 0), np.uint8) if data is None else np.asarray(data))
+
+  def __array__(self, dtype=None, copy=None):
+    return self.data if dtype is None else self.data.astype(dtype)
+
+  @property
+  def width(self):
+    return self.data.shape[1]
+
+  @property
+  def height(self):
+    return self.data.shape[0]
+
+  def get_min_bound(self):
+    return np.zeros(2)
+
+  def get_max_bound(self):
+    """(width, height), as open3d returns it (util/integration.py:92)."""
+    return np.array([self.data.shape[1], self.data.shape[0]], dtype=np.float64)
+
+  def is_empty(self):
+    return self.data.size == 0
+
+  def __repr__(self):
+    return f'Image of size {self.width}x{self.height}, with {1 if self.data.ndim == 2 else self.data.shape[2]} channels.'
+
+
+def read_image(path):
+  """``o3d.io.read_image`` for PNG -> Image."""
+  return Image(read_png(path))
+
+
+class TriangleMesh:
+  """``open3d.geometry.TriangleMesh``: vertices [N, 3] float64, triangles [M, 3] int32, vertex_colors [N, 3] in
+  [0, 1] (empty when the mesh has none)."""
+
+  def __init__(self, vertices=None, triangles=None, vertex_colors=None):
+    self.vertices = np.zeros((0, 3)) if vertices is None else np.asarray(vertices, np.float64).reshape(-1, 3)
+    self.triangles = (np.zeros((0, 3), np.int32) if triangles is None
+                      else np.asarray(triangles, np.int32).reshape(-1, 3))
+    self.vertex_colors = (np.zeros((0, 3)) if vertex_colors is None
+                          else np.asarray(vertex_colors, np.float64).reshape(-1, 3))
+
+  def has_vertex_colors(self):
+    return len(self.vertex_colors) > 0 and len(self.vertex_colors) == len(self.vertices)
+
+  def is_empty(self):
+    return len(self.vertices) == 0
+
+  def __repr__(self):
+    return f'TriangleMesh with {len(self.vertices)} points and {len(self.triangles)} triangles.'
+
+
+def write_triangle_mesh(path, mesh, **kwargs):
+  """Binary little-endian PLY: the vertex element first (float x y z, uchar red green blue when the mesh has
+  colours, round(255 c) clipped), then ``face`` with ``list uchar int vertex_indices``.  read_point_cloud of the file
+  returns the vertices.  -> True (open3d's return)."""
+  V = np.asarray(mesh.vertices, np.float64).reshape(-1, 3)
+  T = np.asarray(mesh.triangles, np.int64).reshape(-1, 3)
+  cols = np.asarray(getattr(mesh, 'vertex_colors', np.zeros((0, 3))), np.float64).reshape(-1, 3)
+  has_c = len(cols) == len(V) and len(V) > 0
+  if len(T) and (T.min() < 0 or T.max() >= len(V)):
+    raise ValueError('triangle index out of range')
+  fields = [('x', '<f4'), ('y', '<f4'), ('z', '<f4')]
+  if has_c:
+    fields += [('red', 'u1'), ('green', 'u1'), ('blue', 'u1')]
+  rec = np.empty(len(V), dtype=fields)
+  for k, a in zip('xyz', V.T):
+    rec[k] = a
+  if has_c:
+    c8 = np.clip(np.round(cols * 255.0), 0, 255).astype(np.uint8)
+    for k, n in enumerate(('red', 'green', 'blue')):
+      rec[n] = c8[:, k]
+  face = np.empty(len(T), dtype=[('n', 'u1'), ('v', '<i4', (3,))])
+  face['n'] = 3
+  face['v'] = T
+  head = ['ply', 'format binary_little_endian 1.0', 'comment dgr-b200', f'element vertex {len(V)}',
+          'property float x', 'property float y', 'property float z']
+  if has_c:
+    head += ['property uchar red', 'property uchar green', 'property uchar blue']
+  head += [f'element face {len(T)}', 'property list uchar int vertex_indices', 'end_header']
+  with open(path, 'wb') as fh:
+    fh.write(('\n'.join(head) + '\n').encode('ascii'))
+    fh.write(rec.tobytes())
+    fh.write(face.tobytes())
+  return True

@@ -47,8 +47,11 @@ def _open3d_stub():
   registration_fast_based_on_feature_matching / FastGlobalRegistrationOption / compute_fpfh_feature for FGR and
   FPFH users, the pose graph and global_optimization for multiway registration, and
   TransformationEstimationPointToPlane with geometry.KDTreeSearchParamHybrid for point-to-plane ICP users) backed
-  by libdgr_b200 (o3d_registration.py) - so the reference's OWN DeepGlobalRegistration class and demo.py run on
-  this stack unmodified.  This package's DeepGlobalRegistration does not go through here: it calls the library."""
+  by libdgr_b200 (o3d_registration.py), and what util/integration.py fuses RGB-D frames with
+  (pipelines.integration.ScalableTSDFVolume, camera.PinholeCameraIntrinsic, geometry.Image / RGBDImage /
+  TriangleMesh, io.read_image / write_triangle_mesh; o3d_integration.py) - so the reference's OWN
+  DeepGlobalRegistration class, demo.py and util/integration.py run on this stack unmodified.  This package's
+  DeepGlobalRegistration does not go through here: it calls the library."""
   import numpy as np
 
   from . import io as dio
@@ -82,6 +85,22 @@ def _open3d_stub():
   sys.modules['open3d.pipelines'] = o3d.pipelines
   sys.modules['open3d.pipelines.registration'] = o3d.pipelines.registration
   sys.modules['open3d.registration'] = o3d.pipelines.registration
+  # RGB-D fusion (util/integration.py): pipelines.integration (integration before 0.12), camera, images, meshes
+  from . import o3d_integration as integ
+  o3d.pipelines.integration = types.ModuleType('open3d.pipelines.integration')
+  for name in ('ScalableTSDFVolume', 'TSDFVolumeColorType'):
+    setattr(o3d.pipelines.integration, name, getattr(integ, name))
+  o3d.integration = o3d.pipelines.integration
+  sys.modules['open3d.pipelines.integration'] = o3d.pipelines.integration
+  sys.modules['open3d.integration'] = o3d.pipelines.integration
+  o3d.camera = types.ModuleType('open3d.camera')
+  o3d.camera.PinholeCameraIntrinsic = integ.PinholeCameraIntrinsic
+  sys.modules['open3d.camera'] = o3d.camera
+  o3d.geometry.Image = dio.Image
+  o3d.geometry.RGBDImage = integ.RGBDImage
+  o3d.geometry.TriangleMesh = dio.TriangleMesh
+  o3d.io.read_image = dio.read_image
+  o3d.io.write_triangle_mesh = dio.write_triangle_mesh
   o3d.utility.VerbosityLevel = types.SimpleNamespace(Error=0, Warning=1, Info=2, Debug=3)
   o3d.utility.set_verbosity_level = lambda level: None
   o3d.visualization = types.ModuleType('open3d.visualization')

@@ -462,3 +462,134 @@ def pose_graph(seed, n_nodes, n_loops, noise=0.01, n_wrong=0, n_corr=(200, 2000)
     info.append(information_from_points(rng.uniform(-1.0, 1.0, size=(int(rng.integers(*n_corr)), 3))))
   return dict(poses_gt=P, ends=np.array(ends, np.int64).reshape(E, 2), T=np.stack(T) if E else np.zeros((0, 4, 4)),
               info=np.stack(info) if E else np.zeros((0, 6, 6)), uncertain=unc, wrong=wrong)
+
+
+# --------------------------------------------------------------------------- #
+# RGB-D sequences (fragment fusion)
+# --------------------------------------------------------------------------- #
+def _look_pose(pos, yaw, pitch):
+  """Camera-to-world pose of a camera at `pos` looking along (yaw, pitch); camera x right, y down, z forward."""
+  f = np.array([np.cos(yaw) * np.cos(pitch), np.sin(yaw) * np.cos(pitch), np.sin(pitch)])
+  r = np.cross(f, [0.0, 0.0, 1.0])
+  r /= np.linalg.norm(r)
+  d = np.cross(f, r)
+  T = np.eye(4)
+  T[:3, 0], T[:3, 1], T[:3, 2], T[:3, 3] = r, d, f, pos
+  return T
+
+
+def _face_colour(box, axis, side, p):
+  """Deterministic uint8 colour of a point p [n, 3] on face (axis, side) of box `box`: a per-face base colour and a
+  10 cm checker."""
+  base = np.array([(53 * box + 97 * axis + 151 * side) % 200 + 40, (89 * box + 31 * axis + 67 * side) % 200 + 40,
+                   (17 * box + 113 * axis + 29 * side) % 200 + 40], dtype=np.int32)
+  o = [a for a in range(3) if a != axis]
+  chk = (np.floor(p[:, o[0]] / 0.1).astype(np.int64) + np.floor(p[:, o[1]] / 0.1).astype(np.int64)) & 1
+  return np.clip(base[None, :] + np.where(chk[:, None] == 1, 25, -25), 0, 255).astype(np.uint8)
+
+
+def rgbd_sequence(seed, n_frames, width=640, height=480, extent=(3.6, 3.0, 2.5), max_depth=4.0, turn=0.5,
+                  radius=0.3, height_m=1.6, pitch=-0.35, focal=None):
+  """Ray-cast the room of room_boxes(seed) from a smooth camera path inside it (a circle of `radius` at height
+  `height_m`, the view turning by `turn` revolutions over the sequence).  Rays leave the room box and enter the
+  furniture boxes.  Depth is along the optical axis, quantised to uint16 millimetres, 0 beyond max_depth; colour is a
+  deterministic uint8 pattern per face.  Intrinsics are 3DMatch's (585, 585, W/2, H/2) at 640 wide; focal (default
+  585 W / 640) keeps the field of view at other widths.
+  -> (colors [n, H, W, 3] uint8, depths [n, H, W] uint16, poses [n, 4, 4] camera to world, (fx, fy, cx, cy))."""
+  boxes = room_boxes(seed, extent)
+  ex = np.asarray(extent, float)
+  f = 585.0 * width / 640.0 if focal is None else float(focal)
+  fx = fy = f
+  cx, cy = width / 2.0, height / 2.0
+  jj, ii = np.meshgrid(np.arange(width, dtype=np.float64), np.arange(height, dtype=np.float64))
+  dirs_c = np.stack([(jj - cx) / fx, (ii - cy) / fy, np.ones_like(jj)], -1).reshape(-1, 3)   # z = 1: t is depth
+  colors = np.zeros((n_frames, height, width, 3), np.uint8)
+  depths = np.zeros((n_frames, height, width), np.uint16)
+  poses = np.zeros((n_frames, 4, 4))
+  phase = 2 * np.pi * (seed % 7) / 7.0
+  for k in range(n_frames):
+    s = k / max(n_frames - 1, 1)
+    pos = np.array([ex[0] / 2 + radius * np.cos(2 * np.pi * s + phase), ex[1] / 2 + radius * np.sin(2 * np.pi * s + phase),
+                    height_m])
+    T = _look_pose(pos, phase + 2 * np.pi * turn * s, pitch)
+    poses[k] = T
+    d = dirs_c @ T[:3, :3].T
+    with np.errstate(divide='ignore', invalid='ignore'):
+      inv = 1.0 / d
+      t_best = np.full(len(d), np.inf)
+      hit_box = np.full(len(d), -1)
+      hit_ax = np.zeros(len(d), np.int64)
+      hit_side = np.zeros(len(d), np.int64)
+      for b, (lo, hi) in enumerate(boxes):
+        t1, t2 = (lo - pos) * inv, (hi - pos) * inv
+        tmin, tmax = np.minimum(t1, t2), np.maximum(t1, t2)
+        if b == 0:                                   # the room: the ray leaves through the nearest exit plane
+          t = np.min(np.where(np.isnan(tmax), np.inf, tmax), axis=1)
+          ax = np.argmin(np.where(np.isnan(tmax), np.inf, tmax), axis=1)
+          side = (d[np.arange(len(d)), ax] > 0).astype(np.int64)
+          ok = np.isfinite(t) & (t > 0)
+        else:                                        # furniture: the ray enters through the farthest entry plane
+          tn = np.max(np.where(np.isnan(tmin), -np.inf, tmin), axis=1)
+          tf = np.min(np.where(np.isnan(tmax), np.inf, tmax), axis=1)
+          ax = np.argmax(np.where(np.isnan(tmin), -np.inf, tmin), axis=1)
+          side = (d[np.arange(len(d)), ax] < 0).astype(np.int64)
+          t = tn
+          ok = (tn <= tf) & (tn > 0)
+        better = ok & (t < t_best)
+        t_best = np.where(better, t, t_best)
+        hit_box = np.where(better, b, hit_box)
+        hit_ax = np.where(better, ax, hit_ax)
+        hit_side = np.where(better, side, hit_side)
+    z = t_best                                        # depth along the optical axis (direction has z = 1)
+    mm = np.where(np.isfinite(z) & (z <= max_depth) & (hit_box >= 0), np.round(z * 1000.0), 0)
+    depths[k] = np.clip(mm, 0, 65535).astype(np.uint16).reshape(height, width)
+    p = pos[None, :] + np.where(np.isfinite(z), z, 0)[:, None] * d
+    col = np.zeros((len(d), 3), np.uint8)
+    for b in range(len(boxes)):
+      for ax in range(3):
+        for side in range(2):
+          m = (hit_box == b) & (hit_ax == ax) & (hit_side == side)
+          if m.any():
+            col[m] = _face_colour(b, ax, side, p[m])
+    colors[k] = col.reshape(height, width, 3)
+  return colors, depths, poses, (fx, fy, cx, cy)
+
+
+def write_rgbd_sequence(root, scene, colors, depths, poses, intrinsics, seq='seq-01'):
+  """Write a sequence in the 3DMatch raw layout: root/scene/seq/frame-000000.{color,depth}.png and .pose.txt, and
+  root/scene/camera-intrinsics.txt (the 3x3 K).  -> the sequence directory."""
+  import os
+
+  from .io import write_png
+  seq_dir = os.path.join(root, scene, seq)
+  os.makedirs(seq_dir, exist_ok=True)
+  fx, fy, cx, cy = intrinsics
+  np.savetxt(os.path.join(root, scene, 'camera-intrinsics.txt'), np.array([[fx, 0, cx], [0, fy, cy], [0, 0, 1]]))
+  for k in range(len(poses)):
+    stem = os.path.join(seq_dir, f'frame-{k:06d}')
+    write_png(stem + '.color.png', colors[k])
+    write_png(stem + '.depth.png', depths[k])
+    np.savetxt(stem + '.pose.txt', poses[k])
+  return seq_dir
+
+
+def box_face_distance(points, boxes):
+  """Distance of every point [n, 3] to the nearest face (a closed rectangle) of any box, and to the nearest box edge."""
+  p = np.asarray(points, np.float64)
+  face = np.full(len(p), np.inf)
+  edge = np.full(len(p), np.inf)
+  for lo, hi in boxes:
+    lo, hi = np.asarray(lo, float), np.asarray(hi, float)
+    q = np.clip(p, lo, hi)
+    for ax in range(3):
+      for v in (lo[ax], hi[ax]):
+        qf = q.copy()
+        qf[:, ax] = v
+        face = np.minimum(face, np.linalg.norm(p - qf, axis=1))
+      o = [a for a in range(3) if a != ax]
+      for v0 in (lo[o[0]], hi[o[0]]):
+        for v1 in (lo[o[1]], hi[o[1]]):
+          qe = q.copy()
+          qe[:, o[0]], qe[:, o[1]] = v0, v1
+          edge = np.minimum(edge, np.linalg.norm(p - qe, axis=1))
+  return face, edge

@@ -265,6 +265,54 @@ int32_t dgr_pose_graph_optimize(const double* poses, int64_t n_nodes, const int3
                                 double upper_scale_factor, double lower_scale_factor, uint64_t* ws, double* poses_out,
                                 int32_t* kept_out, double* l_out, double* stats, void* stream);
 
+/* ---- RGB-D fusion: open3d's ScalableTSDFVolume integrate / extract_triangle_mesh (util/integration.py:44-71),
+ *      csrc/tsdf.cu; oracle/tsdf.py is the arithmetic contract, met bit for bit ------------------------------- */
+/* Units of DGR_TSDF_RES^3 voxels (the only volume_unit_resolution supported) keyed by unit coordinate, each axis in
+ * [DGR_TSDF_COORD_MIN, DGR_TSDF_COORD_MAX] (3 x 21-bit keys).  The volume is owned by the caller:
+ *   table keys[cap] / vals[cap]  unit key -> slot, cap a power of two (cleared by dgr_hash_clear before first use);
+ *   unit_keys[slots][3] int32    unit coordinates in slot order (order of first touch);
+ *   tsdf / weight [slots][4096], rgb [slots][3][4096] fp32 slabs, zero for a slot never integrated.
+ * Voxel (x, y, z) of a unit has index (x * 16 + y) * 16 + z.  intr: host double[4] (fx, fy, cx, cy); pose /
+ * extrinsic: host double[12], rows 0..2 of a 4x4. */
+#define DGR_TSDF_RES 16
+#define DGR_TSDF_COORD_MIN (-1048576)
+#define DGR_TSDF_COORD_MAX 1048574
+/* Candidate units per frame (n_cand: samples x side^3, side = floor(2 sdf_trunc / (16 voxel_length)) + 2) and the
+ * 8-byte words of dgr_tsdf_touch's workspace. */
+int32_t dgr_tsdf_touch_ws_elems(int32_t width, int32_t height, int32_t stride, double voxel_length, double sdf_trunc,
+                                int64_t* n_cand, int64_t* n_elems);
+/* Units touched by a float depth image [height][width] (metres, 0 = none) seen from `pose` (camera to world):
+ * new units get slots n_total, n_total + 1, ... in first-touch order, are inserted in the table and written to
+ * unit_keys; touched[0, n_touched) lists every touched unit's slot in first-touch order.  counts: device int32[3] =
+ * (n_touched, n_total after the frame, 1 if a unit coordinate fell outside the key range).  Requires
+ * unit_cap >= n_total + n_cand and cap >= 2 (n_total + n_cand); touched holds n_cand.  No host read. */
+int32_t dgr_tsdf_touch(const float* depth, int32_t width, int32_t height, const double* intr, const double* pose,
+                       double voxel_length, double sdf_trunc, int32_t res, int32_t stride, uint64_t* table_keys,
+                       int32_t* table_vals, int64_t table_cap, int32_t* unit_keys, int64_t unit_cap, int32_t n_total,
+                       int32_t* touched, int32_t* counts, void* ws, void* stream);
+/* Clear the table and insert slots [0, n_total) of unit_keys (growing the table). */
+int32_t dgr_tsdf_rehash(const int32_t* unit_keys, int32_t n_total, uint64_t* table_keys, int32_t* table_vals,
+                        int64_t table_cap, void* stream);
+/* Integrate one frame into the n_touched touched units (extrinsic: world to camera).  color: device uint8
+ * [height][width][3] with rgb, or both NULL (NoColor).  The slabs must hold every slot in touched. */
+int32_t dgr_tsdf_integrate(const float* depth, const uint8_t* color, int32_t width, int32_t height, const double* intr,
+                           const double* extrinsic, double voxel_length, double sdf_trunc, int32_t res,
+                           const int32_t* unit_keys, const int32_t* touched, int32_t n_touched, float* tsdf,
+                           float* weight, float* rgb, int64_t slab_units, void* stream);
+/* Marching cubes over every unit: count, then write.  ws: dgr_tsdf_extract_ws_elems(n_units) 8-byte words, kept
+ * between the two calls; totals: device int32[2] = (vertices, triangles), read by the caller to size the outputs.
+ * write: vertices [nv][3] fp64 ordered by (slot, voxel, axis), colors [nv][3] fp64 in [0, 1] (NULL with rgb NULL),
+ * triangles [nt][3] int32 ordered by (slot, voxel, table order), wound (e[i], e[i+2], e[i+1]). */
+int32_t dgr_tsdf_extract_ws_elems(int64_t n_units, int64_t* n_elems);
+int32_t dgr_tsdf_extract_count(const int32_t* unit_keys, int32_t n_units, const uint64_t* table_keys,
+                               const int32_t* table_vals, int64_t table_cap, const float* tsdf, const float* weight,
+                               int32_t res, void* ws, int32_t* totals, void* stream);
+int32_t dgr_tsdf_extract_write(const int32_t* unit_keys, int32_t n_units, const float* tsdf, const float* rgb,
+                               double voxel_length, const void* ws, double* vertices, double* colors,
+                               int32_t* triangles, void* stream);
+/* Host copy of the marching-cubes tables: edge_table[256] (bit e: edge e changes sign), tri_table[256][16] (-1 pad). */
+int32_t dgr_tsdf_mc_tables(int32_t* edge_table, int32_t* tri_table);
+
 /* ---- Safeguard RANSAC (SURVEY 8f rank 2): open3d registration_ransac_based_on_correspondence as
  *      called at core/deep_global_registration.py:50-64 (from :302-315) ---------------------- */
 /* Correspondence i pairs x[idx0[i]] with y[idx1[i]] (a null index array means i itself).
