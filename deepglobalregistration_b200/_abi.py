@@ -1,5 +1,8 @@
 """ctypes binding of libdgr_b200.so (include/dgr_b200.h).
 
+Every entry point's argtypes / restype and the integer DGR_* constants are read from the
+header the library is compiled against, so the binding cannot drift from the C ABI.
+
 torch is used here for device memory and the current CUDA stream only; every
 computation happens inside the library.  There is no CPU fallback: importing this
 module without a built library, or calling into it without an sm_90 device,
@@ -8,14 +11,58 @@ raises.
 import ctypes as C
 import math
 import os
+import re
 
 import numpy as np
 import torch
 
+from .build import INCLUDE
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libdgr_b200.so')
+HEADER = os.path.join(INCLUDE, 'dgr_b200.h')
 
-MAX_COLS = 8
+
+class DgrError(RuntimeError):
+  pass
+
+
+# the only C types the binding maps; anything else (int, size_t, a struct by value) is an error, never a guessed width
+_SCALARS = {'int32_t': C.c_int32, 'int64_t': C.c_int64, 'uint64_t': C.c_uint64, 'float': C.c_float,
+            'double': C.c_double}
+
+
+def _ctype(decl, c_type, ret=False):
+  """ctypes type of the C type `c_type` of declaration `decl`: any pointer is c_void_p (c_char_p for a returned
+  const char*)."""
+  words = c_type.replace('*', ' * ').split()
+  if '*' in words:
+    return C.c_char_p if ret and words == ['const', 'char', '*'] else C.c_void_p
+  words = [w for w in words if w != 'const']
+  if len(words) != 1 or words[0] not in _SCALARS:
+    raise DgrError(f'{decl}: no ctypes type for {c_type.strip()!r}')
+  return _SCALARS[words[0]]
+
+
+def read_header(path):
+  """-> ({entry point: (restype, [argtypes])}, {DGR_* integer constant: value}) of a dgr_b200.h: every
+  `<type> dgr_name(<type> name, ...);` declaration and every `#define DGR_NAME <integer>`."""
+  with open(path) as fh:
+    src = re.sub(r'/\*.*?\*/|//[^\n]*', ' ', fh.read(), flags=re.S)
+  consts = {name: int(v.strip('()')) for name, v in
+            re.findall(r'^[ \t]*#[ \t]*define[ \t]+(DGR_\w+)[ \t]+(-?\d+|\(-?\d+\))[ \t]*$', src, re.M)}
+  src = re.sub(r'^[ \t]*#.*$', ' ', src, flags=re.M)
+  decls = {}
+  for ret, name, params in re.findall(r'([\w\s*]*?)\b(dgr_\w+)\s*\(([^;]*?)\)\s*;', src):
+    decl = ' '.join(f'{ret} {name}({params})'.split())
+    args = [] if params.strip() == 'void' else [_ctype(decl, re.sub(r'\w+\s*$', '', p)) for p in params.split(',')]
+    decls[name] = (_ctype(decl, ret, ret=True), args)
+  return decls, consts
+
+
+DECLARATIONS, _DEFINES = read_header(HEADER)
+
+MAX_COLS = _DEFINES['DGR_MAX_COLS']
 TILE_ROWS = 128
 KEY_MARGIN = 32     # spare cells around the bounding box: covers 7^3 kernels and stride-8 flooring
 
@@ -27,116 +74,17 @@ class KeySpec(C.Structure):
 
 KEYSPEC_INTS = C.sizeof(KeySpec) // 4
 
-_p, _i32, _i64, _f32, _f64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_double
-
-# name -> argtypes; every function returns int32 status unless listed in _RESTYPES
-SIGNATURES = {
-    'dgr_version': [],
-    'dgr_last_error': [],
-    'dgr_launch_count': [],
-    'dgr_device_check': [_i32],
-    'dgr_quantize_points': [_p, _i32, _i64, _f64, _i32, _p, _p, _p],
-    'dgr_coords_minmax': [_p, _i64, _i32, _p, _p],
-    'dgr_keyspec_build': [_p, _i32, _i32, _p, _p],
-    'dgr_hash_clear': [_p, _p, _i64, _p],
-    'dgr_unique_first': [_p, _i64, _i32, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _p],
-    'dgr_scan_ws_elems': [_i64],
-    'dgr_hash_find': [_p, _i64, _i32, _p, _p, _p, _i64, _p, _p],
-    'dgr_gather_rows_i32': [_p, _p, _i64, _i32, _p, _p],
-    'dgr_spconv_fwd': [_p, _i32, _p, _i32, _p, _p, _p, _p, _p, _i32, _i32, _i32, _p, _p],
-    'dgr_spconv_tc_supported': [_i32, _i32],
-    'dgr_pack_weight_tf32': [_p, _i32, _i32, _i32, _p, _p],
-    'dgr_spconv_tc_fwd': [_p, _i32, _p, _i32, _p, _p, _p, _p, _p, _i32, _i32, _i32, _p, _p],
-    'dgr_linear_fwd': [_p, _i32, _p, _i32, _i64, _p, _i32, _p, _i32, _i32, _p, _p],
-    'dgr_affine_act': [_p, _i64, _i32, _p, _p, _p, _i32, _p, _p],
-    'dgr_cat2': [_p, _i32, _p, _i32, _i64, _p, _p],
-    'dgr_l2_normalize': [_p, _i64, _i32, _p, _p],
-    'dgr_knn_top1': [_p, _i64, _p, _i64, _i32, _p, _p, _p, _p],
-    'dgr_knn_tc_supported': [_i32],
-    'dgr_knn_tc_ws_elems': [_i64, _i64, _i32],
-    'dgr_knn_top1_tc': [_p, _i64, _p, _i64, _i32, _p, _p, _p, _p, _p],
-    'dgr_inlier_coords': [_p, _p, _p, _i64, _p, _p],
-    'dgr_sigmoid_clip_sum': [_p, _i64, _f32, _p, _p, _p],
-    'dgr_estimate_normals': [_p, _i64, _p, _p, _p, _i64, _i32, _f64, _f64, _i32, _p, _p, _p, _p],
-    'dgr_fpfh_ws_elems': [_i64, _i32, _p],
-    'dgr_compute_fpfh': [_p, _p, _i64, _p, _p, _p, _i64, _i32, _f64, _f64, _i32, _i32, _p, _p, _p, _p],
-    'dgr_icp_ws_elems': [_i64, _p],
-    'dgr_icp': [_p, _i64, _p, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _p, _i32, _f64, _f64, _p, _p, _p],
-    'dgr_information_matrix_ws_elems': [_i64, _p],
-    'dgr_information_matrix': [_p, _i64, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _p, _p, _p, _p],
-    'dgr_pose_graph_ws_elems': [_i64, _i64, _p],
-    'dgr_pose_graph_optimize': [_p, _i64, _p, _p, _p, _p, _p, _i64, _f64, _f64, _f64, _i32, _i32, _f64, _f64, _f64,
-                                _f64, _i32, _f64, _f64, _p, _p, _p, _p, _p, _p],
-    'dgr_tsdf_touch_ws_elems': [_i32, _i32, _i32, _f64, _f64, _p, _p],
-    'dgr_tsdf_touch': [_p, _i32, _i32, _p, _p, _f64, _f64, _i32, _i32, _p, _p, _i64, _p, _i64, _i32, _p, _p, _p, _p],
-    'dgr_tsdf_rehash': [_p, _i32, _p, _p, _i64, _p],
-    'dgr_tsdf_integrate': [_p, _p, _i32, _i32, _p, _p, _f64, _f64, _i32, _p, _p, _i32, _p, _p, _p, _i64, _p],
-    'dgr_tsdf_extract_ws_elems': [_i64, _p],
-    'dgr_tsdf_extract_count': [_p, _i32, _p, _p, _i64, _p, _p, _i32, _p, _p, _p],
-    'dgr_tsdf_extract_write': [_p, _i32, _p, _p, _f64, _p, _p, _p, _p, _p],
-    'dgr_tsdf_mc_tables': [_p, _p],
-    'dgr_ransac_ws_elems': [_i64, _i64, _p],
-    'dgr_ransac_correspondence': [_p, _p, _p, _p, _i64, _f64, _i64, C.c_uint64, _p, _p, _p],
-    'dgr_ransac_fm_ws_elems': [_i64, _i64, _i64, _p],
-    'dgr_ransac_feature_matching': [_p, _i64, _p, _p, _p, _p, _p, _i64, _i32, _f64, _f64, _f64, _f64, _i64, _i64,
-                                    C.c_uint64, _p, _p, _p],
-    'dgr_fgr_ws_elems': [_i64, _i64, _i64, _i32, _p],
-    'dgr_fgr_feature_matching': [_p, _i64, _p, _i64, _p, _p, _f64, _i32, _i32, _f64, _i32, _f64, _i64, _i32, C.c_uint64,
-                                 _p, _p, _p, _p],
-    'dgr_goicp_dt_build': [_p, _i64, _p, _i64, _i32, _f64, _p, _p, _p, _p],
-    'dgr_goicp_ws_elems': [_i64, _i64, _i32, _i64, _i32, _p],
-    'dgr_goicp': [_p, _i64, _p, _i64, _f64, _f64, _i32, _f64, _p, _f64, _p, _f64, _i32, _i32, _i64, _p, _p, _p],
-    'dgr_super4pcs_ws_elems': [_i64, _i64, _i64, _i32, _i32, _i64, _i64, _i32, _p],
-    'dgr_super4pcs': [_p, _i64, _p, _i64, _i64, _f64, _f64, _f64, _i32, _f64, _i32, _i32, _i64, _i64, _i32, _f64,
-                      C.c_uint64, _p, _p, _p, _p],
-    'dgr_pointnet_pack': [_p, _p, _p],
-    'dgr_pointnet_forward': [_p, _i64, _p, _p, _i32, _p, _p, _p],
-    'dgr_pointnetlk_ws_elems': [_i64, _i64, _i32, _p],
-    'dgr_pointnetlk': [_p, _i64, _p, _i64, _p, _f64, _i32, _f64, _p, _p, _p, _p, _p],
-    'dgr_se3_register': [_p, _p, _p, _p, _i64, _f32, _i32, _i32, _f32, _f32, _f32, _p, _p, _p, _p],
-    # ---- round 2: coordinate planning with device-side counts (csrc/coordplan.cu) ----
-    'dgr_spconv_table_fwd_strided': [_p, _i32, _p, _i32, _p, _i32, _i64, _i64, _p, _p, _p, _p],
-    'dgr_compact_voxel_pair': [_p, _p, _p, _i64, _i64, _p, _i32, _p, _i32, _p, _p, _p, _p],
-    'dgr_table_build_unique': [_p, _i64, _p, _i32, _p, _p, _p, _i64, _p],
-    'dgr_coarse_maps': [_p, _i64, _p, _i32, _p, _i32, _p, _p, _p, _i64, _p, _p, _p, _p, _p],
-    'dgr_bloom2_build': [_p, _i64, _p, _i64, _p],
-    'dgr_bloom2_words': [_i64],
-    'dgr_kmap_mask_words': [_i64],
-    'dgr_kmap_cnt_elems': [_i32, _i64],
-    'dgr_kmap_probe': [_p, _i64, _p, _i32, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p, _p, _p, _p, _p],
-    'dgr_kmap_fill': [_p, _p, _i32, _i64, _p, _i32, _p, _p, _p, _i64, _p, _p, _p, _p],
-    'dgr_kernel_map_tiles': [_p, _i32, _i32, _i32, _i32, _p, _p, _p],
-    'dgr_kmap_dense': [_p, _i64, _p, _i32, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p, _i64, _p, _p],
-    'dgr_spconv_ones_bits_fwd': [_p, _i32, _p, _i64, _i32, _i64, _p, _p, _p, _p],
-    'dgr_spconv_wgrad': [_p, _i32, _p, _i32, _p, _p, _p, _i32, _p, _p],
-    'dgr_affine_act_amax': [_p, _i64, _i32, _p, _p, _p, _i32, _p, _p, _p],
-    'dgr_absmax_f32': [_p, _i64, _p, _p],
-    'dgr_spconv_tc_f16_supported': [_i32, _i32],
-    'dgr_pack_weight_f16': [_p, _i32, _i32, _i32, _p, _p, _p],
-    'dgr_spconv_tc_f16_fwd': [_p, _i32, _p, _i32, _p, _p, _p, _p, _p, _i32, _i32, _p, _p, _p, _p],
-    # ---- round 2: native executor (csrc/exec.cu) ----
-    'dgr_ctx_create': [_i32, _p, _p],
-    'dgr_ctx_destroy': [_p],
-    'dgr_ctx_stream': [_p],
-    'dgr_ctx_stats': [_p, _p],
-    'dgr_ctx_profile': [_p, _i32],
-    'dgr_ctx_profile_read': [_p, _p, _i64],
-    'dgr_ctx_stage_times': [_p, _p, _i32],
-    'dgr_net_create': [_i32, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _i32, _p, _p],
-    'dgr_net_destroy': [_p],
-    'dgr_net_forward': [_p, _p, _p, _i64, _p, _p],
-    'dgr_pair_register': [_p, _p, _p, _p, _i64, _i32, _p, _i64, _i32, _i32, _f64, _f32, _i32, _p],
-    'dgr_pair_safeguard': [_p, _f64, _i64, C.c_uint64, _i32, _p],
-    'dgr_pair_tap': [_p, _i32, _p, _p, _p],
-}
-_RESTYPES = {'dgr_kmap_mask_words': _i64, 'dgr_kmap_cnt_elems': _i64, 'dgr_ctx_stream': C.c_void_p,
-             'dgr_ctx_profile_read': _i64, 'dgr_last_error': C.c_char_p, 'dgr_knn_tc_ws_elems': _i64, 'dgr_launch_count': _i64, 'dgr_spconv_tc_supported': _i32, 'dgr_scan_ws_elems': _i64, 'dgr_bloom2_words': _i64}
-
 _lib = None
 
 
-class DgrError(RuntimeError):
-  pass
+def bind(path, names=None):
+  """Load a libdgr_b200.so and set argtypes / restype of the header's entry points (`names`: only these, so that
+  another build lacking newer entry points can be bound for comparison)."""
+  l = C.CDLL(path)
+  for name in DECLARATIONS if names is None else names:
+    fn = getattr(l, name)
+    fn.restype, fn.argtypes = DECLARATIONS[name]
+  return l
 
 
 def lib():
@@ -146,12 +94,7 @@ def lib():
     if not os.path.exists(LIB_PATH):
       raise DgrError(f'{LIB_PATH} is missing: run `python -m deepglobalregistration_b200.build` '
                      '(there is no CPU fallback)')
-    l = C.CDLL(LIB_PATH)
-    for name, args in SIGNATURES.items():
-      fn = getattr(l, name)
-      fn.argtypes = args
-      fn.restype = _RESTYPES.get(name, _i32)
-    _lib = l
+    _lib = bind(LIB_PATH)
   return _lib
 
 
@@ -200,7 +143,10 @@ def require_device(device):
 
 
 def ptr(t):
-  return 0 if t is None else t.data_ptr()
+  """Address of a tensor's or a host numpy array's data; 0 for None."""
+  if t is None:
+    return 0
+  return t.ctypes.data if isinstance(t, np.ndarray) else t.data_ptr()
 
 
 _STREAM = None
@@ -251,6 +197,13 @@ def scratch(name, numel, dtype, device):
     buf = torch.empty(max(int(numel * 1.25), 1024), dtype=dtype, device=device)
     _ARENA[key] = buf
   return buf[:numel]
+
+
+def workspace(name, dtype, device, query, *args):
+  """scratch(name) of the element count the dgr_*_ws_elems entry point `query` gives for args."""
+  n = C.c_int64(0)
+  call(query, *args, C.byref(n))
+  return scratch(name, n.value, dtype, device)
 
 
 # --------------------------------------------------------------------------- #
@@ -677,9 +630,7 @@ def compute_fpfh(xyz, normals, manager_or_table, cell, radius, max_nn, batch=0, 
     raise DgrError('normals must hold one normal per point')
   spec, table = _hash_of(manager_or_table)
   n = xyz.shape[0]
-  words = C.c_int64(0)
-  call('dgr_fpfh_ws_elems', n, int(max_nn), C.byref(words))
-  ws = scratch('fpfh', words.value, torch.int64, xyz.device)
+  ws = workspace('fpfh', torch.int64, xyz.device, 'dgr_fpfh_ws_elems', n, int(max_nn))
   out = torch.empty(max(n, 1), max(int(ld), 1), dtype=torch.float32, device=xyz.device)[:n]
   counts = torch.empty(max(n, 1), dtype=torch.int32, device=xyz.device)[:n]
   call('dgr_compute_fpfh', ptr(xyz), ptr(normals), n, ptr(spec), ptr(table.keys), ptr(table.vals), table.cap,
@@ -697,9 +648,7 @@ def _icp(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter, 
   spec, table = _hash_of(tgt_manager)
   if not (isinstance(T_init, torch.Tensor) and T_init.is_cuda and T_init.numel() == 12):
     T_init = torch.as_tensor(T_init, dtype=torch.float64).reshape(4, 4)[:3].contiguous().to(dev)
-  words = C.c_int64(0)
-  call('dgr_icp_ws_elems', src.shape[0], C.byref(words))
-  ws = scratch('icp', words.value, torch.float64, dev)
+  ws = workspace('icp', torch.float64, dev, 'dgr_icp_ws_elems', src.shape[0])
   res = torch.empty(20, dtype=torch.float64, device=dev)
   # ptr() of an empty tgt_normals is 0, which selects point-to-point; without target points neither update has a
   # correspondence, so both give the same result
@@ -733,17 +682,15 @@ def information_matrix(src, tgt, tgt_manager, cell, max_dist, T, batch=0):
   _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
   spec, table = _hash_of(tgt_manager)
   T = np.ascontiguousarray(np.asarray(T, dtype=np.float64).reshape(4, 4))
-  words = C.c_int64(0)
-  call('dgr_information_matrix_ws_elems', src.shape[0], C.byref(words))
-  ws = scratch('information', words.value, torch.float64, src.device)
+  ws = workspace('information', torch.float64, src.device, 'dgr_information_matrix_ws_elems', src.shape[0])
   out = torch.empty(37, dtype=torch.float64, device=src.device)
   call('dgr_information_matrix', ptr(src), src.shape[0], ptr(tgt), ptr(spec), ptr(table.keys), ptr(table.vals),
-       table.cap, int(batch), float(cell), float(max_dist), T.ctypes.data_as(C.c_void_p), ptr(ws), ptr(out), stream())
+       table.cap, int(batch), float(cell), float(max_dist), ptr(T), ptr(ws), ptr(out), stream())
   return out
 
 
-POSE_GRAPH_MAX_NODES = 256
-POSE_GRAPH_MAX_EDGES = 32640
+POSE_GRAPH_MAX_NODES = _DEFINES['DGR_POSE_GRAPH_MAX_NODES']
+POSE_GRAPH_MAX_EDGES = _DEFINES['DGR_POSE_GRAPH_MAX_EDGES']
 POSE_GRAPH_STATS = ('iterations', 'iterations_pruned', 'cost', 'pruned', 'status', 'mu', 'mu_pruned', 'cost_start',
                     'cost_first_pass', 'factorisations')
 
@@ -766,19 +713,16 @@ def pose_graph_optimize(poses, ends, T, info, uncertain, confidence, max_corresp
   unc = np.ascontiguousarray(np.asarray(uncertain, dtype=np.int32).reshape(e))
   conf = np.ascontiguousarray(np.asarray(confidence, dtype=np.float64).reshape(e))
   dev = require_device(device)
-  words = C.c_int64(0)
-  call('dgr_pose_graph_ws_elems', n, e, C.byref(words))
-  ws = scratch('pose_graph', words.value, torch.int64, dev)
+  ws = workspace('pose_graph', torch.int64, dev, 'dgr_pose_graph_ws_elems', n, e)
   out = np.zeros((max(n, 1), 16))
   kept = np.zeros(max(e, 1), dtype=np.int32)
   lp = np.zeros(max(e, 1))
   st = np.zeros(16)
-  vp = lambda a: a.ctypes.data_as(C.c_void_p)
-  call('dgr_pose_graph_optimize', vp(poses), n, vp(ends), vp(T), vp(info), vp(unc), vp(conf), e,
+  call('dgr_pose_graph_optimize', ptr(poses), n, ptr(ends), ptr(T), ptr(info), ptr(unc), ptr(conf), e,
        float(max_correspondence_distance), float(edge_prune_threshold), float(preference_loop_closure),
        int(reference_node), int(max_iteration), float(min_relative_increment), float(min_relative_residual_increment),
        float(min_right_term), float(min_residual), int(max_iteration_lm), float(upper_scale_factor),
-       float(lower_scale_factor), ptr(ws), vp(out), vp(kept), vp(lp), vp(st), refresh_stream())
+       float(lower_scale_factor), ptr(ws), ptr(out), ptr(kept), ptr(lp), ptr(st), refresh_stream())
   stats = {k: float(st[i]) for i, k in enumerate(POSE_GRAPH_STATS)}
   for k in ('iterations', 'iterations_pruned', 'pruned', 'status', 'factorisations'):
     stats[k] = int(stats[k])
@@ -796,9 +740,7 @@ def ransac_correspondence(x, y, idx0, idx1, max_dist, num_hyp=4000000, seed=0):
   n = len(idx0) if idx0 is not None else (len(idx1) if idx1 is not None else x.shape[0])
   if idx0 is not None and idx1 is not None and len(idx0) != len(idx1):
     raise DgrError('idx0 and idx1 differ in length')
-  words = C.c_int64(0)
-  call('dgr_ransac_ws_elems', n, int(num_hyp), C.byref(words))
-  ws = scratch('ransac', words.value, torch.int64, dev)
+  ws = workspace('ransac', torch.int64, dev, 'dgr_ransac_ws_elems', n, int(num_hyp))
   res = torch.empty(20, dtype=torch.float64, device=dev)
   call('dgr_ransac_correspondence', ptr(x), ptr(y), ptr(idx0) if idx0 is not None else None,
        ptr(idx1) if idx1 is not None else None, n, float(max_dist), int(num_hyp), int(seed) & (2**64 - 1),
@@ -818,9 +760,8 @@ def ransac_feature_matching(src, tgt, nn, spec, table, cell, max_dist, edge_rati
   if nn.numel() != src.shape[0]:
     raise DgrError('nn must hold one target row per source point')
   dev = src.device
-  words = C.c_int64(0)
-  call('dgr_ransac_fm_ws_elems', src.shape[0], int(max_iteration), int(max_validation), C.byref(words))
-  ws = scratch('ransac_fm', words.value, torch.int64, dev)
+  ws = workspace('ransac_fm', torch.int64, dev, 'dgr_ransac_fm_ws_elems', src.shape[0], int(max_iteration),
+                 int(max_validation))
   res = torch.empty(24, dtype=torch.float64, device=dev)
   call('dgr_ransac_feature_matching', ptr(src), src.shape[0], ptr(tgt), ptr(nn), ptr(spec), ptr(table.keys),
        ptr(table.vals), table.cap, int(batch), float(cell), float(max_dist), float(edge_ratio), float(check_dist),
@@ -843,9 +784,8 @@ def fgr_feature_matching(src, tgt, nn_st, nn_ts, division_factor=1.4, use_absolu
   if nn_st.numel() != n_s or nn_ts.numel() != n_t:
     raise DgrError('nn_st / nn_ts must hold one row per source / target point')
   dev = src.device
-  words = C.c_int64(0)
-  call('dgr_fgr_ws_elems', n_s, n_t, int(maximum_tuple_count), int(bool(tuple_test)), C.byref(words))
-  ws = scratch('fgr', words.value, torch.int64, dev)
+  ws = workspace('fgr', torch.int64, dev, 'dgr_fgr_ws_elems', n_s, n_t, int(maximum_tuple_count),
+                 int(bool(tuple_test)))
   res = torch.empty(24, dtype=torch.float64, device=dev)
   corres = None
   if return_correspondences:
@@ -887,10 +827,8 @@ def goicp(src, tgt, mse_thresh=1e-3, trim_fraction=0.0, dt_size=300, dt_expand=2
   (both clouds centred, divided by one scale s).  -> device double [32]: 4x4 pose mapping src into tgt, then the
   fields of GOICP_RESULT."""
   _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
-  args = (src.shape[0], tgt.shape[0], int(dt_size), int(max_rotation_cubes), int(cubes_per_round))
-  words = C.c_int64(0)
-  call('dgr_goicp_ws_elems', *args, C.byref(words))
-  ws = scratch('goicp', words.value, torch.int64, src.device)
+  ws = workspace('goicp', torch.int64, src.device, 'dgr_goicp_ws_elems', src.shape[0], tgt.shape[0], int(dt_size),
+                 int(max_rotation_cubes), int(cubes_per_round))
   res = torch.empty(32, dtype=torch.float64, device=src.device)
   rmin, tmin = (C.c_double * 3)(*map(float, rot_min)), (C.c_double * 3)(*map(float, trans_min))
   call('dgr_goicp', ptr(src), src.shape[0], ptr(tgt), tgt.shape[0], float(mse_thresh), float(trim_fraction),
@@ -913,10 +851,9 @@ def super4pcs(src, tgt, n_sample_tgt=1024, overlap=0.5, delta=0.1, angle_tol=0.0
   then the fields of SUPER4PCS_RESULT; with return_log, also the int32 [max_bases, 16] base log (fields
   SUPER4PCS_LOG, then zeros; -1 rows for bases not run)."""
   _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
-  words = C.c_int64(0)
-  call('dgr_super4pcs_ws_elems', src.shape[0], tgt.shape[0], int(n_sample_tgt), int(dt_size), int(bases_per_round),
-       int(max_pairs), int(max_candidates), int(verify_per_base), C.byref(words))
-  ws = scratch('super4pcs', words.value, torch.int64, src.device)
+  ws = workspace('super4pcs', torch.int64, src.device, 'dgr_super4pcs_ws_elems', src.shape[0], tgt.shape[0],
+                 int(n_sample_tgt), int(dt_size), int(bases_per_round), int(max_pairs), int(max_candidates),
+                 int(verify_per_base))
   res = torch.empty(32, dtype=torch.float64, device=src.device)
   log = torch.empty(max(int(max_bases), 1), 16, dtype=torch.int32, device=src.device) if return_log else None
   call('dgr_super4pcs', ptr(src), src.shape[0], ptr(tgt), tgt.shape[0], int(n_sample_tgt), float(overlap),
@@ -926,8 +863,8 @@ def super4pcs(src, tgt, n_sample_tgt=1024, overlap=0.5, delta=0.1, angle_tol=0.0
   return (res, log) if return_log else res
 
 
-POINTNET_PARAMS = 154368              # DGR_POINTNET_PARAMS
-POINTNET_PACKED_BYTES = 1185792       # DGR_POINTNET_PACKED_BYTES
+POINTNET_PARAMS = _DEFINES['DGR_POINTNET_PARAMS']
+POINTNET_PACKED_BYTES = _DEFINES['DGR_POINTNET_PACKED_BYTES']
 POINTNETLK_RESULT = ('iterations', 'last_dx', 'last_r', 'status', 'n_src', 'n_tgt', 'host_reads')
 POINTNETLK_LOG = ('g00', 'g01', 'g02', 'g03', 'g10', 'g11', 'g12', 'g13', 'g20', 'g21', 'g22', 'g23', 'dx_norm',
                   'r_norm')
@@ -983,9 +920,8 @@ def pointnetlk(src, tgt, packed, delta=1e-2, max_iter=10, xtol=1e-7, return_jaco
     if t.dim() != 2 or t.shape[1] != 3:
       raise DgrError(f'{name}: expected [n, 3], got {tuple(t.shape)}')
   _chk_packed(packed, src.device)
-  words = C.c_int64(0)
-  call('dgr_pointnetlk_ws_elems', src.shape[0], tgt.shape[0], int(max_iter), C.byref(words))
-  ws = scratch('pointnetlk', words.value, torch.int64, src.device)
+  ws = workspace('pointnetlk', torch.int64, src.device, 'dgr_pointnetlk_ws_elems', src.shape[0], tgt.shape[0],
+                 int(max_iter))
   res = torch.empty(32, dtype=torch.float64, device=src.device)
   jac = torch.empty(1024, 6, dtype=torch.float64, device=src.device) if return_jacobian else None
   log = torch.full((max(int(max_iter), 1), 16), float('nan'), dtype=torch.float64, device=src.device) \
@@ -999,7 +935,7 @@ def pointnetlk(src, tgt, packed, delta=1e-2, max_iter=10, xtol=1e-7, return_jaco
 # --------------------------------------------------------------------------- #
 # RGB-D fusion (csrc/tsdf.cu): the device half of o3d_integration.ScalableTSDFVolume
 # --------------------------------------------------------------------------- #
-TSDF_RES = 16
+TSDF_RES = _DEFINES['DGR_TSDF_RES']
 
 
 def _host_f64(a, n, name):
@@ -1024,10 +960,9 @@ def tsdf_touch(depth, intr, pose, voxel_length, sdf_trunc, stride, keys, vals, u
   _chk(depth, torch.float32, 'depth')
   intr = _host_f64(intr, 4, 'intr')
   pose = _host_f64(np.asarray(pose, dtype=np.float64).reshape(4, 4)[:3], 12, 'pose')
-  call('dgr_tsdf_touch', ptr(depth), depth.shape[1], depth.shape[0], intr.ctypes.data_as(C.c_void_p),
-       pose.ctypes.data_as(C.c_void_p), float(voxel_length), float(sdf_trunc), TSDF_RES, int(stride), ptr(keys),
-       ptr(vals), keys.numel(), ptr(unit_keys), unit_keys.shape[0], int(n_total), ptr(touched), ptr(counts), ptr(ws),
-       stream())
+  call('dgr_tsdf_touch', ptr(depth), depth.shape[1], depth.shape[0], ptr(intr), ptr(pose), float(voxel_length),
+       float(sdf_trunc), TSDF_RES, int(stride), ptr(keys), ptr(vals), keys.numel(), ptr(unit_keys), unit_keys.shape[0],
+       int(n_total), ptr(touched), ptr(counts), ptr(ws), stream())
 
 
 def tsdf_rehash(unit_keys, n_total, keys, vals):
@@ -1044,9 +979,9 @@ def tsdf_integrate(depth, color, intr, extrinsic, voxel_length, sdf_trunc, unit_
       raise DgrError(f'color: expected {(depth.shape[0], depth.shape[1], 3)}, got {tuple(color.shape)}')
   intr = _host_f64(intr, 4, 'intr')
   ext = _host_f64(np.asarray(extrinsic, dtype=np.float64).reshape(4, 4)[:3], 12, 'extrinsic')
-  call('dgr_tsdf_integrate', ptr(depth), ptr(color), depth.shape[1], depth.shape[0], intr.ctypes.data_as(C.c_void_p),
-       ext.ctypes.data_as(C.c_void_p), float(voxel_length), float(sdf_trunc), TSDF_RES, ptr(unit_keys), ptr(touched),
-       int(n_touched), ptr(tsdf), ptr(weight), ptr(rgb), tsdf.shape[0], stream())
+  call('dgr_tsdf_integrate', ptr(depth), ptr(color), depth.shape[1], depth.shape[0], ptr(intr), ptr(ext),
+       float(voxel_length), float(sdf_trunc), TSDF_RES, ptr(unit_keys), ptr(touched), int(n_touched), ptr(tsdf),
+       ptr(weight), ptr(rgb), tsdf.shape[0], stream())
 
 
 def tsdf_extract(unit_keys, n_units, keys, vals, tsdf, weight, rgb, voxel_length):
@@ -1072,5 +1007,5 @@ def tsdf_mc_tables():
   """-> (edge_table [256], tri_table [256, 16]) int32 numpy: the library's marching-cubes tables."""
   edge = np.zeros(256, np.int32)
   tri = np.zeros((256, 16), np.int32)
-  call('dgr_tsdf_mc_tables', edge.ctypes.data_as(C.c_void_p), tri.ctypes.data_as(C.c_void_p))
+  call('dgr_tsdf_mc_tables', ptr(edge), ptr(tri))
   return edge, tri

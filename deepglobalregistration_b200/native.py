@@ -51,7 +51,7 @@ class Context:
   def profile_read(self, max_rows=4096):
     """-> float64 [n, 4]: milliseconds, algorithmic flops, gather-scatter-model bytes, kind."""
     buf = np.zeros((max_rows, 4), np.float64)
-    n = _abi.lib().dgr_ctx_profile_read(self.handle, buf.ctypes.data_as(C.c_void_p), max_rows)
+    n = _abi.lib().dgr_ctx_profile_read(self.handle, _abi.ptr(buf), max_rows)
     return buf[:int(n)].copy()
 
   STAGES = ('upload+voxelise', 'fcgf_coordinate_phase', 'read1+fcgf_pair_lists', 'fcgf_convolutions', 'feature_knn',
@@ -175,12 +175,12 @@ def pair_register(ctx, fcgf, inlier, xyz0, xyz1, voxel, clip, use_icp):
     torch.cuda.current_stream(a.device).synchronize()
   res = np.zeros(64, np.float64)
   _abi.call('dgr_pair_register', ctx.handle, fcgf.handle, inlier.handle, pa, na, fa, pb, nb, fb, int(ha),
-            float(voxel), float(clip), int(bool(use_icp)), res.ctypes.data_as(C.c_void_p))
+            float(voxel), float(clip), int(bool(use_icp)), _abi.ptr(res))
   return res
 
 
 def pair_safeguard(ctx, max_dist, num_hyp, seed, use_icp):
   res = np.zeros(40, np.float64)
   _abi.call('dgr_pair_safeguard', ctx.handle, float(max_dist), int(num_hyp), int(seed) & (2**64 - 1),
-            int(bool(use_icp)), res.ctypes.data_as(C.c_void_p))
+            int(bool(use_icp)), _abi.ptr(res))
   return res

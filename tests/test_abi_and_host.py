@@ -18,7 +18,7 @@ def built():
   return build.build()
 
 
-def test_library_exports_every_declared_symbol(built):
+def test_library_exports_and_binds_every_declared_symbol(built):
   header = open(os.path.join(ROOT, 'include', 'dgr_b200.h')).read()
   declared = set(re.findall(r'\b(dgr_[a-z0-9_]+)\s*\(', header))
   declared -= {'dgr_keyspec_t'}
@@ -27,9 +27,34 @@ def test_library_exports_every_declared_symbol(built):
   missing = [s for s in sorted(declared) if not hasattr(lib, s)]
   assert not missing, missing
   from deepglobalregistration_b200 import _abi
-  assert set(_abi.SIGNATURES) == declared, set(_abi.SIGNATURES) ^ declared
+  bound = _abi.bind(built)
+  assert {s for s in declared if getattr(bound, s).argtypes is not None} == declared
+  assert set(_abi.DECLARATIONS) == declared, set(_abi.DECLARATIONS) ^ declared
   assert _abi.lib().dgr_version() == 100
   assert ctypes.sizeof(_abi.KeySpec) == 4 * (2 + 3 * 8)
+
+
+def test_header_binding_types(tmp_path):
+  """The argtypes / restypes and constants read from include/dgr_b200.h, pinned for a few declarations; a C type
+  without a fixed-width ctypes equivalent is rejected, not guessed."""
+  from deepglobalregistration_b200 import _abi
+  p, i32, i64, u64 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_uint64
+  f32, f64 = ctypes.c_float, ctypes.c_double
+  D = _abi.DECLARATIONS
+  assert D['dgr_pose_graph_optimize'] == (i32, [p, i64, p, p, p, p, p, i64, f64, f64, f64, i32, i32, f64, f64, f64,
+                                                f64, i32, f64, f64, p, p, p, p, p, p])
+  assert D['dgr_ransac_correspondence'] == (i32, [p, p, p, p, i64, f64, i64, u64, p, p, p])
+  assert D['dgr_sigmoid_clip_sum'] == (i32, [p, i64, f32, p, p, p])
+  assert D['dgr_version'] == (i32, [])
+  assert D['dgr_last_error'] == (ctypes.c_char_p, [])
+  assert D['dgr_ctx_stream'] == (p, [p])
+  assert D['dgr_kmap_mask_words'] == (i64, [i64])
+  assert _abi.POINTNET_PACKED_BYTES == 1185792 and _abi.POSE_GRAPH_MAX_EDGES == 32640
+  assert _abi.read_header(_abi.HEADER)[1]['DGR_TSDF_COORD_MIN'] == -1048576
+  bad = tmp_path / 'bad.h'
+  bad.write_text('#include <stddef.h>\nint32_t dgr_bad(const float* x, size_t n, void* stream);\n')
+  with pytest.raises(_abi.DgrError, match='dgr_bad.*size_t'):
+    _abi.read_header(str(bad))
 
 
 def test_sm90a_sass_present(built):

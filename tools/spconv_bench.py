@@ -17,7 +17,6 @@ same buffers in this process (the C ABI and the packed weight layouts are the sa
 come from one run.
 """
 import argparse
-import ctypes as C
 import json
 import os
 import subprocess
@@ -72,15 +71,6 @@ def network_launches(coords):
   return out
 
 
-def other_lib(path):
-  lib = C.CDLL(path)
-  for name in ('dgr_spconv_tc_fwd', 'dgr_spconv_tc_f16_fwd', 'dgr_last_error'):
-    fn = getattr(lib, name)
-    fn.argtypes = _abi.SIGNATURES[name]
-    fn.restype = C.c_char_p if name == 'dgr_last_error' else C.c_int32
-  return lib
-
-
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--lib', default=None, help='a second libdgr_b200.so to alternate with')
@@ -91,7 +81,7 @@ def main():
   card = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.sm,clocks.max.sm', '--format=csv,noheader'],
                         capture_output=True, text=True).stdout.strip()
   print(f'card: {card}', flush=True)
-  other = other_lib(args.lib) if args.lib else None
+  other = _abi.bind(args.lib, ('dgr_spconv_tc_fwd', 'dgr_spconv_tc_f16_fwd', 'dgr_last_error')) if args.lib else None
   res = {'card': card, 'other_lib': args.lib, 'rows': []}
   seen = {}
   for D, coords in bench_coords().items():
