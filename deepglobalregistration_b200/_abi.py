@@ -612,6 +612,23 @@ def estimate_normals(xyz, manager_or_table, cell, radius, max_nn, prev=None, ret
   return (normals, counts) if return_counts else normals
 
 
+def color_gradient(xyz, normals, intensity, manager_or_table, cell, radius, max_nn, return_counts=False, batch=0):
+  """Colour gradients (open3d 0.10's InitializePointCloudForColoredICP) of xyz (CUDA float32 [n, 3]) with normals
+  (CUDA float32 [n, 3]) and intensities (CUDA float32 [n]) from the neighbours estimate_normals finds (strictly within
+  `radius`, at most `max_nn` <= 64 by (d^2, row), the cloud's own voxel hash at `cell`).  -> float32 [n, 3] (and the
+  int32 [n] counts within the radius)."""
+  _chk(xyz, torch.float32, 'xyz'); _chk(normals, torch.float32, 'normals'); _chk(intensity, torch.float32, 'intensity')
+  n = xyz.shape[0]
+  if normals.shape != xyz.shape or intensity.shape != (n,):
+    raise DgrError('normals and intensity must hold one row per point')
+  spec, table = _hash_of(manager_or_table)
+  grad = torch.empty(n, 3, dtype=torch.float32, device=xyz.device)
+  counts = torch.empty(max(n, 1), dtype=torch.int32, device=xyz.device)[:n]
+  call('dgr_color_gradient', ptr(xyz), ptr(normals), ptr(intensity), n, ptr(spec), ptr(table.keys), ptr(table.vals),
+       table.cap, int(batch), float(cell), float(radius), int(max_nn), ptr(grad), ptr(counts), stream())
+  return (grad, counts) if return_counts else grad
+
+
 FPFH_MAX_NN = 128      # dgr_compute_fpfh's bound on the neighbours per point (the point itself included)
 FPFH_DIM = 33
 
@@ -672,6 +689,32 @@ def icp_point_to_plane(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_in
   """Point-to-plane ICP (open3d's TransformationEstimationPointToPlane, default criteria) of src onto tgt through
   tgt's voxel hash; arguments as icp_point_to_point plus tgt_normals (CUDA float32 [n_tgt, 3])."""
   return _icp(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter, rel_fitness, rel_rmse, batch)
+
+
+def icp_colored(src, src_intensity, tgt, tgt_normals, tgt_intensity, tgt_grad, tgt_manager, voxel, max_dist,
+                lambda_geometric, T_init, max_iter=30, rel_fitness=1e-6, rel_rmse=1e-6, batch=0):
+  """Colored ICP (open3d's TransformationEstimationForColoredICP(lambda_geometric), default criteria) of src onto tgt
+  through tgt's voxel hash; arguments as icp_point_to_plane plus the intensities (CUDA float32 [n]) of both clouds and
+  the target's colour gradients (color_gradient; CUDA float32 [n_tgt, 3]).  -> device double [20] as icp_point_to_plane."""
+  _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
+  for name, a, shape in (('src_intensity', src_intensity, (src.shape[0],)), ('tgt_normals', tgt_normals, tgt.shape),
+                         ('tgt_intensity', tgt_intensity, (tgt.shape[0],)), ('tgt_grad', tgt_grad, tgt.shape)):
+    _chk(a, torch.float32, name)
+    if a.shape != shape:
+      raise DgrError(f'{name} must hold one row per point')
+  if tgt.shape[0] == 0:
+    raise DgrError('colored ICP needs target points')
+  dev = src.device
+  spec, table = _hash_of(tgt_manager)
+  if not (isinstance(T_init, torch.Tensor) and T_init.is_cuda and T_init.numel() == 12):
+    T_init = torch.as_tensor(T_init, dtype=torch.float64).reshape(4, 4)[:3].contiguous().to(dev)
+  ws = workspace('icp', torch.float64, dev, 'dgr_icp_ws_elems', src.shape[0])
+  res = torch.empty(20, dtype=torch.float64, device=dev)
+  call('dgr_colored_icp', ptr(src), ptr(src_intensity), src.shape[0], ptr(tgt), ptr(tgt_normals), ptr(tgt_intensity),
+       ptr(tgt_grad), ptr(spec), ptr(table.keys), ptr(table.vals), table.cap, int(batch), float(voxel), float(max_dist),
+       float(lambda_geometric), ptr(T_init), int(max_iter), float(rel_fitness), float(rel_rmse), ptr(ws), ptr(res),
+       stream())
+  return res
 
 
 def information_matrix(src, tgt, tgt_manager, cell, max_dist, T, batch=0):

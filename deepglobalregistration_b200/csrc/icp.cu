@@ -1,13 +1,15 @@
-// Normal estimation and ICP: open3d 0.10's EstimateNormals(KDTreeSearchParamHybrid(radius, max_nn)) and
-// RegistrationICP with TransformationEstimationPointToPoint / PointToPlane, restated in oracle/normals.py,
-// oracle/icp.py and oracle/icp_plane.py (which pin every boundary convention).  All search one cloud's voxel hash (a
+// Normal estimation, colour gradients and ICP: open3d 0.10's EstimateNormals(KDTreeSearchParamHybrid(radius,
+// max_nn)), InitializePointCloudForColoredICP and RegistrationICP with TransformationEstimationPointToPoint /
+// PointToPlane / ForColoredICP, restated in oracle/normals.py, oracle/icp.py, oracle/icp_plane.py and
+// oracle/colored_icp.py (which pin every boundary convention).  All search one cloud's voxel hash (a
 // dgr_unique_first table with at most one point per cell): the (2 reach + 1)^3 cells around a point,
 // reach = ceil(radius / cell) <= 4, 8 lanes per point as in dgr_voxel_nearest8.  No atomics: every sum has a fixed
 // order, so a call gives the same bits on every run.
-//   normals_kernel           8 lanes per point, one probe pass: count and fp64 cumulants of the offsets p_j - p_i of
-//                            the rows with |p_j - p_i|^2 < radius^2; a point with <= max_nn of them gets its normal
-//   normals_select_kernel    a warp per point with more than max_nn: the in-radius rows again, in cell order, into
-//                            shared memory; the max_nn smallest (d^2, row) keys by rank; their cumulants
+//   nbr_probe_kernel<S>      8 lanes per point, one probe pass: count and the 9 fp64 sums S adds over the rows with
+//                            |p_j - p_i|^2 < radius^2 (the offsets' cumulants for normals, the gradient rows for
+//                            colour gradients); a point with <= max_nn of them gets its result
+//   nbr_select_kernel<S>     a warp per point with more than max_nn: the in-radius rows again, in cell order, into
+//                            shared memory; the max_nn smallest (d^2, row) keys by rank; their sums
 //   icp_match_kernel<E>      nearest target row within max_dist (dgr_voxel_nearest8); the estimator's sums, the
 //                            count and sum d^2 as per-block partials
 //   icp_update_kernel<E>     the partials reduced in block order, open3d's stopping rule, the estimator's step
@@ -20,7 +22,7 @@
 namespace {
 
 constexpr int kNormThreads = 256;
-constexpr int kSelWarps = 4;                            // normals_select_kernel: warps (points) per block
+constexpr int kSelWarps = 4;                            // nbr_select_kernel: warps (points) per block
 constexpr int kMaxNN = 64;
 constexpr int kIcpThreads = 256;
 constexpr int kIcpMaxBlocks = 2368;
@@ -77,17 +79,85 @@ __device__ void store_normal(const double m[9], int n, const float* __restrict__
   for (int a = 0; a < 3; ++a) normals[3 * i + a] = (float)nv[a];
 }
 
+// The per-point sums of a neighbourhood pass: 9 fp64 sums over the kept rows j of point i (offset e = p_j - p_i),
+// then one result per point.  point(i) loads what add() needs of point i; store() gets the sums and the kept count.
+//   NormalSums    the cumulants of e (add_cumulants); store_normal
+//   GradientSums  open3d's colour-gradient rows u = e - (e.n_i) n_i, b = I_j - I_i: sum u u^T (xx, xy, xz, yy, yz,
+//                 zz) and sum u b; the point's own row adds exact zeros.  store_gradient
+struct NormalSums {
+  const float* prev;
+  float* normals;
+  struct Point {};
+  __device__ __forceinline__ Point point(int64_t) const { return {}; }
+  __device__ __forceinline__ void add(const Point&, double m[9], const double e[3], int32_t) const {
+    add_cumulants(m, e);
+  }
+  __device__ __forceinline__ void store(const double m[9], int n, int64_t i) const {
+    store_normal(m, n, prev, i, normals);
+  }
+};
+
+// open3d's InitializePointCloudForColoredICP at point i from the sums of nn neighbours (i included): g = 0 for
+// nn < 4, else the solution of (sum u u^T + (nn - 1)^2 n n^T) g = sum u b by a 3x3 Cholesky in fp64 (g = 0 on a
+// non-positive pivot, open3d's result when its solve fails), rounded to float once
+__device__ void store_gradient(const double m[9], int nn, const double nv[3], int64_t i, float* __restrict__ grad) {
+  double g[3] = {0.0, 0.0, 0.0};
+  if (nn >= 4) {
+    const double k = (double)(nn - 1) * (double)(nn - 1);
+    const double a00 = m[0] + k * nv[0] * nv[0], a01 = m[1] + k * nv[0] * nv[1], a02 = m[2] + k * nv[0] * nv[2];
+    const double a11 = m[3] + k * nv[1] * nv[1], a12 = m[4] + k * nv[1] * nv[2], a22 = m[5] + k * nv[2] * nv[2];
+    if (a00 > 0.0) {
+      const double l00 = sqrt(a00), l10 = a01 / l00, l20 = a02 / l00;
+      const double d1 = a11 - l10 * l10;
+      if (d1 > 0.0) {
+        const double l11 = sqrt(d1), l21 = (a12 - l20 * l10) / l11;
+        const double d2 = a22 - l20 * l20 - l21 * l21;
+        if (d2 > 0.0) {
+          const double l22 = sqrt(d2);
+          const double y0 = m[6] / l00, y1 = (m[7] - l10 * y0) / l11, y2 = (m[8] - l20 * y0 - l21 * y1) / l22;
+          g[2] = y2 / l22;
+          g[1] = (y1 - l21 * g[2]) / l11;
+          g[0] = (y0 - l10 * g[1] - l20 * g[2]) / l00;
+        }
+      }
+    }
+  }
+  for (int a = 0; a < 3; ++a) grad[3 * i + a] = (float)g[a];
+}
+
+struct GradientSums {
+  const float* nrm;
+  const float* intensity;
+  float* grad;
+  struct Point { double n[3], I; };
+  __device__ __forceinline__ Point point(int64_t i) const {
+    return {{(double)nrm[3 * i], (double)nrm[3 * i + 1], (double)nrm[3 * i + 2]}, (double)intensity[i]};
+  }
+  __device__ __forceinline__ void add(const Point& q, double m[9], const double e[3], int32_t j) const {
+    const double en = e[0] * q.n[0] + e[1] * q.n[1] + e[2] * q.n[2];
+    const double u[3] = {e[0] - en * q.n[0], e[1] - en * q.n[1], e[2] - en * q.n[2]};
+    const double b = (double)__ldg(intensity + j) - q.I;
+    m[0] += u[0] * u[0]; m[1] += u[0] * u[1]; m[2] += u[0] * u[2];
+    m[3] += u[1] * u[1]; m[4] += u[1] * u[2]; m[5] += u[2] * u[2];
+    m[6] += u[0] * b; m[7] += u[1] * b; m[8] += u[2] * b;
+  }
+  __device__ __forceinline__ void store(const double m[9], int n, int64_t i) const {
+    store_gradient(m, n, point(i).n, i, grad);
+  }
+};
+
+template <class S>
 __global__ void __launch_bounds__(kNormThreads)
-normals_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspec_t* __restrict__ spec_p,
-               const uint64_t* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask, int32_t batch,
-               double cell, int reach, double r2, int max_nn, const float* __restrict__ prev,
-               float* __restrict__ normals, int32_t* __restrict__ counts) {
+nbr_probe_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspec_t* __restrict__ spec_p,
+                 const uint64_t* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask, int32_t batch,
+                 double cell, int reach, double r2, int max_nn, const S sums, int32_t* __restrict__ counts) {
   const dgr_keyspec_t s = *spec_p;
   const int64_t i0 = ((int64_t)blockIdx.x * kNormThreads + threadIdx.x) >> 3;
   const int sub = threadIdx.x & 7;
   const bool have = i0 < n;                             // whole warps stay for the shuffles
   const int64_t i = have ? i0 : 0;
   const double p[3] = {(double)xyz[3 * i], (double)xyz[3 * i + 1], (double)xyz[3 * i + 2]};
+  const typename S::Point q = sums.point(i);
   const int side = 2 * reach + 1, n_cells = side * side * side;
   int c3[3];
 #pragma unroll
@@ -100,7 +170,7 @@ normals_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspec_t* __
     double e[3];
     if (offset_d2(xyz, j, p, e) < r2) {
       ++cnt;
-      add_cumulants(m, e);
+      sums.add(q, m, e, j);
     }
   }
 #pragma unroll
@@ -111,7 +181,7 @@ normals_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspec_t* __
   }
   if (!have || sub != 0) return;
   counts[i] = cnt;
-  if (cnt <= max_nn) store_normal(m, cnt, prev, i, normals);
+  if (cnt <= max_nn) sums.store(m, cnt, i);
 }
 
 // (d2, row) of a before b
@@ -119,11 +189,11 @@ __device__ __forceinline__ bool key_less(double da, int32_t ja, double db, int32
   return da < db || (da == db && ja < jb);
 }
 
+template <class S>
 __global__ void __launch_bounds__(kSelWarps * 32)
-normals_select_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspec_t* __restrict__ spec_p,
-                      const uint64_t* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask,
-                      int32_t batch, double cell, int reach, double r2, int max_nn, const float* __restrict__ prev,
-                      float* __restrict__ normals, const int32_t* __restrict__ counts) {
+nbr_select_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspec_t* __restrict__ spec_p,
+                  const uint64_t* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask, int32_t batch,
+                  double cell, int reach, double r2, int max_nn, const S sums, const int32_t* __restrict__ counts) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int side = 2 * reach + 1, n_cells = side * side * side;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -158,6 +228,7 @@ normals_select_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspe
   }
   __syncwarp();
   // candidate k is kept when fewer than max_nn keys rank before it (keys are distinct: rows are)
+  const typename S::Point q = sums.point(i);
   double mm[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   for (int k = lane; k < m_cnt; k += 32) {
     const double dk = kd[k];
@@ -167,14 +238,14 @@ normals_select_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspe
     if (rank < max_nn) {
       double e[3];
       offset_d2(xyz, jk, p, e);
-      add_cumulants(mm, e);
+      sums.add(q, mm, e, jk);
     }
   }
 #pragma unroll
   for (int d = 1; d < 32; d <<= 1)
 #pragma unroll
     for (int k = 0; k < 9; ++k) mm[k] += __shfl_xor_sync(0xffffffffu, mm[k], d);
-  if (lane == 0) store_normal(mm, max_nn, prev, i, normals);
+  if (lane == 0) sums.store(mm, max_nn, i);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -201,12 +272,22 @@ __device__ __forceinline__ void add_sum(double* acc, int sub, int k, double v) {
   if ((k & 7) == sub) acc[k >> 3] += v;
 }
 
+// What the estimators read besides the matched pair: target normals (point-to-plane, colored), and for colored ICP
+// the target colour gradients and intensities, the source intensities and sqrt(lambda), sqrt(1 - lambda)
+struct IcpInputs {
+  const float* tnorm;
+  const float* tgrad;
+  const float* tint;
+  const float* sint;
+  double sqrt_geo, sqrt_photo;
+};
+
 // open3d's TransformationEstimationPointToPoint: sums n, sum d^2, sum p (3), sum q (3), sum q p^T (9) over the
 // correspondences (p = current transformed source point, q its target point); the step is the Kabsch rotation of
 // the centred cross-covariance, composed on the left (the identity without correspondences)
 struct PointToPoint {
   static constexpr int kNv = 17, kCount = 0, kD2 = 1;
-  __device__ __forceinline__ static void accumulate(const double p[3], const double q[3], const float* __restrict__,
+  __device__ __forceinline__ static void accumulate(const double p[3], const double q[3], const IcpInputs&, int64_t,
                                                     int64_t, double d2, int sub, double* acc) {
     add_sum(acc, sub, 0, 1.0);
     add_sum(acc, sub, 1, d2);
@@ -246,9 +327,9 @@ struct PointToPoint {
 // pivot - no match, a single plane - gives the identity) and composes [Rz(x2) Ry(x1) Rx(x0) | x3..5] on the left
 struct PointToPlane {
   static constexpr int kNv = 29, kCount = 27, kD2 = 28;
-  __device__ __forceinline__ static void accumulate(const double p[3], const double q[3],
-                                                    const float* __restrict__ tnorm, int64_t j, double d2, int sub,
-                                                    double* acc) {
+  __device__ __forceinline__ static void accumulate(const double p[3], const double q[3], const IcpInputs& in,
+                                                    int64_t, int64_t j, double d2, int sub, double* acc) {
+    const float* __restrict__ tnorm = in.tnorm;
     const double nv[3] = {tnorm[3 * j], tnorm[3 * j + 1], tnorm[3 * j + 2]};
     const double r = (p[0] - q[0]) * nv[0] + (p[1] - q[1]) * nv[1] + (p[2] - q[2]) * nv[2];
     const double J[6] = {p[1] * nv[2] - p[2] * nv[1], p[2] * nv[0] - p[0] * nv[2], p[0] * nv[1] - p[1] * nv[0],
@@ -272,12 +353,50 @@ struct PointToPlane {
   }
 };
 
+// open3d's TransformationEstimationForColoredICP(lambda): two rows per correspondence (source point s = p, target
+// point q, normal n, colour gradient d, intensities I_s, I_t), both added into PointToPlane's 29 sums and step:
+//   geometric    r = sqrt(lambda) (s - q).n,  J = sqrt(lambda) [s x n, n];
+//   photometric  with s' = s - ((s - q).n) n and m = -(I - n n^T) d = (d.n) n - d:
+//                r = sqrt(1 - lambda) (I_s - (d.(s' - q) + I_t)),  J = sqrt(1 - lambda) [s x m, m].
+// At lambda = 1 the photometric row is exactly zero and the sums are PointToPlane's.
+struct Colored {
+  static constexpr int kNv = PointToPlane::kNv, kCount = PointToPlane::kCount, kD2 = PointToPlane::kD2;
+  __device__ __forceinline__ static void accumulate(const double p[3], const double q[3], const IcpInputs& in,
+                                                    int64_t i, int64_t j, double d2, int sub, double* acc) {
+    const double nv[3] = {in.tnorm[3 * j], in.tnorm[3 * j + 1], in.tnorm[3 * j + 2]};
+    const double dv[3] = {in.tgrad[3 * j], in.tgrad[3 * j + 1], in.tgrad[3 * j + 2]};
+    const double rg = (p[0] - q[0]) * nv[0] + (p[1] - q[1]) * nv[1] + (p[2] - q[2]) * nv[2];
+    const double dn = dv[0] * nv[0] + dv[1] * nv[1] + dv[2] * nv[2];
+    const double mv[3] = {dn * nv[0] - dv[0], dn * nv[1] - dv[1], dn * nv[2] - dv[2]};
+    const double w[3] = {p[0] - rg * nv[0] - q[0], p[1] - rg * nv[1] - q[1], p[2] - rg * nv[2] - q[2]};
+    const double rp = (double)in.sint[i] - ((dv[0] * w[0] + dv[1] * w[1] + dv[2] * w[2]) + (double)in.tint[j]);
+#pragma unroll
+    for (int row = 0; row < 2; ++row) {
+      const double* v = row == 0 ? nv : mv;
+      const double sc = row == 0 ? in.sqrt_geo : in.sqrt_photo;
+      const double r = sc * (row == 0 ? rg : rp);
+      const double J[6] = {sc * (p[1] * v[2] - p[2] * v[1]), sc * (p[2] * v[0] - p[0] * v[2]),
+                           sc * (p[0] * v[1] - p[1] * v[0]), sc * v[0], sc * v[1], sc * v[2]};
+      int k = 0;
+#pragma unroll
+      for (int a = 0; a < 6; ++a)
+#pragma unroll
+        for (int b = a; b < 6; ++b) add_sum(acc, sub, k++, J[a] * J[b]);
+#pragma unroll
+      for (int a = 0; a < 6; ++a) add_sum(acc, sub, 21 + a, J[a] * r);
+    }
+    add_sum(acc, sub, 27, 1.0);
+    add_sum(acc, sub, 28, d2);
+  }
+  __device__ __forceinline__ static void step(const double* tot, double* T) { PointToPlane::step(tot, T); }
+};
+
 // E::kNv sums in (kNv + 7) / 8 accumulators per lane.  Per-block partials: part[block][k], summed lanes by butterfly
 // and warps in order.
 template <class E>
 __global__ void __launch_bounds__(kIcpThreads)
-icp_match_kernel(const float* __restrict__ src, int64_t n_src, const float* __restrict__ tgt,
-                 const float* __restrict__ tnorm, const dgr_keyspec_t* __restrict__ spec_p,
+icp_match_kernel(const float* __restrict__ src, int64_t n_src, const float* __restrict__ tgt, const IcpInputs in,
+                 const dgr_keyspec_t* __restrict__ spec_p,
                  const uint64_t* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask, int32_t batch,
                  double voxel, double max_dist, const IcpState* __restrict__ st, double* __restrict__ part) {
   constexpr int kSlots = (E::kNv + 7) / 8;
@@ -305,7 +424,7 @@ icp_match_kernel(const float* __restrict__ src, int64_t n_src, const float* __re
     if (have && best_j >= 0) {                          // every lane of the group has the match
       const int64_t j = best_j;
       const double q[3] = {tgt[3 * j], tgt[3 * j + 1], tgt[3 * j + 2]};
-      E::accumulate(p, q, tnorm, j, best, sub, acc);
+      E::accumulate(p, q, in, i, j, best, sub, acc);
     }
   }
   __shared__ double red[kIcpThreads / 32][kIcpStride];
@@ -382,16 +501,14 @@ int64_t icp_layout(int64_t n_src, double* base, IcpState** state, double** part)
   return c.words;
 }
 
-}  // namespace
-
-extern "C" {
-
-int32_t dgr_estimate_normals(const float* xyz, int64_t n, const dgr_keyspec_t* spec, const uint64_t* keys,
-                             const int32_t* vals, int64_t cap, int32_t batch, double cell, double radius,
-                             int32_t max_nn, const float* prev, float* normals, int32_t* counts, void* stream) {
+// the two passes of a neighbourhood search over the cloud's own hash (normals, colour gradients), checked first
+template <class S>
+int32_t nbr_launch(const float* xyz, int64_t n, const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals,
+                   int64_t cap, int32_t batch, double cell, double radius, int32_t max_nn, const S& sums,
+                   int32_t* counts, void* stream) {
   DGR_ARG_CHECK(n >= 0 && n < (1ll << 31), "point count out of range");
   DGR_ARG_CHECK(n == 0 || (xyz != nullptr && spec != nullptr && keys != nullptr && vals != nullptr &&
-                           normals != nullptr && counts != nullptr), "null pointer");
+                           counts != nullptr), "null pointer");
   DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
   DGR_ARG_CHECK(cell > 0 && radius > 0, "cell and radius must be positive");
   DGR_ARG_CHECK(radius / cell <= 4.0, "search radius above 4 cells is not supported");
@@ -401,14 +518,55 @@ int32_t dgr_estimate_normals(const float* xyz, int64_t n, const dgr_keyspec_t* s
   const int reach = (int)ceil(radius / cell);
   const int side = 2 * reach + 1, n_cells = side * side * side;
   const double r2 = radius * radius;
-  normals_kernel<<<dgr_blocks(n * 8, kNormThreads), kNormThreads, 0, st>>>(
-      xyz, n, spec, keys, vals, (uint64_t)cap - 1, batch, cell, reach, r2, max_nn, prev, normals, counts);
+  nbr_probe_kernel<S><<<dgr_blocks(n * 8, kNormThreads), kNormThreads, 0, st>>>(
+      xyz, n, spec, keys, vals, (uint64_t)cap - 1, batch, cell, reach, r2, max_nn, sums, counts);
   const size_t smem = (size_t)kSelWarps * n_cells * (sizeof(double) + sizeof(int32_t));   // <= 35 KB
-  normals_select_kernel<<<dgr_blocks(n, kSelWarps), kSelWarps * 32, smem, st>>>(
-      xyz, n, spec, keys, vals, (uint64_t)cap - 1, batch, cell, reach, r2, max_nn, prev, normals, counts);
+  nbr_select_kernel<S><<<dgr_blocks(n, kSelWarps), kSelWarps * 32, smem, st>>>(
+      xyz, n, spec, keys, vals, (uint64_t)cap - 1, batch, cell, reach, r2, max_nn, sums, counts);
   dgr_note_launches(2);
   DGR_LAUNCH_CHECK();
   return DGR_OK;
+}
+
+// enqueue init and max_iter + 1 (match, update) pairs of estimator E; the arguments are checked by the caller
+template <class E>
+void icp_run(const float* src, int64_t n_src, const float* tgt, const IcpInputs& in, const dgr_keyspec_t* spec,
+             const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch, double voxel, double max_dist,
+             const double* T_init, int32_t max_iter, double rel_fitness, double rel_rmse, double* ws, double* result,
+             cudaStream_t st) {
+  IcpState* state;
+  double* part;
+  icp_layout(n_src, ws, &state, &part);
+  const int blocks = icp_blocks(n_src);
+  icp_init_kernel<<<1, 32, 0, st>>>(T_init, state);
+  for (int k = 0; k <= max_iter; ++k) {
+    icp_match_kernel<E><<<blocks, kIcpThreads, 0, st>>>(src, n_src, tgt, in, spec, keys, vals, (uint64_t)cap - 1,
+                                                        batch, voxel, max_dist, state, part);
+    icp_update_kernel<E><<<1, E::kNv * 32, 0, st>>>(state, part, blocks, n_src, max_iter, rel_fitness, rel_rmse,
+                                                    result);
+  }
+  dgr_note_launches(1 + 2 * (max_iter + 1));
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t dgr_estimate_normals(const float* xyz, int64_t n, const dgr_keyspec_t* spec, const uint64_t* keys,
+                             const int32_t* vals, int64_t cap, int32_t batch, double cell, double radius,
+                             int32_t max_nn, const float* prev, float* normals, int32_t* counts, void* stream) {
+  DGR_ARG_CHECK(n == 0 || normals != nullptr, "null pointer");
+  return nbr_launch(xyz, n, spec, keys, vals, cap, batch, cell, radius, max_nn, NormalSums{prev, normals}, counts,
+                    stream);
+}
+
+int32_t dgr_color_gradient(const float* xyz, const float* normals, const float* intensity, int64_t n,
+                           const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap,
+                           int32_t batch, double cell, double radius, int32_t max_nn, float* grad, int32_t* counts,
+                           void* stream) {
+  DGR_ARG_CHECK(n == 0 || (normals != nullptr && intensity != nullptr && grad != nullptr), "null pointer");
+  return nbr_launch(xyz, n, spec, keys, vals, cap, batch, cell, radius, max_nn,
+                    GradientSums{normals, intensity, grad}, counts, stream);
 }
 
 int32_t dgr_icp_ws_elems(int64_t n_src, int64_t* n_elems) {
@@ -427,25 +585,35 @@ int32_t dgr_icp(const float* src, int64_t n_src, const float* tgt, const float* 
   DGR_ARG_CHECK(n_src >= 0 && n_src < (1ll << 31), "point count out of range");
   DGR_ARG_CHECK(T_init != nullptr && ws != nullptr && result != nullptr && spec != nullptr, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  IcpState* state;
-  double* part;
-  icp_layout(n_src, ws, &state, &part);
-  const int blocks = icp_blocks(n_src);
-  const auto iterate = [&](auto estimator) {
-    using E = decltype(estimator);
-    for (int k = 0; k <= max_iter; ++k) {
-      icp_match_kernel<E><<<blocks, kIcpThreads, 0, st>>>(src, n_src, tgt, tgt_normals, spec, keys, vals,
-                                                          (uint64_t)cap - 1, batch, voxel, max_dist, state, part);
-      icp_update_kernel<E><<<1, E::kNv * 32, 0, st>>>(state, part, blocks, n_src, max_iter, rel_fitness, rel_rmse,
-                                                      result);
-    }
-  };
-  icp_init_kernel<<<1, 32, 0, st>>>(T_init, state);
+  const IcpInputs in{tgt_normals, nullptr, nullptr, nullptr, 1.0, 0.0};
   if (tgt_normals != nullptr)
-    iterate(PointToPlane{});
+    icp_run<PointToPlane>(src, n_src, tgt, in, spec, keys, vals, cap, batch, voxel, max_dist, T_init, max_iter,
+                          rel_fitness, rel_rmse, ws, result, st);
   else
-    iterate(PointToPoint{});
-  dgr_note_launches(1 + 2 * (max_iter + 1));
+    icp_run<PointToPoint>(src, n_src, tgt, in, spec, keys, vals, cap, batch, voxel, max_dist, T_init, max_iter,
+                          rel_fitness, rel_rmse, ws, result, st);
+  DGR_LAUNCH_CHECK();
+  return DGR_OK;
+}
+
+int32_t dgr_colored_icp(const float* src, const float* src_intensity, int64_t n_src, const float* tgt,
+                        const float* tgt_normals, const float* tgt_intensity, const float* tgt_grad,
+                        const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap,
+                        int32_t batch, double voxel, double max_dist, double lambda_geometric, const double* T_init,
+                        int32_t max_iter, double rel_fitness, double rel_rmse, double* ws, double* result,
+                        void* stream) {
+  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
+  DGR_ARG_CHECK(voxel > 0 && max_dist > 0 && max_iter >= 0, "bad ICP parameters");
+  DGR_ARG_CHECK(lambda_geometric >= 0.0 && lambda_geometric <= 1.0, "lambda_geometric must lie in [0, 1]");
+  DGR_ARG_CHECK(max_dist / voxel <= 4.0, "search radius above 4 voxels is not supported");
+  DGR_ARG_CHECK(n_src >= 0 && n_src < (1ll << 31), "point count out of range");
+  DGR_ARG_CHECK(T_init != nullptr && ws != nullptr && result != nullptr && spec != nullptr && keys != nullptr &&
+                vals != nullptr && tgt != nullptr && tgt_normals != nullptr && tgt_intensity != nullptr &&
+                tgt_grad != nullptr && (n_src == 0 || (src != nullptr && src_intensity != nullptr)), "null pointer");
+  const IcpInputs in{tgt_normals, tgt_grad, tgt_intensity, src_intensity, sqrt(lambda_geometric),
+                     sqrt(1.0 - lambda_geometric)};
+  icp_run<Colored>(src, n_src, tgt, in, spec, keys, vals, cap, batch, voxel, max_dist, T_init, max_iter, rel_fitness,
+                   rel_rmse, ws, result, (cudaStream_t)stream);
   DGR_LAUNCH_CHECK();
   return DGR_OK;
 }

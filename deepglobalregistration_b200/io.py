@@ -11,7 +11,7 @@ numpy only, nothing here touches the GPU path:
 
 ``PointCloud`` is the small part of ``open3d.geometry.PointCloud`` the reference's demo and
 ``DeepGlobalRegistration.preprocess`` (core/deep_global_registration.py:143-148) rely on:
-``.points``, ``.normals``, ``.transform(T)`` and ``estimate_normals``.  With no argument
+``.points``, ``.normals``, ``.colors`` (what colored ICP registers), ``.transform(T)`` and ``estimate_normals``.  With no argument
 ``estimate_normals()`` does nothing (demo.py calls it for display only); with
 ``KDTreeSearchParamHybrid(radius, max_nn)`` (util/pointcloud.py:60) it computes the normals on the GPU -
 the one call here that leaves the host, through a lazy import of o3d_registration.
@@ -29,13 +29,15 @@ _PLY_TYPES = {
 
 
 class PointCloud:
-  """Points [N, 3] float64 plus optional per-point attributes read alongside them."""
+  """Points [N, 3] float64, optional colours [N, 3] float64 in [0, 1], plus optional per-point attributes read
+  alongside them."""
 
   def __init__(self, points=None, attributes=None, **more_attributes):
     self.points = np.zeros((0, 3)) if points is None else points
     # per-point extras as ONE dict (a PLY property may be called anything, 'points' included)
     self.attributes = dict(attributes or {}, **more_attributes)
     self.normals = None
+    self.colors = None
 
   @property
   def points(self):
@@ -47,6 +49,23 @@ class PointCloud:
     if value.ndim != 2 or value.shape[1] != 3:
       raise ValueError(f'points must be [N, 3], got {value.shape}')
     self._points = np.ascontiguousarray(value)
+
+  @property
+  def colors(self):
+    return self._colors
+
+  @colors.setter
+  def colors(self, value):
+    if value is not None:
+      value = np.asarray(value, dtype=np.float64)
+      if value.ndim != 2 or value.shape[1] != 3:
+        raise ValueError(f'colors must be [N, 3], got {value.shape}')
+      value = np.ascontiguousarray(value)
+    self._colors = value
+
+  def has_colors(self):
+    """open3d's rule: one colour per point of a non-empty cloud."""
+    return self._colors is not None and len(self._colors) == len(self._points) > 0
 
   def __len__(self):
     return len(self._points)
@@ -132,6 +151,11 @@ def _skip_binary_element(fh, el, order):
 
 def read_ply(path):
   """-> (points float64 [N, 3], {other scalar vertex properties: array [N]})."""
+  return _read_ply(path)[:2]
+
+
+def _read_ply(path):
+  """read_ply plus {vertex property name: its PLY type}."""
   with open(path, 'rb') as fh:
     fmt, elements = _ply_header(fh)
     order = {'ascii': '=', 'binary_little_endian': '<', 'binary_big_endian': '>'}[fmt]
@@ -163,7 +187,7 @@ def read_ply(path):
         cols = {n: rec[n] for n in names}
       pts = np.stack([np.asarray(cols[a], dtype=np.float64) for a in 'xyz'], axis=1)
       extra = {n: np.asarray(v) for n, v in cols.items() if n not in ('x', 'y', 'z')}
-      return pts, extra
+      return pts, extra, {p[2]: p[1] for p in el['props']}
   raise ValueError('PLY file has no vertex element')
 
 
@@ -229,12 +253,29 @@ def read_points(path):
   return np.ascontiguousarray(pts[:, :3])
 
 
+def _ply_colors(extra, types):
+  """Colours [N, 3] in [0, 1] from PLY red / green / blue (uchar divided by 255, floating point kept), else None."""
+  names = ('red', 'green', 'blue')
+  if not all(n in extra for n in names):
+    return None
+  kinds = {np.dtype(_PLY_TYPES[types[n]]).kind for n in names}
+  rgb = np.stack([np.asarray(extra[n], np.float64) for n in names], axis=1)
+  if kinds == {'f'}:
+    return rgb
+  if {types[n] for n in names} <= {'uchar', 'uint8'}:
+    return rgb / 255.0
+  return None                                           # other integer widths: left in attributes only
+
+
 def read_point_cloud(path):
   """``o3d.io.read_point_cloud`` for the formats above -> PointCloud (points as float64, which is
-  what open3d holds and why the reference voxelises PLY input in float64)."""
+  what open3d holds and why the reference voxelises PLY input in float64).  PLY red / green / blue also fill
+  ``colors`` (and stay in ``attributes``); a mesh PLY reads as its coloured vertices."""
   if os.path.splitext(path)[1].lower() == '.ply':
-    pts, extra = read_ply(path)
-    return PointCloud(pts, attributes=extra)
+    pts, extra, types = _read_ply(path)
+    pcd = PointCloud(pts, attributes=extra)
+    pcd.colors = _ply_colors(extra, types)
+    return pcd
   return PointCloud(read_points(path))
 
 

@@ -14,6 +14,9 @@ Fragments:
   ``--gt_trajectory LOG`` (one pose per fragment, in order) adds the ATE: the RMS translation error after expressing
   both trajectories relative to fragment 0, next to the ATE of the odometry chain.
 
+``--refine colored_icp`` refines every kept edge by multi-scale colored ICP before the optimisation (open3d's
+refine_registration); the fragments then need colours (PLY red / green / blue).
+
 Output: the trajectory (metadata ``k k N`` and fragment k's pose in fragment 0's frame) written with
 io.write_trajectory, and one JSON summary line."""
 import argparse
@@ -69,6 +72,8 @@ def main(argv=None):
   ap.add_argument('--overlap_thresh', type=float, default=0.3,
                   help='loop closures kept when Lambda[5, 5] / min(n_i, n_j) reaches it')
   ap.add_argument('--info_radius_voxels', type=float, default=2.0, help='information-matrix radius in voxels')
+  ap.add_argument('--refine', choices=['colored_icp'], default=None,
+                  help='refine every kept edge by multi-scale colored ICP (needs coloured fragments)')
   ap.add_argument('--out_dir', default='.')
   args = ap.parse_args(argv)
   ev.check_method_arguments(ap, args)
@@ -87,7 +92,8 @@ def main(argv=None):
     files = fragments_in_dir(args.fragments_dir)
   else:
     files = read_fragment_list(args.fragment_list)
-  mw = MultiwayRegistration(method, overlap_thresh=args.overlap_thresh, info_radius_voxels=args.info_radius_voxels)
+  mw = MultiwayRegistration(method, overlap_thresh=args.overlap_thresh, info_radius_voxels=args.info_radius_voxels,
+                            refine=args.refine)
   poses, report = mw.register_sequence(files, device=device)
   if rank == 0:
     n = len(files)
@@ -97,6 +103,8 @@ def main(argv=None):
                    seconds={k: round(v, 4) for k, v in report['seconds'].items()},
                    iterations=[report['optimiser'].get('iterations'), report['optimiser'].get('iterations_pruned')],
                    method=args.method, world_size=world)
+    if args.refine:
+      summary['refine'] = args.refine
     pairwise = {(e['s'], e['t']): e['T'] for e in edges}
     if args.fragments_dir:
       log = os.path.normpath(args.fragments_dir) + '-evaluation/gt.log'

@@ -18,6 +18,11 @@ It also carries the calls open3d users make beyond DGR's own: point-to-plane ICP
 ``TransformationEstimationPointToPlane``, -> dgr_icp) on target normals from
 ``PointCloud.estimate_normals(KDTreeSearchParamHybrid(radius, max_nn))`` (-> dgr_estimate_normals), and
 
+  registration_colored_icp(source, target, max_distance, init, criteria, lambda_geometric)           (open3d 0.10)
+  registration_colored_icp(source, target, max_correspondence_distance, init, estimation_method, criteria) (>= 0.12)
+      -> dgr_color_gradient on the target, then dgr_colored_icp: ICP with a geometric and a photometric row per
+         correspondence (Park, Zhou & Koltun 2017), the local refinement of open3d's reconstruction system;
+
   registration_fast_based_on_feature_matching(source, target, source_feature, target_feature, option)
       -> dgr_knn_top1 both ways + dgr_fgr_feature_matching: Fast Global Registration (mutual matches, tuple
          test, graduated non-convexity) with FastGlobalRegistrationOption's fields and defaults;
@@ -54,6 +59,18 @@ class TransformationEstimationPointToPlane:
   def __init__(self, kernel=None):
     if kernel is not None:
       raise NotImplementedError('robust kernels (the open3d >= 0.12 form) are not built')
+    self.kernel = None
+
+
+class TransformationEstimationForColoredICP:
+  """lambda_geometric weighs the geometric rows against the photometric ones; outside [0, 1] it falls back to 0.968,
+  as open3d's constructor does."""
+
+  def __init__(self, lambda_geometric=0.968, kernel=None):
+    if kernel is not None:
+      raise NotImplementedError('robust kernels (the open3d >= 0.12 form) are not built')
+    lam = float(lambda_geometric)
+    self.lambda_geometric = lam if 0.0 <= lam <= 1.0 else 0.968
     self.kernel = None
 
 
@@ -242,6 +259,84 @@ def registration_icp(source, target, max_correspondence_distance, init=None, est
   else:
     res = _abi.icp_point_to_point(src, tgt, (spec, table), cell, *args)
   r = res.cpu().numpy()
+  return RegistrationResult(r[:16], r[16], r[17], r[19])
+
+
+_COLORED_ICP_FORMS = (('max_distance', 'init', 'criteria', 'lambda_geometric'),                   # open3d 0.10
+                      ('max_correspondence_distance', 'init', 'estimation_method', 'criteria'))  # >= 0.12
+
+
+def _colored_icp_arguments(args, kwargs):
+  """(max_distance, init, criteria, lambda_geometric) of either argument form; the fifth argument (or a keyword only
+  one form has) tells them apart."""
+  new = ((len(args) >= 3 and isinstance(args[2], TransformationEstimationForColoredICP)) or
+         'estimation_method' in kwargs or 'max_correspondence_distance' in kwargs)
+  names = _COLORED_ICP_FORMS[new]
+  if len(args) > len(names):
+    raise TypeError(f'registration_colored_icp takes at most {len(names) + 2} positional arguments')
+  bound = dict(zip(names, args))
+  for k, v in kwargs.items():
+    if k not in names or k in bound:
+      raise TypeError(f'registration_colored_icp got an unexpected or repeated argument {k!r}')
+    bound[k] = v
+  if names[0] not in bound:
+    raise TypeError(f'registration_colored_icp needs {names[0]}')
+  if new:
+    est = bound.get('estimation_method') or TransformationEstimationForColoredICP()
+    if not isinstance(est, TransformationEstimationForColoredICP):
+      raise NotImplementedError('registration_colored_icp takes TransformationEstimationForColoredICP')
+    lam = est.lambda_geometric
+  else:
+    lam = TransformationEstimationForColoredICP(bound.get('lambda_geometric', 0.968)).lambda_geometric
+  return float(bound[names[0]]), bound.get('init'), bound.get('criteria'), lam
+
+
+def _colors(pcd, which):
+  c = getattr(pcd, 'colors', None)
+  n = len(np.asarray(getattr(pcd, 'points', pcd)).reshape(-1, 3))
+  if c is None or len(np.asarray(c).reshape(-1, 3)) != n or n == 0:
+    raise RuntimeError(f'colored ICP needs colours on the {which} cloud (PointCloud.colors, one row per point)')
+  return np.asarray(c, dtype=np.float64).reshape(-1, 3)
+
+
+def intensity(colors):
+  """open3d's colored-ICP intensity (r + g + b) / 3 of colours [n, 3] in [0, 1], as the float32 the kernels read."""
+  c = np.asarray(colors, dtype=np.float64).reshape(-1, 3)
+  return ((c[:, 0] + c[:, 1] + c[:, 2]) / 3.0).astype(np.float32)
+
+
+def registration_colored_icp(source, target, *args, **kwargs):
+  """open3d's colored ICP (Park, Zhou & Koltun, ICCV 2017) in either argument form: 0.10's (source, target,
+  max_distance, init, criteria, lambda_geometric) or >= 0.12's (source, target, max_correspondence_distance, init,
+  estimation_method, criteria).  The target needs normals and both clouds colours.  As open3d does, the target's
+  colour gradients come from its normals and colours at KDTreeSearchParamHybrid(2 max_distance, 30)
+  (dgr_color_gradient); the ICP (dgr_colored_icp) searches a voxel hash of the target whose cell serves both radii."""
+  max_distance, init, criteria, lam = _colored_icp_arguments(args, kwargs)
+  if not max_distance > 0.0:
+    raise ValueError(f'max_distance must be positive, got {max_distance}')
+  tgt_normals = getattr(target, 'normals', None)
+  if tgt_normals is None:
+    raise RuntimeError('colored ICP needs target normals: call '
+                       'target.estimate_normals(KDTreeSearchParamHybrid(radius, max_nn)) first')
+  c_src, c_tgt = _colors(source, 'source'), _colors(target, 'target')
+  nrm = np.asarray(tgt_normals, dtype=np.float32).reshape(-1, 3)
+  if len(nrm) != len(c_tgt):
+    raise RuntimeError('target normals must hold one row per target point')
+  criteria = criteria or ICPConvergenceCriteria()
+  T0 = np.eye(4) if init is None else np.asarray(init, dtype=np.float64).reshape(4, 4)
+  dev = _abi.require_device('cuda')
+  _abi.refresh_stream()
+  src64, tgt64 = _points(source, dev), _points(target, dev)
+  cell, spec, table = _target_hash(tgt64, 2.0 * max_distance, what='2 max_distance')
+  src, tgt = src64.float().contiguous(), tgt64.float().contiguous()
+  nrm_d = torch.from_numpy(np.ascontiguousarray(nrm)).to(dev)
+  i_src = torch.from_numpy(intensity(c_src)).to(dev)
+  i_tgt = torch.from_numpy(intensity(c_tgt)).to(dev)
+  grad = _abi.color_gradient(tgt, nrm_d, i_tgt, (spec, table), cell, 2.0 * max_distance, 30)
+  T12 = torch.from_numpy(np.ascontiguousarray(T0[:3])).to(dev)
+  r = _abi.icp_colored(src, i_src, tgt, nrm_d, i_tgt, grad, (spec, table), cell, max_distance, lam, T12,
+                       int(criteria.max_iteration), float(criteria.relative_fitness),
+                       float(criteria.relative_rmse)).cpu().numpy()
   return RegistrationResult(r[:16], r[16], r[17], r[19])
 
 

@@ -46,7 +46,8 @@ def _open3d_stub():
   registration_ransac_based_on_feature_matching, Feature, utility vectors; plus
   registration_fast_based_on_feature_matching / FastGlobalRegistrationOption / compute_fpfh_feature for FGR and
   FPFH users, the pose graph and global_optimization for multiway registration, and
-  TransformationEstimationPointToPlane with geometry.KDTreeSearchParamHybrid for point-to-plane ICP users) backed
+  TransformationEstimationPointToPlane with geometry.KDTreeSearchParamHybrid for point-to-plane ICP users, and
+  registration_colored_icp / TransformationEstimationForColoredICP for colored-ICP refinement) backed
   by libdgr_b200 (o3d_registration.py), and what util/integration.py fuses RGB-D frames with
   (pipelines.integration.ScalableTSDFVolume, camera.PinholeCameraIntrinsic, geometry.Image / RGBDImage /
   TriangleMesh, io.read_image / write_triangle_mesh; o3d_integration.py) - so the reference's OWN
@@ -79,7 +80,8 @@ def _open3d_stub():
                'registration_fast_based_on_feature_matching', 'compute_fpfh_feature',
                'get_information_matrix_from_point_clouds', 'PoseGraph', 'PoseGraphNode', 'PoseGraphEdge',
                'GlobalOptimizationLevenbergMarquardt', 'GlobalOptimizationGaussNewton',
-               'GlobalOptimizationConvergenceCriteria', 'GlobalOptimizationOption', 'global_optimization'):
+               'GlobalOptimizationConvergenceCriteria', 'GlobalOptimizationOption', 'global_optimization',
+               'TransformationEstimationForColoredICP', 'registration_colored_icp'):
     setattr(o3d.pipelines.registration, name, getattr(reg, name))
   o3d.registration = o3d.pipelines.registration          # the pre-0.12 module path
   sys.modules['open3d.pipelines'] = o3d.pipelines

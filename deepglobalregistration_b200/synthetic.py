@@ -79,25 +79,29 @@ def _box_faces(lo, hi):
   return lo, hi, faces
 
 
-def _sample_boxes(boxes, n, rng, noise):
-  """Area-uniform samples on the faces of axis-aligned boxes."""
+def _sample_boxes(boxes, n, rng, noise, colours=False):
+  """Area-uniform samples on the faces of axis-aligned boxes; with `colours`, also their uint8 colours [n, 3]
+  (_face_colour of the noise-free sample on its face; the same draws, so the same points)."""
   allf = []
-  for lo, hi in boxes:
+  for b, (lo, hi) in enumerate(boxes):
     lo, hi, faces = _box_faces(lo, hi)
-    for f in faces:
-      allf.append((lo, hi) + f)
+    for k, f in enumerate(faces):
+      allf.append((lo, hi) + f + (b, k % 2))
   areas = np.array([f[5] for f in allf])
   counts = rng.multinomial(n, areas / areas.sum())
-  out = []
-  for (lo, hi, ax, v, o, _), c in zip(allf, counts):
+  out, cols = [], []
+  for (lo, hi, ax, v, o, _, b, side), c in zip(allf, counts):
     p = np.empty((c, 3))
     p[:, ax] = v
     p[:, o[0]] = rng.uniform(lo[o[0]], hi[o[0]], c)
     p[:, o[1]] = rng.uniform(lo[o[1]], hi[o[1]], c)
     out.append(p)
+    if colours:
+      cols.append(_face_colour(b, ax, side, p))
   p = np.concatenate(out)
   p += rng.normal(scale=noise, size=p.shape)
-  return p[rng.permutation(len(p))]
+  perm = rng.permutation(len(p))
+  return (p[perm], np.concatenate(cols)[perm]) if colours else p[perm]
 
 
 def room_boxes(seed, extent=(3.6, 3.0, 2.5), n_furniture=6):
@@ -112,13 +116,14 @@ def room_boxes(seed, extent=(3.6, 3.0, 2.5), n_furniture=6):
   return boxes
 
 
-def room_scan(seed, n_raw=250_000, extent=(3.6, 3.0, 2.5), scene_seed=None, noise=0.005):
+def room_scan(seed, n_raw=250_000, extent=(3.6, 3.0, 2.5), scene_seed=None, noise=0.005, colours=False):
   """3DMatch-shape scan: a box room with furniture boxes, area-uniform surface
   samples with 5 mm noise.  n_raw=250k gives ~52k voxels at 0.05 m (SURVEY §8d
-  config 2).  ``scene_seed`` fixes the geometry; ``seed`` the sampling."""
+  config 2).  ``scene_seed`` fixes the geometry; ``seed`` the sampling.  With ``colours`` -> (points, uint8
+  colours [n, 3] of _face_colour), the points unchanged."""
   boxes = room_boxes(seed if scene_seed is None else scene_seed, extent)
   rng = np.random.default_rng(seed)
-  return _sample_boxes(boxes, n_raw, rng, noise)
+  return _sample_boxes(boxes, n_raw, rng, noise, colours=colours)
 
 
 def room_pair(seed, n_raw=250_000, extent=(3.6, 3.0, 2.5), rigid_copy=False, voxel_size=0.0625):
@@ -375,17 +380,18 @@ def _rot_z(a):
 
 
 def room_fragments(seed, n_frag=6, n_raw=120_000, radius=1.9, extent=(3.6, 3.0, 2.5), loop=(0.7, 0.55),
-                   noise=0.003):
+                   noise=0.003, colours=False):
   """Fragments of one ``room_boxes`` room seen from cameras on a loop inside it.  Camera k sits at angle 2 pi k /
   n_frag on an ellipse of half-axes `loop` [m] around the room's centre, 1.2 m up, turned by that angle about z (plus
   a seeded tilt of up to 5 degrees).  Fragment k holds its own surface samples (n_raw over the whole room, seed and k
   fixing them) within `radius` of camera k, expressed in camera k's frame: consecutive fragments overlap strongly and
   the last closes the loop onto the first.  -> (clouds [n_frag] float64 [n_k, 3], P [n_frag, 4, 4] mapping each
-  fragment into the room frame)."""
+  fragment into the room frame); with `colours` -> (clouds, colours [n_frag] float64 [n_k, 3] in [0, 1], P), the
+  colours rgbd_sequence gives the same surfaces (_face_colour), the points unchanged."""
   boxes = room_boxes(seed, extent)
   ex = np.asarray(extent, float)
   rng = np.random.default_rng(30_000 + seed)
-  clouds, poses = [], []
+  clouds, cols, poses = [], [], []
   for k in range(n_frag):
     th = 2 * math.pi * k / n_frag
     cam = np.array([ex[0] / 2 + loop[0] * math.cos(th), ex[1] / 2 + loop[1] * math.sin(th), 1.2])
@@ -393,11 +399,33 @@ def room_fragments(seed, n_frag=6, n_raw=120_000, radius=1.9, extent=(3.6, 3.0, 
     P = np.eye(4)
     P[:3, :3] = _rot_z(th) @ tilt
     P[:3, 3] = cam
-    pts = _sample_boxes(boxes, n_raw, np.random.default_rng(31_000 + 100 * seed + k), noise)
-    pts = pts[np.linalg.norm(pts - cam, axis=1) < radius]
+    pts = _sample_boxes(boxes, n_raw, np.random.default_rng(31_000 + 100 * seed + k), noise, colours=colours)
+    if colours:
+      pts, c8 = pts
+    near = np.linalg.norm(pts - cam, axis=1) < radius
+    pts = pts[near]
     clouds.append((pts - cam) @ P[:3, :3])                # P^-1 x
+    if colours:
+      cols.append(c8[near] / 255.0)
     poses.append(P)
-  return clouds, np.stack(poses)
+  return (clouds, cols, np.stack(poses)) if colours else (clouds, np.stack(poses))
+
+
+def checker_wall(seed, size=(1.2, 1.2), spacing=0.02, square=0.1, noise=0.001):
+  """A flat wall patch z = 0 of `size` [m] centred on the origin, points on a jittered grid of `spacing` with `noise`
+  normal to the wall, coloured by a checker of `square` [m] (grey levels 0.2 / 0.8 plus a gentle ramp along x, so no
+  two squares are alike).  Point-to-plane ICP cannot see a slide along it; its colours can.
+  -> (points float64 [n, 3], colours float64 [n, 3] in [0, 1])."""
+  rng = np.random.default_rng(50_000 + seed)
+  xs = np.arange(-size[0] / 2, size[0] / 2, spacing)
+  ys = np.arange(-size[1] / 2, size[1] / 2, spacing)
+  x, y = (a.ravel() for a in np.meshgrid(xs, ys))
+  x = x + rng.uniform(-0.3, 0.3, x.shape) * spacing
+  y = y + rng.uniform(-0.3, 0.3, y.shape) * spacing
+  pts = np.stack([x, y, rng.normal(0.0, noise, x.shape)], axis=1)
+  chk = (np.floor(x / square).astype(np.int64) + np.floor(y / square).astype(np.int64)) & 1
+  grey = np.where(chk == 1, 0.8, 0.2) + 0.1 * (x / size[0])
+  return pts, np.repeat(np.clip(grey, 0.0, 1.0)[:, None], 3, axis=1)
 
 
 def _exp6(x):

@@ -209,6 +209,18 @@ int32_t dgr_compute_fpfh(const float* xyz, const float* normals, int64_t n, cons
                          const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch, double cell,
                          double radius, int32_t max_nn, int32_t ld, void* ws, float* out, int32_t* counts,
                          void* stream);
+/* Colour gradients of the cloud xyz[n] (open3d 0.10 InitializePointCloudForColoredICP; oracle/colored_icp.py) with
+ * normals[n, 3] and intensity[n] (float; (r + g + b) / 3 of colours in [0, 1]), through its OWN voxel hash and with
+ * the neighbour sets of dgr_estimate_normals (radius / cell <= 4, the max_nn (1..64) smallest by (d^2, row), point i
+ * included).  With nn kept neighbours, each other one adds the row u = e - (e.n_i) n_i, b = I_j - I_i
+ * (e = p_j - p_i), and a last row (nn - 1) n_i with b = 0; grad[i] solves the normal equations
+ * (sum u u^T + (nn - 1)^2 n n^T) g = sum u b by a 3x3 Cholesky in fp64, rounded to float once.  g = 0 for nn < 4 or
+ * on a non-positive pivot.  grad: float [n, 3]; counts: int32 [n] = rows within the radius (before the max_nn
+ * truncation).  No atomics, the same bits on every run. */
+int32_t dgr_color_gradient(const float* xyz, const float* normals, const float* intensity, int64_t n,
+                           const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap,
+                           int32_t batch, double cell, double radius, int32_t max_nn, float* grad, int32_t* counts,
+                           void* stream);
 /* ICP of src onto tgt.  Correspondences: the nearest target point strictly within max_dist of each transformed
  * source point s, through the TARGET cloud's voxel hash (keys / vals / spec of the table dgr_unique_first built at
  * `voxel`; table rows = rows of tgt; `batch` = the batch index those coordinates carry; max_dist / voxel <= 4).
@@ -225,6 +237,21 @@ int32_t dgr_icp(const float* src, int64_t n_src, const float* tgt, const float* 
                 const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch, double voxel, double max_dist,
                 const double* T_init, int32_t max_iter, double rel_fitness, double rel_rmse, double* ws,
                 double* result, void* stream);
+/* Colored ICP (open3d 0.10 registration_colored_icp with TransformationEstimationForColoredICP(lambda_geometric);
+ * oracle/colored_icp.py): dgr_icp's correspondences, stopping rule, workspace (dgr_icp_ws_elems) and result, with
+ * two rows per correspondence (source point s, target point q, normal n, gradient d = tgt_grad from
+ * dgr_color_gradient, intensities I_s = src_intensity, I_t = tgt_intensity, all float):
+ *   geometric    r = sqrt(lambda) (s - q).n, J = sqrt(lambda) [s x n, n];
+ *   photometric  s' = s - ((s - q).n) n, m = -(I - n n^T) d: r = sqrt(1 - lambda) (I_s - (d.(s' - q) + I_t)),
+ *                J = sqrt(1 - lambda) [s x m, m];
+ * J^T J x = -J^T r by Cholesky (a non-positive pivot gives the identity update), T <- [Rz(x2) Ry(x1) Rx(x0) | x3..5] T.
+ * lambda_geometric in [0, 1]; at 1 the update is dgr_icp's point-to-plane one. */
+int32_t dgr_colored_icp(const float* src, const float* src_intensity, int64_t n_src, const float* tgt,
+                        const float* tgt_normals, const float* tgt_intensity, const float* tgt_grad,
+                        const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap,
+                        int32_t batch, double voxel, double max_dist, double lambda_geometric, const double* T_init,
+                        int32_t max_iter, double rel_fitness, double rel_rmse, double* ws, double* result,
+                        void* stream);
 
 /* ---- Multiway registration: open3d's GetInformationMatrixFromPointClouds and GlobalOptimization with
  *      GlobalOptimizationLevenbergMarquardt (csrc/posegraph.cu; oracle/pose_graph.py) ---------------------- */
