@@ -54,6 +54,12 @@ void dgr_knn_top1_packed(const float* f0, int n0, const float* f1, int n1, int c
     }                                                                 \
   } while (0)
 
+#define DGR_TRY(expr)                 \
+  do {                                \
+    int32_t rc__ = (expr);            \
+    if (rc__ != DGR_OK) return rc__;  \
+  } while (0)
+
 static inline unsigned dgr_blocks(int64_t n, int per_block) {
   int64_t b = (n + per_block - 1) / per_block;
   return (unsigned)(b < 1 ? 1 : b);
@@ -173,6 +179,103 @@ __device__ __forceinline__ void dgr_voxel_nearest8(const double p[3], bool have,
       best_j = oj;
     }
   }
+}
+
+// What every search of a voxel hash requires of its arguments, checked on the host: a power-of-two table capacity,
+// a positive cell and radius, and reach = ceil(radius / cell) <= max_reach (false for NaN)
+inline int32_t dgr_check_hash_search(int64_t cap, double cell, double radius, int max_reach) {
+  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
+  DGR_ARG_CHECK(cell > 0 && radius > 0, "cell and radius must be positive");
+  if (!(ceil(radius / cell) <= (double)max_reach)) {
+    dgr_set_error("%s:%d: bad argument: search radius above %d cells is not supported", __FILE__, __LINE__, max_reach);
+    return DGR_ERR_ARG;
+  }
+  return DGR_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// Radius neighbours of a point in its own cloud's voxel hash (one point per cell): open3d's hybrid search, restated
+// in oracle/normals.py (neighbours).  Row j is in the radius of point i when d2 = |p_j - p_i|^2 < radius^2, and the
+// rows are ranked by (d2, row).  Normals and colour gradients (icp.cu) and FPFH (fpfh.cu) search with these.
+// ---------------------------------------------------------------------------------------
+// offset e = p_j - p_i and d2 = |e|^2 evaluated as numpy does ((ex ex + ey ey) + ez ez, no contraction), so that the
+// strict radius test and the (d2, row) order agree with the oracle bit for bit
+__device__ __forceinline__ double dgr_offset_d2(const float* __restrict__ xyz, int32_t j, const double p[3],
+                                                double e[3]) {
+#pragma unroll
+  for (int a = 0; a < 3; ++a) e[a] = __dsub_rn((double)__ldg(xyz + 3 * (int64_t)j + a), p[a]);
+  return __dadd_rn(__dadd_rn(__dmul_rn(e[0], e[0]), __dmul_rn(e[1], e[1])), __dmul_rn(e[2], e[2]));
+}
+
+// (d2, row) of a before b
+__device__ __forceinline__ bool dgr_key_less(double da, int32_t ja, double db, int32_t jb) {
+  return da < db || (da == db && ja < jb);
+}
+
+// Cell c of the probe block (numbered as in dgr_probe_cell) can hold a point within the radius: sum max(|d| - 1, 0)^2
+// <= gap_limit = (radius / cell)^2 (1 + 1e-6), the margin covering the rounding of p / cell.  A dead cell cannot hold
+// a point strictly inside the radius, so skipping it changes no neighbour list.
+__host__ __device__ __forceinline__ bool dgr_cell_live(int c, int side, int reach, double gap_limit) {
+  const int dx = c % side - reach, dy = (c / side) % side - reach, dz = c / (side * side) - reach;
+  const int gx = dx < 0 ? -dx - 1 : dx - 1, gy = dy < 0 ? -dy - 1 : dy - 1, gz = dz < 0 ? -dz - 1 : dz - 1;
+  const int s = (gx > 0 ? gx * gx : 0) + (gy > 0 ? gy * gy : 0) + (gz > 0 ? gz * gz : 0);
+  return (double)s <= gap_limit;
+}
+
+inline double dgr_gap_limit(double radius, double cell) { return radius * radius * (1.0 + 1e-6) / (cell * cell); }
+
+// The live cells of the probe block: with one point per cell, the most keys dgr_gather_in_radius appends
+inline int dgr_live_cells(int reach, double gap_limit) {
+  const int side = 2 * reach + 1, n_cells = side * side * side;
+  int live = 0;
+  for (int c = 0; c < n_cells; ++c) live += dgr_cell_live(c, side, reach, gap_limit);
+  return live;
+}
+
+// The in-radius keys (d2, row) of point p, appended to kd / kj in cell order (ballot + prefix popcount), dead cells
+// not probed.  A whole warp calls it for one point; it returns the key count in every lane, with the keys visible
+// to the whole warp.  kd / kj have room for dgr_live_cells(reach, gap_limit) keys.
+__device__ __forceinline__ int dgr_gather_in_radius(const float* __restrict__ xyz, const double p[3], double cell,
+                                                    int reach, double r2, double gap_limit, int32_t batch,
+                                                    const dgr_keyspec_t& s, const uint64_t* __restrict__ keys,
+                                                    const int32_t* __restrict__ vals, uint64_t mask, double* kd,
+                                                    int32_t* kj) {
+  const int side = 2 * reach + 1, n_cells = side * side * side;
+  const int lane = threadIdx.x & 31;
+  int c3[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) c3[a] = (int)floor(p[a] / cell);
+  int cnt = 0;
+  for (int c0 = 0; c0 < n_cells; c0 += 32) {
+    const int c = c0 + lane;
+    int32_t j = -1;
+    double d2 = 0.0;
+    if (c < n_cells && dgr_cell_live(c, side, reach, gap_limit)) {
+      j = dgr_probe_cell(c, side, reach, c3, batch, s, keys, vals, mask);
+      if (j >= 0) {
+        double e[3];
+        d2 = dgr_offset_d2(xyz, j, p, e);
+        if (!(d2 < r2)) j = -1;
+      }
+    }
+    const unsigned ball = __ballot_sync(0xffffffffu, j >= 0);
+    if (j >= 0) {
+      const int pos = cnt + __popc(ball & ((1u << lane) - 1u));
+      kd[pos] = d2;
+      kj[pos] = j;
+    }
+    cnt += __popc(ball);
+  }
+  __syncwarp();
+  return cnt;
+}
+
+// Rank of the key (d2, j) among the cnt keys of kd / kj: how many come before it (keys are distinct: rows are).
+// The loop walks pointers: indexed as kd[l], the unrolled loop recomputed the warp's slice base every few keys.
+__device__ __forceinline__ int dgr_key_rank(const double* kd, const int32_t* kj, int cnt, double d2, int32_t j) {
+  int rank = 0;
+  for (const double* end = kd + cnt; kd < end; ++kd, ++kj) rank += dgr_key_less(*kd, *kj, d2, j);
+  return rank;
 }
 
 // ---------------------------------------------------------------------------------------

@@ -46,12 +46,6 @@ constexpr int kKeyMargin = 32;        // spare cells around the bounding box (7^
 bool tc_f16_enabled();
 int tc_f16_min_cout();
 
-#define DGR_TRY(expr)                 \
-  do {                                \
-    int32_t rc__ = (expr);            \
-    if (rc__ != DGR_OK) return rc__;  \
-  } while (0)
-
 __global__ void fill_f32_kernel(float* p, int64_t n, float v) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;

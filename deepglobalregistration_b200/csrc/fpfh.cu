@@ -2,9 +2,8 @@
 // restated in oracle/fpfh.py (which pins every convention).  The cloud is searched through its own voxel hash (a
 // dgr_unique_first table with at most one point per cell), reach = ceil(radius / cell) <= 6.  No atomics: every
 // sum has a fixed order, so a call gives the same bits on every run.
-//   fpfh_neighbour_kernel  a warp per point: the in-radius rows in cell order into shared memory (ballot + prefix
-//                          popcount), ranked by (d^2, row); the first max_nn without the point itself, with their
-//                          fp64 d^2, into the workspace in rank order
+//   fpfh_neighbour_kernel  a warp per point: the in-radius keys (dgr_gather_in_radius); the first max_nn without the
+//                          point itself, with their fp64 d^2, into the workspace in rank order
 //   fpfh_spfh_kernel       a warp per point: the fp64 pair features of its list, the 33 bin counts by ballot, each
 //                          bin = 100 / m added count times
 //   fpfh_kernel            4 threads per point: threads 0..2 the weighted sums of one 11-bin group over the
@@ -26,15 +25,6 @@ constexpr int kMaxReach = 6;
 constexpr int kMaxNN = 128;
 constexpr int kFpfhThreads = 128;                       // fpfh_kernel: 32 points x 4 threads
 
-// offset e = p_j - p_i and d2 = |e|^2 evaluated as numpy does ((ex ex + ey ey) + ez ez, no contraction): the
-// strict radius test and the (d^2, row) order agree with oracle/normals.py bit for bit
-__device__ __forceinline__ double offset_d2(const float* __restrict__ xyz, int32_t j, const double p[3]) {
-  double e[3];
-#pragma unroll
-  for (int a = 0; a < 3; ++a) e[a] = __dsub_rn((double)__ldg(xyz + 3 * (int64_t)j + a), p[a]);
-  return __dadd_rn(__dadd_rn(__dmul_rn(e[0], e[0]), __dmul_rn(e[1], e[1])), __dmul_rn(e[2], e[2]));
-}
-
 struct FpfhWs {
   double* d2;          // [n, max_nn] d^2 of the kept neighbours, rank order
   double* spfh;        // [n, 33]
@@ -55,28 +45,12 @@ int64_t fpfh_layout(int64_t n, int max_nn, void* base, FpfhWs* ws) {
   return c.words;
 }
 
-// Cell c of the probe block can hold a point within the radius: sum max(|d| - 1, 0)^2 <= gap_limit, gap_limit =
-// (radius / cell)^2 (1 + 1e-6) (the margin covers the rounding of p / cell).  The host counts these cells with the
-// same test to size the shared list: with one point per cell the list never holds more.
-__host__ __device__ __forceinline__ bool cell_live(int c, int side, int reach, double gap_limit) {
-  const int dx = c % side - reach, dy = (c / side) % side - reach, dz = c / (side * side) - reach;
-  const int gx = dx < 0 ? -dx - 1 : dx - 1, gy = dy < 0 ? -dy - 1 : dy - 1, gz = dz < 0 ? -dz - 1 : dz - 1;
-  const int s = (gx > 0 ? gx * gx : 0) + (gy > 0 ? gy * gy : 0) + (gz > 0 ? gz * gz : 0);
-  return (double)s <= gap_limit;
-}
-
-// (d2, row) of a before b
-__device__ __forceinline__ bool key_less(double da, int32_t ja, double db, int32_t jb) {
-  return da < db || (da == db && ja < jb);
-}
-
 __global__ void __launch_bounds__(kWarps * 32)
 fpfh_neighbour_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspec_t* __restrict__ spec_p,
                       const uint64_t* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask,
                       int32_t batch, double cell, int reach, double r2, double gap_limit, int slots, int max_nn,
                       FpfhWs ws, int32_t* __restrict__ counts) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  const int side = 2 * reach + 1, n_cells = side * side * side;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t i = (int64_t)blockIdx.x * kWarps + warp;
   if (i >= n) return;                                   // uniform per warp
@@ -85,34 +59,7 @@ fpfh_neighbour_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspe
                 (size_t)warp * slots;
   const dgr_keyspec_t s = *spec_p;
   const double p[3] = {(double)xyz[3 * i], (double)xyz[3 * i + 1], (double)xyz[3 * i + 2]};
-  int c3[3];
-#pragma unroll
-  for (int a = 0; a < 3; ++a) c3[a] = (int)floor(p[a] / cell);
-  // the in-radius rows in cell order (ordered append: ballot + prefix popcount); cells that cannot meet the ball
-  // are not probed
-  int cnt = 0;
-  for (int c0 = 0; c0 < n_cells; c0 += 32) {
-    const int c = c0 + lane;
-    int32_t j = -1;
-    double d2 = 0.0;
-    if (c < n_cells) {
-      if (cell_live(c, side, reach, gap_limit)) {
-        j = dgr_probe_cell(c, side, reach, c3, batch, s, keys, vals, mask);
-        if (j >= 0) {
-          d2 = offset_d2(xyz, j, p);
-          if (!(d2 < r2)) j = -1;
-        }
-      }
-    }
-    const unsigned ball = __ballot_sync(0xffffffffu, j >= 0);
-    if (j >= 0) {
-      const int pos = cnt + __popc(ball & ((1u << lane) - 1u));
-      kd[pos] = d2;
-      kj[pos] = j;
-    }
-    cnt += __popc(ball);
-  }
-  __syncwarp();
+  const int cnt = dgr_gather_in_radius(xyz, p, cell, reach, r2, gap_limit, batch, s, keys, vals, mask, kd, kj);
   // the point itself (d^2 = 0: rank 0 when present, rows being distinct points) is dropped; the others keep
   // their rank among the first max_nn, shifted down by one
   bool self = false;
@@ -123,8 +70,7 @@ fpfh_neighbour_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspe
     const double dk = kd[k];
     const int32_t jk = kj[k];
     if (jk == (int32_t)i) continue;
-    int rank = 0;
-    for (int l = 0; l < cnt; ++l) rank += key_less(kd[l], kj[l], dk, jk);
+    const int rank = dgr_key_rank(kd, kj, cnt, dk, jk);
     if (rank < max_nn) {
       const int pos = rank - has_self;
       ws.nb[i * K + pos] = jk;
@@ -283,9 +229,7 @@ int32_t dgr_compute_fpfh(const float* xyz, const float* normals, int64_t n, cons
   DGR_ARG_CHECK(normals != nullptr, "normals are required");
   DGR_ARG_CHECK(n == 0 || (xyz != nullptr && spec != nullptr && keys != nullptr && vals != nullptr && ws != nullptr &&
                            out != nullptr && counts != nullptr), "null pointer");
-  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
-  DGR_ARG_CHECK(cell > 0 && radius > 0, "cell and radius must be positive");
-  DGR_ARG_CHECK(ceil(radius / cell) <= (double)kMaxReach, "search radius above 6 cells is not supported");
+  DGR_TRY(dgr_check_hash_search(cap, cell, radius, kMaxReach));
   DGR_ARG_CHECK(max_nn >= 1 && max_nn <= kMaxNN, "max_nn must lie in [1, 128]");
   DGR_ARG_CHECK(ld >= kDim, "row stride ld must be at least 33");
   if (n == 0) return DGR_OK;
@@ -293,10 +237,8 @@ int32_t dgr_compute_fpfh(const float* xyz, const float* normals, int64_t n, cons
   FpfhWs w;
   fpfh_layout(n, max_nn, ws, &w);
   const int reach = (int)ceil(radius / cell);
-  const int side = 2 * reach + 1, n_cells = side * side * side;
-  const double gap_limit = radius * radius * (1.0 + 1e-6) / (cell * cell);
-  int slots = 0;
-  for (int c = 0; c < n_cells; ++c) slots += cell_live(c, side, reach, gap_limit);
+  const double gap_limit = dgr_gap_limit(radius, cell);
+  const int slots = dgr_live_cells(reach, gap_limit);
   const size_t smem = (size_t)kWarps * slots * (sizeof(double) + sizeof(int32_t));     // < 103 KB (reach 6)
   DGR_ENSURE_SMEM(fpfh_neighbour_kernel, smem);
   fpfh_neighbour_kernel<<<dgr_blocks(n, kWarps), kWarps * 32, smem, st>>>(

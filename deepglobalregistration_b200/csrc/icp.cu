@@ -8,8 +8,8 @@
 //   nbr_probe_kernel<S>      8 lanes per point, one probe pass: count and the 9 fp64 sums S adds over the rows with
 //                            |p_j - p_i|^2 < radius^2 (the offsets' cumulants for normals, the gradient rows for
 //                            colour gradients); a point with <= max_nn of them gets its result
-//   nbr_select_kernel<S>     a warp per point with more than max_nn: the in-radius rows again, in cell order, into
-//                            shared memory; the max_nn smallest (d^2, row) keys by rank; their sums
+//   nbr_select_kernel<S>     a warp per point with more than max_nn: the in-radius keys again (dgr_gather_in_radius);
+//                            the sums of the max_nn ranked first
 //   icp_match_kernel<E>      nearest target row within max_dist (dgr_voxel_nearest8); the estimator's sums, the
 //                            count and sum d^2 as per-block partials
 //   icp_update_kernel<E>     the partials reduced in block order, open3d's stopping rule, the estimator's step
@@ -23,19 +23,12 @@ namespace {
 
 constexpr int kNormThreads = 256;
 constexpr int kSelWarps = 4;                            // nbr_select_kernel: warps (points) per block
+constexpr int kMaxReach = 4;                            // normals, colour gradients and ICP
 constexpr int kMaxNN = 64;
 constexpr int kIcpThreads = 256;
 constexpr int kIcpMaxBlocks = 2368;
 constexpr int kIcpStride = 32;                          // doubles per block partial
 constexpr int kIcpState = 32;                           // doubles of IcpState (static_assert below)
-
-// offset e = p_j - p_i and d2 = |e|^2 evaluated as numpy does ((ex ex + ey ey) + ez ez, no contraction), so that
-// the strict radius test and the (d^2, row) order agree with the oracle bit for bit
-__device__ __forceinline__ double offset_d2(const float* __restrict__ xyz, int32_t j, const double p[3], double e[3]) {
-#pragma unroll
-  for (int a = 0; a < 3; ++a) e[a] = __dsub_rn((double)__ldg(xyz + 3 * (int64_t)j + a), p[a]);
-  return __dadd_rn(__dadd_rn(__dmul_rn(e[0], e[0]), __dmul_rn(e[1], e[1])), __dmul_rn(e[2], e[2]));
-}
 
 // m[0..3) += e, m[3..9) += e e^T (xx, xy, xz, yy, yz, zz)
 __device__ __forceinline__ void add_cumulants(double m[9], const double e[3]) {
@@ -168,7 +161,7 @@ nbr_probe_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspec_t* 
     const int32_t j = dgr_probe_cell(c, side, reach, c3, batch, s, keys, vals, mask);
     if (j < 0) continue;
     double e[3];
-    if (offset_d2(xyz, j, p, e) < r2) {
+    if (dgr_offset_d2(xyz, j, p, e) < r2) {
       ++cnt;
       sums.add(q, m, e, j);
     }
@@ -184,60 +177,30 @@ nbr_probe_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspec_t* 
   if (cnt <= max_nn) sums.store(m, cnt, i);
 }
 
-// (d2, row) of a before b
-__device__ __forceinline__ bool key_less(double da, int32_t ja, double db, int32_t jb) {
-  return da < db || (da == db && ja < jb);
-}
-
 template <class S>
 __global__ void __launch_bounds__(kSelWarps * 32)
 nbr_select_kernel(const float* __restrict__ xyz, int64_t n, const dgr_keyspec_t* __restrict__ spec_p,
                   const uint64_t* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask, int32_t batch,
-                  double cell, int reach, double r2, int max_nn, const S sums, const int32_t* __restrict__ counts) {
+                  double cell, int reach, double r2, double gap_limit, int slots, int max_nn, const S sums,
+                  const int32_t* __restrict__ counts) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  const int side = 2 * reach + 1, n_cells = side * side * side;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t i = (int64_t)blockIdx.x * kSelWarps + warp;
   if (i >= n || counts[i] <= max_nn) return;            // uniform per warp
-  double* kd = reinterpret_cast<double*>(smem_raw) + (size_t)warp * n_cells;
-  int32_t* kj = reinterpret_cast<int32_t*>(reinterpret_cast<double*>(smem_raw) + (size_t)kSelWarps * n_cells) +
-                (size_t)warp * n_cells;
+  double* kd = reinterpret_cast<double*>(smem_raw) + (size_t)warp * slots;
+  int32_t* kj = reinterpret_cast<int32_t*>(reinterpret_cast<double*>(smem_raw) + (size_t)kSelWarps * slots) +
+                (size_t)warp * slots;
   const dgr_keyspec_t s = *spec_p;
   const double p[3] = {(double)xyz[3 * i], (double)xyz[3 * i + 1], (double)xyz[3 * i + 2]};
-  int c3[3];
-#pragma unroll
-  for (int a = 0; a < 3; ++a) c3[a] = (int)floor(p[a] / cell);
-  // the in-radius rows in cell order (ordered append: ballot + prefix popcount)
-  int m_cnt = 0;
-  for (int c0 = 0; c0 < n_cells; c0 += 32) {
-    const int c = c0 + lane;
-    int32_t j = c < n_cells ? dgr_probe_cell(c, side, reach, c3, batch, s, keys, vals, mask) : -1;
-    double d2 = 0.0;
-    if (j >= 0) {
-      double e[3];
-      d2 = offset_d2(xyz, j, p, e);
-      if (!(d2 < r2)) j = -1;
-    }
-    const unsigned ball = __ballot_sync(0xffffffffu, j >= 0);
-    if (j >= 0) {
-      const int pos = m_cnt + __popc(ball & ((1u << lane) - 1u));
-      kd[pos] = d2;
-      kj[pos] = j;
-    }
-    m_cnt += __popc(ball);
-  }
-  __syncwarp();
-  // candidate k is kept when fewer than max_nn keys rank before it (keys are distinct: rows are)
+  const int cnt = dgr_gather_in_radius(xyz, p, cell, reach, r2, gap_limit, batch, s, keys, vals, mask, kd, kj);
+  // candidate k is kept when fewer than max_nn keys rank before it
   const typename S::Point q = sums.point(i);
   double mm[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-  for (int k = lane; k < m_cnt; k += 32) {
-    const double dk = kd[k];
+  for (int k = lane; k < cnt; k += 32) {
     const int32_t jk = kj[k];
-    int rank = 0;
-    for (int l = 0; l < m_cnt; ++l) rank += key_less(kd[l], kj[l], dk, jk);
-    if (rank < max_nn) {
+    if (dgr_key_rank(kd, kj, cnt, kd[k], jk) < max_nn) {
       double e[3];
-      offset_d2(xyz, jk, p, e);
+      dgr_offset_d2(xyz, jk, p, e);
       sums.add(q, mm, e, jk);
     }
   }
@@ -509,20 +472,18 @@ int32_t nbr_launch(const float* xyz, int64_t n, const dgr_keyspec_t* spec, const
   DGR_ARG_CHECK(n >= 0 && n < (1ll << 31), "point count out of range");
   DGR_ARG_CHECK(n == 0 || (xyz != nullptr && spec != nullptr && keys != nullptr && vals != nullptr &&
                            counts != nullptr), "null pointer");
-  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
-  DGR_ARG_CHECK(cell > 0 && radius > 0, "cell and radius must be positive");
-  DGR_ARG_CHECK(radius / cell <= 4.0, "search radius above 4 cells is not supported");
+  DGR_TRY(dgr_check_hash_search(cap, cell, radius, kMaxReach));
   DGR_ARG_CHECK(max_nn >= 1 && max_nn <= kMaxNN, "max_nn must lie in [1, 64]");
   if (n == 0) return DGR_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const int reach = (int)ceil(radius / cell);
-  const int side = 2 * reach + 1, n_cells = side * side * side;
-  const double r2 = radius * radius;
+  const double r2 = radius * radius, gap_limit = dgr_gap_limit(radius, cell);
+  const int slots = dgr_live_cells(reach, gap_limit);
   nbr_probe_kernel<S><<<dgr_blocks(n * 8, kNormThreads), kNormThreads, 0, st>>>(
       xyz, n, spec, keys, vals, (uint64_t)cap - 1, batch, cell, reach, r2, max_nn, sums, counts);
-  const size_t smem = (size_t)kSelWarps * n_cells * (sizeof(double) + sizeof(int32_t));   // <= 35 KB
+  const size_t smem = (size_t)kSelWarps * slots * (sizeof(double) + sizeof(int32_t));   // <= 35 KB (reach 4)
   nbr_select_kernel<S><<<dgr_blocks(n, kSelWarps), kSelWarps * 32, smem, st>>>(
-      xyz, n, spec, keys, vals, (uint64_t)cap - 1, batch, cell, reach, r2, max_nn, sums, counts);
+      xyz, n, spec, keys, vals, (uint64_t)cap - 1, batch, cell, reach, r2, gap_limit, slots, max_nn, sums, counts);
   dgr_note_launches(2);
   DGR_LAUNCH_CHECK();
   return DGR_OK;
@@ -579,9 +540,8 @@ int32_t dgr_icp(const float* src, int64_t n_src, const float* tgt, const float* 
                 const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch, double voxel, double max_dist,
                 const double* T_init, int32_t max_iter, double rel_fitness, double rel_rmse, double* ws,
                 double* result, void* stream) {
-  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
-  DGR_ARG_CHECK(voxel > 0 && max_dist > 0 && max_iter >= 0, "bad ICP parameters");
-  DGR_ARG_CHECK(max_dist / voxel <= 4.0, "search radius above 4 voxels is not supported");
+  DGR_TRY(dgr_check_hash_search(cap, voxel, max_dist, kMaxReach));
+  DGR_ARG_CHECK(max_iter >= 0, "bad ICP parameters");
   DGR_ARG_CHECK(n_src >= 0 && n_src < (1ll << 31), "point count out of range");
   DGR_ARG_CHECK(T_init != nullptr && ws != nullptr && result != nullptr && spec != nullptr, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
@@ -602,10 +562,9 @@ int32_t dgr_colored_icp(const float* src, const float* src_intensity, int64_t n_
                         int32_t batch, double voxel, double max_dist, double lambda_geometric, const double* T_init,
                         int32_t max_iter, double rel_fitness, double rel_rmse, double* ws, double* result,
                         void* stream) {
-  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
-  DGR_ARG_CHECK(voxel > 0 && max_dist > 0 && max_iter >= 0, "bad ICP parameters");
+  DGR_TRY(dgr_check_hash_search(cap, voxel, max_dist, kMaxReach));
+  DGR_ARG_CHECK(max_iter >= 0, "bad ICP parameters");
   DGR_ARG_CHECK(lambda_geometric >= 0.0 && lambda_geometric <= 1.0, "lambda_geometric must lie in [0, 1]");
-  DGR_ARG_CHECK(max_dist / voxel <= 4.0, "search radius above 4 voxels is not supported");
   DGR_ARG_CHECK(n_src >= 0 && n_src < (1ll << 31), "point count out of range");
   DGR_ARG_CHECK(T_init != nullptr && ws != nullptr && result != nullptr && spec != nullptr && keys != nullptr &&
                 vals != nullptr && tgt != nullptr && tgt_normals != nullptr && tgt_intensity != nullptr &&

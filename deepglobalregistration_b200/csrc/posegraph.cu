@@ -717,9 +717,7 @@ int32_t dgr_information_matrix(const float* src, int64_t n_src, const float* tgt
                 vals != nullptr, "null pointer");
   DGR_ARG_CHECK(n_src >= 0 && n_src < (1ll << 31), "point count out of range");
   DGR_ARG_CHECK(n_src == 0 || (src != nullptr && tgt != nullptr), "null pointer");
-  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
-  DGR_ARG_CHECK(cell > 0 && max_dist > 0, "cell and max_dist must be positive");
-  DGR_ARG_CHECK(max_dist / cell <= 4.0, "search radius above 4 cells is not supported");
+  DGR_TRY(dgr_check_hash_search(cap, cell, max_dist, 4));
   DGR_ARG_CHECK(finite_all(T, 16), "transformation must be finite");
   cudaStream_t st = (cudaStream_t)stream;
   Pose12 P;

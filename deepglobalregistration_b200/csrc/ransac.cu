@@ -482,9 +482,7 @@ int32_t dgr_ransac_feature_matching(const float* src, int64_t n_src, const float
   DGR_ARG_CHECK(n_src >= 1 && n_src <= kFmChunk * kFmMaxChunks, "source point count out of range");
   DGR_ARG_CHECK(max_iteration >= 1 && max_iteration <= (1ll << 30), "hypothesis count out of range");
   DGR_ARG_CHECK(max_validation >= 1, "max_validation must be positive");
-  DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
-  DGR_ARG_CHECK(cell > 0 && max_dist > 0, "cell and max_dist must be positive");
-  DGR_ARG_CHECK(max_dist / cell <= 4.0, "search radius above 4 cells is not supported");
+  DGR_TRY(dgr_check_hash_search(cap, cell, max_dist, 4));
   DGR_ARG_CHECK(edge_ratio >= 0, "edge_ratio must be >= 0 (0 = no edge-length checker)");
   cudaStream_t st = (cudaStream_t)stream;
   FmWs w;
