@@ -3,8 +3,8 @@
 Every entry point's argtypes / restype and the integer DGR_* constants are read from the
 header the library is compiled against, so the binding cannot drift from the C ABI.
 
-torch is used here for device memory and the current CUDA stream only; every
-computation happens inside the library.  There is no CPU fallback: importing this
+torch is used here for device memory, the current CUDA stream and dtype conversions
+(float32_in_cells) only; every computation happens inside the library.  There is no CPU fallback: importing this
 module without a built library, or calling into it without an sm_90 device,
 raises.
 """
@@ -293,6 +293,25 @@ def voxelise(xyz, voxel, batch=0):
   table, sel, inverse, cnt = unique_first(raw, spec)
   n = read_count(cnt)
   return raw, spec, table, sel[:n], inverse, n
+
+
+CELL_NUDGE_STEPS = 4   # float32 ulps a row may move; a float64 row needs 1, a row quantised in float32 at most 2
+
+
+def float32_in_cells(xyz, cells, cell):
+  """xyz float64/float32 [n, 3] as the float32 rows a hash search may read: floor(double(x) / cell) - the cell every
+  search kernel computes - equals the row's stored cell `cells` (int [n, 3]; voxelise's raw coords [:, 1:]) in every
+  coordinate.  A table keyed in float64 (or by a float32 division) can hold a row whose float32 value lies across a
+  cell boundary; such a coordinate is moved toward its cell one float32 ulp at a time, every other one is exactly
+  xyz.float().  Without this a search can miss an in-radius row (DESIGN.md §3)."""
+  x32 = xyz.float()
+  k = cells.double()
+  c = torch.tensor(float(cell), dtype=torch.float64, device=xyz.device)   # a scalar divisor becomes a reciprocal
+  for _ in range(CELL_NUDGE_STEPS):
+    xd = x32.double()
+    off = k - torch.floor(xd / c)
+    x32 = torch.where(off == 0, x32, torch.nextafter(x32, (off * math.inf).float()))
+  return x32.contiguous()
 
 
 def hash_find(coords, spec, table):

@@ -132,7 +132,8 @@ class DeepGlobalRegistration:
       dxyz = self._upload(xyz, _slot)
     raw_coords, spec, table, sel, _, npts = _abi.voxelise(dxyz, self.voxel_size, batch=_batch)
     coords = _abi.gather_rows_i32(raw_coords, sel, npts)
-    xyz_sel = dxyz[sel.long()].float()
+    # float32 rows the ICP refine and the baselines search this table with: in the cells they are stored under
+    xyz_sel = _abi.float32_in_cells(dxyz[sel.long()], coords[:, 1:], self.voxel_size)
     # the dedup table already maps voxel key -> row of `coords`: hand it to SparseTensor
     coords._dgr_manager = CoordinateManager(_parts=(coords, spec, table))
     self._last_sel_value, self._last_ctx = sel, None

@@ -117,8 +117,9 @@ class MultiwayRegistration:
     if isinstance(cloud, (str, bytes)) or hasattr(cloud, '__fspath__'):
       cloud = sharding._cloud(cloud)
     x64 = torch.from_numpy(np.ascontiguousarray(np.asarray(cloud, dtype=np.float64).reshape(-1, 3))).to(dev)
-    _, spec, table, sel, _, n = _abi.voxelise(x64, self.voxel_size)
-    return x64[sel.long()].float().contiguous(), (spec, table), n
+    raw, spec, table, sel, _, n = _abi.voxelise(x64, self.voxel_size)
+    sel = sel.long()
+    return _abi.float32_in_cells(x64[sel], raw[sel, 1:], self.voxel_size), (spec, table), n
 
   def edges(self, clouds, pairs, X, device='cuda'):
     """The information matrix of every pair (i, j) under X[k], on the voxelised fragments.
@@ -140,8 +141,8 @@ class MultiwayRegistration:
     and colour gradients at radius 2 sigma, max_nn 30."""
     from ..o3d_registration import intensity
     x64 = torch.from_numpy(np.ascontiguousarray(pts)).to(dev)
-    _, spec, table, sel, _, _ = _abi.voxelise(x64, sigma)
-    x = x64[sel.long()].float().contiguous()
+    raw, spec, table, sel, _, _ = _abi.voxelise(x64, sigma)
+    x = _abi.float32_in_cells(x64[sel.long()], raw[sel.long(), 1:], sigma)
     inten = torch.from_numpy(intensity(colors)).to(dev)[sel.long()].contiguous()
     nrm = _abi.estimate_normals(x, (spec, table), sigma, 2 * sigma, 30)
     grad = _abi.color_gradient(x, nrm, inten, (spec, table), sigma, 2 * sigma, 30)

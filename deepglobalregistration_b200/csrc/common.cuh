@@ -182,10 +182,11 @@ __device__ __forceinline__ void dgr_voxel_nearest8(const double p[3], bool have,
 }
 
 // What every search of a voxel hash requires of its arguments, checked on the host: a power-of-two table capacity,
-// a positive cell and radius, and reach = ceil(radius / cell) <= max_reach (false for NaN)
+// a positive finite cell, a positive radius, and reach = ceil(radius / cell) <= max_reach (false for NaN and an
+// infinite radius; an infinite cell would give reach 0)
 inline int32_t dgr_check_hash_search(int64_t cap, double cell, double radius, int max_reach) {
   DGR_ARG_CHECK(cap > 0 && (cap & (cap - 1)) == 0, "capacity must be a power of two");
-  DGR_ARG_CHECK(cell > 0 && radius > 0, "cell and radius must be positive");
+  DGR_ARG_CHECK(cell > 0 && cell < INFINITY && radius > 0, "cell and radius must be positive, the cell finite");
   if (!(ceil(radius / cell) <= (double)max_reach)) {
     dgr_set_error("%s:%d: bad argument: search radius above %d cells is not supported", __FILE__, __LINE__, max_reach);
     return DGR_ERR_ARG;

@@ -121,10 +121,9 @@ def estimate_normals(points, search_param, prev=None):
   dev = _abi.require_device('cuda')
   _abi.refresh_stream()
   p64 = torch.from_numpy(np.ascontiguousarray(pts)).to(dev)
-  cell, spec, table = _target_hash(p64, search_param.radius)
+  cell, spec, table, p32 = _target_hash(p64, search_param.radius, rows=True)
   prev_d = None if prev is None else torch.from_numpy(np.ascontiguousarray(prev, dtype=np.float32)).to(dev)
-  nrm = _abi.estimate_normals(p64.float().contiguous(), (spec, table), cell, search_param.radius, search_param.max_nn,
-                              prev=prev_d)
+  nrm = _abi.estimate_normals(p32, (spec, table), cell, search_param.radius, search_param.max_nn, prev=prev_d)
   return nrm.cpu().numpy().astype(np.float64)
 
 
@@ -185,18 +184,20 @@ def _points(pcd, device):
   return torch.from_numpy(np.ascontiguousarray(pts)).to(device)
 
 
-def _target_hash(tgt64, max_dist, max_reach=4, what='max_correspondence_distance'):
+def _target_hash(tgt64, max_dist, max_reach=4, what='max_correspondence_distance', rows=False):
   """Voxel hash of the target with at most one point per cell (what the ICP, normal and FPFH kernels search): cell =
   max_dist / 2 as in DGR (voxelised clouds, radius 2 voxels); a cloud with several points per cell gets finer
   cells up to the kernel's reach (4 for ICP and normals, 6 for FPFH, whose 5-voxel radius needs cell = max_dist / 5).
-  A cell whose quotient max_dist / cell rounds above the reach is widened by one ulp."""
+  A cell whose quotient max_dist / cell rounds above the reach is widened by one ulp.  -> (cell, spec, table), and with
+  rows=True also the target as the float32 rows a search of this table must read (_abi.float32_in_cells of the
+  table's cells)."""
   for div in range(2, max_reach + 1):
     cell = max_dist / div
     if math.ceil(max_dist / cell) > max_reach:
       cell = float(np.nextafter(cell, np.inf))
-    _, spec, table, _, _, n = _abi.voxelise(tgt64, cell)
-    if n == tgt64.shape[0]:
-      return cell, spec, table
+    raw, spec, table, _, _, n = _abi.voxelise(tgt64, cell)
+    if n == tgt64.shape[0]:                 # every row kept: raw row i is target row i
+      return (cell, spec, table, _abi.float32_in_cells(tgt64, raw[:, 1:], cell)) if rows else (cell, spec, table)
   raise NotImplementedError(f'target has several points within {what} / {max_reach} of each other: '
                             'voxel-downsample it first (DGR always passes voxelised clouds)')
 
@@ -221,8 +222,8 @@ def compute_fpfh_feature(input, search_param):
   dev = _abi.require_device('cuda')
   _abi.refresh_stream()
   p64 = torch.from_numpy(np.ascontiguousarray(pts)).to(dev)
-  cell, spec, table = _target_hash(p64, search_param.radius, max_reach=6, what='the radius')
-  f = _abi.compute_fpfh(p64.float().contiguous(), torch.from_numpy(np.ascontiguousarray(nrm)).to(dev), (spec, table),
+  cell, spec, table, p32 = _target_hash(p64, search_param.radius, max_reach=6, what='the radius', rows=True)
+  f = _abi.compute_fpfh(p32, torch.from_numpy(np.ascontiguousarray(nrm)).to(dev), (spec, table),
                         cell, search_param.radius, search_param.max_nn)
   feature.data = f.cpu().numpy().astype(np.float64).T.copy()
   return feature
@@ -245,8 +246,8 @@ def registration_icp(source, target, max_correspondence_distance, init=None, est
   T0 = np.eye(4) if init is None else np.asarray(init, dtype=np.float64).reshape(4, 4)
   if len(src64) == 0 or len(tgt64) == 0:
     return RegistrationResult(T0)
-  cell, spec, table = _target_hash(tgt64, float(max_correspondence_distance))
-  src, tgt = src64.float().contiguous(), tgt64.float().contiguous()
+  cell, spec, table, tgt = _target_hash(tgt64, float(max_correspondence_distance), rows=True)
+  src = src64.float().contiguous()
   T12 = torch.from_numpy(np.ascontiguousarray(T0[:3])).to(dev)
   args = (float(max_correspondence_distance), T12, int(criteria.max_iteration), float(criteria.relative_fitness),
           float(criteria.relative_rmse))
@@ -327,8 +328,8 @@ def registration_colored_icp(source, target, *args, **kwargs):
   dev = _abi.require_device('cuda')
   _abi.refresh_stream()
   src64, tgt64 = _points(source, dev), _points(target, dev)
-  cell, spec, table = _target_hash(tgt64, 2.0 * max_distance, what='2 max_distance')
-  src, tgt = src64.float().contiguous(), tgt64.float().contiguous()
+  cell, spec, table, tgt = _target_hash(tgt64, 2.0 * max_distance, what='2 max_distance', rows=True)
+  src = src64.float().contiguous()
   nrm_d = torch.from_numpy(np.ascontiguousarray(nrm)).to(dev)
   i_src = torch.from_numpy(intensity(c_src)).to(dev)
   i_tgt = torch.from_numpy(intensity(c_tgt)).to(dev)
@@ -403,9 +404,9 @@ def registration_ransac_based_on_feature_matching(source, target, source_feature
   if len(src64) == 0 or len(tgt64) == 0:
     return RegistrationResult(np.eye(4))
   d = float(max_correspondence_distance)
-  cell, spec, table = _target_hash(tgt64, d)
+  cell, spec, table, tgt = _target_hash(tgt64, d, rows=True)
   nn = _abi.knn_top1(torch.from_numpy(np.ascontiguousarray(fs)).to(dev), torch.from_numpy(np.ascontiguousarray(ft)).to(dev))
-  r = _abi.ransac_feature_matching(src64.float().contiguous(), tgt64.float().contiguous(), nn, spec, table, cell, d,
+  r = _abi.ransac_feature_matching(src64.float().contiguous(), tgt, nn, spec, table, cell, d,
                                    edge_ratio, check_dist, criteria.max_iteration, criteria.max_validation,
                                    seed=seed).cpu().numpy()
   return RegistrationResult(r[:16], r[16], r[17], r[19])
@@ -492,8 +493,8 @@ def get_information_matrix_from_point_clouds(source, target, max_correspondence_
   dev = _abi.require_device('cuda')
   _abi.refresh_stream()
   src64, tgt64 = _points(source, dev), _points(target, dev)
-  cell, spec, table = _target_hash(tgt64, d)
-  out = _abi.information_matrix(src64.float().contiguous(), tgt64.float().contiguous(), (spec, table), cell, d, T)
+  cell, spec, table, tgt = _target_hash(tgt64, d, rows=True)
+  out = _abi.information_matrix(src64.float().contiguous(), tgt, (spec, table), cell, d, T)
   return out.cpu().numpy()[:36].reshape(6, 6).copy()
 
 

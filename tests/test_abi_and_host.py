@@ -2,6 +2,7 @@
 include/dgr_b200.h (no compute calls without a GPU); the ME-shaped host API has the
 surface the reference touches; product code fails loudly without CUDA."""
 import ctypes
+import math
 import os
 import re
 
@@ -142,3 +143,99 @@ def test_native_layer_table_parameter_order():
     # folded BatchNorm: scale = weight / sqrt(var + eps)
     bn = m.norm1.bn
     assert torch.allclose(ps[1], bn.weight / torch.sqrt(bn.running_var + bn.eps))
+
+
+# The argument check every voxel-hash search shares (dgr_check_hash_search), host-only: each call also breaks one
+# argument checked after it (max_nn 0, max_iter -1, a non-finite pose, edge_ratio -1), so that no call launches.
+HASH_SEARCHES = {'dgr_estimate_normals': (4, 'max_nn'), 'dgr_color_gradient': (4, 'max_nn'),
+                 'dgr_compute_fpfh': (6, 'max_nn'), 'dgr_icp': (4, 'bad ICP parameters'),
+                 'dgr_colored_icp': (4, 'bad ICP parameters'), 'dgr_information_matrix': (4, 'must be finite'),
+                 'dgr_ransac_feature_matching': (4, 'edge_ratio')}
+HASH_REFUSALS = ('capacity must be a power of two', 'must be positive', 'search radius above')
+
+
+def hash_search_refusal(name, cap, cell, radius):
+  """Which dgr_check_hash_search refusal entry point `name` gives for (cap, cell, radius); None when it passes."""
+  from deepglobalregistration_b200 import _abi
+  keep = [(ctypes.c_double * 16)(*[math.nan] * 16)]
+  nz = ctypes.addressof(keep[0])                      # a host address where only null is checked
+  args = {
+      'dgr_estimate_normals': (None, 0, None, None, None, cap, 0, cell, radius, 0, None, None, None, None),
+      'dgr_color_gradient': (None, None, None, 0, None, None, None, cap, 0, cell, radius, 0, None, None, None),
+      'dgr_compute_fpfh': (None, nz, 0, None, None, None, cap, 0, cell, radius, 0, 33, None, None, None, None),
+      'dgr_icp': (None, 0, None, None, nz, nz, nz, cap, 0, cell, radius, nz, -1, 1e-6, 1e-6, nz, nz, None),
+      'dgr_colored_icp': (None, None, 0, nz, nz, nz, nz, nz, nz, nz, cap, 0, cell, radius, 0.968, nz, -1, 1e-6, 1e-6,
+                          nz, nz, None),
+      'dgr_information_matrix': (None, 0, None, nz, nz, nz, cap, 0, cell, radius, nz, nz, nz, None),
+      'dgr_ransac_feature_matching': (nz, 1, nz, nz, nz, nz, nz, cap, 0, cell, radius, -1.0, 0.0, 1, 1, 0, nz, nz,
+                                      None),
+  }[name]
+  assert getattr(_abi.lib(), name)(*args) == _abi._DEFINES['DGR_ERR_ARG']
+  msg = _abi.lib().dgr_last_error().decode()
+  hit = [m for m in HASH_REFUSALS if m in msg]
+  assert hit or HASH_SEARCHES[name][1] in msg, msg
+  return hit[0] if hit else None
+
+
+def largest_radius(reach, cell):
+  """The largest double radius with ceil(radius / cell) <= reach."""
+  r = reach * cell
+  while math.ceil(r / cell) > reach:
+    r = float(np.nextafter(r, 0.0))
+  while math.ceil(float(np.nextafter(r, math.inf)) / cell) <= reach:
+    r = float(np.nextafter(r, math.inf))
+  return r
+
+
+@pytest.mark.parametrize('name', sorted(HASH_SEARCHES))
+def test_hash_search_argument_boundaries(built, name):
+  reach = HASH_SEARCHES[name][0]
+  for cell in (0.0625, 0.05, 0.3, 0.07, 1e-3):
+    r = largest_radius(reach, cell)
+    assert hash_search_refusal(name, 1024, cell, r) is None, (cell, r)
+    assert hash_search_refusal(name, 1024, cell, float(np.nextafter(r, math.inf))) == 'search radius above'
+    assert hash_search_refusal(name, 1024, cell, 0.5 * cell) is None
+  assert hash_search_refusal(name, 1024, 0.0625, reach * 0.0625) is None          # an exact ratio at the reach
+  assert hash_search_refusal(name, 1024, 0.0625, (reach + 1) * 0.0625) == 'search radius above'
+  for bad in (math.nan, math.inf, -math.inf, 0.0, -0.0, -0.05, 5e-324 * -1):
+    assert hash_search_refusal(name, 1024, bad, 0.1) == 'must be positive', bad
+    if bad != math.inf:
+      assert hash_search_refusal(name, 1024, 0.05, bad) == 'must be positive', bad
+  assert hash_search_refusal(name, 1024, 0.05, math.inf) == 'search radius above'
+  for cap in (0, 3, 6, 1000, -8, 2 ** 62 + 2 ** 61):
+    assert hash_search_refusal(name, cap, 0.05, 0.1) == 'capacity must be a power of two', cap
+  for cap in (1, 2, 2 ** 20, 2 ** 62):
+    assert hash_search_refusal(name, cap, 0.05, 0.1) is None, cap
+
+
+def ordered(x32):
+  """float32 bits as integers in value order (-0.0 and +0.0 both 0): differences count ulps."""
+  b = np.asarray(x32, np.float32).view(np.int32).astype(np.int64)
+  return np.where(b < 0, -(b & 0x7FFFFFFF), b)
+
+
+def test_float32_in_cells_moves_only_boundary_rows():
+  """_abi.float32_in_cells (on CPU tensors) over the hash-search test clouds: every row ends in its stored cell, a row
+  whose float32 value is already there keeps its bits, and no coordinate moves more than CELL_NUDGE_STEPS ulps; keys
+  from float64 (the stand-ins, multiway) and from a float32 division (preprocess() of float32 input)."""
+  from deepglobalregistration_b200 import _abi
+  from test_gpu_hash_search_edges import rows_in_cells, snapped_cloud, straddling_pairs
+  clouds = [(np.array([[-127.9000015258789, 0.0, 0.0], [-127.79999993771924, -0.0, 1e-30]]), 0.05)]
+  clouds += [(straddling_pairs(cell, R).reshape(-1, 3), cell) for cell in (0.03, 0.05, 0.07) for R in (1, 2, 3, 6)]
+  clouds += [(snapped_cloud(s, cell, off), cell) for s, cell in enumerate((0.05, 0.3, 0.0625, 0.02))
+             for off in (0.0, -100.0, 1000.0)]
+  moved_rows = 0
+  for x64, cell in clouds:
+    x32 = x64.astype(np.float32)
+    for x, keys in ((x64, np.floor(x64 / cell)), (x32, np.floor(x32 / np.float32(cell)).astype(np.float64))):
+      y = _abi.float32_in_cells(torch.from_numpy(x), torch.from_numpy(keys.astype(np.int32)), cell)
+      assert y.dtype == torch.float32 and y.is_contiguous()
+      y = y.numpy()
+      assert np.array_equal(np.floor(y.astype(np.float64) / cell), keys)
+      agree = np.floor(x32.astype(np.float64) / cell) == keys
+      assert y[agree].tobytes() == x32[agree].tobytes()
+      assert np.abs(ordered(y) - ordered(x32)).max() <= _abi.CELL_NUDGE_STEPS
+      moved_rows += int((~agree).any(1).sum())
+      if x is x64:
+        assert y.tobytes() == rows_in_cells(x64, cell).tobytes()
+  assert moved_rows > 1000
