@@ -39,26 +39,23 @@ __global__ void inlier_coords_kernel(const int32_t* __restrict__ c0, const int32
   o[4] = b.y; o[5] = b.z; o[6] = b.w;
 }
 
-__global__ void sigmoid_clip_sum_kernel(const float* __restrict__ logit, int64_t n, float clip,
-                                        float* __restrict__ w, double* wsum) {
-  double acc = 0.0;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
-       i += (int64_t)gridDim.x * blockDim.x) {
+// One CTA: thread k sums rows k, k + 1024, ... in fp64, then dgr_block_sum, so the gate sum that picks Procrustes or
+// the safeguard has the same bits on every run.
+constexpr int kGateThreads = 1024;
+
+__global__ void __launch_bounds__(kGateThreads)
+sigmoid_clip_sum_kernel(const float* __restrict__ logit, int64_t n, float clip, float* __restrict__ w,
+                        double* wsum) {
+  __shared__ double part[kGateThreads / 32][1];
+  double acc[1] = {0.0};
+  for (int64_t i = threadIdx.x; i < n; i += kGateThreads) {
     float s = 1.f / (1.f + expf(-logit[i]));
     if (clip > 0.f && s < clip) s = 0.f;
     w[i] = s;
-    acc += (double)s;
+    acc[0] += (double)s;
   }
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, d);
-  __shared__ double ws[8];
-  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int k = 0; k < (int)(blockDim.x >> 5); ++k) t += ws[k];
-    atomicAdd(wsum, t);
-  }
+  const double t = dgr_block_sum<kGateThreads>(acc, part);
+  if (threadIdx.x == 0) *wsum = t;
 }
 
 // gather the correspondences into structure-of-arrays form: 7 arrays of length n
@@ -215,20 +212,22 @@ se3_register_kernel(const float* __restrict__ pack, int64_t n, float q, int max_
   };
 
   // ---- weighted Procrustes: first moments -------------------------------------------------
+  // Procrustes normalises by sum |w| (core/registration.py:96), the loss by sum w (core/loss.py:61)
   {
-    double v[7] = {0, 0, 0, 0, 0, 0, 0};
-    float a[7] = {0, 0, 0, 0, 0, 0, 0};
+    double v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    float a[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     for (int64_t k = tid; k < cnt; k += kRegThreads) {
       float x[3], y[3], w;
       load_pt(k, x, y, w);
       a[0] += fabsf(w);
       a[1] += w * x[0]; a[2] += w * x[1]; a[3] += w * x[2];
       a[4] += w * y[0]; a[5] += w * y[1]; a[6] += w * y[2];
+      a[7] += w;
     }
-    for (int k = 0; k < 7; ++k) v[k] = (double)a[k];
+    for (int k = 0; k < 8; ++k) v[k] = (double)a[k];
     dgr_allreduce<kClusterSize>(sh.red, v, parity);
   }
-  const double W1 = sh.red.tot[0];
+  const double W1 = sh.red.tot[0], Wsum = sh.red.tot[7];
   const float wden = (float)W1 + eps;
   float mux[3], muy[3];
   for (int k = 0; k < 3; ++k) {
@@ -332,7 +331,7 @@ se3_register_kernel(const float* __restrict__ pack, int64_t n, float q, int max_
     for (int k = 0; k < 13; ++k) v[k] = (double)a[k];
     dgr_allreduce<kClusterSize>(sh.red, v, parity);
     // every thread evaluates the stop rule on identical data so the cluster stays in lock step
-    const double w1 = W1;   // weights are >= 0: sum w == sum |w|
+    const double w1 = Wsum;
     loss = (float)(sh.red.tot[0] / w1);
     if (it == 0) loss_prev = loss;   // the reference evaluates loss_prev on the initial pose
     if (loss < 1e-7f) break;
@@ -397,11 +396,7 @@ int32_t dgr_inlier_coords(const int32_t* coords0, const int32_t* coords1, const 
 int32_t dgr_sigmoid_clip_sum(const float* logit, int64_t n, float clip, float* w, double* wsum,
                              void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
-  DGR_CUDA_CHECK(cudaMemsetAsync(wsum, 0, sizeof(double), st));
-  if (n == 0) return DGR_OK;
-  unsigned blocks = dgr_blocks(n, 256 * 4);
-  if (blocks > 592) blocks = 592;
-  sigmoid_clip_sum_kernel<<<blocks, 256, 0, st>>>(logit, n, clip, w, wsum);
+  sigmoid_clip_sum_kernel<<<1, kGateThreads, 0, st>>>(logit, n, clip, w, wsum);
   dgr_note_launches(1);
   DGR_LAUNCH_CHECK();
   return DGR_OK;

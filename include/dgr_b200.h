@@ -166,7 +166,8 @@ int32_t dgr_knn_top1_tc(const float* f0, int64_t n0, const float* f1, int64_t n1
 /* out[i] = (coords0[i, 0..3], coords1[idx1[i], 1..3]) int32 [n0, 7]. */
 int32_t dgr_inlier_coords(const int32_t* coords0, const int32_t* coords1, const int32_t* idx1,
                           int64_t n0, int32_t* out, void* stream);
-/* w = sigmoid(logit); w[w < clip] = 0 (if clip > 0); *wsum (device double) = sum w. */
+/* w = sigmoid(logit); w[w < clip] = 0 (if clip > 0); *wsum (device double) = sum w in fp64, in a fixed order
+ * (the same bits on every run). */
 int32_t dgr_sigmoid_clip_sum(const float* logit, int64_t n, float clip, float* w, double* wsum,
                              void* stream);
 
@@ -175,7 +176,8 @@ int32_t dgr_sigmoid_clip_sum(const float* logit, int64_t n, float clip, float* w
 /* Correspondence i pairs x[i] with y[idx1[i]] (idx1 may be NULL: y[i]).
  * result (device float[16]): R row-major [0..9), t [9..12), iterations, final loss,
  * break_count, n_active (correspondences with non-zero weight).
- * max_iter == 0 returns the closed-form weighted Procrustes solution only.
+ * max_iter == 0 returns the closed-form weighted Procrustes solution only.  Procrustes normalises by sum |w|,
+ * the loss by sum w (core/registration.py:96, core/loss.py:61).
  * pack_ws: float workspace of 7 * n elements; cnt_ws: int32[4]. */
 int32_t dgr_se3_register(const float* x, const float* y, const int32_t* idx1, const float* w,
                          int64_t n, float quantization_size, int32_t max_iter,
