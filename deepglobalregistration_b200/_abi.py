@@ -631,6 +631,40 @@ def estimate_normals(xyz, manager_or_table, cell, radius, max_nn, prev=None, ret
   return (normals, counts) if return_counts else normals
 
 
+def estimate_covariances(xyz, manager_or_table, cell, radius, max_nn, return_counts=False, batch=0):
+  """Per-point covariances (open3d's EstimatePerPointCovariances) of xyz (CUDA float32 [n, 3]) over the neighbours
+  estimate_normals finds (strictly within `radius`, at most `max_nn` <= 64 by (d^2, row), the cloud's own voxel hash
+  at `cell`); the identity below 3 neighbours.  -> float64 [n, 6] (xx, xy, xz, yy, yz, zz) (and the int32 [n] counts
+  within the radius, equal to estimate_normals')."""
+  _chk(xyz, torch.float32, 'xyz')
+  spec, table = _hash_of(manager_or_table)
+  n = xyz.shape[0]
+  cov = torch.empty(max(n, 1), 6, dtype=torch.float64, device=xyz.device)[:n]
+  counts = torch.empty(max(n, 1), dtype=torch.int32, device=xyz.device)[:n]
+  call('dgr_estimate_covariances', ptr(xyz), n, ptr(spec), ptr(table.keys), ptr(table.vals), table.cap, int(batch),
+       float(cell), float(radius), int(max_nn), ptr(cov), ptr(counts), stream())
+  return (cov, counts) if return_counts else cov
+
+
+def covariances_from_normals(normals, epsilon=1e-3):
+  """Generalized-ICP covariances R diag(epsilon, 1, 1) R^T of normals (CUDA float32 [n, 3]; open3d's
+  InitializePointCloudForGeneralizedICP).  -> float64 [n, 6] as estimate_covariances."""
+  _chk(normals, torch.float32, 'normals')
+  n = normals.shape[0]
+  cov = torch.empty(max(n, 1), 6, dtype=torch.float64, device=normals.device)[:n]
+  call('dgr_covariances_from_normals', ptr(normals), n, float(epsilon), ptr(cov), stream())
+  return cov
+
+
+LOSS_IDS = {name: _DEFINES[f'DGR_LOSS_{name.upper()}'] for name in ('L2', 'L1', 'Huber', 'Cauchy', 'GM', 'Tukey')}
+
+
+def _loss_id(loss):
+  if loss not in LOSS_IDS:
+    raise DgrError(f'loss must be one of {sorted(LOSS_IDS)}, got {loss!r}')
+  return LOSS_IDS[loss]
+
+
 def color_gradient(xyz, normals, intensity, manager_or_table, cell, radius, max_nn, return_counts=False, batch=0):
   """Colour gradients (open3d 0.10's InitializePointCloudForColoredICP) of xyz (CUDA float32 [n, 3]) with normals
   (CUDA float32 [n, 3]) and intensities (CUDA float32 [n]) from the neighbours estimate_normals finds (strictly within
@@ -674,7 +708,14 @@ def compute_fpfh(xyz, normals, manager_or_table, cell, radius, max_nn, batch=0, 
   return (out, counts) if return_counts else out
 
 
-def _icp(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter, rel_fitness, rel_rmse, batch):
+def _pose12(T_init, dev):
+  if not (isinstance(T_init, torch.Tensor) and T_init.is_cuda and T_init.numel() == 12):
+    T_init = torch.as_tensor(T_init, dtype=torch.float64).reshape(4, 4)[:3].contiguous().to(dev)
+  return T_init
+
+
+def _icp(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter, rel_fitness, rel_rmse, batch,
+         loss=None, loss_k=1.0):
   _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
   if tgt_normals is not None:
     _chk(tgt_normals, torch.float32, 'tgt_normals')
@@ -682,10 +723,14 @@ def _icp(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter, 
       raise DgrError('tgt_normals must hold one normal per target point')
   dev = src.device
   spec, table = _hash_of(tgt_manager)
-  if not (isinstance(T_init, torch.Tensor) and T_init.is_cuda and T_init.numel() == 12):
-    T_init = torch.as_tensor(T_init, dtype=torch.float64).reshape(4, 4)[:3].contiguous().to(dev)
+  T_init = _pose12(T_init, dev)
   ws = workspace('icp', torch.float64, dev, 'dgr_icp_ws_elems', src.shape[0])
   res = torch.empty(20, dtype=torch.float64, device=dev)
+  if loss is not None:
+    call('dgr_icp_loss', ptr(src), src.shape[0], ptr(tgt), ptr(tgt_normals), ptr(spec), ptr(table.keys),
+         ptr(table.vals), table.cap, int(batch), float(voxel), float(max_dist), _loss_id(loss), float(loss_k),
+         ptr(T_init), int(max_iter), float(rel_fitness), float(rel_rmse), ptr(ws), ptr(res), stream())
+    return res
   # ptr() of an empty tgt_normals is 0, which selects point-to-point; without target points neither update has a
   # correspondence, so both give the same result
   call('dgr_icp', ptr(src), src.shape[0], ptr(tgt), ptr(tgt_normals), ptr(spec), ptr(table.keys), ptr(table.vals),
@@ -704,17 +749,24 @@ def icp_point_to_point(src, tgt, tgt_manager, voxel, max_dist, T_init, max_iter=
 
 
 def icp_point_to_plane(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter=30, rel_fitness=1e-6,
-                       rel_rmse=1e-6, batch=0):
+                       rel_rmse=1e-6, batch=0, loss=None, loss_k=1.0):
   """Point-to-plane ICP (open3d's TransformationEstimationPointToPlane, default criteria) of src onto tgt through
-  tgt's voxel hash; arguments as icp_point_to_point plus tgt_normals (CUDA float32 [n_tgt, 3])."""
-  return _icp(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter, rel_fitness, rel_rmse, batch)
+  tgt's voxel hash; arguments as icp_point_to_point plus tgt_normals (CUDA float32 [n_tgt, 3]).  loss: None (the
+  plain estimator) or a robust loss of LOSS_IDS with scale loss_k, each row weighted by it (dgr_icp_loss)."""
+  if loss is not None and tgt_normals is None:
+    raise DgrError('point-to-plane ICP with a loss needs tgt_normals')
+  return _icp(src, tgt, tgt_normals, tgt_manager, voxel, max_dist, T_init, max_iter, rel_fitness, rel_rmse, batch,
+              loss, loss_k)
 
 
 def icp_colored(src, src_intensity, tgt, tgt_normals, tgt_intensity, tgt_grad, tgt_manager, voxel, max_dist,
-                lambda_geometric, T_init, max_iter=30, rel_fitness=1e-6, rel_rmse=1e-6, batch=0):
+                lambda_geometric, T_init, max_iter=30, rel_fitness=1e-6, rel_rmse=1e-6, batch=0, loss=None,
+                loss_k=1.0):
   """Colored ICP (open3d's TransformationEstimationForColoredICP(lambda_geometric), default criteria) of src onto tgt
   through tgt's voxel hash; arguments as icp_point_to_plane plus the intensities (CUDA float32 [n]) of both clouds and
-  the target's colour gradients (color_gradient; CUDA float32 [n_tgt, 3]).  -> device double [20] as icp_point_to_plane."""
+  the target's colour gradients (color_gradient; CUDA float32 [n_tgt, 3]).  loss / loss_k: as icp_point_to_plane,
+  each of the two rows weighted on its own scaled residual (dgr_colored_icp_loss).  -> device double [20] as
+  icp_point_to_plane."""
   _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
   for name, a, shape in (('src_intensity', src_intensity, (src.shape[0],)), ('tgt_normals', tgt_normals, tgt.shape),
                          ('tgt_intensity', tgt_intensity, (tgt.shape[0],)), ('tgt_grad', tgt_grad, tgt.shape)):
@@ -725,14 +777,43 @@ def icp_colored(src, src_intensity, tgt, tgt_normals, tgt_intensity, tgt_grad, t
     raise DgrError('colored ICP needs target points')
   dev = src.device
   spec, table = _hash_of(tgt_manager)
-  if not (isinstance(T_init, torch.Tensor) and T_init.is_cuda and T_init.numel() == 12):
-    T_init = torch.as_tensor(T_init, dtype=torch.float64).reshape(4, 4)[:3].contiguous().to(dev)
+  T_init = _pose12(T_init, dev)
   ws = workspace('icp', torch.float64, dev, 'dgr_icp_ws_elems', src.shape[0])
   res = torch.empty(20, dtype=torch.float64, device=dev)
+  if loss is not None:
+    call('dgr_colored_icp_loss', ptr(src), ptr(src_intensity), src.shape[0], ptr(tgt), ptr(tgt_normals),
+         ptr(tgt_intensity), ptr(tgt_grad), ptr(spec), ptr(table.keys), ptr(table.vals), table.cap, int(batch),
+         float(voxel), float(max_dist), float(lambda_geometric), _loss_id(loss), float(loss_k), ptr(T_init),
+         int(max_iter), float(rel_fitness), float(rel_rmse), ptr(ws), ptr(res), stream())
+    return res
   call('dgr_colored_icp', ptr(src), ptr(src_intensity), src.shape[0], ptr(tgt), ptr(tgt_normals), ptr(tgt_intensity),
        ptr(tgt_grad), ptr(spec), ptr(table.keys), ptr(table.vals), table.cap, int(batch), float(voxel), float(max_dist),
        float(lambda_geometric), ptr(T_init), int(max_iter), float(rel_fitness), float(rel_rmse), ptr(ws), ptr(res),
        stream())
+  return res
+
+
+def icp_generalized(src, src_cov, tgt, tgt_cov, tgt_manager, voxel, max_dist, T_init, max_iter=30, rel_fitness=1e-6,
+                    rel_rmse=1e-6, batch=0, loss=None, loss_k=1.0):
+  """Generalized ICP (open3d's TransformationEstimationForGeneralizedICP, default criteria) of src onto tgt through
+  tgt's voxel hash; arguments as icp_point_to_point plus both clouds' covariances (CUDA float64 [n, 6], from
+  estimate_covariances or covariances_from_normals) and an optional robust loss as icp_point_to_plane
+  (dgr_generalized_icp).  -> device double [20] as icp_point_to_point."""
+  _chk(src, torch.float32, 'src'); _chk(tgt, torch.float32, 'tgt')
+  for name, a, n in (('src_cov', src_cov, src.shape[0]), ('tgt_cov', tgt_cov, tgt.shape[0])):
+    _chk(a, torch.float64, name)
+    if a.shape != (n, 6):
+      raise DgrError(f'{name} must hold one [6] covariance row per point')
+  if tgt.shape[0] == 0:
+    raise DgrError('generalized ICP needs target points')
+  dev = src.device
+  spec, table = _hash_of(tgt_manager)
+  T_init = _pose12(T_init, dev)
+  ws = workspace('icp', torch.float64, dev, 'dgr_icp_ws_elems', src.shape[0])
+  res = torch.empty(20, dtype=torch.float64, device=dev)
+  call('dgr_generalized_icp', ptr(src), ptr(src_cov), src.shape[0], ptr(tgt), ptr(tgt_cov), ptr(spec), ptr(table.keys),
+       ptr(table.vals), table.cap, int(batch), float(voxel), float(max_dist), _loss_id('L2' if loss is None else loss),
+       float(loss_k), ptr(T_init), int(max_iter), float(rel_fitness), float(rel_rmse), ptr(ws), ptr(res), stream())
   return res
 
 

@@ -1,6 +1,6 @@
 """``ICPBaseline``: ICP from a fixed initial pose (identity by default), the ``ICP (Point-to-point)`` and
-``ICP (Point-to-plane)`` rows of the reference's results, on the same voxelisation, GPU and evaluation protocol as
-``DeepGlobalRegistration``.
+``ICP (Point-to-plane)`` rows of the reference's results and generalized ICP, on the same voxelisation, GPU and
+evaluation protocol as ``DeepGlobalRegistration``.
 
     dgr = DeepGlobalRegistration(config)
     T = ICPBaseline(dgr, method='point_to_plane').register(xyz0, xyz1)
@@ -8,7 +8,8 @@
 Voxelise both clouds (the wrapped object's ``preprocess`` and ``voxel_size``; no FCGF) -> point_to_plane: target
 normals from neighbours within 2 voxels, at most 30 (dgr_estimate_normals, util/pointcloud.py:60's setting), through
 cloud 1's voxel table -> ICP from ``init`` through the same table (dgr_icp, with or without the normals)
--> one readback.
+-> one readback.  generalized: both clouds' normals at the same setting, each through its own table, covariances
+R diag(1e-3, 1, 1) R^T from them (dgr_covariances_from_normals) -> dgr_generalized_icp.
 """
 import numpy as np
 import torch
@@ -16,12 +17,13 @@ import torch
 from .. import _abi
 from ..util.timer import Timer
 
-METHODS = {'point_to_point': 'icp', 'point_to_plane': 'icp_plane'}
+METHODS = {'point_to_point': 'icp', 'point_to_plane': 'icp_plane', 'generalized': 'icp_generalized'}
 
 
 class ICPBaseline:
   normal_radius_voxels = 2.0
   normal_max_nn = 30
+  gicp_epsilon = 1e-3
 
   def __init__(self, dgr, method='point_to_plane', max_correspondence_distance=None, max_iteration=30, init=None):
     if method not in METHODS:
@@ -60,12 +62,19 @@ class ICPBaseline:
     _abi.refresh_stream()
     vs, dist = self.voxel_size, self._distance()
     with torch.no_grad():
-      p0, _, _ = d.preprocess(xyz0, 0, _batch=0)
+      p0, c0, _ = d.preprocess(xyz0, 0, _batch=0)
       p1, c1, _ = d.preprocess(xyz1, 1, _batch=1)
       m = c1._dgr_manager
       T0 = torch.from_numpy(np.ascontiguousarray(self.init[:3])).to(p0.device)
-      if self.method == 'point_to_plane':
-        normals = _abi.estimate_normals(p1, m, vs, self.normal_radius_voxels * vs, self.normal_max_nn, batch=1)
+      radius = self.normal_radius_voxels * vs
+      if self.method == 'generalized':
+        n0 = _abi.estimate_normals(p0, c0._dgr_manager, vs, radius, self.normal_max_nn, batch=0)
+        n1 = _abi.estimate_normals(p1, m, vs, radius, self.normal_max_nn, batch=1)
+        res = _abi.icp_generalized(p0, _abi.covariances_from_normals(n0, self.gicp_epsilon), p1,
+                                   _abi.covariances_from_normals(n1, self.gicp_epsilon), m, vs, dist, T0,
+                                   self.max_iteration, batch=1)
+      elif self.method == 'point_to_plane':
+        normals = _abi.estimate_normals(p1, m, vs, radius, self.normal_max_nn, batch=1)
         res = _abi.icp_point_to_plane(p0, p1, normals, m, vs, dist, T0, self.max_iteration, batch=1)
       else:
         res = _abi.icp_point_to_point(p0, p1, m, vs, dist, T0, self.max_iteration, batch=1)

@@ -1,13 +1,14 @@
-// Normal estimation, colour gradients and ICP: open3d 0.10's EstimateNormals(KDTreeSearchParamHybrid(radius,
-// max_nn)), InitializePointCloudForColoredICP and RegistrationICP with TransformationEstimationPointToPoint /
-// PointToPlane / ForColoredICP, restated in oracle/normals.py, oracle/icp.py, oracle/icp_plane.py and
-// oracle/colored_icp.py (which pin every boundary convention).  All search one cloud's voxel hash (a
+// Normal estimation, covariances, colour gradients and ICP: open3d 0.10's EstimateNormals(KDTreeSearchParamHybrid(
+// radius, max_nn)), EstimatePerPointCovariances, InitializePointCloudForColoredICP and RegistrationICP with
+// TransformationEstimationPointToPoint / PointToPlane / ForColoredICP / ForGeneralizedICP and the robust kernels of
+// open3d >= 0.12, restated in oracle/normals.py, oracle/icp.py, oracle/icp_plane.py, oracle/colored_icp.py and
+// oracle/gicp.py (which pin every boundary convention).  All search one cloud's voxel hash (a
 // dgr_unique_first table with at most one point per cell): the (2 reach + 1)^3 cells around a point,
 // reach = ceil(radius / cell) <= 4, 8 lanes per point as in dgr_voxel_nearest8.  No atomics: every sum has a fixed
 // order, so a call gives the same bits on every run.
 //   nbr_probe_kernel<S>      8 lanes per point, one probe pass: count and the 9 fp64 sums S adds over the rows with
-//                            |p_j - p_i|^2 < radius^2 (the offsets' cumulants for normals, the gradient rows for
-//                            colour gradients); a point with <= max_nn of them gets its result
+//                            |p_j - p_i|^2 < radius^2 (the offsets' cumulants for normals and covariances, the
+//                            gradient rows for colour gradients); a point with <= max_nn of them gets its result
 //   nbr_select_kernel<S>     a warp per point with more than max_nn: the in-radius keys again (dgr_gather_in_radius);
 //                            the sums of the max_nn ranked first
 //   icp_match_kernel<E>      nearest target row within max_dist (dgr_voxel_nearest8); the estimator's sums, the
@@ -89,6 +90,53 @@ struct NormalSums {
     store_normal(m, n, prev, i, normals);
   }
 };
+
+// open3d's EstimatePerPointCovariances: C = E[e e^T] - mu mu^T over the n kept offsets (NormalSums' cumulants), the
+// identity for n < 3; cov[i] = (xx, xy, xz, yy, yz, zz) in fp64
+struct CovarianceSums {
+  double* cov;
+  struct Point {};
+  __device__ __forceinline__ Point point(int64_t) const { return {}; }
+  __device__ __forceinline__ void add(const Point&, double m[9], const double e[3], int32_t) const {
+    add_cumulants(m, e);
+  }
+  __device__ __forceinline__ void store(const double m[9], int n, int64_t i) const {
+    double c[6] = {1.0, 0.0, 0.0, 1.0, 0.0, 1.0};
+    if (n >= 3) {
+      const double inv = 1.0 / (double)n;
+      const double mu[3] = {m[0] * inv, m[1] * inv, m[2] * inv};
+      c[0] = m[3] * inv - mu[0] * mu[0]; c[1] = m[4] * inv - mu[0] * mu[1]; c[2] = m[5] * inv - mu[0] * mu[2];
+      c[3] = m[6] * inv - mu[1] * mu[1]; c[4] = m[7] * inv - mu[1] * mu[2]; c[5] = m[8] * inv - mu[2] * mu[2];
+    }
+    for (int a = 0; a < 6; ++a) cov[6 * i + a] = c[a];
+  }
+};
+
+// InitializePointCloudForGeneralizedICP: C = R diag(eps, 1, 1) R^T with R = GetRotationFromE1ToX(n), evaluated
+// literally in fp64: v = e1 x n, c = e1.n, R = I + [v]x + [v]x^2 / (1 + c), or diag(-1, -1, 1) when c < -0.99
+__global__ void cov_from_normals_kernel(const float* __restrict__ normals, int64_t n, double eps,
+                                        double* __restrict__ cov) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double x = normals[3 * i], y = normals[3 * i + 1], z = normals[3 * i + 2];
+  double R[3][3] = {{-1.0, 0.0, 0.0}, {0.0, -1.0, 0.0}, {0.0, 0.0, 1.0}};
+  if (!(x < -0.99)) {
+    const double v[3] = {0.0, -z, y};
+    const double S[3][3] = {{0.0, -v[2], v[1]}, {v[2], 0.0, -v[0]}, {-v[1], v[0], 0.0}};
+    const double f = 1.0 / (1.0 + x);
+    for (int a = 0; a < 3; ++a)
+      for (int b = 0; b < 3; ++b) {
+        const double s2 = S[a][0] * S[0][b] + S[a][1] * S[1][b] + S[a][2] * S[2][b];
+        R[a][b] = (a == b ? 1.0 : 0.0) + S[a][b] + s2 * f;
+      }
+  }
+  const double d[3] = {eps, 1.0, 1.0};
+  double c[6];
+  int k = 0;
+  for (int a = 0; a < 3; ++a)
+    for (int b = a; b < 3; ++b) c[k++] = R[a][0] * d[0] * R[b][0] + R[a][1] * d[1] * R[b][1] + R[a][2] * d[2] * R[b][2];
+  for (int q = 0; q < 6; ++q) cov[6 * i + q] = c[q];
+}
 
 // open3d's InitializePointCloudForColoredICP at point i from the sums of nn neighbours (i included): g = 0 for
 // nn < 4, else the solution of (sum u u^T + (nn - 1)^2 n n^T) g = sum u b by a 3x3 Cholesky in fp64 (g = 0 on a
@@ -235,23 +283,58 @@ __device__ __forceinline__ void add_sum(double* acc, int sub, int k, double v) {
   if ((k & 7) == sub) acc[k >> 3] += v;
 }
 
-// What the estimators read besides the matched pair: target normals (point-to-plane, colored), and for colored ICP
-// the target colour gradients and intensities, the source intensities and sqrt(lambda), sqrt(1 - lambda)
+// What the estimators read besides the matched pair: target normals (point-to-plane, colored), for colored ICP the
+// target colour gradients and intensities, the source intensities and sqrt(lambda), sqrt(1 - lambda), for
+// generalized ICP both clouds' covariances, and the robust loss (DGR_LOSS_*) and its scale k of a weighted estimator
 struct IcpInputs {
   const float* tnorm;
   const float* tgrad;
   const float* tint;
   const float* sint;
   double sqrt_geo, sqrt_photo;
+  const double* scov;
+  const double* tcov;
+  int loss;
+  double loss_k;
 };
+
+// open3d's RobustKernel::Weight(r) of the DGR_LOSS_* losses, scale k; L1 gives 0 at r = 0 (open3d: infinity)
+__device__ __forceinline__ double loss_weight(int loss, double k, double r) {
+  const double a = fabs(r);
+  switch (loss) {
+    case DGR_LOSS_L1: return a > 0.0 ? 1.0 / a : 0.0;
+    case DGR_LOSS_HUBER: return a <= k ? 1.0 : k / a;
+    case DGR_LOSS_CAUCHY: { const double u = r / k; return 1.0 / (1.0 + u * u); }
+    case DGR_LOSS_GM: { const double d = k + r * r; return k / (d * d); }
+    case DGR_LOSS_TUKEY: { const double u = fmin(1.0, a / k), e = 1.0 - u * u; return e * e; }
+    default: return 1.0;
+  }
+}
+
+// One residual row r, J into the 29 sums J^T J (upper triangle, 21) and J^T r (6); weighted (kW): w J J^T and w J r.
+// The unweighted instantiation is the plain products, not a multiply by 1.
+template <bool kW>
+__device__ __forceinline__ void add_row(double* acc, int sub, const double J[6], double r, double w) {
+  int k = 0;
+#pragma unroll
+  for (int a = 0; a < 6; ++a) {
+    const double wa = kW ? w * J[a] : J[a];
+#pragma unroll
+    for (int b = a; b < 6; ++b) add_sum(acc, sub, k++, wa * J[b]);
+  }
+#pragma unroll
+  for (int a = 0; a < 6; ++a) add_sum(acc, sub, 21 + a, (kW ? w * J[a] : J[a]) * r);
+}
 
 // open3d's TransformationEstimationPointToPoint: sums n, sum d^2, sum p (3), sum q (3), sum q p^T (9) over the
 // correspondences (p = current transformed source point, q its target point); the step is the Kabsch rotation of
 // the centred cross-covariance, composed on the left (the identity without correspondences)
 struct PointToPoint {
+  using Update = PointToPoint;
   static constexpr int kNv = 17, kCount = 0, kD2 = 1;
-  __device__ __forceinline__ static void accumulate(const double p[3], const double q[3], const IcpInputs&, int64_t,
-                                                    int64_t, double d2, int sub, double* acc) {
+  __device__ __forceinline__ static void accumulate(const double p[3], const double q[3], const IcpInputs&,
+                                                    const double*, int64_t, int64_t, double d2, int sub,
+                                                    double* acc) {
     add_sum(acc, sub, 0, 1.0);
     add_sum(acc, sub, 1, d2);
 #pragma unroll
@@ -287,23 +370,21 @@ struct PointToPoint {
 
 // open3d's TransformationEstimationPointToPlane: with the target normal n, r = (s - q).n and J = [s x n, n]; sums
 // J^T J (upper triangle, 21), J^T r (6), n, sum d^2; the step solves J^T J x = -J^T r by Cholesky (a non-positive
-// pivot - no match, a single plane - gives the identity) and composes [Rz(x2) Ry(x1) Rx(x0) | x3..5] on the left
-struct PointToPlane {
+// pivot - no match, a single plane - gives the identity) and composes [Rz(x2) Ry(x1) Rx(x0) | x3..5] on the left.
+// kW: the row weighted by loss_weight(r) (open3d >= 0.12's kernel argument).
+template <bool kW>
+struct PointToPlaneT {
+  using Update = PointToPlaneT<false>;
   static constexpr int kNv = 29, kCount = 27, kD2 = 28;
   __device__ __forceinline__ static void accumulate(const double p[3], const double q[3], const IcpInputs& in,
-                                                    int64_t, int64_t j, double d2, int sub, double* acc) {
+                                                    const double*, int64_t, int64_t j, double d2, int sub,
+                                                    double* acc) {
     const float* __restrict__ tnorm = in.tnorm;
     const double nv[3] = {tnorm[3 * j], tnorm[3 * j + 1], tnorm[3 * j + 2]};
     const double r = (p[0] - q[0]) * nv[0] + (p[1] - q[1]) * nv[1] + (p[2] - q[2]) * nv[2];
     const double J[6] = {p[1] * nv[2] - p[2] * nv[1], p[2] * nv[0] - p[0] * nv[2], p[0] * nv[1] - p[1] * nv[0],
                          nv[0], nv[1], nv[2]};
-    int k = 0;
-#pragma unroll
-    for (int a = 0; a < 6; ++a)
-#pragma unroll
-      for (int b = a; b < 6; ++b) add_sum(acc, sub, k++, J[a] * J[b]);
-#pragma unroll
-    for (int a = 0; a < 6; ++a) add_sum(acc, sub, 21 + a, J[a] * r);
+    add_row<kW>(acc, sub, J, r, kW ? loss_weight(in.loss, in.loss_k, r) : 1.0);
     add_sum(acc, sub, 27, 1.0);
     add_sum(acc, sub, 28, d2);
   }
@@ -315,17 +396,21 @@ struct PointToPlane {
     zyx_update_left(x, T0, T);
   }
 };
+using PointToPlane = PointToPlaneT<false>;
 
 // open3d's TransformationEstimationForColoredICP(lambda): two rows per correspondence (source point s = p, target
 // point q, normal n, colour gradient d, intensities I_s, I_t), both added into PointToPlane's 29 sums and step:
 //   geometric    r = sqrt(lambda) (s - q).n,  J = sqrt(lambda) [s x n, n];
 //   photometric  with s' = s - ((s - q).n) n and m = -(I - n n^T) d = (d.n) n - d:
 //                r = sqrt(1 - lambda) (I_s - (d.(s' - q) + I_t)),  J = sqrt(1 - lambda) [s x m, m].
-// At lambda = 1 the photometric row is exactly zero and the sums are PointToPlane's.
-struct Colored {
-  static constexpr int kNv = PointToPlane::kNv, kCount = PointToPlane::kCount, kD2 = PointToPlane::kD2;
+// At lambda = 1 the photometric row is exactly zero and the sums are PointToPlane's.  kW: each row weighted by
+// loss_weight of its own (scaled) residual, as open3d >= 0.12 does.
+template <bool kW>
+struct ColoredT {
+  using Update = PointToPlane;
   __device__ __forceinline__ static void accumulate(const double p[3], const double q[3], const IcpInputs& in,
-                                                    int64_t i, int64_t j, double d2, int sub, double* acc) {
+                                                    const double*, int64_t i, int64_t j, double d2, int sub,
+                                                    double* acc) {
     const double nv[3] = {in.tnorm[3 * j], in.tnorm[3 * j + 1], in.tnorm[3 * j + 2]};
     const double dv[3] = {in.tgrad[3 * j], in.tgrad[3 * j + 1], in.tgrad[3 * j + 2]};
     const double rg = (p[0] - q[0]) * nv[0] + (p[1] - q[1]) * nv[1] + (p[2] - q[2]) * nv[2];
@@ -340,29 +425,80 @@ struct Colored {
       const double r = sc * (row == 0 ? rg : rp);
       const double J[6] = {sc * (p[1] * v[2] - p[2] * v[1]), sc * (p[2] * v[0] - p[0] * v[2]),
                            sc * (p[0] * v[1] - p[1] * v[0]), sc * v[0], sc * v[1], sc * v[2]};
-      int k = 0;
-#pragma unroll
-      for (int a = 0; a < 6; ++a)
-#pragma unroll
-        for (int b = a; b < 6; ++b) add_sum(acc, sub, k++, J[a] * J[b]);
-#pragma unroll
-      for (int a = 0; a < 6; ++a) add_sum(acc, sub, 21 + a, J[a] * r);
+      add_row<kW>(acc, sub, J, r, kW ? loss_weight(in.loss, in.loss_k, r) : 1.0);
     }
     add_sum(acc, sub, 27, 1.0);
     add_sum(acc, sub, 28, d2);
   }
-  __device__ __forceinline__ static void step(const double* tot, double* T) { PointToPlane::step(tot, T); }
 };
 
-// E::kNv sums in (kNv + 7) / 8 accumulators per lane.  Per-block partials: part[block][k], summed lanes by butterfly
-// and warps in order.
+// open3d's TransformationEstimationForGeneralizedICP (Segal, Haehnel & Thrun 2009): with the source covariance
+// rotated by the current pose, C_s' = R C_s R^T, and M = C_s' + C_t, three rows per correspondence k = 0..2 with
+// v = W[k], W = M^(-1/2) (the principal root, from the eigenvectors jacobi_svd3 gives for a positive-definite M):
+// r = v.(s - q), J = [s x v, v], into PointToPlane's 29 sums and step.  A correspondence whose M fails a 3x3
+// Cholesky (a non-positive pivot) adds no row; it still counts towards fitness and RMSE.  kW: each row weighted by
+// loss_weight(r).
+template <bool kW>
+struct GeneralizedT {
+  using Update = PointToPlane;
+  __device__ __forceinline__ static void accumulate(const double p[3], const double q[3], const IcpInputs& in,
+                                                    const double T[12], int64_t i, int64_t j, double d2, int sub,
+                                                    double* acc) {
+    const double* cs = in.scov + 6 * i;
+    const double* ct = in.tcov + 6 * j;
+    const double C[3][3] = {{cs[0], cs[1], cs[2]}, {cs[1], cs[3], cs[4]}, {cs[2], cs[4], cs[5]}};
+    double RC[3][3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int b = 0; b < 3; ++b) RC[a][b] = T[4 * a] * C[0][b] + T[4 * a + 1] * C[1][b] + T[4 * a + 2] * C[2][b];
+    double M[3][3];
+    M[0][0] = RC[0][0] * T[0] + RC[0][1] * T[1] + RC[0][2] * T[2] + ct[0];
+    M[0][1] = RC[0][0] * T[4] + RC[0][1] * T[5] + RC[0][2] * T[6] + ct[1];
+    M[0][2] = RC[0][0] * T[8] + RC[0][1] * T[9] + RC[0][2] * T[10] + ct[2];
+    M[1][1] = RC[1][0] * T[4] + RC[1][1] * T[5] + RC[1][2] * T[6] + ct[3];
+    M[1][2] = RC[1][0] * T[8] + RC[1][1] * T[9] + RC[1][2] * T[10] + ct[4];
+    M[2][2] = RC[2][0] * T[8] + RC[2][1] * T[9] + RC[2][2] * T[10] + ct[5];
+    M[1][0] = M[0][1]; M[2][0] = M[0][2]; M[2][1] = M[1][2];
+    add_sum(acc, sub, 27, 1.0);
+    add_sum(acc, sub, 28, d2);
+    // M's Cholesky pivots in order; W needs a positive-definite M
+    const double d0 = M[0][0];
+    if (!(d0 > 0.0)) return;
+    const double l10 = M[1][0] / sqrt(d0), l20 = M[2][0] / sqrt(d0);
+    const double d1 = M[1][1] - l10 * l10;
+    if (!(d1 > 0.0)) return;
+    const double l21 = (M[2][1] - l20 * l10) / sqrt(d1);
+    if (!(M[2][2] - l20 * l20 - l21 * l21 > 0.0)) return;
+    double A[3][3], V[3][3], sig[3];
+    jacobi_svd3(M, A, V, sig);
+    const double is[3] = {1.0 / sqrt(sig[0]), 1.0 / sqrt(sig[1]), 1.0 / sqrt(sig[2])};
+    const double e[3] = {p[0] - q[0], p[1] - q[1], p[2] - q[2]};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      double v[3];
+#pragma unroll
+      for (int b = 0; b < 3; ++b)
+        v[b] = V[k][0] * is[0] * V[b][0] + V[k][1] * is[1] * V[b][1] + V[k][2] * is[2] * V[b][2];
+      const double r = v[0] * e[0] + v[1] * e[1] + v[2] * e[2];
+      const double J[6] = {p[1] * v[2] - p[2] * v[1], p[2] * v[0] - p[0] * v[2], p[0] * v[1] - p[1] * v[0],
+                           v[0], v[1], v[2]};
+      add_row<kW>(acc, sub, J, r, kW ? loss_weight(in.loss, in.loss_k, r) : 1.0);
+    }
+  }
+};
+
+// Every estimator E names the estimator whose sums layout (kNv, kCount, kD2) and step icp_update_kernel runs
+// (E::Update): its own, or PointToPlane's for those that add rows into the same 29 sums.
+// kNv = E::Update::kNv sums in (kNv + 7) / 8 accumulators per lane.  Per-block partials: part[block][k], summed lanes
+// by butterfly and warps in order.
 template <class E>
 __global__ void __launch_bounds__(kIcpThreads)
 icp_match_kernel(const float* __restrict__ src, int64_t n_src, const float* __restrict__ tgt, const IcpInputs in,
                  const dgr_keyspec_t* __restrict__ spec_p,
                  const uint64_t* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask, int32_t batch,
                  double voxel, double max_dist, const IcpState* __restrict__ st, double* __restrict__ part) {
-  constexpr int kSlots = (E::kNv + 7) / 8;
+  constexpr int kNv = E::Update::kNv, kSlots = (kNv + 7) / 8;
   if (st->done) return;
   const dgr_keyspec_t s = *spec_p;
   double T[12];
@@ -387,7 +523,7 @@ icp_match_kernel(const float* __restrict__ src, int64_t n_src, const float* __re
     if (have && best_j >= 0) {                          // every lane of the group has the match
       const int64_t j = best_j;
       const double q[3] = {tgt[3 * j], tgt[3 * j + 1], tgt[3 * j + 2]};
-      E::accumulate(p, q, in, i, j, best, sub, acc);
+      E::accumulate(p, q, in, T, i, j, best, sub, acc);
     }
   }
   __shared__ double red[kIcpThreads / 32][kIcpStride];
@@ -400,7 +536,7 @@ icp_match_kernel(const float* __restrict__ src, int64_t n_src, const float* __re
     if (lane < 8) red[warp][8 * a + lane] = v;
   }
   __syncthreads();
-  if (threadIdx.x < E::kNv) {
+  if (threadIdx.x < kNv) {
     double v = 0.0;
     for (int w = 0; w < kIcpThreads / 32; ++w) v += red[w][threadIdx.x];
     part[(int64_t)blockIdx.x * kIcpStride + threadIdx.x] = v;
@@ -503,10 +639,42 @@ void icp_run(const float* src, int64_t n_src, const float* tgt, const IcpInputs&
   for (int k = 0; k <= max_iter; ++k) {
     icp_match_kernel<E><<<blocks, kIcpThreads, 0, st>>>(src, n_src, tgt, in, spec, keys, vals, (uint64_t)cap - 1,
                                                         batch, voxel, max_dist, state, part);
-    icp_update_kernel<E><<<1, E::kNv * 32, 0, st>>>(state, part, blocks, n_src, max_iter, rel_fitness, rel_rmse,
-                                                    result);
+    icp_update_kernel<typename E::Update><<<1, E::Update::kNv * 32, 0, st>>>(state, part, blocks, n_src, max_iter,
+                                                                     rel_fitness, rel_rmse, result);
   }
   dgr_note_launches(1 + 2 * (max_iter + 1));
+}
+
+// estimator E<false> for the L2 loss (today's unweighted code), E<true> with the loss weight otherwise
+template <template <bool> class E>
+void icp_run_loss(const float* src, int64_t n_src, const float* tgt, const IcpInputs& in, const dgr_keyspec_t* spec,
+                  const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch, double voxel, double max_dist,
+                  const double* T_init, int32_t max_iter, double rel_fitness, double rel_rmse, double* ws,
+                  double* result, cudaStream_t st) {
+  if (in.loss == DGR_LOSS_L2)
+    icp_run<E<false>>(src, n_src, tgt, in, spec, keys, vals, cap, batch, voxel, max_dist, T_init, max_iter,
+                      rel_fitness, rel_rmse, ws, result, st);
+  else
+    icp_run<E<true>>(src, n_src, tgt, in, spec, keys, vals, cap, batch, voxel, max_dist, T_init, max_iter,
+                     rel_fitness, rel_rmse, ws, result, st);
+}
+
+// a DGR_LOSS_* id, and for the losses with a scale a finite k > 0
+int32_t check_loss(int32_t loss, double loss_k) {
+  DGR_ARG_CHECK(loss >= DGR_LOSS_L2 && loss <= DGR_LOSS_TUKEY, "unknown loss");
+  DGR_ARG_CHECK(loss == DGR_LOSS_L2 || loss == DGR_LOSS_L1 || (loss_k > 0.0 && loss_k < INFINITY),
+                "loss_k must be finite and positive");
+  return DGR_OK;
+}
+
+// the checks every ICP entry point makes before it enqueues
+int32_t check_icp(int64_t cap, double voxel, double max_dist, int32_t max_iter, int64_t n_src, const double* T_init,
+                  const double* ws, const double* result, const dgr_keyspec_t* spec) {
+  DGR_TRY(dgr_check_hash_search(cap, voxel, max_dist, kMaxReach));
+  DGR_ARG_CHECK(max_iter >= 0, "bad ICP parameters");
+  DGR_ARG_CHECK(n_src >= 0 && n_src < (1ll << 31), "point count out of range");
+  DGR_ARG_CHECK(T_init != nullptr && ws != nullptr && result != nullptr && spec != nullptr, "null pointer");
+  return DGR_OK;
 }
 
 }  // namespace
@@ -530,6 +698,24 @@ int32_t dgr_color_gradient(const float* xyz, const float* normals, const float* 
                     GradientSums{normals, intensity, grad}, counts, stream);
 }
 
+int32_t dgr_estimate_covariances(const float* xyz, int64_t n, const dgr_keyspec_t* spec, const uint64_t* keys,
+                                 const int32_t* vals, int64_t cap, int32_t batch, double cell, double radius,
+                                 int32_t max_nn, double* cov, int32_t* counts, void* stream) {
+  DGR_ARG_CHECK(n == 0 || cov != nullptr, "null pointer");
+  return nbr_launch(xyz, n, spec, keys, vals, cap, batch, cell, radius, max_nn, CovarianceSums{cov}, counts, stream);
+}
+
+int32_t dgr_covariances_from_normals(const float* normals, int64_t n, double epsilon, double* cov, void* stream) {
+  DGR_ARG_CHECK(n >= 0 && n < (1ll << 31), "point count out of range");
+  DGR_ARG_CHECK(epsilon > 0.0 && epsilon < INFINITY, "epsilon must be finite and positive");
+  DGR_ARG_CHECK(n == 0 || (normals != nullptr && cov != nullptr), "null pointer");
+  if (n == 0) return DGR_OK;
+  cov_from_normals_kernel<<<dgr_blocks(n, 256), 256, 0, (cudaStream_t)stream>>>(normals, n, epsilon, cov);
+  dgr_note_launches(1);
+  DGR_LAUNCH_CHECK();
+  return DGR_OK;
+}
+
 int32_t dgr_icp_ws_elems(int64_t n_src, int64_t* n_elems) {
   DGR_ARG_CHECK(n_elems != nullptr && n_src >= 0, "bad arguments");
   *n_elems = icp_layout(n_src, nullptr, nullptr, nullptr);
@@ -540,12 +726,9 @@ int32_t dgr_icp(const float* src, int64_t n_src, const float* tgt, const float* 
                 const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch, double voxel, double max_dist,
                 const double* T_init, int32_t max_iter, double rel_fitness, double rel_rmse, double* ws,
                 double* result, void* stream) {
-  DGR_TRY(dgr_check_hash_search(cap, voxel, max_dist, kMaxReach));
-  DGR_ARG_CHECK(max_iter >= 0, "bad ICP parameters");
-  DGR_ARG_CHECK(n_src >= 0 && n_src < (1ll << 31), "point count out of range");
-  DGR_ARG_CHECK(T_init != nullptr && ws != nullptr && result != nullptr && spec != nullptr, "null pointer");
+  DGR_TRY(check_icp(cap, voxel, max_dist, max_iter, n_src, T_init, ws, result, spec));
   cudaStream_t st = (cudaStream_t)stream;
-  const IcpInputs in{tgt_normals, nullptr, nullptr, nullptr, 1.0, 0.0};
+  const IcpInputs in{tgt_normals, nullptr, nullptr, nullptr, 1.0, 0.0, nullptr, nullptr, DGR_LOSS_L2, 0.0};
   if (tgt_normals != nullptr)
     icp_run<PointToPlane>(src, n_src, tgt, in, spec, keys, vals, cap, batch, voxel, max_dist, T_init, max_iter,
                           rel_fitness, rel_rmse, ws, result, st);
@@ -556,23 +739,65 @@ int32_t dgr_icp(const float* src, int64_t n_src, const float* tgt, const float* 
   return DGR_OK;
 }
 
+int32_t dgr_icp_loss(const float* src, int64_t n_src, const float* tgt, const float* tgt_normals,
+                     const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch,
+                     double voxel, double max_dist, int32_t loss, double loss_k, const double* T_init,
+                     int32_t max_iter, double rel_fitness, double rel_rmse, double* ws, double* result,
+                     void* stream) {
+  DGR_TRY(check_icp(cap, voxel, max_dist, max_iter, n_src, T_init, ws, result, spec));
+  DGR_TRY(check_loss(loss, loss_k));
+  DGR_ARG_CHECK(tgt_normals != nullptr, "null pointer: point-to-plane ICP needs target normals");
+  const IcpInputs in{tgt_normals, nullptr, nullptr, nullptr, 1.0, 0.0, nullptr, nullptr, loss, loss_k};
+  icp_run_loss<PointToPlaneT>(src, n_src, tgt, in, spec, keys, vals, cap, batch, voxel, max_dist, T_init, max_iter,
+                              rel_fitness, rel_rmse, ws, result, (cudaStream_t)stream);
+  DGR_LAUNCH_CHECK();
+  return DGR_OK;
+}
+
+int32_t dgr_colored_icp_loss(const float* src, const float* src_intensity, int64_t n_src, const float* tgt,
+                             const float* tgt_normals, const float* tgt_intensity, const float* tgt_grad,
+                             const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap,
+                             int32_t batch, double voxel, double max_dist, double lambda_geometric, int32_t loss,
+                             double loss_k, const double* T_init, int32_t max_iter, double rel_fitness,
+                             double rel_rmse, double* ws, double* result, void* stream) {
+  DGR_TRY(check_icp(cap, voxel, max_dist, max_iter, n_src, T_init, ws, result, spec));
+  DGR_TRY(check_loss(loss, loss_k));
+  DGR_ARG_CHECK(lambda_geometric >= 0.0 && lambda_geometric <= 1.0, "lambda_geometric must lie in [0, 1]");
+  DGR_ARG_CHECK(keys != nullptr && vals != nullptr && tgt != nullptr && tgt_normals != nullptr &&
+                tgt_intensity != nullptr && tgt_grad != nullptr &&
+                (n_src == 0 || (src != nullptr && src_intensity != nullptr)), "null pointer");
+  const IcpInputs in{tgt_normals, tgt_grad, tgt_intensity, src_intensity, sqrt(lambda_geometric),
+                     sqrt(1.0 - lambda_geometric), nullptr, nullptr, loss, loss_k};
+  icp_run_loss<ColoredT>(src, n_src, tgt, in, spec, keys, vals, cap, batch, voxel, max_dist, T_init, max_iter,
+                         rel_fitness, rel_rmse, ws, result, (cudaStream_t)stream);
+  DGR_LAUNCH_CHECK();
+  return DGR_OK;
+}
+
 int32_t dgr_colored_icp(const float* src, const float* src_intensity, int64_t n_src, const float* tgt,
                         const float* tgt_normals, const float* tgt_intensity, const float* tgt_grad,
                         const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap,
                         int32_t batch, double voxel, double max_dist, double lambda_geometric, const double* T_init,
                         int32_t max_iter, double rel_fitness, double rel_rmse, double* ws, double* result,
                         void* stream) {
-  DGR_TRY(dgr_check_hash_search(cap, voxel, max_dist, kMaxReach));
-  DGR_ARG_CHECK(max_iter >= 0, "bad ICP parameters");
-  DGR_ARG_CHECK(lambda_geometric >= 0.0 && lambda_geometric <= 1.0, "lambda_geometric must lie in [0, 1]");
-  DGR_ARG_CHECK(n_src >= 0 && n_src < (1ll << 31), "point count out of range");
-  DGR_ARG_CHECK(T_init != nullptr && ws != nullptr && result != nullptr && spec != nullptr && keys != nullptr &&
-                vals != nullptr && tgt != nullptr && tgt_normals != nullptr && tgt_intensity != nullptr &&
-                tgt_grad != nullptr && (n_src == 0 || (src != nullptr && src_intensity != nullptr)), "null pointer");
-  const IcpInputs in{tgt_normals, tgt_grad, tgt_intensity, src_intensity, sqrt(lambda_geometric),
-                     sqrt(1.0 - lambda_geometric)};
-  icp_run<Colored>(src, n_src, tgt, in, spec, keys, vals, cap, batch, voxel, max_dist, T_init, max_iter, rel_fitness,
-                   rel_rmse, ws, result, (cudaStream_t)stream);
+  return dgr_colored_icp_loss(src, src_intensity, n_src, tgt, tgt_normals, tgt_intensity, tgt_grad, spec, keys, vals,
+                              cap, batch, voxel, max_dist, lambda_geometric, DGR_LOSS_L2, 0.0, T_init, max_iter,
+                              rel_fitness, rel_rmse, ws, result, stream);
+}
+
+int32_t dgr_generalized_icp(const float* src, const double* src_cov, int64_t n_src, const float* tgt,
+                            const double* tgt_cov, const dgr_keyspec_t* spec, const uint64_t* keys,
+                            const int32_t* vals, int64_t cap, int32_t batch, double voxel, double max_dist,
+                            int32_t loss, double loss_k, const double* T_init, int32_t max_iter, double rel_fitness,
+                            double rel_rmse, double* ws, double* result, void* stream) {
+  DGR_TRY(check_icp(cap, voxel, max_dist, max_iter, n_src, T_init, ws, result, spec));
+  DGR_TRY(check_loss(loss, loss_k));
+  DGR_ARG_CHECK(src_cov != nullptr && tgt_cov != nullptr, "null pointer: generalized ICP needs both covariances");
+  DGR_ARG_CHECK(keys != nullptr && vals != nullptr && tgt != nullptr && (n_src == 0 || src != nullptr),
+                "null pointer");
+  const IcpInputs in{nullptr, nullptr, nullptr, nullptr, 1.0, 0.0, src_cov, tgt_cov, loss, loss_k};
+  icp_run_loss<GeneralizedT>(src, n_src, tgt, in, spec, keys, vals, cap, batch, voxel, max_dist, T_init, max_iter,
+                             rel_fitness, rel_rmse, ws, result, (cudaStream_t)stream);
   DGR_LAUNCH_CHECK();
   return DGR_OK;
 }

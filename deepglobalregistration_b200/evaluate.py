@@ -189,12 +189,13 @@ def add_method_arguments(ap):
   ap.add_argument('--success_rre_thresh', type=float, default=15.0, help='deg (config.py:128; KITTI: 5)')
   ap.add_argument('--no_icp', action='store_true')
   ap.add_argument('--method', choices=('dgr', 'fcgf_ransac', 'fcgf_fgr', 'fpfh_ransac', 'fpfh_fgr', 'icp_point_to_point',
-                                       'icp_point_to_plane', 'goicp', 'super4pcs', 'pointnetlk'),
+                                       'icp_point_to_plane', 'icp_generalized', 'goicp', 'super4pcs', 'pointnetlk'),
                   default='dgr',
                   help='dgr: DeepGlobalRegistration.register; fcgf_ransac: the FCGF + RANSAC baseline on the same '
                   'checkpoint (core/fcgf_ransac.py); fcgf_fgr: FCGF + Fast Global Registration with open3d\'s '
                   'default options (core/fcgf_fgr.py); fpfh_ransac / fpfh_fgr: the same two searches on FPFH features '
-                  'instead of FCGF (core/fpfh_baseline.py); icp_point_to_point / icp_point_to_plane: ICP from the identity '
+                  'instead of FCGF (core/fpfh_baseline.py); icp_point_to_point / icp_point_to_plane / icp_generalized: ICP '
+                  '(generalized: plane-to-plane on covariances from both clouds\' normals) from the identity '
                   'on the checkpoint\'s voxelisation (core/icp_baseline.py); goicp: globally optimal Go-ICP on the same '
                   'voxelisation (core/goicp.py); super4pcs: 4-point congruent sets on the same voxelisation '
                   '(core/super4pcs.py); pointnetlk: PointNetLK on the same voxelisation with the network of '
@@ -248,7 +249,7 @@ def build_method(args, device):
   elif args.method == 'fpfh_fgr':
     from .core.fpfh_baseline import FPFHFastGlobal
     method = FPFHFastGlobal(dgr)
-  elif args.method in ('icp_point_to_point', 'icp_point_to_plane'):
+  elif args.method in ('icp_point_to_point', 'icp_point_to_plane', 'icp_generalized'):
     from .core.icp_baseline import ICPBaseline
     method = ICPBaseline(dgr, args.method[len('icp_'):], args.icp_max_correspondence_distance, args.icp_max_iteration)
   elif args.method == 'goicp':
@@ -311,6 +312,7 @@ def main(argv=None):
                   'fcgf_fgr': ('fcgf-fgr-b200', 'FGR'), 'fpfh_ransac': ('fpfh-ransac-b200', 'FPFH + RANSAC'),
                   'fpfh_fgr': ('fpfh-fgr-b200', 'FPFH + FGR'), 'icp_point_to_point': ('icp-p2p-b200', 'ICP (Point-to-point)'),
                   'icp_point_to_plane': ('icp-p2plane-b200', 'ICP (Point-to-plane)'),
+                  'icp_generalized': ('icp-gicp-b200', 'Generalized ICP'),
                   'goicp': ('goicp-b200', 'Go-ICP'), 'super4pcs': ('super4pcs-b200', 'Super4PCS'),
                   'pointnetlk': ('pointnetlk-b200', 'PointNetLK')}[args.method]
     out = os.path.join(out_dir, f'{stem}-stats.npz')

@@ -38,6 +38,7 @@ class PointCloud:
     self.attributes = dict(attributes or {}, **more_attributes)
     self.normals = None
     self.colors = None
+    self.covariances = None
 
   @property
   def points(self):
@@ -67,6 +68,23 @@ class PointCloud:
     """open3d's rule: one colour per point of a non-empty cloud."""
     return self._colors is not None and len(self._colors) == len(self._points) > 0
 
+  @property
+  def covariances(self):
+    return self._covariances
+
+  @covariances.setter
+  def covariances(self, value):
+    if value is not None:
+      value = np.asarray(value, dtype=np.float64)
+      if value.ndim != 3 or value.shape[1:] != (3, 3):
+        raise ValueError(f'covariances must be [N, 3, 3], got {value.shape}')
+      value = np.ascontiguousarray(value)
+    self._covariances = value
+
+  def has_covariances(self):
+    """open3d's rule: one covariance per point of a non-empty cloud."""
+    return self._covariances is not None and len(self._covariances) == len(self._points) > 0
+
   def __len__(self):
     return len(self._points)
 
@@ -80,6 +98,9 @@ class PointCloud:
     self._points = self._points @ T[:3, :3].T + T[:3, 3]
     if self.normals is not None:
       self.normals = np.asarray(self.normals, dtype=np.float64) @ T[:3, :3].T
+    if self._covariances is not None:
+      R = T[:3, :3]
+      self._covariances = np.ascontiguousarray(np.einsum('ab,nbc,dc->nad', R, self._covariances, R))
     return self
 
   def has_normals(self):
@@ -95,6 +116,18 @@ class PointCloud:
       return self
     from .o3d_registration import estimate_normals
     self.normals = estimate_normals(self._points, search_param, prev=self.normals)
+    return self
+
+  def estimate_covariances(self, search_param=None):
+    """``estimate_covariances(KDTreeSearchParamHybrid(radius, max_nn))`` computes per-point covariances on the GPU
+    (o3d_registration.estimate_covariances; max_nn <= 64) into ``covariances`` (float64 [N, 3, 3]).  Without an
+    argument it raises NotImplementedError: open3d's default there is KDTreeSearchParamKNN(30), an unbounded search
+    the voxel-hash kernel cannot do."""
+    if search_param is None:
+      raise NotImplementedError('estimate_covariances() defaults to KDTreeSearchParamKNN(30), which is not built: pass '
+                                'KDTreeSearchParamHybrid(radius, max_nn)')
+    from .o3d_registration import estimate_covariances
+    self.covariances = estimate_covariances(self._points, search_param)
     return self
 
   def __repr__(self):

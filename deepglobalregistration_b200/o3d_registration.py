@@ -23,6 +23,12 @@ It also carries the calls open3d users make beyond DGR's own: point-to-plane ICP
       -> dgr_color_gradient on the target, then dgr_colored_icp: ICP with a geometric and a photometric row per
          correspondence (Park, Zhou & Koltun 2017), the local refinement of open3d's reconstruction system;
 
+  registration_generalized_icp(source, target, max_correspondence_distance, init, estimation_method, criteria)
+      -> dgr_generalized_icp on covariances from estimate_covariances (-> dgr_estimate_covariances) or built from
+         normals (-> dgr_covariances_from_normals): plane-to-plane ICP (Segal, Haehnel & Thrun 2009);
+  L2Loss / L1Loss / HuberLoss / CauchyLoss / GMLoss / TukeyLoss as the kernel of the point-to-plane, colored and
+  generalized estimators -> dgr_icp_loss, dgr_colored_icp_loss, dgr_generalized_icp;
+
   registration_fast_based_on_feature_matching(source, target, source_feature, target_feature, option)
       -> dgr_knn_top1 both ways + dgr_fgr_feature_matching: Fast Global Registration (mutual matches, tuple
          test, graduated non-convexity) with FastGlobalRegistrationOption's fields and defaults;
@@ -55,11 +61,72 @@ class TransformationEstimationPointToPoint:
     self.with_scaling = False
 
 
+class RobustKernel:
+  """open3d >= 0.12's robust loss: each residual row r of an estimator is weighted by Weight(r) (_abi.LOSS_IDS)."""
+  loss = None
+
+  def __init__(self, k=1.0):
+    k = float(k)
+    if self.loss in ('Huber', 'Cauchy', 'GM', 'Tukey') and not 0.0 < k < math.inf:
+      raise ValueError(f'{type(self).__name__}: k must be finite and positive, got {k}')
+    self.k = k
+
+  def __repr__(self):
+    return f'{type(self).__name__}(k={self.k})'
+
+
+class L2Loss(RobustKernel):
+  """Weight 1: the estimator without a kernel."""
+  loss = 'L2'
+
+  def __init__(self):
+    super().__init__(1.0)
+
+
+class L1Loss(RobustKernel):
+  """Weight 1 / |r| (0 at r = 0, where open3d's is infinite)."""
+  loss = 'L1'
+
+  def __init__(self):
+    super().__init__(1.0)
+
+
+class HuberLoss(RobustKernel):
+  """Weight 1 for |r| <= k, else k / |r|."""
+  loss = 'Huber'
+
+
+class CauchyLoss(RobustKernel):
+  """Weight 1 / (1 + (r / k)^2)."""
+  loss = 'Cauchy'
+
+
+class GMLoss(RobustKernel):
+  """Geman-McClure: weight k / (k + r^2)^2."""
+  loss = 'GM'
+
+
+class TukeyLoss(RobustKernel):
+  """Weight (1 - min(1, |r| / k)^2)^2: 0 beyond k."""
+  loss = 'Tukey'
+
+
+def _kernel_check(kernel):
+  """None or one of the six losses; any other object raises NotImplementedError."""
+  if kernel is not None and not isinstance(kernel, RobustKernel):
+    raise NotImplementedError(f'{type(kernel).__name__}: only L2Loss, L1Loss, HuberLoss, CauchyLoss, GMLoss and '
+                              'TukeyLoss are built')
+  return kernel
+
+
+def _loss_args(kernel):
+  """(loss, loss_k) of the _abi ICP wrappers: (None, 1.0) without a kernel."""
+  return (None, 1.0) if kernel is None else (kernel.loss, kernel.k)
+
+
 class TransformationEstimationPointToPlane:
   def __init__(self, kernel=None):
-    if kernel is not None:
-      raise NotImplementedError('robust kernels (the open3d >= 0.12 form) are not built')
-    self.kernel = None
+    self.kernel = _kernel_check(kernel)
 
 
 class TransformationEstimationForColoredICP:
@@ -67,11 +134,21 @@ class TransformationEstimationForColoredICP:
   as open3d's constructor does."""
 
   def __init__(self, lambda_geometric=0.968, kernel=None):
-    if kernel is not None:
-      raise NotImplementedError('robust kernels (the open3d >= 0.12 form) are not built')
+    self.kernel = _kernel_check(kernel)
     lam = float(lambda_geometric)
     self.lambda_geometric = lam if 0.0 <= lam <= 1.0 else 0.968
-    self.kernel = None
+
+
+class TransformationEstimationForGeneralizedICP:
+  """Generalized ICP (Segal, Haehnel & Thrun 2009): plane-to-plane residuals weighted by both clouds' surface
+  covariances.  epsilon: the covariance built from a normal n is R diag(epsilon, 1, 1) R^T (flat along n)."""
+
+  def __init__(self, epsilon=1e-3, kernel=None):
+    self.kernel = _kernel_check(kernel)
+    epsilon = float(epsilon)
+    if not 0.0 < epsilon < math.inf:
+      raise ValueError(f'epsilon must be finite and positive, got {epsilon}')
+    self.epsilon = epsilon
 
 
 class KDTreeSearchParamHybrid:
@@ -125,6 +202,26 @@ def estimate_normals(points, search_param, prev=None):
   prev_d = None if prev is None else torch.from_numpy(np.ascontiguousarray(prev, dtype=np.float32)).to(dev)
   nrm = _abi.estimate_normals(p32, (spec, table), cell, search_param.radius, search_param.max_nn, prev=prev_d)
   return nrm.cpu().numpy().astype(np.float64)
+
+
+def estimate_covariances(points, search_param):
+  """Per-point covariances of points [N, 3] (open3d's EstimatePerPointCovariances) from KDTreeSearchParamHybrid
+  neighbours, through a voxel hash of the cloud (dgr_estimate_covariances).  -> float64 [N, 3, 3]."""
+  _hybrid_check(search_param)
+  pts = np.asarray(points, dtype=np.float64).reshape(-1, 3)
+  if len(pts) == 0:
+    return np.zeros((0, 3, 3))
+  dev = _abi.require_device('cuda')
+  _abi.refresh_stream()
+  p64 = torch.from_numpy(np.ascontiguousarray(pts)).to(dev)
+  cell, spec, table, p32 = _target_hash(p64, search_param.radius, rows=True)
+  cov = _abi.estimate_covariances(p32, (spec, table), cell, search_param.radius, search_param.max_nn)
+  return _cov33(cov.cpu().numpy())
+
+
+def _cov33(c6):
+  """[N, 6] (xx, xy, xz, yy, yz, zz) -> [N, 3, 3]."""
+  return np.ascontiguousarray(np.stack([c6[:, [0, 1, 2]], c6[:, [1, 3, 4]], c6[:, [2, 4, 5]]], axis=1))
 
 
 class ICPConvergenceCriteria:
@@ -230,11 +327,20 @@ def compute_fpfh_feature(input, search_param):
 
 
 def registration_icp(source, target, max_correspondence_distance, init=None, estimation_method=None, criteria=None):
-  """Point-to-point (the default, what DGR calls) or point-to-plane ICP; point-to-plane needs target normals
-  (``target.estimate_normals(KDTreeSearchParamHybrid(radius, max_nn))``)."""
+  """Point-to-point (the default, what DGR calls), point-to-plane or generalized ICP; point-to-plane needs target
+  normals (``target.estimate_normals(KDTreeSearchParamHybrid(radius, max_nn))``), generalized ICP covariances on both
+  clouds (``estimate_covariances``; unlike open3d, which returns ``init`` unchanged, it raises without them)."""
+  if isinstance(estimation_method, TransformationEstimationForGeneralizedICP):
+    for pcd, which in ((source, 'source'), (target, 'target')):
+      if getattr(pcd, 'covariances', None) is None:
+        raise RuntimeError(f'registration_icp with TransformationEstimationForGeneralizedICP needs covariances on the '
+                           f'{which} cloud: call estimate_covariances(KDTreeSearchParamHybrid(radius, max_nn)) first, '
+                           'or use registration_generalized_icp')
+    return registration_generalized_icp(source, target, max_correspondence_distance, init, estimation_method,
+                                        criteria)
   plane = isinstance(estimation_method, TransformationEstimationPointToPlane)
   if not (plane or estimation_method is None or isinstance(estimation_method, TransformationEstimationPointToPoint)):
-    raise NotImplementedError('only point-to-point and point-to-plane ICP are built')
+    raise NotImplementedError('only point-to-point, point-to-plane and generalized ICP are built')
   tgt_normals = getattr(target, 'normals', None) if plane else None
   if plane and tgt_normals is None:
     raise RuntimeError('TransformationEstimationPointToPlane needs target normals: call '
@@ -255,8 +361,9 @@ def registration_icp(source, target, max_correspondence_distance, init=None, est
     nrm = np.asarray(tgt_normals, dtype=np.float32).reshape(-1, 3)
     if len(nrm) != len(tgt):
       raise RuntimeError('target normals must hold one row per target point')
+    loss, loss_k = _loss_args(estimation_method.kernel)
     res = _abi.icp_point_to_plane(src, tgt, torch.from_numpy(np.ascontiguousarray(nrm)).to(dev), (spec, table), cell,
-                                  *args)
+                                  *args, loss=loss, loss_k=loss_k)
   else:
     res = _abi.icp_point_to_point(src, tgt, (spec, table), cell, *args)
   r = res.cpu().numpy()
@@ -313,6 +420,8 @@ def registration_colored_icp(source, target, *args, **kwargs):
   colour gradients come from its normals and colours at KDTreeSearchParamHybrid(2 max_distance, 30)
   (dgr_color_gradient); the ICP (dgr_colored_icp) searches a voxel hash of the target whose cell serves both radii."""
   max_distance, init, criteria, lam = _colored_icp_arguments(args, kwargs)
+  est = kwargs.get('estimation_method', args[2] if len(args) >= 3 else None)
+  kernel = est.kernel if isinstance(est, TransformationEstimationForColoredICP) else None     # the >= 0.12 form
   if not max_distance > 0.0:
     raise ValueError(f'max_distance must be positive, got {max_distance}')
   tgt_normals = getattr(target, 'normals', None)
@@ -335,9 +444,67 @@ def registration_colored_icp(source, target, *args, **kwargs):
   i_tgt = torch.from_numpy(intensity(c_tgt)).to(dev)
   grad = _abi.color_gradient(tgt, nrm_d, i_tgt, (spec, table), cell, 2.0 * max_distance, 30)
   T12 = torch.from_numpy(np.ascontiguousarray(T0[:3])).to(dev)
+  loss, loss_k = _loss_args(kernel)
   r = _abi.icp_colored(src, i_src, tgt, nrm_d, i_tgt, grad, (spec, table), cell, max_distance, lam, T12,
                        int(criteria.max_iteration), float(criteria.relative_fitness),
-                       float(criteria.relative_rmse)).cpu().numpy()
+                       float(criteria.relative_rmse), loss=loss, loss_k=loss_k).cpu().numpy()
+  return RegistrationResult(r[:16], r[16], r[17], r[19])
+
+
+def _gicp_covariances(pcd, which, epsilon, dev):
+  """The cloud's covariances as the device float64 [N, 6] dgr_generalized_icp reads: its own if it has them, else
+  built from its normals with epsilon (dgr_covariances_from_normals); open3d's precedence."""
+  n = len(np.asarray(getattr(pcd, 'points', pcd)).reshape(-1, 3))
+  cov = getattr(pcd, 'covariances', None)
+  if cov is not None:
+    cov = np.asarray(cov, dtype=np.float64).reshape(-1, 3, 3)
+    if len(cov) != n:
+      raise RuntimeError(f'{which} covariances must hold one [3, 3] matrix per point')
+    c6 = np.stack([cov[:, 0, 0], cov[:, 0, 1], cov[:, 0, 2], cov[:, 1, 1], cov[:, 1, 2], cov[:, 2, 2]], axis=1)
+    return torch.from_numpy(np.ascontiguousarray(c6)).to(dev)
+  nrm = getattr(pcd, 'normals', None)
+  if nrm is None:
+    raise RuntimeError(f'generalized ICP needs covariances or normals on the {which} cloud: call '
+                       'estimate_covariances(KDTreeSearchParamHybrid(radius, max_nn)) or '
+                       'estimate_normals(KDTreeSearchParamHybrid(radius, max_nn)) first')
+  nrm = np.asarray(nrm, dtype=np.float32).reshape(-1, 3)
+  if len(nrm) != n:
+    raise RuntimeError(f'{which} normals must hold one row per point')
+  return _abi.covariances_from_normals(torch.from_numpy(np.ascontiguousarray(nrm)).to(dev), epsilon)
+
+
+def registration_generalized_icp(source, target, max_correspondence_distance, init=None, estimation_method=None,
+                                 criteria=None):
+  """open3d's generalized ICP (Segal, Haehnel & Thrun 2009; plane-to-plane).  Each cloud uses its own covariances
+  if it has them, else covariances built from its normals with estimation_method.epsilon; a cloud with neither is an
+  error (open3d would estimate normals with KDTreeSearchParamKNN, which is not built).  dgr_generalized_icp searches
+  a voxel hash of the target as registration_icp does."""
+  est = TransformationEstimationForGeneralizedICP() if estimation_method is None else estimation_method
+  if not isinstance(est, TransformationEstimationForGeneralizedICP):
+    raise NotImplementedError('registration_generalized_icp takes TransformationEstimationForGeneralizedICP')
+  d = float(max_correspondence_distance)
+  if not d > 0.0:
+    raise ValueError(f'max_correspondence_distance must be positive, got {max_correspondence_distance}')
+  for pcd, which in ((source, 'source'), (target, 'target')):
+    if getattr(pcd, 'covariances', None) is None and getattr(pcd, 'normals', None) is None:
+      raise RuntimeError(f'generalized ICP needs covariances or normals on the {which} cloud: call '
+                         'estimate_covariances(KDTreeSearchParamHybrid(radius, max_nn)) or '
+                         'estimate_normals(KDTreeSearchParamHybrid(radius, max_nn)) first')
+  criteria = criteria or ICPConvergenceCriteria()
+  T0 = np.eye(4) if init is None else np.asarray(init, dtype=np.float64).reshape(4, 4)
+  dev = _abi.require_device('cuda')
+  _abi.refresh_stream()
+  src64, tgt64 = _points(source, dev), _points(target, dev)
+  if len(src64) == 0 or len(tgt64) == 0:
+    return RegistrationResult(T0)
+  c_src = _gicp_covariances(source, 'source', est.epsilon, dev)
+  c_tgt = _gicp_covariances(target, 'target', est.epsilon, dev)
+  cell, spec, table, tgt = _target_hash(tgt64, d, rows=True)
+  T12 = torch.from_numpy(np.ascontiguousarray(T0[:3])).to(dev)
+  loss, loss_k = _loss_args(est.kernel)
+  r = _abi.icp_generalized(src64.float().contiguous(), c_src, tgt, c_tgt, (spec, table), cell, d, T12,
+                           int(criteria.max_iteration), float(criteria.relative_fitness),
+                           float(criteria.relative_rmse), loss=loss, loss_k=loss_k).cpu().numpy()
   return RegistrationResult(r[:16], r[16], r[17], r[19])
 
 

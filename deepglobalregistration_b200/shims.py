@@ -47,7 +47,9 @@ def _open3d_stub():
   registration_fast_based_on_feature_matching / FastGlobalRegistrationOption / compute_fpfh_feature for FGR and
   FPFH users, the pose graph and global_optimization for multiway registration, and
   TransformationEstimationPointToPlane with geometry.KDTreeSearchParamHybrid for point-to-plane ICP users, and
-  registration_colored_icp / TransformationEstimationForColoredICP for colored-ICP refinement) backed
+  registration_colored_icp / TransformationEstimationForColoredICP for colored-ICP refinement,
+  registration_generalized_icp / TransformationEstimationForGeneralizedICP / estimate_covariances and the six robust
+  losses) backed
   by libdgr_b200 (o3d_registration.py), and what util/integration.py fuses RGB-D frames with
   (pipelines.integration.ScalableTSDFVolume, camera.PinholeCameraIntrinsic, geometry.Image / RGBDImage /
   TriangleMesh, io.read_image / write_triangle_mesh; o3d_integration.py) - so the reference's OWN
@@ -81,7 +83,9 @@ def _open3d_stub():
                'get_information_matrix_from_point_clouds', 'PoseGraph', 'PoseGraphNode', 'PoseGraphEdge',
                'GlobalOptimizationLevenbergMarquardt', 'GlobalOptimizationGaussNewton',
                'GlobalOptimizationConvergenceCriteria', 'GlobalOptimizationOption', 'global_optimization',
-               'TransformationEstimationForColoredICP', 'registration_colored_icp'):
+               'TransformationEstimationForColoredICP', 'registration_colored_icp',
+               'TransformationEstimationForGeneralizedICP', 'registration_generalized_icp', 'estimate_covariances',
+               'RobustKernel', 'L2Loss', 'L1Loss', 'HuberLoss', 'CauchyLoss', 'GMLoss', 'TukeyLoss'):
     setattr(o3d.pipelines.registration, name, getattr(reg, name))
   o3d.registration = o3d.pipelines.registration          # the pre-0.12 module path
   sys.modules['open3d.pipelines'] = o3d.pipelines

@@ -211,6 +211,19 @@ int32_t dgr_compute_fpfh(const float* xyz, const float* normals, int64_t n, cons
                          const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch, double cell,
                          double radius, int32_t max_nn, int32_t ld, void* ws, float* out, int32_t* counts,
                          void* stream);
+/* Per-point covariances of the cloud xyz[n] (open3d EstimatePerPointCovariances(KDTreeSearchParamHybrid(radius,
+ * max_nn)); oracle/gicp.py): the arguments, checks and neighbour sets (point i included) of dgr_estimate_normals,
+ * and C = E[e e^T] - mu mu^T over the kept offsets in fp64; the identity for fewer than 3 neighbours.
+ * cov: double [n, 6] = (xx, xy, xz, yy, yz, zz); counts: int32 [n] = rows within the radius (before the max_nn
+ * truncation), equal to dgr_estimate_normals'.  No atomics, the same bits on every run. */
+int32_t dgr_estimate_covariances(const float* xyz, int64_t n, const dgr_keyspec_t* spec, const uint64_t* keys,
+                                 const int32_t* vals, int64_t cap, int32_t batch, double cell, double radius,
+                                 int32_t max_nn, double* cov, int32_t* counts, void* stream);
+/* Generalized-ICP covariances from normals (open3d InitializePointCloudForGeneralizedICP; oracle/gicp.py): per point,
+ * C = R diag(epsilon, 1, 1) R^T with R = GetRotationFromE1ToX(n) in fp64 (v = e1 x n, c = e1.n,
+ * R = I + [v]x + [v]x^2 / (1 + c), or diag(-1, -1, 1) when c < -0.99).  normals: float [n, 3]; epsilon finite and
+ * > 0; cov: double [n, 6] as dgr_estimate_covariances. */
+int32_t dgr_covariances_from_normals(const float* normals, int64_t n, double epsilon, double* cov, void* stream);
 /* Colour gradients of the cloud xyz[n] (open3d 0.10 InitializePointCloudForColoredICP; oracle/colored_icp.py) with
  * normals[n, 3] and intensity[n] (float; (r + g + b) / 3 of colours in [0, 1]), through its OWN voxel hash and with
  * the neighbour sets of dgr_estimate_normals (radius / cell <= 4, the max_nn (1..64) smallest by (d^2, row), point i
@@ -254,6 +267,42 @@ int32_t dgr_colored_icp(const float* src, const float* src_intensity, int64_t n_
                         int32_t batch, double voxel, double max_dist, double lambda_geometric, const double* T_init,
                         int32_t max_iter, double rel_fitness, double rel_rmse, double* ws, double* result,
                         void* stream);
+/* Robust losses of the ICP estimators (open3d >= 0.12's RobustKernel; oracle/gicp.py): each residual row r is
+ * weighted by w(r) in J^T J and J^T r.  w: L2 1; L1 1 / |r| (0 at r = 0); Huber(k) 1 for |r| <= k, else k / |r|;
+ * Cauchy(k) 1 / (1 + (r / k)^2); GM(k) k / (k + r^2)^2; Tukey(k) (1 - min(1, |r| / k)^2)^2.  loss_k: finite and
+ * > 0 for Huber, Cauchy, GM and Tukey.  DGR_LOSS_L2 runs the unweighted code: the bits of the call without a loss. */
+#define DGR_LOSS_L2 0
+#define DGR_LOSS_L1 1
+#define DGR_LOSS_HUBER 2
+#define DGR_LOSS_CAUCHY 3
+#define DGR_LOSS_GM 4
+#define DGR_LOSS_TUKEY 5
+/* dgr_icp's point-to-plane ICP (tgt_normals required) with a robust loss. */
+int32_t dgr_icp_loss(const float* src, int64_t n_src, const float* tgt, const float* tgt_normals,
+                     const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap, int32_t batch,
+                     double voxel, double max_dist, int32_t loss, double loss_k, const double* T_init,
+                     int32_t max_iter, double rel_fitness, double rel_rmse, double* ws, double* result,
+                     void* stream);
+/* dgr_colored_icp with a robust loss; each of the two rows is weighted on its own sqrt(lambda)-scaled residual. */
+int32_t dgr_colored_icp_loss(const float* src, const float* src_intensity, int64_t n_src, const float* tgt,
+                             const float* tgt_normals, const float* tgt_intensity, const float* tgt_grad,
+                             const dgr_keyspec_t* spec, const uint64_t* keys, const int32_t* vals, int64_t cap,
+                             int32_t batch, double voxel, double max_dist, double lambda_geometric, int32_t loss,
+                             double loss_k, const double* T_init, int32_t max_iter, double rel_fitness,
+                             double rel_rmse, double* ws, double* result, void* stream);
+/* Generalized ICP (Segal, Haehnel & Thrun 2009; open3d >= 0.13 registration_generalized_icp with
+ * TransformationEstimationForGeneralizedICP; oracle/gicp.py): dgr_icp's correspondences, stopping rule, workspace
+ * (dgr_icp_ws_elems) and result, with the covariances src_cov [n_src, 6] and tgt_cov [n_tgt, 6] (double, as
+ * dgr_estimate_covariances writes them).  Per correspondence (s = current transformed source point, q its target
+ * point, R the current rotation): M = R C_s R^T + C_t, W = M^(-1/2) (principal root), three rows k = 0..2 with
+ * v = W[k]: r = v.(s - q), J = [s x v, v], weighted by the loss; J^T J x = -J^T r by Cholesky (a non-positive pivot
+ * gives the identity update), T <- [Rz(x2) Ry(x1) Rx(x0) | x3..5] T.  A correspondence whose M has a non-positive
+ * Cholesky pivot adds no row but counts towards fitness and RMSE. */
+int32_t dgr_generalized_icp(const float* src, const double* src_cov, int64_t n_src, const float* tgt,
+                            const double* tgt_cov, const dgr_keyspec_t* spec, const uint64_t* keys,
+                            const int32_t* vals, int64_t cap, int32_t batch, double voxel, double max_dist,
+                            int32_t loss, double loss_k, const double* T_init, int32_t max_iter, double rel_fitness,
+                            double rel_rmse, double* ws, double* result, void* stream);
 
 /* ---- Multiway registration: open3d's GetInformationMatrixFromPointClouds and GlobalOptimization with
  *      GlobalOptimizationLevenbergMarquardt (csrc/posegraph.cu; oracle/pose_graph.py) ---------------------- */
