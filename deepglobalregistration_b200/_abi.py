@@ -1152,3 +1152,49 @@ def tsdf_mc_tables():
   tri = np.zeros((256, 16), np.int32)
   call('dgr_tsdf_mc_tables', ptr(edge), ptr(tri))
   return edge, tri
+
+
+ODOMETRY_MAX_LEVELS = _DEFINES['DGR_ODOMETRY_MAX_LEVELS']
+ODOMETRY_MAX_ITERATIONS = _DEFINES['DGR_ODOMETRY_MAX_ITERATIONS']
+ODOMETRY_RESULT = _DEFINES['DGR_ODOMETRY_RESULT']
+ODOMETRY_RESULT_HEAD = _DEFINES['DGR_ODOMETRY_RESULT_HEAD']
+ODOMETRY_JACOBIANS = {'hybrid': _DEFINES['DGR_ODOMETRY_JACOBIAN_HYBRID'], 'color': _DEFINES['DGR_ODOMETRY_JACOBIAN_COLOR']}
+
+
+def rgbd_odometry_ws_layout(width, height, levels):
+  """Word offsets of the images dgr_rgbd_odometry leaves in its workspace (dgr_b200.h)."""
+  off = np.zeros(8 * int(levels) + 3, dtype=np.int64)
+  call('dgr_rgbd_odometry_ws_layout', int(width), int(height), int(levels), ptr(off))
+  return off
+
+
+def rgbd_odometry(src_intensity, src_depth, tgt_intensity, tgt_depth, intrinsic, odo_init, jacobian='hybrid',
+                  iterations=(20, 10, 5), max_depth_diff=0.03, min_depth=0.0, max_depth=4.0, ws=None, result=None):
+  """open3d's legacy compute_rgbd_odometry (dgr_rgbd_odometry), enqueued without a host read.  Images: CUDA float32
+  [H, W] intensity and metric depth of both frames; intrinsic: (fx, fy, cx, cy); odo_init: 4x4 mapping the source
+  camera into the target camera; iterations: per level, coarsest first.  ws: a uint64 workspace of
+  dgr_rgbd_odometry_ws_elems words (an arena buffer by default); result: a CUDA float64 [ODOMETRY_RESULT] to write.
+  -> result (pose 16, success, steps, info 36, its count, per-step counts)."""
+  H, W = src_depth.shape if src_depth.dim() == 2 else (0, 0)
+  for name, a in (('src_intensity', src_intensity), ('src_depth', src_depth), ('tgt_intensity', tgt_intensity),
+                  ('tgt_depth', tgt_depth)):
+    _chk(a, torch.float32, name)
+    if a.shape != (H, W):
+      raise DgrError(f'{name} must be [H, W] = [{H}, {W}], got {tuple(a.shape)}')
+  if jacobian not in ODOMETRY_JACOBIANS:
+    raise DgrError(f'jacobian must be one of {sorted(ODOMETRY_JACOBIANS)}, got {jacobian!r}')
+  dev = src_depth.device
+  intr = np.ascontiguousarray(np.asarray(intrinsic, dtype=np.float64).reshape(4))
+  init = np.ascontiguousarray(np.asarray(odo_init, dtype=np.float64).reshape(4, 4))
+  its = np.ascontiguousarray(np.asarray(iterations, dtype=np.int32).reshape(-1))
+  L = len(its)
+  if ws is None:
+    n = C.c_int64(0)
+    call('dgr_rgbd_odometry_ws_elems', int(W), int(H), L, C.byref(n))
+    ws = scratch('rgbd_odometry', n.value, torch.int64, dev)
+  if result is None:
+    result = torch.empty(ODOMETRY_RESULT, dtype=torch.float64, device=dev)
+  call('dgr_rgbd_odometry', ptr(src_intensity), ptr(src_depth), ptr(tgt_intensity), ptr(tgt_depth), int(W), int(H),
+       ptr(intr), ptr(init), ODOMETRY_JACOBIANS[jacobian], ptr(its), L, float(max_depth_diff), float(min_depth),
+       float(max_depth), ptr(ws), ptr(result), stream())
+  return result

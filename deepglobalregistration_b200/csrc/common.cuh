@@ -16,6 +16,11 @@ void dgr_note_launches(int n);   // bookkeeping for dgr_launch_count()
 void dgr_knn_top1_packed(const float* f0, int n0, const float* f1, int n1, int c, uint64_t* packed,
                          const int32_t* live, cudaStream_t st);
 
+// posegraph.cu: open3d's 6x6 information matrix [[tr(Q) I - Q, [S]x], [[S]x^T, n I]] from per-CTA partials
+// part[b][10] = (n, sum q, sum q q^T (xx, xy, xz, yy, yz, zz)), b < n_blocks, added in a fixed order; out[37] = the
+// matrix row-major, then n.  One launch (not counted: its callers count it).
+void dgr_info_final(const double* part, int n_blocks, double* out, cudaStream_t st);
+
 #define DGR_CUDA_CHECK(expr)                                                            \
   do {                                                                                  \
     cudaError_t e__ = (expr);                                                           \

@@ -278,11 +278,6 @@ __global__ void icp_init_kernel(const double* __restrict__ T_init, IcpState* st)
   }
 }
 
-// Lane `sub` of a point's group of 8 owns the sums k = 8 a + sub, in its accumulator a
-__device__ __forceinline__ void add_sum(double* acc, int sub, int k, double v) {
-  if ((k & 7) == sub) acc[k >> 3] += v;
-}
-
 // What the estimators read besides the matched pair: target normals (point-to-plane, colored), for colored ICP the
 // target colour gradients and intensities, the source intensities and sqrt(lambda), sqrt(1 - lambda), for
 // generalized ICP both clouds' covariances, and the robust loss (DGR_LOSS_*) and its scale k of a weighted estimator
@@ -309,21 +304,6 @@ __device__ __forceinline__ double loss_weight(int loss, double k, double r) {
     case DGR_LOSS_TUKEY: { const double u = fmin(1.0, a / k), e = 1.0 - u * u; return e * e; }
     default: return 1.0;
   }
-}
-
-// One residual row r, J into the 29 sums J^T J (upper triangle, 21) and J^T r (6); weighted (kW): w J J^T and w J r.
-// The unweighted instantiation is the plain products, not a multiply by 1.
-template <bool kW>
-__device__ __forceinline__ void add_row(double* acc, int sub, const double J[6], double r, double w) {
-  int k = 0;
-#pragma unroll
-  for (int a = 0; a < 6; ++a) {
-    const double wa = kW ? w * J[a] : J[a];
-#pragma unroll
-    for (int b = a; b < 6; ++b) add_sum(acc, sub, k++, wa * J[b]);
-  }
-#pragma unroll
-  for (int a = 0; a < 6; ++a) add_sum(acc, sub, 21 + a, (kW ? w * J[a] : J[a]) * r);
 }
 
 // open3d's TransformationEstimationPointToPoint: sums n, sum d^2, sum p (3), sum q (3), sum q p^T (9) over the

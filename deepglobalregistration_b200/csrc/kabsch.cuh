@@ -1,6 +1,6 @@
 // Small fp64 solvers shared by registration.cu (weighted Procrustes), ransac.cu (4-point hypotheses), fgr.cu and
-// pointnetlk.cu (Gauss-Newton / Lucas-Kanade steps), icp.cu (normals, ICP steps), goicp.cu (trimmed ICP) and
-// super4pcs.cu (congruent-set fits).
+// pointnetlk.cu (Gauss-Newton / Lucas-Kanade steps), icp.cu (normals, ICP steps), goicp.cu (trimmed ICP),
+// super4pcs.cu (congruent-set fits) and odometry.cu (RGB-D odometry steps).
 #pragma once
 
 // ---------------------------------------------------------------------------------------
@@ -141,6 +141,29 @@ __device__ __forceinline__ void zyx_update_left(const double x[6], const double 
   for (int r = 0; r < 3; ++r)
     for (int c = 0; c < 4; ++c)
       Tn[4 * r + c] = D[r][0] * T[c] + D[r][1] * T[4 + c] + D[r][2] * T[8 + c] + (c == 3 ? x[3 + r] : 0.0);
+}
+
+// ---------------------------------------------------------------------------------------
+// The 29 fixed-order Gauss-Newton sums (icp.cu's estimators, odometry.cu): a point's group of 8 lanes shares its rows
+// ---------------------------------------------------------------------------------------
+// Lane `sub` of a point's group of 8 owns the sums k = 8 a + sub, in its accumulator a
+__device__ __forceinline__ void add_sum(double* acc, int sub, int k, double v) {
+  if ((k & 7) == sub) acc[k >> 3] += v;
+}
+
+// One residual row r, J into the 29 sums J^T J (upper triangle, 21) and J^T r (6); weighted (kW): w J J^T and w J r.
+// The unweighted instantiation is the plain products, not a multiply by 1.
+template <bool kW>
+__device__ __forceinline__ void add_row(double* acc, int sub, const double J[6], double r, double w) {
+  int k = 0;
+#pragma unroll
+  for (int a = 0; a < 6; ++a) {
+    const double wa = kW ? w * J[a] : J[a];
+#pragma unroll
+    for (int b = a; b < 6; ++b) add_sum(acc, sub, k++, wa * J[b]);
+  }
+#pragma unroll
+  for (int a = 0; a < 6; ++a) add_sum(acc, sub, 21 + a, (kW ? w * J[a] : J[a]) * r);
 }
 
 // ---------------------------------------------------------------------------------------

@@ -702,6 +702,12 @@ int64_t count_pairs(const int32_t* ends, int64_t E, int64_t N, std::vector<int32
 
 }  // namespace
 
+// the information matrix of kInfoNv (= 10) sums per CTA in part[n_blocks][10], written to out[37]; odometry.cu's
+// information pass shares it
+void dgr_info_final(const double* part, int n_blocks, double* out, cudaStream_t st) {
+  info_final_kernel<<<1, 32 * kInfoNv, 0, st>>>(part, n_blocks, out);
+}
+
 extern "C" {
 
 int32_t dgr_information_matrix_ws_elems(int64_t n_src, int64_t* n_elems) {
@@ -725,7 +731,7 @@ int32_t dgr_information_matrix(const float* src, int64_t n_src, const float* tgt
   const int blocks = info_blocks(n_src);
   info_match_kernel<<<blocks, kInfoThreads, 0, st>>>(src, n_src, tgt, spec, keys, vals, (uint64_t)cap - 1, batch, cell,
                                                      (int)ceil(max_dist / cell), max_dist, P, ws);
-  info_final_kernel<<<1, 32 * kInfoNv, 0, st>>>(ws, blocks, out);
+  dgr_info_final(ws, blocks, out, st);
   dgr_note_launches(2);
   DGR_LAUNCH_CHECK();
   return DGR_OK;

@@ -52,7 +52,8 @@ def _open3d_stub():
   losses) backed
   by libdgr_b200 (o3d_registration.py), and what util/integration.py fuses RGB-D frames with
   (pipelines.integration.ScalableTSDFVolume, camera.PinholeCameraIntrinsic, geometry.Image / RGBDImage /
-  TriangleMesh, io.read_image / write_triangle_mesh; o3d_integration.py) - so the reference's OWN
+  TriangleMesh, io.read_image / write_triangle_mesh; o3d_integration.py) and poses raw frames with
+  (pipelines.odometry.compute_rgbd_odometry; o3d_odometry.py) - so the reference's OWN
   DeepGlobalRegistration class, demo.py and util/integration.py run on this stack unmodified.  This package's
   DeepGlobalRegistration does not go through here: it calls the library."""
   import numpy as np
@@ -99,6 +100,15 @@ def _open3d_stub():
   o3d.integration = o3d.pipelines.integration
   sys.modules['open3d.pipelines.integration'] = o3d.pipelines.integration
   sys.modules['open3d.integration'] = o3d.pipelines.integration
+  # RGB-D odometry (make_fragments): pipelines.odometry (odometry before 0.12)
+  from . import o3d_odometry as odo
+  o3d.pipelines.odometry = types.ModuleType('open3d.pipelines.odometry')
+  for name in ('OdometryOption', 'RGBDOdometryJacobianFromHybridTerm', 'RGBDOdometryJacobianFromColorTerm',
+               'compute_rgbd_odometry'):
+    setattr(o3d.pipelines.odometry, name, getattr(odo, name))
+  o3d.odometry = o3d.pipelines.odometry
+  sys.modules['open3d.pipelines.odometry'] = o3d.pipelines.odometry
+  sys.modules['open3d.odometry'] = o3d.pipelines.odometry
   o3d.camera = types.ModuleType('open3d.camera')
   o3d.camera.PinholeCameraIntrinsic = integ.PinholeCameraIntrinsic
   sys.modules['open3d.camera'] = o3d.camera

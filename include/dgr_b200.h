@@ -343,6 +343,43 @@ int32_t dgr_pose_graph_optimize(const double* poses, int64_t n_nodes, const int3
                                 double upper_scale_factor, double lower_scale_factor, uint64_t* ws, double* poses_out,
                                 int32_t* kept_out, double* l_out, double* stats, void* stream);
 
+/* ---- RGB-D odometry: open3d's legacy compute_rgbd_odometry (csrc/odometry.cu; oracle/rgbd_odometry.py states
+ *      every reading of open3d and every departure) ------------------------------------------------------------- */
+/* Relative pose of two RGB-D frames of one pinhole camera (intrinsic: HOST double[4] = fx, fy, cx, cy at full
+ * resolution).  Inputs: device float [height][width] intensity and metric depth of the source and of the target.
+ * Preparation: depth outside [min_depth, max_depth] or <= 0 becomes NaN; a separable {0.25, 0.5, 0.25} filter
+ * (replicated border, float products summed in fp64, rounded once per pass); both intensities scaled by 0.5 / mean
+ * over the correspondences at odo_init; `levels` 2x2-average pyramid levels, camera K / 2^l; target Sobel gradients.
+ * Then, from the coarsest level (iterations[0] steps) to the finest (iterations[levels - 1]), every step finds the
+ * correspondences (one per target pixel: the nearest transformed depth, then the lowest source pixel, within
+ * max_depth_diff of the target depth), sums J^T J and J^T r of the hybrid (Park, Zhou & Koltun 2017) or colour
+ * (Steinbruecker et al. 2011) rows in a fixed order, solves by Cholesky and composes [Rz Ry Rx | t] on the left.  A
+ * failed solve, or no correspondence at odo_init, ends the call unsuccessfully.  Finally the information matrix over
+ * the full-resolution correspondences at the final pose (the target points, as dgr_information_matrix).
+ * odo_init: HOST double[16] row-major, finite (all zero reads as the identity).  Every argument is checked before the
+ * device is touched.  No host round trip; the same bits on every run.  ws: dgr_rgbd_odometry_ws_elems 8-byte words
+ * (none read before the call writes it).  result: device double[DGR_ODOMETRY_RESULT] = 4x4 pose (the identity on
+ * failure), success (1 / 0), steps run (a failed one included), 6x6 information (the identity on failure), its
+ * correspondence count, then the correspondence count of every step in order (0 for steps not run). */
+#define DGR_ODOMETRY_JACOBIAN_HYBRID 0
+#define DGR_ODOMETRY_JACOBIAN_COLOR 1
+#define DGR_ODOMETRY_MAX_LEVELS 6
+#define DGR_ODOMETRY_MAX_ITERATIONS 100      /* per level */
+#define DGR_ODOMETRY_RESULT_HEAD 55
+#define DGR_ODOMETRY_RESULT 655              /* head + max levels x max iterations */
+int32_t dgr_rgbd_odometry_ws_elems(int32_t width, int32_t height, int32_t levels, int64_t* n_elems);
+/* Word offsets into the workspace of the images a call leaves there (inspection and tests): per level l (full
+ * resolution first) the float images source intensity, source depth, target intensity, target depth, target
+ * intensity d/dx, d/dy, target depth d/dx, d/dy (Sobel, unscaled); then the two filtered full-resolution intensities
+ * before scaling, and the uint64 [height][width] correspondence buffer of the information pass (source pixel index in
+ * the low 32 bits, all ones where none).  offsets: HOST int64[8 levels + 3]. */
+int32_t dgr_rgbd_odometry_ws_layout(int32_t width, int32_t height, int32_t levels, int64_t* offsets);
+int32_t dgr_rgbd_odometry(const float* src_intensity, const float* src_depth, const float* tgt_intensity,
+                          const float* tgt_depth, int32_t width, int32_t height, const double* intrinsic,
+                          const double* odo_init, int32_t jacobian, const int32_t* iterations, int32_t levels,
+                          double max_depth_diff, double min_depth, double max_depth, uint64_t* ws, double* result,
+                          void* stream);
+
 /* ---- RGB-D fusion: open3d's ScalableTSDFVolume integrate / extract_triangle_mesh (util/integration.py:44-71),
  *      csrc/tsdf.cu; oracle/tsdf.py is the arithmetic contract, met bit for bit ------------------------------- */
 /* Units of DGR_TSDF_RES^3 voxels (the only volume_unit_resolution supported) keyed by unit coordinate, each axis in
