@@ -3,8 +3,8 @@
 Every entry point's argtypes / restype and the integer DGR_* constants are read from the
 header the library is compiled against, so the binding cannot drift from the C ABI.
 
-torch is used here for device memory, the current CUDA stream and dtype conversions
-(float32_in_cells) only; every computation happens inside the library.  There is no CPU fallback: importing this
+torch is used here for device memory and the current CUDA stream only; every computation happens inside the
+library.  There is no CPU fallback: importing this
 module without a built library, or calling into it without an sm_90 device,
 raises.
 """
@@ -280,14 +280,14 @@ def read_count(cnt):
   n, overflow = cnt.cpu().tolist()
   D2H_BYTES += 8
   if overflow:
-    raise DgrError('coordinate extent does not fit a 63-bit packed key')
+    raise DgrError('coordinates are not finite, or their extent does not fit a 63-bit packed key')
   return n
 
 
 def voxelise(xyz, voxel, batch=0):
   """The first point of every voxel of xyz CUDA float64/float32 [n, 3]: floor(xyz / voxel) in the input dtype,
   kept rows ascending, one host read.  -> (raw coords int32 [n, 4], spec, table (voxel key -> index into sel),
-  sel int32 [m], inverse int32 [n], m); raises on key overflow."""
+  sel int32 [m], inverse int32 [n], m); raises on key overflow and on non-finite coordinates."""
   raw, minmax = quantize_points(xyz, voxel, batch)
   spec = keyspec_build(minmax, 4)
   table, sel, inverse, cnt = unique_first(raw, spec)
@@ -295,23 +295,30 @@ def voxelise(xyz, voxel, batch=0):
   return raw, spec, table, sel[:n], inverse, n
 
 
-CELL_NUDGE_STEPS = 4   # float32 ulps a row may move; a float64 row needs 1, a row quantised in float32 at most 2
+CELL_NUDGE_STEPS = _DEFINES['DGR_CELL_NUDGE_STEPS']   # float32 ulps a row may move (dgr_float32_in_cells)
 
 
 def float32_in_cells(xyz, cells, cell):
-  """xyz float64/float32 [n, 3] as the float32 rows a hash search may read: floor(double(x) / cell) - the cell every
-  search kernel computes - equals the row's stored cell `cells` (int [n, 3]; voxelise's raw coords [:, 1:]) in every
-  coordinate.  A table keyed in float64 (or by a float32 division) can hold a row whose float32 value lies across a
-  cell boundary; such a coordinate is moved toward its cell one float32 ulp at a time, every other one is exactly
-  xyz.float().  Without this a search can miss an in-radius row (DESIGN.md §3)."""
-  x32 = xyz.float()
-  k = cells.double()
-  c = torch.tensor(float(cell), dtype=torch.float64, device=xyz.device)   # a scalar divisor becomes a reciprocal
-  for _ in range(CELL_NUDGE_STEPS):
-    xd = x32.double()
-    off = k - torch.floor(xd / c)
-    x32 = torch.where(off == 0, x32, torch.nextafter(x32, (off * math.inf).float()))
-  return x32.contiguous()
+  """xyz CUDA float64/float32 [n, 3] as the float32 rows a hash search may read: floor(double(x) / cell) - the cell
+  every search kernel computes - equals the row's stored cell `cells` (CUDA int [n, 3]; voxelise's raw coords
+  [:, 1:]) in every coordinate.  A table keyed in float64 (or by a float32 division) can hold a row whose float32
+  value lies across a cell boundary; such a coordinate is moved toward its cell one float32 ulp at a time, every
+  other one is exactly xyz.float().  Without this a search can miss an in-radius row (DESIGN.md §3)."""
+  if xyz.dtype not in (torch.float32, torch.float64):
+    xyz = xyz.double()
+  xyz = xyz.contiguous()
+  if cells.dtype != torch.int32 or cells.stride(-1) != 1:
+    cells = cells.to(torch.int32).contiguous()
+  n = xyz.shape[0]
+  if xyz.shape != (n, 3) or cells.shape != (n, 3):
+    raise DgrError(f'float32_in_cells: xyz and cells must be [n, 3], got {list(xyz.shape)} and {list(cells.shape)}')
+  _chk(xyz, xyz.dtype, 'xyz')
+  if not cells.is_cuda or cells.device != xyz.device:
+    raise DgrError(f'float32_in_cells: cells must be on {xyz.device}, got {cells.device}')
+  out = torch.empty(n, 3, dtype=torch.float32, device=xyz.device)
+  call('dgr_float32_in_cells', ptr(xyz), int(xyz.dtype == torch.float64), n, ptr(cells), cells.stride(0),
+       float(cell), ptr(out), stream())
+  return out
 
 
 def hash_find(coords, spec, table):

@@ -199,6 +199,21 @@ inline int32_t dgr_check_hash_search(int64_t cap, double cell, double radius, in
   return DGR_OK;
 }
 
+// The float32 coordinate a search may read for a coordinate x stored under cell k of size `cell`: every search finds
+// a row's cell as floor(double(x32) / cell), so (float)x is moved toward cell k one ulp at a time while that cell
+// differs (a float64 x needs 1 step, an x keyed by a float32 division at most 2).  A coordinate already in its cell
+// keeps its (float)x bits.  dgr_float32_in_cells (coords.cu) and the pair compaction (coordplan.cu) write rows with it.
+__device__ __forceinline__ float dgr_float32_in_cell(double x, int32_t k, double cell) {
+  float x32 = __double2float_rn(x);
+#pragma unroll
+  for (int s = 0; s < DGR_CELL_NUDGE_STEPS; ++s) {
+    const double c = floor(__ddiv_rn((double)x32, cell));
+    if (c == (double)k) break;
+    x32 = nextafterf(x32, c < (double)k ? INFINITY : -INFINITY);
+  }
+  return x32;
+}
+
 // ---------------------------------------------------------------------------------------
 // Radius neighbours of a point in its own cloud's voxel hash (one point per cell): open3d's hybrid search, restated
 // in oracle/normals.py (neighbours).  Row j is in the radius of point i when d2 = |p_j - p_i|^2 < radius^2, and the

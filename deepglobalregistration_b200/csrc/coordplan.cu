@@ -35,7 +35,7 @@ constexpr int kProbeThreads = 512;    // 16 warps = 512 output rows per probe bl
 template <typename T0, typename T1>
 __global__ void compact_voxels_kernel(const int32_t* __restrict__ raw, const int32_t* __restrict__ sel,
                                       const int32_t* __restrict__ n_unique, int64_t n_raw0,
-                                      const T0* __restrict__ xyz0, const T1* __restrict__ xyz1,
+                                      const T0* __restrict__ xyz0, const T1* __restrict__ xyz1, double cell,
                                       int32_t* __restrict__ coords, float* __restrict__ xyz,
                                       int32_t* __restrict__ counts) {
   const int n = n_unique[0];
@@ -53,15 +53,19 @@ __global__ void compact_voxels_kernel(const int32_t* __restrict__ raw, const int
   }
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = sel[i];
-    reinterpret_cast<int4*>(coords)[i] = reinterpret_cast<const int4*>(raw)[r];
-    float x, y, z;
+    const int4 k = reinterpret_cast<const int4*>(raw)[r];
+    reinterpret_cast<int4*>(coords)[i] = k;
+    double x, y, z;
     if (r < n_raw0) {
-      x = (float)xyz0[3 * r]; y = (float)xyz0[3 * r + 1]; z = (float)xyz0[3 * r + 2];
+      x = (double)xyz0[3 * r]; y = (double)xyz0[3 * r + 1]; z = (double)xyz0[3 * r + 2];
     } else {
       const int64_t q = r - n_raw0;
-      x = (float)xyz1[3 * q]; y = (float)xyz1[3 * q + 1]; z = (float)xyz1[3 * q + 2];
+      x = (double)xyz1[3 * q]; y = (double)xyz1[3 * q + 1]; z = (double)xyz1[3 * q + 2];
     }
-    xyz[3 * i] = x; xyz[3 * i + 1] = y; xyz[3 * i + 2] = z;
+    // the rows the pair's ICP searches its voxel hash with: in the cells they are keyed under (DESIGN.md §3)
+    xyz[3 * i] = dgr_float32_in_cell(x, k.y, cell);
+    xyz[3 * i + 1] = dgr_float32_in_cell(y, k.z, cell);
+    xyz[3 * i + 2] = dgr_float32_in_cell(z, k.w, cell);
   }
 }
 
@@ -349,15 +353,16 @@ extern "C" {
 
 int32_t dgr_compact_voxel_pair(const int32_t* raw_coords, const int32_t* sel, const int32_t* n_unique,
                                int64_t n_raw0, int64_t n_raw1, const void* xyz0, int32_t is_f64_0,
-                               const void* xyz1, int32_t is_f64_1, int32_t* coords, float* xyz,
+                               const void* xyz1, int32_t is_f64_1, double cell, int32_t* coords, float* xyz,
                                int32_t* counts, void* stream) {
+  DGR_ARG_CHECK(cell > 0 && cell < INFINITY, "cell must be positive and finite");
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t n_max = n_raw0 + n_raw1;
   unsigned blocks = dgr_blocks(n_max > 0 ? n_max : 1, kThreads);
   if (blocks > 1184) blocks = 1184;
 #define DGR_CV(T0, T1)                                                                                         \
   compact_voxels_kernel<T0, T1><<<blocks, kThreads, 0, st>>>(raw_coords, sel, n_unique, n_raw0, (const T0*)xyz0, \
-                                                             (const T1*)xyz1, coords, xyz, counts)
+                                                             (const T1*)xyz1, cell, coords, xyz, counts)
   if (is_f64_0 && is_f64_1) DGR_CV(double, double);
   else if (is_f64_0) DGR_CV(double, float);
   else if (is_f64_1) DGR_CV(float, double);

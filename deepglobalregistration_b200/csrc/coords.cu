@@ -19,6 +19,15 @@ constexpr int kMaxLevels = 4;      // strides per first-occurrence pass
 // ---------------------------------------------------------------------------------------
 // voxelisation
 // ---------------------------------------------------------------------------------------
+// The cell of quotient q.  A float-to-int conversion of NaN is no cell at all, so a non-finite q (NaN or infinite
+// input, or a division that overflows) goes to INT_MIN explicitly: below INT_MIN + the key margin, where
+// keyspec_kernel sets the overflow flag and the cloud is refused, whichever point of its voxel comes first.  A finite
+// q out of range saturates and is refused the same way.
+template <typename T>
+__device__ __forceinline__ int32_t cell_of(T q) {
+  return isfinite(q) ? (int32_t)floor(q) : INT_MIN;
+}
+
 template <typename T>
 __global__ void quantize_kernel(const T* __restrict__ xyz, int64_t n, T voxel, int32_t batch,
                                 int32_t* __restrict__ coords) {
@@ -28,10 +37,19 @@ __global__ void quantize_kernel(const T* __restrict__ xyz, int64_t n, T voxel, i
   T x = xyz[3 * r + 0] / voxel, y = xyz[3 * r + 1] / voxel, z = xyz[3 * r + 2] / voxel;
   int4 c;
   c.x = batch;
-  c.y = (int32_t)floor(x);
-  c.z = (int32_t)floor(y);
-  c.w = (int32_t)floor(z);
+  c.y = cell_of(x);
+  c.z = cell_of(y);
+  c.w = cell_of(z);
   reinterpret_cast<int4*>(coords)[r] = c;
+}
+
+template <typename T>
+__global__ void float32_in_cells_kernel(const T* __restrict__ xyz, int64_t n, const int32_t* __restrict__ cells,
+                                        int64_t cells_stride, double cell, float* __restrict__ out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 3 * n) return;
+  const int64_t r = i / 3;
+  out[i] = dgr_float32_in_cell((double)xyz[i], cells[r * cells_stride + (i - 3 * r)], cell);
 }
 
 __global__ void minmax_init_kernel(int32_t* minmax, int ncols) {
@@ -360,6 +378,24 @@ int32_t dgr_quantize_points(const void* xyz, int32_t is_f64, int64_t n, double v
     DGR_LAUNCH_CHECK();
   }
   return dgr_coords_minmax(coords, n, 4, minmax, stream);
+}
+
+int32_t dgr_float32_in_cells(const void* xyz, int32_t is_f64, int64_t n, const int32_t* cells, int64_t cells_stride,
+                             double cell, float* out, void* stream) {
+  DGR_ARG_CHECK(cell > 0 && cell < INFINITY, "cell must be positive and finite");
+  DGR_ARG_CHECK(n >= 0 && n < (1ll << 40), "row count out of range");
+  if (n == 0) return DGR_OK;
+  DGR_ARG_CHECK(xyz != nullptr && cells != nullptr && out != nullptr, "null argument");
+  DGR_ARG_CHECK(cells_stride >= 3, "cells rows must hold at least 3 ints");
+  const unsigned blocks = dgr_blocks(3 * n, kThreads);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (is_f64)
+    float32_in_cells_kernel<double><<<blocks, kThreads, 0, st>>>((const double*)xyz, n, cells, cells_stride, cell, out);
+  else
+    float32_in_cells_kernel<float><<<blocks, kThreads, 0, st>>>((const float*)xyz, n, cells, cells_stride, cell, out);
+  dgr_note_launches(1);
+  DGR_LAUNCH_CHECK();
+  return DGR_OK;
 }
 
 int32_t dgr_keyspec_build(const int32_t* minmax, int32_t ncols, int32_t margin, dgr_keyspec_t* spec,

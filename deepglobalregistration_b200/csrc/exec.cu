@@ -898,6 +898,8 @@ int32_t dgr_pair_register(dgr_ctx_t* c, dgr_net_t* fcgf, dgr_net_t* inlier, cons
   DGR_CUDA_CHECK(cudaStreamSynchronize(c->stream));
   DGR_TRY(c->arena.reset());
   c->reads = c->d2h_bytes = c->h2d_bytes = 0;
+  for (auto& t : c->taps) t = dgr_ctx::Tap{};       // the arena is reused: a refused pair leaves no stale taps
+  c->pair_xyz = nullptr;
   void* st = c->stream;
   const int64_t n_raw = n_raw0 + n_raw1;
   for (auto e : c->stage_marks) c->event_pool.push_back(e);
@@ -939,7 +941,7 @@ int32_t dgr_pair_register(dgr_ctx_t* c, dgr_net_t* fcgf, dgr_net_t* inlier, cons
   DGR_TRY(dgr_unique_first(raw, n_raw, 4, spec, keys, vals, cap, sel, inverse, n_unique, slot_ws, scan_ws, st));
   DGR_TRY(aalloc(c, n_raw * 4, &coords));
   DGR_TRY(aalloc(c, n_raw * 3, &xyz));
-  DGR_TRY(dgr_compact_voxel_pair(raw, sel, n_unique, n_raw0, n_raw1, d0, is_f64_0, d1, is_f64_1, coords, xyz,
+  DGR_TRY(dgr_compact_voxel_pair(raw, sel, n_unique, n_raw0, n_raw1, d0, is_f64_0, d1, is_f64_1, voxel, coords, xyz,
                                  c->meta_dev, st));
 
   mark_stage(c, ranges, 1);                                        // 1: upload + voxelisation enqueued
@@ -960,7 +962,7 @@ int32_t dgr_pair_register(dgr_ctx_t* c, dgr_net_t* fcgf, dgr_net_t* inlier, cons
   DGR_TRY(read_meta(c, meta_ints(pf)));                 // host read 1
   const int N = c->meta_host[0], N0 = c->meta_host[1], N1 = c->meta_host[2];
   if (c->meta_host[3] != 0) {
-    dgr_set_error("coordinate extent does not fit a 63-bit packed key");
+    dgr_set_error("coordinates are not finite, or their extent does not fit a 63-bit packed key");
     return DGR_ERR_ARG;
   }
   if (N0 < 1 || N1 < 1) {

@@ -42,8 +42,9 @@ extern "C" {
  *   key = sum_i (uint64)(c[i] - lo[i]) << shift[i]
  * Lives in DEVICE memory (written by dgr_keyspec_build, read by every kernel that hashes
  * coordinates) so that building it costs no host round trip.  `overflow` != 0 means the
- * coordinate extent does not fit 63 bits and every later result is invalid; the host
- * checks it at its next natural synchronisation point and raises. */
+ * coordinate extent does not fit 63 bits (a non-finite input coordinate quantises to INT_MIN,
+ * outside every accepted extent) and every later result is invalid; the host checks it at its
+ * next natural synchronisation point and raises. */
 typedef struct dgr_keyspec {
   int32_t ncols;
   int32_t overflow;
@@ -64,9 +65,18 @@ int32_t dgr_device_check(int32_t device);
  *      (core/deep_global_registration.py:152-158) ------------------------------------- */
 /* coords[r] = (batch, floor(xyz[r] / voxel)) with the division in the input dtype
  * (is_f64 ? double : float), plus per-column min/max into minmax[2*4] (device int32:
- * mins then maxes; initialised by the call). */
+ * mins then maxes; initialised by the call).  A non-finite quotient gives INT_MIN, so that the
+ * key spec built from minmax flags the cloud as overflowing. */
 int32_t dgr_quantize_points(const void* xyz, int32_t is_f64, int64_t n, double voxel, int32_t batch,
                             int32_t* coords, int32_t* minmax, void* stream);
+/* The float32 rows a voxel-hash search may read (DESIGN.md §3): out[i, a] = (float)xyz[i, a], moved toward
+ * cells[i * cells_stride + a] one float32 ulp at a time, at most DGR_CELL_NUDGE_STEPS times, while
+ * floor(double(out) / cell) - the cell every search computes - differs from it.  A coordinate already in its
+ * cell keeps its (float) bits.  xyz [n, 3] is float64 (is_f64) or float32, cells int32 rows of cells_stride >= 3
+ * ints; all device memory.  cell must be positive and finite. */
+#define DGR_CELL_NUDGE_STEPS 4
+int32_t dgr_float32_in_cells(const void* xyz, int32_t is_f64, int64_t n, const int32_t* cells, int64_t cells_stride,
+                             double cell, float* out, void* stream);
 /* Per-column min/max of an existing coordinate matrix into minmax[2*ncols]. */
 int32_t dgr_coords_minmax(const int32_t* coords, int64_t n, int32_t ncols, int32_t* minmax,
                           void* stream);
@@ -640,11 +650,13 @@ int32_t dgr_spconv_ones_bits_fwd(const float* weight, int32_t cout, const uint32
  * manager behind ME.SparseTensor / MinkowskiConvolution (core/deep_global_registration.py:167,214,
  * model/residual_block.py:31-80). */
 /* After dgr_unique_first over the concatenated raw voxel coordinates [n_raw0 + n_raw1, 4] of a scan pair:
- * coords[i] = raw[sel[i]], xyz[i] = float(point sel[i]) for i < n_unique[0]; counts[4] = (N, N0, N1,
- * key-overflow flag) with N0 = kept points of cloud 0 (sel ascending: cloud 0 rows first). */
+ * coords[i] = raw[sel[i]], xyz[i] = point sel[i] as the float32 row of dgr_float32_in_cells in the cells
+ * raw[sel[i]] of size `cell`, for i < n_unique[0]; counts[4] = (N, N0, N1, key-overflow flag) with N0 = kept
+ * points of cloud 0 (sel ascending: cloud 0 rows first). */
 int32_t dgr_compact_voxel_pair(const int32_t* raw_coords, const int32_t* sel, const int32_t* n_unique,
                                int64_t n_raw0, int64_t n_raw1, const void* xyz0, int32_t is_f64_0, const void* xyz1,
-                               int32_t is_f64_1, int32_t* coords, float* xyz, int32_t* counts, void* stream);
+                               int32_t is_f64_1, double cell, int32_t* coords, float* xyz, int32_t* counts,
+                               void* stream);
 /* Table key -> row index of rows known to be distinct (clears the table first). */
 int32_t dgr_table_build_unique(const int32_t* coords, int64_t n_max, const int32_t* n_dev, int32_t ncols,
                                const dgr_keyspec_t* spec, uint64_t* keys, int32_t* vals, int64_t cap, void* stream);

@@ -214,28 +214,25 @@ def ordered(x32):
   return np.where(b < 0, -(b & 0x7FFFFFFF), b)
 
 
-def test_float32_in_cells_moves_only_boundary_rows():
-  """_abi.float32_in_cells (on CPU tensors) over the hash-search test clouds: every row ends in its stored cell, a row
-  whose float32 value is already there keeps its bits, and no coordinate moves more than CELL_NUDGE_STEPS ulps; keys
-  from float64 (the stand-ins, multiway) and from a float32 division (preprocess() of float32 input)."""
+def test_float32_in_cells_argument_checks(built):
+  """dgr_float32_in_cells refuses a NaN, infinite, zero or negative cell and null pointers before any launch; an
+  empty call is a no-op."""
   from deepglobalregistration_b200 import _abi
-  from test_gpu_hash_search_edges import rows_in_cells, snapped_cloud, straddling_pairs
-  clouds = [(np.array([[-127.9000015258789, 0.0, 0.0], [-127.79999993771924, -0.0, 1e-30]]), 0.05)]
-  clouds += [(straddling_pairs(cell, R).reshape(-1, 3), cell) for cell in (0.03, 0.05, 0.07) for R in (1, 2, 3, 6)]
-  clouds += [(snapped_cloud(s, cell, off), cell) for s, cell in enumerate((0.05, 0.3, 0.0625, 0.02))
-             for off in (0.0, -100.0, 1000.0)]
-  moved_rows = 0
-  for x64, cell in clouds:
-    x32 = x64.astype(np.float32)
-    for x, keys in ((x64, np.floor(x64 / cell)), (x32, np.floor(x32 / np.float32(cell)).astype(np.float64))):
-      y = _abi.float32_in_cells(torch.from_numpy(x), torch.from_numpy(keys.astype(np.int32)), cell)
-      assert y.dtype == torch.float32 and y.is_contiguous()
-      y = y.numpy()
-      assert np.array_equal(np.floor(y.astype(np.float64) / cell), keys)
-      agree = np.floor(x32.astype(np.float64) / cell) == keys
-      assert y[agree].tobytes() == x32[agree].tobytes()
-      assert np.abs(ordered(y) - ordered(x32)).max() <= _abi.CELL_NUDGE_STEPS
-      moved_rows += int((~agree).any(1).sum())
-      if x is x64:
-        assert y.tobytes() == rows_in_cells(x64, cell).tobytes()
-  assert moved_rows > 1000
+  lib = _abi.lib()
+  keep = (ctypes.c_double * 16)()
+  nz = ctypes.addressof(keep)                         # a host address where only null is checked
+  launches = lib.dgr_launch_count()
+
+  def refusal(xyz, n, cells, stride, cell, out):
+    assert lib.dgr_float32_in_cells(xyz, 1, n, cells, stride, cell, out, None) == _abi._DEFINES['DGR_ERR_ARG']
+    return lib.dgr_last_error().decode()
+
+  for bad in (math.nan, math.inf, -math.inf, 0.0, -0.0, -0.05, -5e-324):
+    assert 'cell must be positive and finite' in refusal(nz, 4, nz, 3, bad, nz), bad
+  for xyz, cells, out in ((None, nz, nz), (nz, None, nz), (nz, nz, None)):
+    assert 'null argument' in refusal(xyz, 4, cells, 3, 0.05, out)
+  assert 'at least 3 ints' in refusal(nz, 4, nz, 2, 0.05, nz)
+  assert 'row count' in refusal(nz, -1, nz, 3, 0.05, nz)
+  assert lib.dgr_float32_in_cells(None, 1, 0, None, 3, 0.05, None, None) == 0
+  assert lib.dgr_launch_count() == launches
+  assert _abi.CELL_NUDGE_STEPS == 4
