@@ -1086,6 +1086,7 @@ def pointnetlk(src, tgt, packed, delta=1e-2, max_iter=10, xtol=1e-7, return_jaco
 # RGB-D fusion (csrc/tsdf.cu): the device half of o3d_integration.ScalableTSDFVolume
 # --------------------------------------------------------------------------- #
 TSDF_RES = _DEFINES['DGR_TSDF_RES']
+TSDF_RAYCAST_MAX_STEPS = _DEFINES['DGR_TSDF_RAYCAST_MAX_STEPS']
 
 
 def _host_f64(a, n, name):
@@ -1151,6 +1152,24 @@ def tsdf_extract(unit_keys, n_units, keys, vals, tsdf, weight, rgb, voxel_length
   call('dgr_tsdf_extract_write', ptr(unit_keys), int(n_units), ptr(tsdf), ptr(rgb), float(voxel_length), ptr(ws),
        ptr(verts), ptr(cols), ptr(tris), stream())
   return verts, cols, tris
+
+
+def tsdf_raycast(keys, vals, tsdf, weight, rgb, width, height, intr, pose, voxel_length, sdf_trunc, depth_min,
+                 depth_max, weight_threshold, depth, intensity=None, colour=None):
+  """Render one camera from the volume (dgr_tsdf_raycast, one launch, no host read): pose is camera_pose = inv(extrinsic)
+  (4x4 host); keys / vals None for an empty volume.  Writes the CUDA float32 outputs depth [H, W] and, for an RGB8
+  volume (rgb not None), intensity [H, W] and colour [H, W, 3] when given."""
+  for name, t, shape in (('depth', depth, (height, width)), ('intensity', intensity, (height, width)),
+                         ('colour', colour, (height, width, 3))):
+    if t is not None:
+      _chk(t, torch.float32, name)
+      if tuple(t.shape) != shape:
+        raise DgrError(f'{name}: expected {shape}, got {tuple(t.shape)}')
+  intr = _host_f64(intr, 4, 'intr')
+  pose = _host_f64(np.asarray(pose, dtype=np.float64).reshape(4, 4)[:3], 12, 'pose')
+  call('dgr_tsdf_raycast', ptr(keys), ptr(vals), 0 if keys is None else keys.numel(), ptr(tsdf), ptr(weight),
+       ptr(rgb), int(width), int(height), ptr(intr), ptr(pose), float(voxel_length), float(sdf_trunc), TSDF_RES,
+       float(depth_min), float(depth_max), float(weight_threshold), ptr(depth), ptr(intensity), ptr(colour), stream())
 
 
 def tsdf_mc_tables():

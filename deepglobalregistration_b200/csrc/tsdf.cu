@@ -19,7 +19,12 @@
 //                        same on every run), per-unit triangle counts; popcount word prefixes and vertex counts per
 //                        unit; two count scans.  write: vertices by (slot, voxel, axis) from the masks, triangles by
 //                        (slot, voxel, table order) with a block scan per 256 voxels.
+//   dgr_tsdf_raycast     a thread per pixel marches its ray through the unit table (a missing unit is jumped past its
+//                        exit plane, a known voxel by its tsdf distance, an unknown one by a voxel) to the first
+//                        + to - crossing; depth, and for RGB8 the trilinear colour and its intensity.  Read-only.
 #include <limits.h>
+#include <math.h>
+#include <math_constants.h>
 #include <stdio.h>
 
 #include "common.cuh"
@@ -509,6 +514,147 @@ __global__ void __launch_bounds__(kThreads) write_triangles_kernel(ExtractWs w, 
   }
 }
 
+// ---------------------------------------------------------------------------------------
+// ray cast (oracle/tsdf_raycast.py states the contract)
+// ---------------------------------------------------------------------------------------
+constexpr int kRayBx = 8, kRayBy = 16;         // 128 threads; a warp covers an 8 x 4 pixel tile
+
+// Slot of the unit holding lattice voxel g (fp64 integers), its local index in lv; -1 when the unit is missing or
+// outside the key range.  U receives the unit coordinates (fp64) either way.
+__device__ __forceinline__ int ray_unit(const double g[3], const uint64_t* __restrict__ keys,
+                                        const int32_t* __restrict__ vals, uint64_t mask, bool have_table, double U[3],
+                                        int& lv) {
+  bool in = have_table;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    U[k] = floor(__dmul_rn(g[k], 0.0625));
+    in = in && U[k] >= (double)DGR_TSDF_COORD_MIN && U[k] <= (double)DGR_TSDF_COORD_MAX;
+  }
+  if (!in) return -1;
+  const int ux = (int)U[0], uy = (int)U[1], uz = (int)U[2];
+  lv = (((int)g[0] - kRes * ux) * kRes + ((int)g[1] - kRes * uy)) * kRes + ((int)g[2] - kRes * uz);
+  return dgr_hash_lookup(keys, vals, mask, unit_key(ux, uy, uz));
+}
+
+// Steps a ray of the launch may take: ceil(((2 s_max) depth_max) / voxel_length) + 1, where s_max is the largest
+// world length per unit of t over the image.  s = |R (a, b, 1)| is convex in (a, b), so its maximum over the image
+// lies at a corner pixel.  Every step advances t by at least (0.5 voxel_length) / s, so no ray needs more.
+double raycast_max_steps(int W, int H, const double* intr, const double* M, double vl, double dmax) {
+  double s_max = 0.0;
+  for (int c = 0; c < 4; ++c) {
+    const double a = ((double)((c & 1) ? W - 1 : 0) - intr[2]) / intr[0];
+    const double b = ((double)((c & 2) ? H - 1 : 0) - intr[3]) / intr[1];
+    double d[3];
+    for (int k = 0; k < 3; ++k) d[k] = (M[4 * k] * a + M[4 * k + 1] * b) + M[4 * k + 2];
+    const double s = sqrt((d[0] * d[0] + d[1] * d[1]) + d[2] * d[2]);
+    s_max = s > s_max ? s : s_max;
+  }
+  return ceil(((2.0 * s_max) * dmax) / vl) + 1.0;
+}
+
+// One thread per pixel (u, v): march p(t) = C + t d from depth_min, sample the voxel holding p, stop at the first
+// (known > 0, known <= 0) pair of consecutive known samples; a missing-unit jump breaks the pair, an unknown voxel
+// does not.  Read-only on the volume; writes every output pixel.
+__global__ void __launch_bounds__(kRayBx* kRayBy)
+raycast_kernel(const uint64_t* __restrict__ keys, const int32_t* __restrict__ vals, uint64_t mask, bool have_table,
+               const float* __restrict__ tsdf, const float* __restrict__ weight, const float* __restrict__ rgb, int W,
+               int H, Cam cam, double vl, double trunc, double dmin, double dmax, double wthr, int max_steps,
+               float* __restrict__ depth, float* __restrict__ intensity, float* __restrict__ colour) {
+  const int u = blockIdx.x * kRayBx + threadIdx.x, v = blockIdx.y * kRayBy + threadIdx.y;
+  if (u >= W || v >= H) return;
+  const double a = __ddiv_rn(__dsub_rn((double)u, cam.cx), cam.fx);
+  const double b = __ddiv_rn(__dsub_rn((double)v, cam.cy), cam.fy);
+  double C[3], d[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    d[k] = __dadd_rn(__dadd_rn(__dmul_rn(cam.M[4 * k], a), __dmul_rn(cam.M[4 * k + 1], b)), cam.M[4 * k + 2]);
+    C[k] = cam.M[4 * k + 3];
+  }
+  const double s = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(d[0], d[0]), __dmul_rn(d[1], d[1])), __dmul_rn(d[2], d[2])));
+  const double dt_vox = __ddiv_rn(vl, s), dt_half = __ddiv_rn(__dmul_rn(0.5, vl), s);
+  double t = dmin, tp = 0.0, t_hit = 0.0;
+  float fp = 0.f;
+  bool prev = false, hit = false;
+  for (int n = 0; n < max_steps && t <= dmax; ++n) {    // the cap is the host's bound: it never cuts a ray short
+    double g[3], U[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) g[k] = floor(__ddiv_rn(__dadd_rn(C[k], __dmul_rn(t, d[k])), vl));
+    int lv = 0;
+    const int slot = ray_unit(g, keys, vals, mask, have_table, U, lv);
+    if (slot < 0) {                                    // missing unit: past its exit plane, plus half a voxel
+      double te = CUDART_INF;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        if (d[k] == 0.0) continue;
+        const double bnd = __dmul_rn(__dadd_rn(__dmul_rn(U[k], 16.0), d[k] > 0.0 ? 16.0 : 0.0), vl);
+        const double tk = __ddiv_rn(__dsub_rn(bnd, C[k]), d[k]);
+        te = tk < te ? tk : te;
+      }
+      t = __dadd_rn(te > t ? te : t, dt_half);
+      prev = false;
+      continue;
+    }
+    const int64_t at = (int64_t)slot * kVox + lv;
+    const float w = weight[at];
+    if (!((double)w >= wthr)) {                        // unknown voxel of an existing unit: one voxel on
+      t = __dadd_rn(t, dt_vox);
+      continue;
+    }
+    const float f = tsdf[at];
+    if (prev && fp > 0.f && f <= 0.f) {
+      t_hit = __dadd_rn(tp, __dmul_rn(__dsub_rn(t, tp), __ddiv_rn((double)fp, __dsub_rn((double)fp, (double)f))));
+      hit = t_hit >= dmin && t_hit <= dmax;
+      break;
+    }
+    prev = true;
+    fp = f;
+    tp = t;
+    const double step = __dmul_rn((double)f, trunc);
+    t = __dadd_rn(t, __ddiv_rn(step > vl ? step : vl, s));
+  }
+  const int64_t px = (int64_t)v * W + u;
+  depth[px] = hit ? __double2float_rn(t_hit) : 0.f;
+  if (intensity == nullptr && colour == nullptr) return;
+  float c32[3] = {0.f, 0.f, 0.f};
+  if (hit) {                                           // trilinear over the 8 voxels around p(t_hit) with weight > 0
+    double q[3], g0[3], fr[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      q[k] = __dsub_rn(__ddiv_rn(__dadd_rn(C[k], __dmul_rn(t_hit, d[k])), vl), 0.5);
+      g0[k] = floor(q[k]);
+      fr[k] = __dsub_rn(q[k], g0[k]);
+    }
+    double acc[3] = {0.0, 0.0, 0.0}, wsum = 0.0;
+    for (int c = 0; c < 8; ++c) {
+      const int o[3] = {c >> 2, (c >> 1) & 1, c & 1};
+      double g[3], U[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) g[k] = __dadd_rn(g0[k], (double)o[k]);
+      int lv = 0;
+      const int slot = ray_unit(g, keys, vals, mask, have_table, U, lv);
+      const int64_t at = (int64_t)slot * kVox + lv;
+      if (slot < 0 || !(weight[at] > 0.f)) continue;
+      const double tw = __dmul_rn(__dmul_rn(o[0] ? fr[0] : __dsub_rn(1.0, fr[0]), o[1] ? fr[1] : __dsub_rn(1.0, fr[1])),
+                                  o[2] ? fr[2] : __dsub_rn(1.0, fr[2]));
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+        acc[k] = __dadd_rn(acc[k], __dmul_rn(tw, (double)rgb[((int64_t)slot * 3 + k) * kVox + lv]));
+      wsum = __dadd_rn(wsum, tw);
+    }
+    if (wsum > 0.0) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) c32[k] = __double2float_rn(__ddiv_rn(acc[k], wsum));
+    }
+  }
+  if (intensity != nullptr)                            // create_from_color_and_depth's intensity, fp32
+    intensity[px] = __fdiv_rn(__fadd_rn(__fadd_rn(__fmul_rn(c32[0], 0.299f), __fmul_rn(c32[1], 0.587f)),
+                                        __fmul_rn(c32[2], 0.114f)), 255.f);
+  if (colour != nullptr) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) colour[3 * px + k] = __fdiv_rn(c32[k], 255.f);
+  }
+}
+
 struct TouchWs {
   dgr_keyspec_t* spec;
   int32_t *cand, *sel, *inverse, *n_unique, *slot_ws, *scan_ws, *flag, *blk, *sel_new, *tslot, *dvals;
@@ -702,6 +848,39 @@ int32_t dgr_tsdf_extract_write(const int32_t* unit_keys, int32_t n_units, const 
   write_vertices_kernel<<<n_units, kThreads, 0, st>>>(unit_keys, tsdf, rgb, voxel_length, w, vertices, colors);
   write_triangles_kernel<<<n_units, kThreads, 0, st>>>(w, triangles);
   dgr_note_launches(2);
+  DGR_LAUNCH_CHECK();
+  return DGR_OK;
+}
+
+int32_t dgr_tsdf_raycast(const uint64_t* table_keys, const int32_t* table_vals, int64_t table_cap, const float* tsdf,
+                         const float* weight, const float* rgb, int32_t width, int32_t height, const double* intr,
+                         const double* pose, double voxel_length, double sdf_trunc, int32_t res, double depth_min,
+                         double depth_max, double weight_threshold, float* depth, float* intensity, float* colour,
+                         void* stream) {
+  if (int32_t e = check_frame(width, height, intr, voxel_length, sdf_trunc, res)) return e;
+  DGR_ARG_CHECK(isfinite(intr[0]) && isfinite(intr[1]) && isfinite(intr[2]) && isfinite(intr[3]),
+                "the intrinsic must be finite");
+  DGR_ARG_CHECK(pose != nullptr && depth != nullptr, "null argument");
+  bool finite = true;
+  for (int i = 0; i < 12; ++i) finite = finite && isfinite(pose[i]);
+  DGR_ARG_CHECK(finite, "the camera pose must be finite");
+  DGR_ARG_CHECK(depth_min >= 0.0 && depth_min < depth_max && isfinite(depth_max), "need 0 <= depth_min < depth_max");
+  DGR_ARG_CHECK(weight_threshold > 0.0 && isfinite(weight_threshold), "weight_threshold must be positive");
+  DGR_ARG_CHECK(rgb != nullptr || table_cap == 0 || (intensity == nullptr && colour == nullptr),
+                "intensity and colour need a colour (RGB8) volume");
+  DGR_ARG_CHECK(table_cap == 0 || ((table_cap & (table_cap - 1)) == 0 && table_keys != nullptr &&
+                                   table_vals != nullptr && tsdf != nullptr && weight != nullptr),
+                "table capacity must be 0 (an empty volume) or a power of two with its table and slabs");
+  const double max_steps = raycast_max_steps(width, height, intr, pose, voxel_length, depth_max);
+  DGR_ARG_CHECK(max_steps <= (double)DGR_TSDF_RAYCAST_MAX_STEPS,
+                "a ray could take more than DGR_TSDF_RAYCAST_MAX_STEPS steps: ceil(2 s_max depth_max / voxel_length) + 1, "
+                "s_max the largest |R (a, b, 1)| over the image's corner pixels");
+  const dim3 block(kRayBx, kRayBy), grid((width + kRayBx - 1) / kRayBx, (height + kRayBy - 1) / kRayBy);
+  raycast_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(
+      table_keys, table_vals, (uint64_t)(table_cap > 0 ? table_cap - 1 : 0), table_cap > 0, tsdf, weight, rgb, width,
+      height, make_cam(intr, pose), voxel_length, sdf_trunc, depth_min, depth_max, weight_threshold, (int)max_steps, depth,
+      intensity, colour);
+  dgr_note_launches(1);
   DGR_LAUNCH_CHECK();
   return DGR_OK;
 }

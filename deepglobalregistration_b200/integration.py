@@ -15,7 +15,13 @@ into the node poses) and between keyframes every ``--keyframe_every`` frames (un
 odometry succeeds), then the pose graph's global optimisation - and the fragment's trajectory is written beside its
 mesh as ``fragment-<k>.log``.  The mesh is then in the frame of the fragment's first camera.  open3d starts a loop
 closure from OpenCV's 5-point ORB pose (and skips it without OpenCV); here it starts from the odometry chain's relative
-pose."""
+pose.
+
+With ``--poses model`` (a project extension) each frame is instead tracked against the model fused so far, as
+KinectFusion and open3d's dense SLAM do: the fragment's volume is ray-cast at the previous pose and the frame is
+registered to that rendering by RGB-D odometry, then fused (track_model).  There is no pose graph, so
+``--frames_per_fragment`` is not capped; the mesh and ``fragment-<k>.log`` come from the tracker's own volume, and
+the summary reports ``tracked_frames`` and ``tracking_failures``."""
 import argparse
 import json
 import os
@@ -115,6 +121,54 @@ def odometry_poses(seq_path, frames, intrinsic, start, end, keyframe_every=5):
                                                         loop_closures=n_loops, loop_closures_kept=kept)
 
 
+def track_model(images, intrinsic, voxel_length=0.008, sdf_trunc=0.04, max_depth=4.5):
+  """Frame-to-model tracking, as open3d's dense SLAM (t.pipelines.slam.Model) tracks: frame 0 is fused at the
+  identity; every later frame k is registered by RGB-D odometry (hybrid Jacobian, ODOMETRY_OPTION, from the identity)
+  against the model ray-cast at P_{k-1} with weight_threshold min(k, 3) over [min_depth, max_depth] of the option,
+  posed P_k = P_{k-1} T and fused at P_k.  A failed odometry keeps P_k = P_{k-1} and the frame is not fused.
+  images: (colour [H, W, 3] uint8, depth [H, W] uint16 mm) per frame.  One result read per tracked frame, besides the
+  integration's own.  -> (poses [n, 4, 4] (frame k -> the first camera), the RGB8 volume, stats dict)."""
+  option = odo.OdometryOption(**ODOMETRY_OPTION)
+  volume = integ.ScalableTSDFVolume(voxel_length=voxel_length, sdf_trunc=sdf_trunc,
+                                    color_type=integ.TSDFVolumeColorType.RGB8)
+  dev = volume.device
+  intr = intrinsic._params()
+  its = option.iteration_number_per_pyramid_level
+  poses, failures = [], 0
+  for k, (color, depth) in enumerate(images):
+    fuse = integ.RGBDImage.create_from_color_and_depth(color, depth, depth_trunc=max_depth,
+                                                       convert_rgb_to_intensity=False)
+    if k == 0:
+      poses.append(np.eye(4))
+      volume.integrate(fuse, intrinsic, np.eye(4))
+      continue
+    src = integ.RGBDImage.create_from_color_and_depth(color, depth, depth_trunc=option.max_depth,
+                                                      convert_rgb_to_intensity=True)
+    Is, Ds = (torch.from_numpy(np.ascontiguousarray(np.asarray(a))).to(dev) for a in (src.color, src.depth))
+    P = poses[-1]
+    model = volume.raycast_tensors(intrinsic, np.linalg.inv(P), option.min_depth, option.max_depth,
+                                   float(min(k, 3)), outputs=('depth', 'intensity'))
+    r = _abi.rgbd_odometry(Is, Ds, model['intensity'], model['depth'], intr, np.eye(4), 'hybrid', its,
+                           option.max_depth_diff, option.min_depth, option.max_depth)
+    ok, T, _ = odo.unpack_result(r.cpu().numpy())
+    if not ok:
+      failures += 1
+      poses.append(P)
+      continue
+    poses.append(P @ T)
+    volume.integrate(fuse, intrinsic, np.linalg.inv(poses[-1]))
+  n = len(poses)
+  return np.stack(poses), volume, dict(tracked_frames=max(n - 1, 0) - failures, tracking_failures=failures)
+
+
+def model_poses(seq_path, frames, intrinsic, start, end, voxel_length=0.008, sdf_trunc=0.04, max_depth=4.5):
+  """track_model over frames [start, end) of a sequence: -> (poses [n, 4, 4], volume, stats)."""
+  color, depth = frames[0], frames[1]
+  images = ((dio.read_image(os.path.join(seq_path, color[i])), dio.read_image(os.path.join(seq_path, depth[i])))
+            for i in range(start, end))
+  return track_model(images, intrinsic, voxel_length, sdf_trunc, max_depth)
+
+
 def integrate_fragment(seq_path, frames, intrinsic, start, end, voxel_length=0.008, sdf_trunc=0.04, max_depth=4.5,
                        poses=None):
   """Mesh of frames [start, end) of a sequence (util/integration.py:44-71); poses: camera-to-world poses of the
@@ -140,8 +194,9 @@ def main(argv=None):
   ap.add_argument('--sdf_trunc', type=float, default=0.04)
   ap.add_argument('--max_depth', type=float, default=4.5)
   ap.add_argument('--overwrite', action='store_true', help='write into an existing OUTPUT/<scene>')
-  ap.add_argument('--poses', choices=('file', 'odometry'), default='file',
-                  help='frame poses: the .pose.txt files, or RGB-D odometry and a pose graph per fragment')
+  ap.add_argument('--poses', choices=('file', 'odometry', 'model'), default='file',
+                  help='frame poses: the .pose.txt files, RGB-D odometry and a pose graph per fragment, or each frame '
+                       'tracked against the fragment\'s fused model')
   ap.add_argument('--keyframe_every', type=int, default=5, help='--poses odometry: loop closures between keyframes')
   args = ap.parse_args(argv)
   if args.frames_per_fragment < 1:
@@ -162,7 +217,7 @@ def main(argv=None):
     return 2
   t0 = time.time()
   written, n_frames, n_vertices, n_triangles = [], 0, 0, 0
-  odo_stats = dict(odometry_pairs=0, loop_closures_kept=0, ate=[])
+  odo_stats = dict(odometry_pairs=0, loop_closures_kept=0, tracked_frames=0, tracking_failures=0, ate=[])
   for seq in seqs:
     seq_path = os.path.join(args.dataset, seq)
     frames = sequence_frames(seq_path, need_poses=args.poses == 'file')
@@ -173,19 +228,28 @@ def main(argv=None):
     n = len(frames[0])
     for k in range((n + args.frames_per_fragment - 1) // args.frames_per_fragment):
       start, end = k * args.frames_per_fragment, min((k + 1) * args.frames_per_fragment, n)
-      poses = None
+      poses, volume = None, None
       if args.poses == 'odometry':
         poses, st = odometry_poses(seq_path, frames, intrinsic, start, end, args.keyframe_every)
-        dio.write_trajectory(os.path.join(out_seq, f'fragment-{k}.log'),
-                            [((i, i, len(poses)), P) for i, P in enumerate(poses)])
         odo_stats['odometry_pairs'] += st['odometry_pairs']
         odo_stats['loop_closures_kept'] += st['loop_closures_kept']
+      elif args.poses == 'model':                       # the tracker's own volume gives the mesh
+        poses, volume, st = model_poses(seq_path, frames, intrinsic, start, end, args.voxel_length, args.sdf_trunc,
+                                        args.max_depth)
+        odo_stats['tracked_frames'] += st['tracked_frames']
+        odo_stats['tracking_failures'] += st['tracking_failures']
+      if poses is not None:
+        dio.write_trajectory(os.path.join(out_seq, f'fragment-{k}.log'),
+                            [((i, i, len(poses)), P) for i, P in enumerate(poses)])
         if frames[2] is not None:                       # ATE against the first frame's frame of the files
           gt = np.stack([np.loadtxt(os.path.join(seq_path, frames[2][i])) for i in range(start, end)])
           gt = np.linalg.inv(gt[0]) @ gt
           odo_stats['ate'].append(float(absolute_trajectory_error(poses, gt)))
-      mesh, _ = integrate_fragment(seq_path, frames, intrinsic, start, end, args.voxel_length, args.sdf_trunc,
-                                   args.max_depth, poses)
+      if volume is not None:
+        mesh = volume.extract_triangle_mesh()
+      else:
+        mesh, _ = integrate_fragment(seq_path, frames, intrinsic, start, end, args.voxel_length, args.sdf_trunc,
+                                     args.max_depth, poses)
       path = os.path.join(out_seq, f'fragment-{k}.ply')
       dio.write_triangle_mesh(path, mesh)
       written.append(path)
@@ -197,8 +261,10 @@ def main(argv=None):
              'output': out_scene}
   if args.poses == 'odometry':
     summary.update(odometry_pairs=odo_stats['odometry_pairs'], loop_closures_kept=odo_stats['loop_closures_kept'])
-    if odo_stats['ate']:
-      summary['fragment_ate'] = odo_stats['ate']
+  elif args.poses == 'model':
+    summary.update(tracked_frames=odo_stats['tracked_frames'], tracking_failures=odo_stats['tracking_failures'])
+  if odo_stats['ate']:
+    summary['fragment_ate'] = odo_stats['ate']
   print(json.dumps(summary))
   return 0
 

@@ -40,6 +40,20 @@ class PinholeCameraIntrinsic:
     return f'PinholeCameraIntrinsic with width = {self.width} and height = {self.height}.'
 
 
+def _raycast_max_steps(W, H, intr, pose, voxel_length, depth_max):
+  """dgr_tsdf_raycast's step bound, ceil(((2 s_max) depth_max) / voxel_length) + 1: s = |R (a, b, 1)| is the ray's
+  world length per unit of t, convex in (a, b), so its largest value s_max is at a corner pixel."""
+  fx, fy, cx, cy = intr
+  s_max = 0.0
+  for c in range(4):
+    a = (float(W - 1 if c & 1 else 0) - cx) / fx
+    b = (float(H - 1 if c & 2 else 0) - cy) / fy
+    d = [(pose[r, 0] * a + pose[r, 1] * b) + pose[r, 2] for r in range(3)]
+    s = float(np.sqrt((d[0] * d[0] + d[1] * d[1]) + d[2] * d[2]))
+    s_max = s if s > s_max else s_max
+  return float(np.ceil(((2.0 * s_max) * depth_max) / voxel_length) + 1.0)
+
+
 class RGBDImage:
   def __init__(self, color=None, depth=None):
     self.color = color if color is not None else Image()
@@ -186,6 +200,74 @@ class ScalableTSDFVolume:
                              torch.full((1,), -1, dtype=torch.int64, device=self.device), self._vals if
                              self._vals.numel() else torch.zeros(1, dtype=torch.int32, device=self.device),
                              self._tsdf, self._weight, self._rgb, self.voxel_length)
+
+  def raycast(self, intrinsic, extrinsic, depth_min=0.1, depth_max=3.0, weight_threshold=3.0,
+              convert_rgb_to_intensity=True):
+    """Render the volume seen by `intrinsic` from `extrinsic` (4x4 world to camera) - a project extension; legacy
+    open3d has no ray cast, and the defaults follow open3d's VoxelBlockGrid.ray_cast.  -> RGBDImage of float32 depth
+    in metres (0 where the ray meets no surface) and float32 colour: the intensity, or RGB in [0, 1] with
+    convert_rgb_to_intensity=False.  A NoColor volume renders depth only (its colour image is empty).  One host read:
+    the outputs share one device buffer, copied once."""
+    want = 'intensity' if convert_rgb_to_intensity else 'colour'
+    flat, out = self._raycast(intrinsic, extrinsic, depth_min, depth_max, weight_threshold,
+                              ('depth', want) if self._color else ('depth',))
+    host = flat.cpu().numpy()
+    H, W = out['depth'].shape
+    depth = host[:H * W].reshape(H, W)
+    color = Image(host[H * W:].reshape(out[want].shape)) if self._color else Image()
+    return RGBDImage(color, Image(depth))
+
+  def raycast_tensors(self, intrinsic, extrinsic, depth_min=0.1, depth_max=3.0, weight_threshold=3.0,
+                      outputs=('depth', 'intensity', 'colour')):
+    """raycast() on the device, without a host read: -> {name: CUDA float32 tensor} for the requested outputs of
+    'depth' [H, W], 'intensity' [H, W] and 'colour' [H, W, 3] (the last two RGB8 volumes only), views of one buffer
+    in that order.  One launch."""
+    return self._raycast(intrinsic, extrinsic, depth_min, depth_max, weight_threshold, tuple(outputs))[1]
+
+  def _raycast(self, intrinsic, extrinsic, depth_min, depth_max, weight_threshold, outputs):
+    """Check every argument, then launch dgr_tsdf_raycast -> (the flat device buffer, {name: view of it})."""
+    if 'depth' not in outputs or any(o not in ('depth', 'intensity', 'colour') for o in outputs):
+      raise ValueError(f"outputs must include 'depth' and name only depth / intensity / colour, got {outputs}")
+    if not self._color and len(outputs) > 1:
+      raise ValueError('a NoColor volume renders depth only')
+    W, H = intrinsic.width, intrinsic.height
+    if W < 1 or H < 1:
+      raise ValueError(f'image size must be positive, got {W} x {H}')
+    intr = intrinsic._params()
+    if not (intr[0] > 0 and intr[1] > 0 and np.isfinite(intr).all()):
+      raise ValueError('focal lengths must be finite and positive, the principal point finite')
+    ext = np.asarray(extrinsic, dtype=np.float64)
+    if ext.shape != (4, 4) or not np.isfinite(ext).all():
+      raise ValueError(f'extrinsic must be a finite 4x4 matrix, got shape {ext.shape}')
+    try:
+      pose = np.linalg.inv(ext)
+    except np.linalg.LinAlgError:
+      raise ValueError('extrinsic must be invertible') from None
+    if not np.isfinite(pose).all():
+      raise ValueError('extrinsic must be invertible')
+    if not (0.0 <= depth_min < depth_max < np.inf):
+      raise ValueError(f'need 0 <= depth_min < depth_max < inf, got {depth_min}, {depth_max}')
+    if not 0.0 < weight_threshold < np.inf:
+      raise ValueError(f'weight_threshold must be finite and positive, got {weight_threshold}')
+    steps = _raycast_max_steps(W, H, intr, pose, self.voxel_length, depth_max)
+    if not steps <= _abi.TSDF_RAYCAST_MAX_STEPS:
+      raise ValueError(f'a ray could take {steps:g} steps, more than {_abi.TSDF_RAYCAST_MAX_STEPS}: the focal '
+                       'length, principal point, extrinsic scale, depth_max or voxel_length is out of range')
+    _abi.refresh_stream()
+    self._grow_slabs(self.n_units)
+    sizes = {'depth': (H, W), 'intensity': (H, W), 'colour': (H, W, 3)}
+    names = [o for o in ('depth', 'intensity', 'colour') if o in outputs]
+    flat = torch.empty(sum(int(np.prod(sizes[o])) for o in names), dtype=torch.float32, device=self.device)
+    out, at = {}, 0
+    for o in names:
+      n = int(np.prod(sizes[o]))
+      out[o] = flat[at:at + n].view(sizes[o])
+      at += n
+    empty = self.n_units == 0
+    _abi.tsdf_raycast(None if empty else self._keys, None if empty else self._vals, self._tsdf, self._weight,
+                      self._rgb, W, H, intr, pose, self.voxel_length, self.sdf_trunc, depth_min, depth_max,
+                      weight_threshold, out['depth'], out.get('intensity'), out.get('colour'))
+    return flat, out
 
   def extract_point_cloud(self):
     raise NotImplementedError('ScalableTSDFVolume.extract_point_cloud is not implemented')

@@ -435,6 +435,23 @@ int32_t dgr_tsdf_extract_count(const int32_t* unit_keys, int32_t n_units, const 
 int32_t dgr_tsdf_extract_write(const int32_t* unit_keys, int32_t n_units, const float* tsdf, const float* rgb,
                                double voxel_length, const void* ws, double* vertices, double* colors,
                                int32_t* triangles, void* stream);
+/* Ray cast one pinhole camera through the volume (a project extension: legacy open3d has none;
+ * oracle/tsdf_raycast.py is the contract, met bit for bit).  pose: HOST double[12], rows 0..2 of camera_pose =
+ * inv(extrinsic), finite.  Pixel (u, v) marches p(t) = C + t R ((u - cx) / fx, (v - cy) / fy, 1) from t = depth_min
+ * (0 <= depth_min < depth_max); a sample is known when its voxel's unit exists and its weight is >= weight_threshold
+ * (> 0).  Every step advances t by at least (0.5 voxel_length) / s, s = |R (a, b, 1)| the ray's world length per unit
+ * of t, so a ray takes at most ceil(2 s_max depth_max / voxel_length) + 1 steps, s_max the largest s over the image's
+ * four corner pixels; arguments whose bound passes DGR_TSDF_RAYCAST_MAX_STEPS are refused, and the kernel stops every
+ * ray at the bound.  Writes depth [height][width] fp32 (t of the first known + to - crossing, 0 where none) and, for
+ * RGB8 volumes only (rgb non-NULL), intensity [height][width] and / or colour [height][width][3] in [0, 1] (either may
+ * be NULL; 0 where no hit).  table_cap 0 is an empty volume: table and slabs may be NULL, and every output is 0.  One
+ * launch, no workspace, no atomics, no host read. */
+#define DGR_TSDF_RAYCAST_MAX_STEPS 65536
+int32_t dgr_tsdf_raycast(const uint64_t* table_keys, const int32_t* table_vals, int64_t table_cap, const float* tsdf,
+                         const float* weight, const float* rgb, int32_t width, int32_t height, const double* intr,
+                         const double* pose, double voxel_length, double sdf_trunc, int32_t res, double depth_min,
+                         double depth_max, double weight_threshold, float* depth, float* intensity, float* colour,
+                         void* stream);
 /* Host copy of the marching-cubes tables: edge_table[256] (bit e: edge e changes sign), tri_table[256][16] (-1 pad). */
 int32_t dgr_tsdf_mc_tables(int32_t* edge_table, int32_t* tri_table);
 
