@@ -382,10 +382,27 @@ class KernelMap:
     return t
 
 
-def kernel_map(out_coords, spec, in_table, n_in, offsets, keep_table=False):
+KMAP_GENERAL, KMAP_SAME, KMAP_DOWN = (_DEFINES['DGR_KMAP_GENERAL'], _DEFINES['DGR_KMAP_SAME'],
+                                     _DEFINES['DGR_KMAP_DOWN'])
+
+
+def kmap_mode(s_in, s_out, kernel_size):
+  """Probe mode of dgr_kmap_probe_mode for the map of a convolution from tensor stride s_in to s_out with the
+  centred cube of kernel_offsets: same-stride maps mirror half their offsets, kernel-3 down maps are enumerated
+  from their input rows."""
+  if s_out == s_in and kernel_size % 2 == 1 and kernel_size > 1:
+    return KMAP_SAME
+  if s_out == 2 * s_in and kernel_size == 3:
+    return KMAP_DOWN
+  return KMAP_GENERAL
+
+
+def kernel_map(out_coords, spec, in_table, n_in, offsets, keep_table=False, mode=KMAP_GENERAL, in_coords=None,
+               in_stride=0, out_table=None):
   """offsets: CUDA int32 [K, D] (scaled by the input tensor stride).  Occupancy bits + bucket offsets (and the
   dense neighbour table when kept), then ONE host read of the bucket offsets sizes the pair lists and the work
-  list."""
+  list.  mode (kmap_mode): KMAP_SAME needs in_table to be the table of out_coords; KMAP_DOWN reads the input
+  rows in_coords at tensor stride in_stride and the table out_table of out_coords."""
   global D2H_BYTES
   _chk(out_coords, torch.int32, 'out_coords')
   _chk(offsets, torch.int32, 'offsets')
@@ -399,12 +416,15 @@ def kernel_map(out_coords, spec, in_table, n_in, offsets, keep_table=False):
   meta = scratch('km_meta', 5, torch.int32, dev)          # written by the probe, read by nobody here
   # the miss filter pays off when most probes miss: many offsets per row (6-D, 5^3, 7^3 kernels)
   bloom, n_words = None, 0
-  if K > 27:
+  if K > 27 and mode != KMAP_DOWN:
     n_words = lib().dgr_bloom2_words(n_in)
     bloom = scratch('km_bloom', n_words, torch.int32, dev)
     call('dgr_bloom2_build', ptr(in_table.keys), in_table.cap, ptr(bloom), n_words, stream())
   table = (ptr(in_table.keys), ptr(in_table.vals), in_table.cap)
-  call('dgr_kmap_probe', ptr(out_coords), n_out, None, ncols, ptr(spec), *table, ptr(bloom), n_words, ptr(offsets), K,
+  down = mode == KMAP_DOWN
+  call('dgr_kmap_probe_mode', mode, ptr(out_coords), n_out, None, ncols, ptr(spec), *table, ptr(bloom), n_words,
+       ptr(offsets), K, ptr(in_coords) if down else None, n_in if down else 0, None, in_stride if down else 0,
+       ptr(out_table.keys) if down else None, ptr(out_table.vals) if down else None, out_table.cap if down else 0,
        ptr(bits), ptr(cnt), ptr(kofs), ptr(meta), stream())
   km = KernelMap()
   km.nbr = None

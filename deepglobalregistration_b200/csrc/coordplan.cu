@@ -107,14 +107,19 @@ __global__ void bloom2_build_kernel(const uint64_t* __restrict__ keys, int64_t c
 // passes the filter (a 3 % pass rate per lane is 62 % per warp) with one or two lanes doing useful work.
 // Output: kDense ? nbr[kappa * nbr_stride + j] = input row or -1
 //                : bits[kappa * W + w] = ballot of warp w's rows (+ per-(kappa, 256-word block) counts)
-template <bool kBloom, bool kDense>
+// kSym (a same-stride map: the input table is the output table, the offsets a centred odd cube, so offset
+// k_last - kappa is the negation of offset kappa): only the buckets kappa < k_last / 2 are probed (K of them).
+// A hit j -> i of bucket kappa is also the pair i -> j of the mirror bucket k_last - kappa: bit i of that bucket
+// is set with a global atomicOr (its words zeroed by the caller).  The centre bucket k_last / 2 (offset 0) holds
+// every live row and is written from the row count without a probe.  kmap_count_kernel counts both afterwards.
+template <bool kBloom, bool kDense, bool kSym>
 __global__ void __launch_bounds__(kProbeThreads, 2)
 kmap_probe_kernel(const int32_t* __restrict__ out_coords, const int32_t* __restrict__ n_out_dev, int64_t n_out_max,
                   int ncols, const dgr_keyspec_t* __restrict__ spec_p, const uint64_t* __restrict__ keys,
                   const int32_t* __restrict__ vals, uint64_t mask, const uint32_t* __restrict__ bloom,
                   uint32_t n_bloom_words, const int32_t* __restrict__ offsets, int K, int k_per_block,
                   uint32_t* __restrict__ bits, int W, int32_t* block_cnt, int bpk, int32_t* __restrict__ nbr,
-                  int64_t nbr_stride, int32_t* hit_count) {
+                  int64_t nbr_stride, int32_t* hit_count, int k_last) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   constexpr int kWarps = kProbeThreads / 32;
   long long* delta = reinterpret_cast<long long*>(smem_raw);                               // [k_per_block]
@@ -155,6 +160,13 @@ kmap_probe_kernel(const int32_t* __restrict__ out_coords, const int32_t* __restr
   uint16_t* q = queue + warp * 64;
   uint32_t* mt = mtile + warp * k_per_block;
   int qn = 0;                                          // queued candidates (warp-uniform)
+  auto mirror = [&](int kappa, int32_t i) {            // kSym: hit (kappa, in i, out j) is the pair (k_last - kappa, in j, out i)
+    atomicOr(bits + (int64_t)(k_last - kappa) * W + (i >> 5), 1u << (i & 31));
+  };
+  if (kSym && blockIdx.y == 0) {                       // centre bucket: the identity pair of every live row
+    const uint32_t m = __ballot_sync(0xffffffffu, live);
+    if (lane == 0 && (j >> 5) < W) bits[(int64_t)(k_last / 2) * W + (j >> 5)] = m;
+  }
 
   auto drain = [&](int count) {                        // lanes < count take one candidate each
     __syncwarp();
@@ -173,6 +185,7 @@ kmap_probe_kernel(const int32_t* __restrict__ out_coords, const int32_t* __restr
         }
       } else if (i >= 0) {
         atomicOr(mt + kq, 1u << src);
+        if (kSym) mirror(k0 + kq, i);
       }
     }
     __syncwarp();
@@ -189,14 +202,15 @@ kmap_probe_kernel(const int32_t* __restrict__ out_coords, const int32_t* __restr
     const int w = (int)(j >> 5);
     const int cnt_col = w / kCntWords;
     for (int kk = 0; kk < kn; kk += 4) {
-      bool found[4];
+      int32_t found[4];
 #pragma unroll
       for (int u = 0; u < 4; ++u)
-        found[u] = live && kk + u < kn && dgr_hash_lookup(keys, vals, mask, key + (uint64_t)delta[min(kk + u, kn - 1)]) >= 0;
+        found[u] = live && kk + u < kn ? dgr_hash_lookup(keys, vals, mask, key + (uint64_t)delta[min(kk + u, kn - 1)]) : -1;
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
         if (kk + u >= kn) break;                                     // uniform
-        const uint32_t m = __ballot_sync(0xffffffffu, found[u]);
+        if (kSym && found[u] >= 0) mirror(k0 + kk + u, found[u]);
+        const uint32_t m = __ballot_sync(0xffffffffu, found[u] >= 0);
         if (lane == 0 && w < W) {
           bits[(int64_t)(k0 + kk + u) * W + w] = m;
           if (m) atomicAdd(block_cnt + (int64_t)(k0 + kk + u) * bpk + cnt_col, __popc(m));
@@ -233,6 +247,63 @@ kmap_probe_kernel(const int32_t* __restrict__ out_coords, const int32_t* __restr
       }
     }
   }
+}
+
+// Down map (kernel 3, input tensor stride s, output stride 2s) enumerated from the input side.
+// Output rows are multiples of 2s and input rows multiples of s, so input row c reaches output o = c - offset
+// only where, on every spatial axis, o = c if c / s is even and o = c -/+ s (offset +s / -s) if it is odd:
+// 2^(odd axes) candidates per input row (one of them, the floor parent, always exists), each looked up in the
+// OUTPUT table.  kDownLanes lanes share a row and take its candidates in turn, so a row with every axis odd
+// (64 candidates in 6-D) is not one thread's chain of 64 dependent L2 round trips.  A hit sets bit o of bucket
+// kappa with atomicOr (words zeroed by the caller): the masks equal those of probing all 3^D offsets per output
+// row.  Offsets are enumerated axis 0 fastest, digit 0 / 1 / 2 = offset -s / 0 / +s.
+constexpr int kDownLanes = 8;
+__global__ void __launch_bounds__(kThreads)
+kmap_down_kernel(const int32_t* __restrict__ in_coords, const int32_t* __restrict__ n_in_dev, int64_t n_in_max,
+                 int ncols, int stride, const dgr_keyspec_t* __restrict__ spec_p, const uint64_t* __restrict__ out_keys,
+                 const int32_t* __restrict__ out_vals, uint64_t out_mask, uint32_t* __restrict__ bits, int W) {
+  const int n_in = dgr_dev_count(n_in_dev, n_in_max);
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t i = t / kDownLanes;
+  if (i >= n_in) return;
+  const dgr_keyspec_t s = *spec_p;
+  const int32_t* c = in_coords + i * ncols;
+  const uint64_t key = dgr_pack_key(c, s);
+  uint32_t odd = 0;
+#pragma unroll
+  for (int a = 1; a < DGR_MAX_COLS; ++a)
+    if (a < ncols) odd |= (uint32_t)((c[a] / stride) & 1) << a;   // exact division; & 1 is floor parity for c < 0 too
+  const uint32_t n_cand = 1u << __popc(odd);
+  for (uint32_t sub = (uint32_t)(t % kDownLanes); sub < n_cand; sub += kDownLanes) {
+    int kappa = 0, p = 1, b = 0;
+    long long d = 0;
+#pragma unroll
+    for (int a = 1; a < DGR_MAX_COLS; ++a) {
+      if (a < ncols) {
+        int digit = 1;
+        if ((odd >> a) & 1u) {
+          const long long step = (long long)stride << s.shift[a];
+          if ((sub >> b++) & 1u) { digit = 2; d -= step; }      // offset +s: o = c - s
+          else { digit = 0; d += step; }                        // offset -s: o = c + s
+        }
+        kappa += digit * p;
+        p *= 3;
+      }
+    }
+    const int32_t o = dgr_hash_lookup(out_keys, out_vals, out_mask, key + (uint64_t)d);
+    if (o >= 0) atomicOr(bits + (int64_t)kappa * W + (o >> 5), 1u << (o & 31));
+  }
+}
+
+// Per-(kappa, 256-word block) pair counts of the buckets k_lo + blockIdx.y from their finished masks (the buckets
+// the down and mirror paths set with atomicOr); grid (bpk, buckets).
+__global__ void __launch_bounds__(kThreads)
+kmap_count_kernel(const uint32_t* __restrict__ bits, int W, int bpk, int k_lo, int32_t* __restrict__ block_cnt) {
+  const int64_t kappa = k_lo + blockIdx.y;
+  const int w = blockIdx.x * kCntWords + threadIdx.x;
+  int total;
+  dgr_block_exclusive_scan<kThreads>(w < W ? __popc(bits[kappa * W + w]) : 0, &total);
+  if (threadIdx.x == 0) block_cnt[kappa * bpk + blockIdx.x] = total;
 }
 
 // exclusive scan of the K x bpk block counts (one block), bucket offsets, work-list sizes
@@ -415,39 +486,79 @@ static int probe_k_per_block(int K, unsigned row_blocks) {
   return (k_per_block + 3) & ~3;
 }
 
-int32_t dgr_kmap_probe(const int32_t* out_coords, int64_t n_out_max, const int32_t* n_out_dev, int32_t ncols,
-                       const dgr_keyspec_t* spec, const uint64_t* in_keys, const int32_t* in_vals, int64_t in_cap,
-                       const uint32_t* bloom_words, int64_t n_bloom_words, const int32_t* offsets, int32_t K,
-                       uint32_t* bits, int32_t* block_cnt, int32_t* kofs, int32_t* meta, void* stream) {
+int32_t dgr_kmap_probe_mode(int32_t mode, const int32_t* out_coords, int64_t n_out_max, const int32_t* n_out_dev,
+                            int32_t ncols, const dgr_keyspec_t* spec, const uint64_t* in_keys, const int32_t* in_vals,
+                            int64_t in_cap, const uint32_t* bloom_words, int64_t n_bloom_words, const int32_t* offsets,
+                            int32_t K, const int32_t* in_coords, int64_t n_in_max, const int32_t* n_in_dev,
+                            int32_t in_stride, const uint64_t* out_keys, const int32_t* out_vals, int64_t out_cap,
+                            uint32_t* bits, int32_t* block_cnt, int32_t* kofs, int32_t* meta, void* stream) {
+  DGR_ARG_CHECK(mode == DGR_KMAP_GENERAL || mode == DGR_KMAP_SAME || mode == DGR_KMAP_DOWN, "unknown probe mode");
   DGR_ARG_CHECK(in_cap > 0 && (in_cap & (in_cap - 1)) == 0, "capacity must be a power of two");
   DGR_ARG_CHECK(K >= 1 && K <= 65535, "K out of range");
   DGR_ARG_CHECK(bloom_words == nullptr || (n_bloom_words >= 32 && (n_bloom_words & (n_bloom_words - 1)) == 0 &&
                                            n_bloom_words <= 32768),
                 "bloom: power of two, 32..32768 words");
+  DGR_ARG_CHECK(mode != DGR_KMAP_SAME || (K > 1 && (K & 1)), "same-stride mode: a centred odd cube of offsets");
+  if (mode == DGR_KMAP_DOWN) {
+    int64_t k3 = 1;
+    for (int a = 1; a < ncols; ++a) k3 *= 3;
+    DGR_ARG_CHECK(K == k3, "down mode: kernel size 3");
+    DGR_ARG_CHECK(in_coords != nullptr && in_stride >= 1 && n_in_max >= 0, "down mode: input rows and stride");
+    DGR_ARG_CHECK(out_keys != nullptr && out_vals != nullptr && out_cap > 0 && (out_cap & (out_cap - 1)) == 0,
+                  "down mode: output table, capacity a power of two");
+  }
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t nmx = n_out_max > 0 ? n_out_max : 1;
   const int W = (int)dgr_kmap_mask_words(nmx);
   const int bpk = (W + kCntWords - 1) / kCntWords;
   DGR_CUDA_CHECK(cudaMemsetAsync(block_cnt, 0, (size_t)dgr_kmap_cnt_elems(K, nmx) * sizeof(int32_t), st));
-  const unsigned row_blocks = dgr_blocks(nmx, kProbeThreads);
-  const int k_per_block = probe_k_per_block(K, row_blocks);
-  const dim3 grid(row_blocks, (K + k_per_block - 1) / k_per_block);
-  if (bloom_words != nullptr) {
-    const size_t smem = probe_smem_bytes(k_per_block, n_bloom_words);
-    DGR_ENSURE_SMEM((kmap_probe_kernel<true, false>), smem);
-    kmap_probe_kernel<true, false><<<grid, kProbeThreads, smem, st>>>(
-        out_coords, n_out_dev, n_out_max, ncols, spec, in_keys, in_vals, (uint64_t)in_cap - 1, bloom_words,
-        (uint32_t)n_bloom_words, offsets, K, k_per_block, bits, W, block_cnt, bpk, nullptr, 0, nullptr);
+  int k_counted = K;                                   // buckets [k_counted, K) are counted from their masks
+  if (mode == DGR_KMAP_DOWN) {
+    DGR_CUDA_CHECK(cudaMemsetAsync(bits, 0, (size_t)K * W * sizeof(uint32_t), st));
+    if (n_in_max > 0)
+      kmap_down_kernel<<<dgr_blocks(n_in_max * kDownLanes, kThreads), kThreads, 0, st>>>(
+          in_coords, n_in_dev, n_in_max, ncols, in_stride, spec, out_keys, out_vals, (uint64_t)out_cap - 1, bits, W);
+    k_counted = 0;
   } else {
-    const size_t smem = probe_smem_bytes(k_per_block, 0);
-    kmap_probe_kernel<false, false><<<grid, kProbeThreads, smem, st>>>(
-        out_coords, n_out_dev, n_out_max, ncols, spec, in_keys, in_vals, (uint64_t)in_cap - 1, nullptr, 1u, offsets, K,
-        k_per_block, bits, W, block_cnt, bpk, nullptr, 0, nullptr);
+    // same-stride mode: probe the buckets below the centre, the rest are mirrored (and set with atomicOr)
+    const bool sym = mode == DGR_KMAP_SAME;
+    const int Kp = sym ? (K - 1) / 2 : K;
+    if (sym) DGR_CUDA_CHECK(cudaMemsetAsync(bits + (int64_t)Kp * W, 0, (size_t)(K - Kp) * W * sizeof(uint32_t), st));
+    k_counted = Kp;
+    const unsigned row_blocks = dgr_blocks(nmx, kProbeThreads);
+    const int k_per_block = probe_k_per_block(Kp, row_blocks);
+    const dim3 grid(row_blocks, (Kp + k_per_block - 1) / k_per_block);
+    const uint32_t* bw = bloom_words;
+    const uint32_t nbw = bloom_words != nullptr ? (uint32_t)n_bloom_words : 1u;
+    const size_t smem = probe_smem_bytes(k_per_block, bloom_words != nullptr ? n_bloom_words : 0);
+#define DGR_PROBE(B, S)                                                                                             \
+  do {                                                                                                              \
+    DGR_ENSURE_SMEM((kmap_probe_kernel<B, false, S>), smem);                                                       \
+    kmap_probe_kernel<B, false, S><<<grid, kProbeThreads, smem, st>>>(                                              \
+        out_coords, n_out_dev, n_out_max, ncols, spec, in_keys, in_vals, (uint64_t)in_cap - 1, bw, nbw, offsets, Kp, \
+        k_per_block, bits, W, block_cnt, bpk, nullptr, 0, nullptr, K - 1);                                          \
+  } while (0)
+    if (bloom_words != nullptr) {
+      if (sym) DGR_PROBE(true, true); else DGR_PROBE(true, false);
+    } else {
+      if (sym) DGR_PROBE(false, true); else DGR_PROBE(false, false);
+    }
+#undef DGR_PROBE
   }
+  if (k_counted < K) kmap_count_kernel<<<dim3(bpk, K - k_counted), kThreads, 0, st>>>(bits, W, bpk, k_counted, block_cnt);
   kmap_scan_kernel<<<1, 1024, 0, st>>>(block_cnt, K, bpk, 128, kofs, meta, spec);
-  dgr_note_launches(2);
+  dgr_note_launches(k_counted < K ? 3 : 2);
   DGR_LAUNCH_CHECK();
   return DGR_OK;
+}
+
+int32_t dgr_kmap_probe(const int32_t* out_coords, int64_t n_out_max, const int32_t* n_out_dev, int32_t ncols,
+                       const dgr_keyspec_t* spec, const uint64_t* in_keys, const int32_t* in_vals, int64_t in_cap,
+                       const uint32_t* bloom_words, int64_t n_bloom_words, const int32_t* offsets, int32_t K,
+                       uint32_t* bits, int32_t* block_cnt, int32_t* kofs, int32_t* meta, void* stream) {
+  return dgr_kmap_probe_mode(DGR_KMAP_GENERAL, out_coords, n_out_max, n_out_dev, ncols, spec, in_keys, in_vals, in_cap,
+                             bloom_words, n_bloom_words, offsets, K, nullptr, 0, nullptr, 0, nullptr, nullptr, 0, bits,
+                             block_cnt, kofs, meta, stream);
 }
 
 int32_t dgr_kmap_fill(const uint32_t* bits, const int32_t* block_cnt, int32_t K, int64_t n_out_max,
@@ -482,15 +593,15 @@ int32_t dgr_kmap_dense(const int32_t* out_coords, int64_t n_out_max, const int32
   const dim3 grid(row_blocks, (K + k_per_block - 1) / k_per_block);
   if (bloom_words != nullptr) {
     const size_t smem = probe_smem_bytes(k_per_block, n_bloom_words);
-    DGR_ENSURE_SMEM((kmap_probe_kernel<true, true>), smem);
-    kmap_probe_kernel<true, true><<<grid, kProbeThreads, smem, st>>>(
+    DGR_ENSURE_SMEM((kmap_probe_kernel<true, true, false>), smem);
+    kmap_probe_kernel<true, true, false><<<grid, kProbeThreads, smem, st>>>(
         out_coords, n_out_dev, n_out_max, ncols, spec, in_keys, in_vals, (uint64_t)in_cap - 1, bloom_words,
-        (uint32_t)n_bloom_words, offsets, K, k_per_block, nullptr, 0, nullptr, 0, nbr, nbr_stride, hit_count);
+        (uint32_t)n_bloom_words, offsets, K, k_per_block, nullptr, 0, nullptr, 0, nbr, nbr_stride, hit_count, 0);
   } else {
     const size_t smem = probe_smem_bytes(k_per_block, 0);
-    kmap_probe_kernel<false, true><<<grid, kProbeThreads, smem, st>>>(
+    kmap_probe_kernel<false, true, false><<<grid, kProbeThreads, smem, st>>>(
         out_coords, n_out_dev, n_out_max, ncols, spec, in_keys, in_vals, (uint64_t)in_cap - 1, nullptr, 1u, offsets, K,
-        k_per_block, nullptr, 0, nullptr, 0, nbr, nbr_stride, hit_count);
+        k_per_block, nullptr, 0, nullptr, 0, nbr, nbr_stride, hit_count, 0);
   }
   dgr_note_launches(1);
   DGR_LAUNCH_CHECK();

@@ -414,10 +414,15 @@ int32_t plan_begin(dgr_ctx* c, const dgr_net* net, Plan& p) {
     DGR_TRY(aalloc(c, (int64_t)m.K * m.W, &m.bits));
     DGR_TRY(aalloc(c, dgr_kmap_cnt_elems(m.K, nmx), &m.cnt));
     DGR_TRY(aalloc(c, m.K + 2, &m.kofs));
-    const bool bloom = Lin.bloom != nullptr && m.K > 27;
-    DGR_TRY(dgr_kmap_probe(Lout.coords, Lout.n_max, Lout.n_dev, ncols, p.spec, Lin.keys, Lin.vals, Lin.cap,
-                           bloom ? Lin.bloom : nullptr, bloom ? Lin.n_bloom : 0, m.offsets, m.K, m.bits, m.cnt, m.kofs,
-                           m.meta, st));
+    // same-stride maps probe half the offsets and mirror the rest; down maps enumerate from the input rows
+    const bool down = m.lout == m.lin + 1 && m.ksize == 3;
+    const int mode = m.lout == m.lin ? DGR_KMAP_SAME : (down ? DGR_KMAP_DOWN : DGR_KMAP_GENERAL);
+    const bool bloom = Lin.bloom != nullptr && m.K > 27 && !down;
+    DGR_TRY(dgr_kmap_probe_mode(mode, Lout.coords, Lout.n_max, Lout.n_dev, ncols, p.spec, Lin.keys, Lin.vals, Lin.cap,
+                                bloom ? Lin.bloom : nullptr, bloom ? Lin.n_bloom : 0, m.offsets, m.K,
+                                down ? Lin.coords : nullptr, down ? Lin.n_max : 0, down ? Lin.n_dev : nullptr,
+                                down ? 1 << m.lin : 0, down ? Lout.keys : nullptr, down ? Lout.vals : nullptr,
+                                down ? Lout.cap : 0, m.bits, m.cnt, m.kofs, m.meta, st));
   }
   return DGR_OK;
 }

@@ -125,7 +125,9 @@ class CoordinateManager:
       # the dense neighbour table is kept only where the output-stationary conv1 kernel reads it
       keep = self.D == 3 and conv_stride == 1 and kernel_size > 3
       self._kmaps[ck] = _abi.kernel_map(m_out.coords, self.spec, m_in.table, m_in.n,
-                                        self._offs(kernel_size, s_in), keep_table=keep)
+                                        self._offs(kernel_size, s_in), keep_table=keep,
+                                        mode=_abi.kmap_mode(s_in, s_out, kernel_size), in_coords=m_in.coords,
+                                        in_stride=s_in, out_table=m_out.table)
     return CoordinateMapKey(s_out), self._kmaps[ck]
 
   def transpose_kernel_map(self, in_key, conv_stride, kernel_size):

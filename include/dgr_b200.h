@@ -704,6 +704,24 @@ int32_t dgr_kmap_probe(const int32_t* out_coords, int64_t n_out_max, const int32
                        const dgr_keyspec_t* spec, const uint64_t* in_keys, const int32_t* in_vals, int64_t in_cap,
                        const uint32_t* bloom_words, int64_t n_bloom_words, const int32_t* offsets, int32_t K,
                        uint32_t* bits, int32_t* block_cnt, int32_t* kofs, int32_t* meta, void* stream);
+/* The same phase 1 with the probe mode explicit; every mode writes the same bits / block_cnt / kofs / meta as
+ * DGR_KMAP_GENERAL (dgr_kmap_probe: every offset probed for every output row).
+ * DGR_KMAP_SAME: a same-stride map (the input table is the output rows' table, offsets the centred odd cube of
+ *   kernel_offsets, axis 0 fastest): only the offsets below the centre are probed; offset K-1-kappa is the
+ *   negation of offset kappa, so each hit also gives the mirrored pair, and the centre holds every row.
+ * DGR_KMAP_DOWN: a kernel-3 map from tensor stride in_stride to 2 in_stride, enumerated from the input rows
+ *   in_coords[n_in] (multiples of in_stride; n_in_dev as n_out_dev): 2^(odd axes) candidate outputs per row,
+ *   looked up in the output rows' table out_keys / out_vals / out_cap; no Bloom filter.
+ * in_coords .. out_cap are read by DGR_KMAP_DOWN only (NULL / 0 otherwise). */
+#define DGR_KMAP_GENERAL 0
+#define DGR_KMAP_SAME 1
+#define DGR_KMAP_DOWN 2
+int32_t dgr_kmap_probe_mode(int32_t mode, const int32_t* out_coords, int64_t n_out_max, const int32_t* n_out_dev,
+                            int32_t ncols, const dgr_keyspec_t* spec, const uint64_t* in_keys, const int32_t* in_vals,
+                            int64_t in_cap, const uint32_t* bloom_words, int64_t n_bloom_words, const int32_t* offsets,
+                            int32_t K, const int32_t* in_coords, int64_t n_in_max, const int32_t* n_in_dev,
+                            int32_t in_stride, const uint64_t* out_keys, const int32_t* out_vals, int64_t out_cap,
+                            uint32_t* bits, int32_t* block_cnt, int32_t* kofs, int32_t* meta, void* stream);
 /* Kernel map, phase 2 (after the caller has read P from meta): in_idx[P], out_idx[P] sorted by (kappa, j),
  * the same lists as the oracle's buckets (oracle/sparse_ops.py). */
 int32_t dgr_kmap_fill(const uint32_t* bits, const int32_t* block_cnt, int32_t K, int64_t n_out_max,
